@@ -1,4 +1,4 @@
-"""3dssd_b200 -- B200 (sm_100a) set-abstraction operators behind the tf_ops / layers_util surface of
+"""3dssd_b200 -- H100 (sm_90a) set-abstraction operators behind the tf_ops / layers_util surface of
 dvlab-research/3DSSD.  Import with importlib.import_module("3dssd_b200") or through the `ssd3d_b200` alias.
 """
 from . import config, dist, head, kitti_io, layers_util, params, tf_ops  # noqa: F401

@@ -1,4 +1,4 @@
-"""Builds libssd3d.so in-tree with nvcc for sm_100a (no torch / pybind dependency: the library is a plain
+"""Builds libssd3d.so in-tree with nvcc for sm_90a (H100) (no torch / pybind dependency: the library is a plain
 C-ABI shared object, see include/ssd3d.h)."""
 import glob
 import os
@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libssd3d.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-fmad=true",
 ]
 
@@ -52,7 +52,7 @@ def _build_to(lib_path, obj_dir, defines, verbose):
         out, _ = p.communicate()
         if p.returncode != 0:
             raise RuntimeError("nvcc failed on %s:\n%s" % (src, out.decode()))
-    cmd = [nvcc, "-shared", "-o", lib_path] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", lib_path] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     subprocess.check_call(cmd)
     return lib_path
 

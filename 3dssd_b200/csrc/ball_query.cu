@@ -1,4 +1,4 @@
-// ball_query.cu -- radius neighbour search for sm_100a.
+// ball_query.cu -- radius neighbour search for sm_90a.
 //
 // Replaces query_ball_point_gpu / query_ball_point_dilated_gpu
 // (/root/reference/lib/utils/tf_ops/grouping/tf_grouping_g.cu:215-255, :308-357).
@@ -116,21 +116,21 @@ ball_query_kernel(const float *__restrict__ xyz1, const float *__restrict__ xyz2
 
         if (!warp_done) {
             const int nsteps = (npts + 31) >> 5;
-            // squared distances of one candidate (32 per step, one per lane) to the warp's 4 queries.  Packed fp32
-            // (FADD2 / FMUL2 / FFMA2, sm_100): two queries per instruction, each lane-half an independent IEEE operation
-            // -> same bits as the reference recipe t = dy*dy ; t = fma(dx,dx,t) ; t = fma(dz,dz,t)
+            // squared distances of one candidate (32 per step, one per lane) to the warp's 4 queries, two queries per
+            // fp32 pair, each half an independent IEEE operation -> same bits as the reference recipe
+            // t = dy*dy ; t = fma(dx,dx,t) ; t = fma(dz,dz,t)
             auto dist4 = [&](int li, float (&tt)[BQ_QW]) -> bool {
                 const float cx = pts[li * 3], cy = pts[li * 3 + 1], cz = pts[li * 3 + 2];
                 const float2 ncx = make_float2(-cx, -cx), ncy = make_float2(-cy, -cy), ncz = make_float2(-cz, -cz);
                 bool near_any = false;
 #pragma unroll
                 for (int q = 0; q < BQ_QW; q += 2) {
-                    const float2 dx = __fadd2_rn(make_float2(qx[q], qx[q + 1]), ncx);
-                    const float2 dy = __fadd2_rn(make_float2(qy[q], qy[q + 1]), ncy);
-                    const float2 dz = __fadd2_rn(make_float2(qz[q], qz[q + 1]), ncz);
-                    float2 t = __fmul2_rn(dy, dy);
-                    t = __ffma2_rn(dx, dx, t);
-                    t = __ffma2_rn(dz, dz, t);
+                    const float2 dx = add2_rn(make_float2(qx[q], qx[q + 1]), ncx);
+                    const float2 dy = add2_rn(make_float2(qy[q], qy[q + 1]), ncy);
+                    const float2 dz = add2_rn(make_float2(qz[q], qz[q + 1]), ncz);
+                    float2 t = mul2_rn(dy, dy);
+                    t = fma2_rn(dx, dx, t);
+                    t = fma2_rn(dz, dz, t);
                     tt[q] = t.x; tt[q + 1] = t.y;
                     near_any = near_any || (DILATED ? (t.x < p.t_max) : !(t.x >= p.t_max)) ||
                                (DILATED ? (t.y < p.t_max) : !(t.y >= p.t_max));

@@ -106,7 +106,7 @@ extern "C" int ssd3d_bn_train(long rows, int c, const float *x, int ldx, const f
     rc = cuda_status(cudaGetLastError(), "bn_finalize_kernel");
     if (rc) return rc;
     const long total = rows * c;
-    const int blocks = (int)((total + 255) / 256 < 148L * 16 ? (total + 255) / 256 : 148L * 16);
+    const int blocks = (int)((total + 255) / 256 < (long)kNumSMs * 16 ? (total + 255) / 256 : (long)kNumSMs * 16);
     scale_shift_act_kernel<<<blocks, 256, 0, st>>>(rows, c, x, ldx, scale, shift, relu, out, ldo);
     SSD3D_LAUNCH_CHECK("scale_shift_act_kernel");
 }

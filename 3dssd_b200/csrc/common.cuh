@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sm_100a kernels of libssd3d.so.
+// common.cuh -- shared helpers for the sm_90a kernels of libssd3d.so.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,9 +23,17 @@ int cuda_status(cudaError_t e, const char *what);
 // cudaGetLastError (capture-safe) reports a failed launch once AND clears it, so later calls do not inherit it
 #define SSD3D_LAUNCH_CHECK(what) return ::ssd3d::cuda_status(cudaGetLastError(), what)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 static inline int ceil_div(long a, long b) { return (int)((a + b - 1) / b); }
+
+// Element-wise fp32 pairs: two independent IEEE round-to-nearest operations each, the same bits as the scalar chain.
+__device__ __forceinline__ float2 add2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c)
+{
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 
 // ---- PTX wrappers ------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -76,7 +84,7 @@ __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity)
         "DONE_%=:\n\t}"
         ::"r"(bar), "r"(parity) : "memory");
 }
-// One lane of a converged warp (for single-thread instructions such as tcgen05.mma / commit issued from code the
+// One lane of a converged warp (for single-thread instructions issued from code the
 // whole warp runs, so that their operands stay in uniform registers).
 __device__ __forceinline__ bool elect_one()
 {

@@ -1,4 +1,4 @@
-// fps.cu -- farthest point sampling for sm_100a.
+// fps.cu -- farthest point sampling for sm_90a.
 //
 // Replaces the reference kernels farthestpointsamplingKernel / farthestpointsamplingwithdistKernel
 // (/root/reference/lib/utils/tf_ops/sampling/tf_sampling_g.cu:124-178, :181-230).
@@ -270,16 +270,16 @@ fps3_direct_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
         // round.  Ties keep the lower slot (a higher slot wins only when STRICTLY greater), i.e. the scan's answer.
         float tv[P];
         {
-            // packed fp32 pairs (FADD2 / FMUL2 / FFMA2): same IEEE operations as d = fma(dz,dz, fma(dy,dy, dx*dx))
+            // fp32 pairs: same IEEE operations as d = fma(dz,dz, fma(dy,dy, dx*dx))
             const float2 nox = make_float2(-ox, -ox), noy = make_float2(-oy, -oy), noz = make_float2(-oz, -oz);
 #pragma unroll
             for (int i = 0; i + 1 < P; i += 2) {
-                const float2 dx = __fadd2_rn(make_float2(px[i], px[i + 1]), nox);
-                const float2 dy = __fadd2_rn(make_float2(py[i], py[i + 1]), noy);
-                const float2 dz = __fadd2_rn(make_float2(pz[i], pz[i + 1]), noz);
-                float2 d = __fmul2_rn(dx, dx);
-                d = __ffma2_rn(dy, dy, d);
-                d = __ffma2_rn(dz, dz, d);
+                const float2 dx = add2_rn(make_float2(px[i], px[i + 1]), nox);
+                const float2 dy = add2_rn(make_float2(py[i], py[i + 1]), noy);
+                const float2 dz = add2_rn(make_float2(pz[i], pz[i + 1]), noz);
+                float2 d = mul2_rn(dx, dx);
+                d = fma2_rn(dy, dy, d);
+                d = fma2_rn(dz, dz, d);
                 td[i] = fminf(d.x, td[i]); td[i + 1] = fminf(d.y, td[i + 1]);
                 tv[i] = td[i]; tv[i + 1] = td[i + 1];
             }

@@ -4,7 +4,7 @@
 // Replaces scatteraddpointKernel (/root/reference/lib/utils/tf_ops/sampling/tf_sampling_g.cu:335-346),
 // group_point_grad_gpu (grouping/tf_grouping_g.cu:383-398) and three_interpolate_grad_gpu
 // (interpolation/tf_interpolate_g.cu:115-140).  Like the reference they scatter with fp32 atomicAdd (RED.ADD on
-// sm_100a), so sums over repeated indices are order-dependent in the last bits: tolerance parity, not bit parity.
+// sm_90a), so sums over repeated indices are order-dependent in the last bits: tolerance parity, not bit parity.
 // The zero-fill the reference's TF op does with cudaMemset before the launcher (tf_sampling.cpp:286,
 // tf_grouping.cpp:510, tf_interpolate.cpp:398) is part of these entry points (cudaMemsetAsync on the same stream).
 #include "common.cuh"

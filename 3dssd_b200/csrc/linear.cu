@@ -6,7 +6,7 @@
 // one kernel per layer instead of ~5 TF kernels that each stream [B,M,K,C] through HBM.
 //
 // This is the exact-fp32 path (CUDA-core FFMA, sequential-k accumulation per output): it serves the layers
-// tensor cores cannot fill (Cin=4 first layer) and is the numerical cross-check of the tcgen05 path
+// tensor cores cannot fill (Cin=4 first layer) and is the numerical cross-check of the wgmma path
 // (mlp_tc.cu).  128x64 output tile per block, 8x4 outputs per thread, k-step 16.
 #include "common.cuh"
 

@@ -1,4 +1,4 @@
-// mlp_tc.cu -- the grouped-MLP layers on the 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// mlp_tc.cu -- the grouped-MLP layers on the Hopper tensor cores (wgmma + TMA + mbarrier pipeline).
 //
 // One layer of the SA point MLP, y = act((x . W) * scale + shift) [+ max-pool over the neighbour axis], i.e. the
 // conv2d/bias/BN/ReLU/reduce_max chain of /root/reference/lib/utils/tf_util.py:127-201, :424-444 and
@@ -7,17 +7,19 @@
 // Precision (DESIGN.md "Grouped MLP"): the reference computes in fp32 and the parity budget is 1e-3 relative.
 // A single TF32/BF16 pass does not hold that through three chained layers, so every fp32 operand is split into
 // two bf16 terms, x = x_hi + x_lo (16 mantissa bits), and the product is evaluated as three bf16 MMAs
-//     x.W ~= x_hi.W_hi + x_lo.W_hi + x_hi.W_lo          (error ~2^-16, fp32 accumulation in TMEM)
+//     x.W ~= x_hi.W_hi + x_lo.W_hi + x_hi.W_lo          (error ~2^-16, fp32 accumulation in registers)
 // at 3x the bf16 tensor rate instead of the 2x-slower TF32 pipe.  Activations travel between layers already
 // split (two bf16 matrices, row-major == K-major), so every operand tile is a plain TMA box in the 128B-swizzled
-// canonical UMMA layout and no conversion happens on the load path.
+// K-major layout the wgmma descriptors read, and no conversion happens on the load path.
 //
-// Kernel shape: 576 threads; warp 0 = TMA producer, warp 1 = MMA issuer (whole warp runs the loop, one elect.sync lane
-// issues), warps 2-9 = operand producers of the gather modes (warp 2 also allocates TMEM), warps 10-17 = epilogue
-// (TMEM -> registers -> scale/shift/ReLU -> fp32 / split-bf16 through TMA tensor stores, or max-pool as a shuffle
-// reduce-and-transpose butterfly; two warps per TMEM lane quarter share the 32-column chunks).
-// Tile 128 rows x BN<=256 columns, K streamed in 64-element blocks through a multi-stage mbarrier ring;
-// two TMEM accumulator buffers let the epilogue of tile i overlap the MMAs of tile i+1.
+// Kernel shape: 640 threads = 5 warpgroups; warp 0 = TMA producer (warps 1-3 idle), warps 4-11 = operand producers of
+// the gather modes, warps 12-19 = two consumer warpgroups.  Consumer warpgroup g owns rows 64g..64g+63 of the tile: it
+// issues the wgmma chain into its registers, stages the fp32 accumulator in shared memory (row-per-thread order), then
+// runs the epilogue (scale/shift/ReLU -> fp32 / split-bf16 through TMA tensor stores, or max-pool as a shuffle
+// reduce-and-transpose butterfly; two warps per 32-row quarter share the 32-column chunks).
+// Tile 128 rows x BN<=64 columns (BN = 32 or 64, a template parameter: the wgmma width is part of the
+// instruction), K streamed in 64-element blocks through a multi-stage mbarrier ring; a stage is released as soon as
+// the wgmma group that read it has retired, so the TMA loads of the next k-blocks overlap the MMAs.
 // Gather modes (TcParams::gather): the operand tile is not read from memory but built in shared memory by the
 // producer warps from neighbour indices (1: concat(features, xyz - centre); 2: the hoisted first conv) and kept
 // resident across the n-tiles of its m-tile (TcParams::astat).
@@ -32,17 +34,20 @@
 
 #include "common.cuh"
 #include "pool.cuh"
+#include "wgmma.cuh"
 
 namespace ssd3d {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;                 // bf16 elements per k-block = one 128-byte swizzle row
-constexpr int TC_PROD_WARP0 = 2;          // warps 2..9: A-operand producers of the gather modes: two threads per tile row, each
-constexpr int TC_PROD_WARPS = 8;          // builds 4 of the 8 16-byte chunks of a k-block (round 2: with 4 warps the producers
-                                          // were busy 50% of the kernel while the MMA warp waited for them 35% of it)
-constexpr int TC_EPI_WARP0 = TC_PROD_WARP0 + TC_PROD_WARPS;   // warps 6..13: epilogue (warp%4 selects the TMEM lane quarter)
+constexpr int TC_PROD_WARP0 = 4;          // warps 4..11: A-operand producers of the gather modes: two threads per tile row, each
+constexpr int TC_PROD_WARPS = 8;          // builds 4 of the 8 16-byte chunks of a k-block
+constexpr int TC_EPI_WARP0 = TC_PROD_WARP0 + TC_PROD_WARPS;   // warps 12..19: the two consumer warpgroups (MMA + epilogue)
 constexpr int TC_EPI_WARPS = 8;
 constexpr int TC_THREADS = (TC_EPI_WARP0 + TC_EPI_WARPS) * 32;
+// 640 threads leave 96 registers per thread: at BN = 64 the consumer already spills 68 bytes (stores) / 76 bytes (loads)
+// per thread to local memory, at BN = 128 about 1 KB, so tiles stop at 64 columns.
+constexpr int TC_MAX_BN = 64;
 constexpr int TC_MAX_STAGES = 4;
 constexpr int TC_MAX_AKB = 4;            // A-stationary mode: k-blocks of an m-tile resident at once (K <= 256)
 constexpr uint32_t TC_A_BYTES = TC_BM * TC_BK * 2;   // one A tile (hi or lo): 16 KiB
@@ -92,32 +97,6 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, uint32_t src, int x, int y)
 {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
@@ -127,12 +106,7 @@ __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// K-major, 128B-swizzled operand tile: rows are 128 bytes, 8-row groups are 1024 bytes apart (SBO), version 1
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr)
-{
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-           (2ull << 61);
-}
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ---- epilogue helpers ---------------------------------------------------------------------------------------
 // order-preserving float <-> uint map (so that an unsigned redux.max is a float max, also for negative values)
@@ -206,7 +180,7 @@ __device__ __forceinline__ void pooled_units_chunk(const TcParams &p, float (&v)
 
 // Developer instrumentation (nvcc -DTC_PROFILE): CTA 0 accumulates, per role, the cycles spent waiting on each barrier
 // and the cycles spent working; printed by the launcher.  Slots: 0 total | 1 tma wait-empty | 2 mma wait-afull |
-// 3 mma wait-full(B) | 4 mma wait-tempty | 5 mma issue | 6 prod wait-slot | 7 prod load+math | 8 epi wait-tfull | 9 epi work
+// 3 mma wait-full(B) | 4 - | 5 mma issue | 6 prod wait-slot | 7 prod load+math | 8 mma drain | 9 epi work
 #ifdef TC_PROFILE
 __device__ long long tc_prof[16];
 #define TCP_DECL long long tcp_t = clock64(); const bool tcp_on = blockIdx.x == 0 && lane == 0
@@ -216,7 +190,13 @@ __device__ long long tc_prof[16];
 #define TCP(i) do { } while (0)
 #endif
 
+// Accumulator staging of one consumer warpgroup: 64 rows x (BN + 4) fp32 (the pad keeps both the fragment writes
+// and the row-per-thread float4 reads free of bank conflicts)
+template <int BN> __host__ __device__ constexpr int tc_acc_pitch() { return BN + 4; }
+static size_t tc_acc_bytes(int bn) { return (size_t)TC_BM * (bn + 4) * sizeof(float); }
+
 // ---------------------------------------------------------------------------------------------------------
+template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
                  const __grid_constant__ CUtensorMap map_bhi, const __grid_constant__ CUtensorMap map_blo,
@@ -224,8 +204,9 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                  const __grid_constant__ CUtensorMap map_of32, const TcParams p)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [stages] x { A_hi | A_lo | B_hi | B_lo }, per-warp output blocks (4 KiB each), then scale/shift
-    const uint32_t b_bytes = (uint32_t)p.bn * TC_BK * 2;
+    // carve: [resident A tiles] [stages] x { A_hi | A_lo | B_hi | B_lo }, per-warp output blocks (4 KiB each),
+    // accumulator staging, then scale/shift
+    const uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;
     const int nkb = (p.kp + TC_BK - 1) / TC_BK;
     const uint32_t a_tile = (uint32_t)nkb * 2u * TC_A_BYTES;                        // one resident A tile: [nkb] x { A_hi | A_lo }
     const uint32_t a_region = (uint32_t)p.astat * a_tile;
@@ -237,13 +218,13 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
     const int ncov = p.n_tiles * p.bn + 32;
     uint8_t *ring = smem + a_region;
     uint8_t *out_stage = ring + (size_t)p.stages * stage_bytes;          // [8 warps][4 KiB], 4 KiB aligned
-    float *s_scale = reinterpret_cast<float *>(out_stage + (p.tma_store ? TC_EPI_WARPS * 4096 : 0));
+    float *s_acc = reinterpret_cast<float *>(out_stage + (p.tma_store ? TC_EPI_WARPS * 4096 : 0));   // [2 wg][64][BN+4]
+    float *s_scale = s_acc + TC_BM * tc_acc_pitch<BN>();
     float *s_shift = s_scale + ncov;
     float *s_wx = s_shift + ncov;                                        // [3][kp] (hoisted mode only)
 
-    __shared__ unsigned long long full_bar[TC_MAX_STAGES], empty_bar[TC_MAX_STAGES], tfull_bar[2], tempty_bar[2];
+    __shared__ unsigned long long full_bar[TC_MAX_STAGES], empty_bar[TC_MAX_STAGES];
     __shared__ unsigned long long afull_bar[2 * TC_MAX_AKB], aempty_bar[2 * TC_MAX_AKB];   // [A buffer][k-block]
-    __shared__ uint32_t tmem_base_smem;
     __shared__ float pool_xs[2 * 4 * 32];
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // provably warp-uniform
@@ -265,15 +246,11 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
     };
 
     if (threadIdx.x == 0) {
-        // full barrier: the TMA thread's expect_tx arrival (+ one arrival per producer warp in gather mode)
-        for (int s = 0; s < p.stages; s++) { mbar_init(smem_u32(&full_bar[s]), (p.gather && !p.astat) ? 1 + TC_PROD_WARPS : 1); mbar_init(smem_u32(&empty_bar[s]), 1); }
-        for (int k = 0; k < 2 * TC_MAX_AKB; k++) { mbar_init(smem_u32(&afull_bar[k]), TC_PROD_WARPS); mbar_init(smem_u32(&aempty_bar[k]), 1); }
-        for (int a = 0; a < 2; a++) { mbar_init(smem_u32(&tfull_bar[a]), 1); mbar_init(smem_u32(&tempty_bar[a]), TC_EPI_WARPS); }
+        // full barrier: the TMA thread's expect_tx arrival (+ one arrival per producer warp in gather mode);
+        // empty barriers: one arrival per consumer warp once its wgmma group reading the slot has retired
+        for (int s = 0; s < p.stages; s++) { mbar_init(smem_u32(&full_bar[s]), (p.gather && !p.astat) ? 1 + TC_PROD_WARPS : 1); mbar_init(smem_u32(&empty_bar[s]), TC_EPI_WARPS); }
+        for (int k = 0; k < 2 * TC_MAX_AKB; k++) { mbar_init(smem_u32(&afull_bar[k]), TC_PROD_WARPS); mbar_init(smem_u32(&aempty_bar[k]), TC_EPI_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     for (int i = threadIdx.x; i < ncov; i += TC_THREADS) {      // columns >= n: scale = shift = 0 -> exact zeros
         s_scale[i] = i < p.n ? __ldg(p.scale + i) : 0.0f;
@@ -284,11 +261,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
             const int a = i / p.kp, k = i - a * p.kp;
             s_wx[i] = k < p.g_c ? __ldg(p.g_wx + a * p.g_c + k) : 0.0f;
         }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-
     if (warp == 0) {
         // ===== TMA producer =====
         if (lane == 0) {
@@ -317,58 +290,10 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: the whole warp runs the loop (uniform control flow keeps descriptors in uniform registers
-        // and tcgen05.mma free of a per-instruction election loop), one elected lane issues =====
-        {
-            // instruction descriptor: D=f32, A=B=bf16, both K-major, N = bn, M = 128
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.bn >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-            int it = 0, tcount = 0, mi = 0, mt, nt;
-            TCP_DECL;
-            for (int i = 0; tile_at(i, mt, nt); i++, tcount++) {
-                const int acc = tcount & 1;
-                TCP(5);
-                mbar_wait_cta(smem_u32(&tempty_bar[acc]), (((uint32_t)(tcount >> 1)) & 1u) ^ 1u);
-                TCP(4);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.bn);
-                const bool last_nt = nt == p.n_tiles - 1;
-                for (int kb = 0; kb < nkb; kb++, it++) {
-                    const int s = it % p.stages;
-                    TCP(5);
-                    const int ab = p.astat == 2 ? (mi & 1) : 0;                 // resident A buffer of this m-tile
-                    const uint32_t aph = (uint32_t)(p.astat == 2 ? (mi >> 1) : mi) & 1u;   // how often it has been used before
-                    if (p.astat && nt == 0) mbar_wait_cta(smem_u32(&afull_bar[ab * TC_MAX_AKB + kb]), aph);   // this m-tile's A k-block
-                    TCP(2);
-                    mbar_wait_cta(smem_u32(&full_bar[s]), (uint32_t)(it / p.stages) & 1u);
-                    TCP(3);
-                    tc_fence_after();
-                    const uint32_t base = smem_u32(ring + (size_t)s * stage_bytes);
-                    const uint32_t abase = p.astat ? smem_u32(smem) + (uint32_t)ab * a_tile + (uint32_t)kb * 2u * TC_A_BYTES : base;
-                    const int ksteps = min(TC_BK, p.kp - kb * TC_BK) / 16;
-                    const uint64_t a_hi = umma_desc(abase), a_lo = umma_desc(abase + TC_A_BYTES);
-                    const uint64_t b_hi = umma_desc(base + b_off), b_lo = umma_desc(base + b_off + b_bytes);
-                    if (elect_one()) {
-                        for (int ks = 0; ks < ksteps; ks++) {          // +2 per k-step: 32 bytes in the address field
-                            const uint32_t first = (kb | ks) ? 1u : 0u;
-                            umma_bf16(d_tmem, a_hi + 2 * ks, b_hi + 2 * ks, idesc, first);
-                            umma_bf16(d_tmem, a_lo + 2 * ks, b_hi + 2 * ks, idesc, 1u);
-                            umma_bf16(d_tmem, a_hi + 2 * ks, b_lo + 2 * ks, idesc, 1u);
-                        }
-                        umma_commit(smem_u32(&empty_bar[s]));   // ring stage free once these MMAs retire
-                        if (p.astat && last_nt) umma_commit(smem_u32(&aempty_bar[ab * TC_MAX_AKB + kb]));   // A k-block free again
-                    }
-                    __syncwarp();
-                }
-                if (elect_one()) umma_commit(smem_u32(&tfull_bar[acc]));   // accumulator ready for the epilogue
-                __syncwarp();
-                if (last_nt) mi++;
-            }
-        }
     } else if (warp >= TC_PROD_WARP0 && warp < TC_EPI_WARP0) {
         // ===== A-operand producers (gather mode): 128 threads, one row of the tile each.  A row's source features are
         // one contiguous run (16-byte loads when c % 4 == 0); all loads of a 64-wide k-block are issued before the
-        // values are split into bf16 hi/lo and stored as 16-byte chunks in the K-major SWIZZLE_128B layout the UMMA
+        // values are split into bf16 hi/lo and stored as 16-byte chunks in the K-major SWIZZLE_128B layout the wgmma
         // descriptor expects.
         if (p.gather) {
             const int pt = threadIdx.x - TC_PROD_WARP0 * 32;
@@ -463,34 +388,83 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
             }
         }
     } else if (warp >= TC_EPI_WARP0) {
-        // ===== epilogue: 8 warps; warp%4 = TMEM lane quarter (rows), (warp-4)/4 = which half of the 32-column chunks
-        const int q = warp & 3;
-        const int h = (warp - TC_EPI_WARP0) >> 2;
-        const int nchunks = (p.bn + 31) / 32;
-        int tcount = 0, mt, nt;
+        // ===== consumers: warpgroup g = rows 64g..64g+63 of the tile.  MMAs: the whole warpgroup issues the wgmma chain
+        // of every k-block into its registers.  Epilogue: warp w of the group handles the 32-row quarter q = 2g + (w & 1)
+        // and the 32-column chunks of parity h = w >> 1, one row per thread, from the staged accumulator.
+        constexpr int PITCH = tc_acc_pitch<BN>();
+        const int g = (warp - TC_EPI_WARP0) >> 2, w = warp & 3;
+        const int q = 2 * g + (w & 1);
+        const int h = w >> 1;
+        const int wg_bar = 4 + g;                                        // named barrier of this warpgroup (2, 3: pooling)
+        float *acc_g = s_acc + g * 64 * PITCH;
+        constexpr int nchunks = BN / 32;
+        int it = 0, mi = 0, mt, nt;
         TCP_DECL;
-        for (int i = 0; tile_at(i, mt, nt); i++, tcount++) {
-            const int acc = tcount & 1;
-            if (warp == TC_EPI_WARP0) TCP(9);
-            mbar_wait_cta(smem_u32(&tfull_bar[acc]), ((uint32_t)(tcount >> 1)) & 1u);
+        for (int i = 0; tile_at(i, mt, nt); i++) {
+            const bool last_nt = nt == p.n_tiles - 1;
+            float d[BN / 2];
+            int prev_s = -1, prev_kb = 0;
+            const int ab = p.astat == 2 ? (mi & 1) : 0;                  // resident A buffer of this m-tile
+            const uint32_t aph = (uint32_t)(p.astat == 2 ? (mi >> 1) : mi) & 1u;   // how often it has been used before
+            // a ring stage (and, after the last n-tile, a resident A k-block) is free once the wgmma group reading it retired
+            auto release = [&](int s, int kb) {
+                if (lane == 0) {
+                    mbar_arrive(smem_u32(&empty_bar[s]));
+                    if (p.astat && last_nt) mbar_arrive(smem_u32(&aempty_bar[ab * TC_MAX_AKB + kb]));
+                }
+            };
+            for (int kb = 0; kb < nkb; kb++, it++) {
+                const int s = it % p.stages;
+                if (warp == TC_EPI_WARP0) TCP(5);
+                if (p.astat && nt == 0) mbar_wait_cta(smem_u32(&afull_bar[ab * TC_MAX_AKB + kb]), aph);   // this m-tile's A k-block
+                if (warp == TC_EPI_WARP0) TCP(2);
+                mbar_wait_cta(smem_u32(&full_bar[s]), (uint32_t)(it / p.stages) & 1u);
+                if (warp == TC_EPI_WARP0) TCP(3);
+                const uint32_t base = smem_u32(ring + (size_t)s * stage_bytes);
+                const uint32_t abase = (p.astat ? smem_u32(smem) + (uint32_t)ab * a_tile + (uint32_t)kb * 2u * TC_A_BYTES : base) +
+                                       (uint32_t)g * (64u * 128u);        // this warpgroup's 64 rows (8 swizzle atoms)
+                const int ksteps = min(TC_BK, p.kp - kb * TC_BK) / 16;
+                const uint64_t a_hi = wg_desc(abase, 128), a_lo = wg_desc(abase + TC_A_BYTES, 128);
+                const uint64_t b_hi = wg_desc(base + b_off, 128), b_lo = wg_desc(base + b_off + b_bytes, 128);
+                wg_fence();
+                for (int ks = 0; ks < ksteps; ks++)                      // +2 per k-step: 32 bytes in the address field
+                    wg_mma3<BN>(d, a_hi + 2 * ks, a_lo + 2 * ks, b_hi + 2 * ks, b_lo + 2 * ks, (kb | ks) ? 1u : 0u);
+                wg_commit();
+                wg_wait<1>();                                            // the previous k-block's group has retired
+                if (prev_s >= 0) release(prev_s, prev_kb);
+                prev_s = s; prev_kb = kb;
+            }
+            wg_wait<0>();
+            release(prev_s, prev_kb);
+            if (last_nt) mi++;
             if (warp == TC_EPI_WARP0) TCP(8);
-            tc_fence_after();
+            // stage the accumulator: fragment rows 16w + lane/4 (+8), columns 8j + 2(lane%4)
+            named_bar_sync(wg_bar, 128);                                 // the previous tile's epilogue has read the buffer
+            {
+                const int r0 = w * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < BN / 8; j++) {
+                    *reinterpret_cast<float2 *>(acc_g + r0 * PITCH + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+                    *reinterpret_cast<float2 *>(acc_g + (r0 + 8) * PITCH + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+                }
+            }
+            named_bar_sync(wg_bar, 128);
             const long row = (long)mt * TC_BM + q * 32 + lane;
             const bool row_ok = row < rows;
+            const float *acc_row = acc_g + ((w & 1) * 32 + lane) * PITCH;
             for (int ci = h; ci < nchunks; ci += 2) {
                 const int c0 = ci * 32;
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * p.bn + c0), r);
                 const int col0 = nt * p.bn + c0;
                 float v[32];
 #pragma unroll
                 for (int j4 = 0; j4 < 32; j4 += 4) {
+                    const float4 a4 = *reinterpret_cast<const float4 *>(acc_row + c0 + j4);
                     const float4 sc = *reinterpret_cast<const float4 *>(s_scale + col0 + j4);
                     const float4 sh = *reinterpret_cast<const float4 *>(s_shift + col0 + j4);
-                    v[j4 + 0] = fmaf(__uint_as_float(r[j4 + 0]), sc.x, sh.x);
-                    v[j4 + 1] = fmaf(__uint_as_float(r[j4 + 1]), sc.y, sh.y);
-                    v[j4 + 2] = fmaf(__uint_as_float(r[j4 + 2]), sc.z, sh.z);
-                    v[j4 + 3] = fmaf(__uint_as_float(r[j4 + 3]), sc.w, sh.w);
+                    v[j4 + 0] = fmaf(a4.x, sc.x, sh.x);
+                    v[j4 + 1] = fmaf(a4.y, sc.y, sh.y);
+                    v[j4 + 2] = fmaf(a4.z, sc.z, sh.z);
+                    v[j4 + 3] = fmaf(a4.w, sc.w, sh.w);
                 }
                 if (p.relu) {
 #pragma unroll
@@ -571,18 +545,9 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&tempty_bar[acc]));   // 8 arrivals (one per epilogue warp) free the buffer
+            if (warp == TC_EPI_WARP0) TCP(9);
         }
         if (p.tma_store && lane == 0) tma_store_wait_all();           // global writes complete before the CTA retires
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
     }
 }
 
@@ -867,47 +832,31 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     // when split outputs are requested the tile must also cover (and zero) the padding columns n..ld_split-1
     const int ncover = out_hi && pool <= 1 ? (ld_split > n16 ? ld_split : n16) : n16;
     // Non-pooled outputs go through TMA tensor stores when exactly one kind is requested and it is 16-byte
-    // addressable; their tiles are capped at 128 columns to leave shared memory for the per-warp store blocks.
+    // addressable.
     const bool want_f32 = out_f32 != nullptr, want_split = out_hi != nullptr;
     bool tma_store = pool <= 1 && (want_f32 != want_split);
     if (tma_store && want_f32) tma_store = (ld_f32 % 4 == 0) && ((reinterpret_cast<uintptr_t>(out_f32) & 15u) == 0);
     p.tma_store = tma_store ? 1 : 0;
     const size_t budget = 224 * 1024 - 1024;   // 227 KiB per CTA minus static barriers and the 1 KiB alignment slack
     const int nkb = (kp + TC_BK - 1) / TC_BK;
-    auto misc_bytes = [&](int bn) {            // scale/shift (+ hoisted Wx) + per-warp store blocks
+    auto misc_bytes = [&](int bn) {            // scale/shift (+ hoisted Wx) + per-warp store blocks + accumulator staging
         const int nt = (ncover + bn - 1) / bn;
         return 2 * ((size_t)nt * bn + 32) * sizeof(float) + (tma_store ? TC_EPI_WARPS * 4096 : 0) +
-               (g && g->wx ? (size_t)3 * kp * sizeof(float) : 0);
+               (g && g->wx ? (size_t)3 * kp * sizeof(float) : 0) + tc_acc_bytes(bn);
     };
-    // gather modes keep the produced A tile resident (A-stationary) when all its k-blocks fit next to a >= 2-stage
-    // weight ring: the producers then build it once per m-tile, not once per (m, n) tile
+    // Tile widths are multiples of 32 (columns beyond the weight rows come in as TMA zero fill and are never stored),
+    // widest first: every wgmma re-reads its 64-row A slab from shared memory, so a wide tile reads A fewer times.
+    const int ncover32 = (ncover + 31) / 32 * 32;
+    const int cands[2] = {TC_MAX_BN, 32};
     int bn = 0, stages = 0;
     p.astat = 0;
+    // gather modes keep the produced A tile resident (A-stationary) when all its k-blocks fit next to a >= 2-stage
+    // weight ring: the producers then build it once per m-tile, not once per (m, n) tile.  (The kernel can also
+    // alternate between two resident tiles, TcParams::astat == 2; this planner does not choose it.)
     if (g && nkb <= TC_MAX_AKB) {
         const size_t a_tile = (size_t)nkb * 2 * TC_A_BYTES;
-        // TWO resident A tiles would let the producers build m-tile i+1 while the MMAs of m-tile i run (with one tile the two
-        // alternate).  The second tile has to be paid for with the per-warp TMA store blocks -- split outputs then leave as
-        // direct 16-byte stores -- and that trade LOSES on the layer-3 shapes: 33 / 43 / 47 us with one tile + TMA stores vs
-        // 57 / 71 / 80 us with two tiles + direct stores (round 2, profiles/r02_bench_1gpu_run4_two_a_tiles.json).  The kernel
-        // keeps the capability (TcParams::astat == 2); the planner does not choose it.
-        constexpr bool kTwoATiles = false;
-        if (kTwoATiles && pool <= 1 && want_split && !want_f32) {
-            const bool saved = tma_store;
-            tma_store = false;
-            const int b = ncover < 128 ? ncover : 128;
-            const size_t need = 2 * a_tile + misc_bytes(b);
-            if (need + 2 * (size_t)(2 * b * TC_BK * 2) <= budget) {
-                bn = b;
-                stages = (int)((budget - need) / (size_t)(2 * b * TC_BK * 2));
-                p.astat = 2;
-            } else {
-                tma_store = saved;
-            }
-        }
-        const int cands[4] = {256, 128, 96, 64};            // widest tile first: a tcgen05.mma has a fixed cost per instruction
-        for (int ci = tma_store ? 1 : 0; ci < 4 && !bn; ci++) {
-            const int cand = cands[ci];
-            const int b = ncover < cand ? ncover : cand;
+        for (int ci = 0; ci < 2 && !bn; ci++) {
+            const int b = ncover32 < cands[ci] ? ncover32 : cands[ci];
             const size_t need = a_tile + misc_bytes(b);
             if (need + 2 * (size_t)(2 * b * TC_BK * 2) <= budget) {
                 bn = b;
@@ -916,13 +865,14 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
             }
         }
     }
-    p.tma_store = tma_store ? 1 : 0;
-    if (!bn) {
-        const int bn_cap = tma_store ? 128 : 256;
-        bn = ncover < bn_cap ? ncover : bn_cap;
-        stages = (int)((budget - misc_bytes(bn)) / (2 * (size_t)TC_A_BYTES + 2 * (size_t)bn * TC_BK * 2));
+    for (int ci = 0; ci < 2 && !bn; ci++) {
+        const int b = ncover32 < cands[ci] ? ncover32 : cands[ci];
+        const size_t misc = misc_bytes(b);
+        const int st = misc < budget ? (int)((budget - misc) / (2 * (size_t)TC_A_BYTES + 2 * (size_t)b * TC_BK * 2)) : 0;
+        if (st >= 2) { bn = b; stages = st; }
     }
     p.bn = bn;
+    SSD3D_REQUIRE(bn > 0, "linear_tc: tile does not fit shared memory");
     p.n_tiles = (ncover + p.bn - 1) / p.bn;
     p.m_tiles = (int)((rows + TC_BM - 1) / TC_BM);
     const size_t stage_bytes = (p.astat ? 0 : 2 * (size_t)TC_A_BYTES) + 2 * (size_t)p.bn * TC_BK * 2;
@@ -953,7 +903,8 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     if (tma_store && want_f32 && (rc = make_out_map(&mof, out_f32, rows, n, ld_f32, true)) != 0) return rc;
 
     const size_t smem = stages * stage_bytes + pool_bytes + 1024;
-    cudaError_t e = cudaFuncSetAttribute((const void *)linear_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const void *kern = p.bn == 32 ? (const void *)linear_tc_kernel<32> : (const void *)linear_tc_kernel<TC_MAX_BN>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return cuda_status(e, "linear_tc attr");
     const int total = p.astat ? p.m_tiles : p.m_tiles * p.n_tiles;    // A-stationary CTAs own whole m-tiles
     const int grid = total < kNumSMs ? total : kNumSMs;
@@ -964,7 +915,10 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     cudaEventCreate(&pe0); cudaEventCreate(&pe1);
     cudaEventRecord(pe0, stream);
 #endif
-    linear_tc_kernel<<<grid, TC_THREADS, smem, stream>>>(mah, mal, mbh, mbl, moh, mol, mof, p);
+    switch (p.bn) {
+        case 32: linear_tc_kernel<32><<<grid, TC_THREADS, smem, stream>>>(mah, mal, mbh, mbl, moh, mol, mof, p); break;
+        default: linear_tc_kernel<TC_MAX_BN><<<grid, TC_THREADS, smem, stream>>>(mah, mal, mbh, mbl, moh, mol, mof, p); break;
+    }
 #ifdef TC_PROFILE
     {
         cudaEventRecord(pe1, stream);

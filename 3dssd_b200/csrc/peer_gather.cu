@@ -2,9 +2,8 @@
 //
 // The reference has no multi-GPU inference (lib/core/evaluator.py:145-147 runs one GPU, batch 1); the sharded step of
 // this repo ends with an all-gather of the per-scene detection block every rank's NMS produced (3dssd_b200/dist.py).
-// ncclAllGather does that correctly, but captured into 8-24 concurrently replayed step graphs it capped the step at
-// 1.19 ms on 2 and 8 GPUs while one GPU ran 1.01 ms (profiles/r02_bench_2gpu_nccl_p24.json).  The exchange is 3.6 KB per
-// scene: all it needs is  store my slice into every peer's buffer -> publish a flag -> wait for the peers' flags.
+// ncclAllGather does that correctly, but captured into 8-24 concurrently replayed step graphs it adds a per-step cost
+// that a one-GPU step does not have.  The exchange is 3.6 KB per scene: all it needs is  store my slice into every peer's buffer -> publish a flag -> wait for the peers' flags.
 //
 // Buffers (3dssd_b200/dist.py PeerGather): every rank owns a SYMMETRIC allocation, mapped into all peers
 // (torch.distributed._symmetric_memory: cuMem + fabric / fd handles), holding for each of two parities a receive area

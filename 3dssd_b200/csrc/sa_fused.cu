@@ -1,20 +1,23 @@
-// sa_fused.cu -- one SA scale in ONE kernel: gather + concat + (conv+BN+ReLU) x L + max-pool + mask, tcgen05.
+// sa_fused.cu -- one SA scale in ONE kernel: gather + concat + (conv+BN+ReLU) x L + max-pool + mask, wgmma.
 //
 // Fuses lib/utils/layers_util.py:157-180 of the reference (idx masking, 2x group_point, centre subtraction, concat,
 // the conv2d/bias/BN/ReLU stack, reduce_max, mask multiply -- ~25 TF kernels per scale, each streaming [B,M,K,C]
 // through HBM) for the layers whose weights fit in shared memory (3DSSD layer1/layer2: 93% of the grouped rows).
 // Nothing but the neighbour indices, the gathered source rows (L2-resident) and the pooled [B,M,C3] result touches
-// global memory; activations go TMEM -> registers -> shared memory (already split in bf16 hi/lo and already in the
-// 128B-swizzled K-major layout the next layer's UMMA descriptor expects).
+// global memory; activations go wgmma registers -> fp32 staging in shared memory -> registers -> shared memory (already
+// split in bf16 hi/lo and already in the swizzled K-major layout the next layer's wgmma descriptors expect).
 //
 // Per CTA: S "slots" of 128*WG threads (a slot works on one 128-row tile = 128/K neighbour groups; its WG warpgroups
 // split the 16-byte chunks of the gather and the 32-column chunks of every epilogue):
 //   weights of all layers (hi+lo images, pre-swizzled on the host) are bulk-copied to shared memory once and shared
-//   by the slots; each slot owns ONE operand buffer, one TMEM accumulator and one mbarrier and loops over tiles:
-//   gather+split -> [fence.proxy.async] -> layer-0 MMAs (one thread) -> epilogue (tcgen05.ld, scale/shift/ReLU,
-//   split) written IN PLACE over the operand the finished MMAs no longer need -> ... -> last layer: max-pool.
-// Small stacks (layer1: ~30 KiB) run S=1 with up to 6 CTAs per SM; stacks whose weights fill most of shared memory
-// (layer2: 68-92 KiB) run one CTA per SM with S=2..3 slots, so gather / MMA / epilogue phases still overlap.
+//   by the slots; each slot owns ONE operand buffer and one fp32 accumulator staging buffer and loops over tiles:
+//   gather+split -> [fence.proxy.async] -> layer-0 MMAs (the slot's warpgroups split the 64-row halves of the tile and
+//   the <= 64-column chunks of the layer; each chunk is one wgmma chain into registers, staged row-major) -> epilogue
+//   (scale/shift/ReLU, split) written IN PLACE over the operand the finished MMAs no longer need -> ... -> last layer:
+//   max-pool.
+// Small stacks (layer1) run S=1 with several CTAs per SM; stacks whose weights fill most of shared memory (layer2) run
+// one CTA per SM with as many slots as fit, each of two warpgroups -- one slot for the layer-2 stacks, whose staged
+// accumulator (128 x 132 fp32) and weights leave no room for a second, so their tiles overlap only across SMs.
 // Hoisted mode (SfParams::hoist): the scale's first conv has been moved to a per-point table z (include/ssd3d.h,
 // ssd3d_sa_mlp_fused_hoisted); the gather then builds relu(z[idx] + (xyz[idx] - centre) . Wx') and the stack starts at
 // the second conv.
@@ -32,6 +35,7 @@
 
 #include "common.cuh"
 #include "pool.cuh"
+#include "wgmma.cuh"
 
 namespace ssd3d {
 
@@ -67,48 +71,13 @@ struct SfParams {
     int nfull[SF_MAX_LAYERS];        // layer l's K = nfull 64-wide k-blocks (128-byte rows) + one tail block
     int rbt[SF_MAX_LAYERS];          // bytes per row of the tail block: 0 (none), 32 (16 wide), 64 (32), 128 (48)
     uint32_t abuf_bytes;             // operand buffer of one slot
-    uint32_t tmem_cols;              // accumulator columns of one slot
-    uint32_t tmem_alloc;             // power of two >= slots * tmem_cols
+    uint32_t acc_cols;               // staged accumulator columns of one slot (widest layer, rounded up to 32)
     float *out_f32; int ld_f32;
     __nv_bfloat16 *out_hi, *out_lo; int ld_split;
     int pool_first;                  // caller guarantees scale >= 0 in the LAST layer: pool raw accumulators, affine after
 };
 
-__device__ __forceinline__ void sf_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void sf_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void sf_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// K-major operand descriptor; rb = bytes per row = swizzle span (128 -> SWIZZLE_128B, 64 -> _64B, 32 -> _32B),
-// 8-row groups are 8*rb bytes apart (SBO), descriptor version 1
-__device__ __forceinline__ uint64_t sf_desc(uint32_t smem_addr, int rb)
-{
-    const uint64_t layout = rb == 128 ? 2ull : (rb == 64 ? 4ull : 6ull);
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)((8 * rb) >> 4) << 32) | (1ull << 46) |
-           (layout << 61);
-}
-__device__ __forceinline__ void sf_mma(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a), "l"(b), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void sf_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void sf_tmem_ld32(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 // x = hi + lo with hi = bf16(x), lo = bf16(x - hi); two values per call, packed {x1 : x0} like two adjacent bf16
 __device__ __forceinline__ void sf_split_pair(float x0, float x1, uint32_t &hw, uint32_t &lw)
 {
@@ -160,8 +129,8 @@ __device__ __forceinline__ float sf_ord2f(uint32_t u) { return __uint_as_float((
 // layer, block layout, blob offsets, neighbours per group).  SfDyn reads the answers from the parameter block at run
 // time (any stack the planner accepts); SfStat<...> answers at COMPILE time for the stacks of the shipped 3DSSD
 // configuration, so that after unrolling the layer loop every address computation, chunk bound and pooling width is a
-// literal: profiling the dynamic kernel showed ~50% of its issued instructions to be integer / branch / uniform-register
-// bookkeeping of exactly these questions (profiles/r02_fused_instruction_mix.txt).
+// literal (integer / branch / uniform-register bookkeeping of exactly these questions is otherwise a large share of the
+// kernel's issued instructions).
 __host__ __device__ constexpr int sf_r16(int x) { return (x + 15) / 16 * 16; }
 __host__ __device__ constexpr int sf_rbt_of(int kp) { return kp % 64 == 0 ? 0 : (kp % 64 <= 16 ? 32 : (kp % 64 <= 32 ? 64 : 128)); }
 __host__ __device__ constexpr uint32_t sf_abuf_of(int kp)
@@ -189,7 +158,7 @@ struct SfDyn {
     __device__ __forceinline__ uint32_t w_total() const { return p.w_total; }
     __device__ __forceinline__ uint32_t ss_total() const { return p.ss_total; }
     __device__ __forceinline__ uint32_t abuf_bytes() const { return p.abuf_bytes; }
-    __device__ __forceinline__ uint32_t tmem_cols() const { return p.tmem_cols; }
+    __device__ __forceinline__ uint32_t acc_cols() const { return p.acc_cols; }
 };
 
 // Hoisted stacks of two convs (the shipped configuration): operand width K0 = n1 of the hoisted first conv, then
@@ -215,10 +184,7 @@ struct SfStat {
     __device__ __forceinline__ constexpr uint32_t w_total() const { return 2u * w_half(0) + 2u * w_half(1); }
     __device__ __forceinline__ constexpr uint32_t ss_total() const { return 2u * (uint32_t)sspad(0) + 2u * (uint32_t)sspad(1); }
     __device__ __forceinline__ constexpr uint32_t abuf_bytes() const { return sf_abuf_of(KP0) > sf_abuf_of(NP0) ? sf_abuf_of(KP0) : sf_abuf_of(NP0); }
-    __device__ __forceinline__ constexpr uint32_t tmem_cols() const
-    {
-        return (NP0 > NP1 ? NP0 : NP1) <= 32 ? 32u : ((NP0 > NP1 ? NP0 : NP1) <= 64 ? 64u : ((NP0 > NP1 ? NP0 : NP1) <= 128 ? 128u : 256u));
-    }
+    __device__ __forceinline__ constexpr uint32_t acc_cols() const { return (uint32_t)((NP0 > NP1 ? NP0 : NP1) + 31) / 32 * 32; }
 };
 
 #ifdef SF_PROFILE
@@ -290,6 +256,51 @@ __device__ __forceinline__ void sf_pool_atomic8(const SfParams &p, float (&v)[32
     }
 }
 
+// One work item of a layer's MMAs: rows 64*hf .. 64*hf+63 of the slot's tile, output columns n0 .. n0+W-1, over the
+// whole K of layer l (full 64-wide blocks + the tail block), issued by one warpgroup as a single wgmma chain; the fp32
+// result is staged row-major in acc (pitch floats per row), where the row-per-thread epilogue reads it.
+template <int W, class C>
+__device__ __forceinline__ void sf_mma_chunk(const C &cfg, int l, uint32_t abase, uint32_t wbase, int hf, int n0, float *acc,
+                                             int pitch, int wq, int lane)
+{
+    float d[W / 2];
+    const int nfull = cfg.nfull(l), rbt = cfg.rbt(l);
+    const uint32_t npad = (uint32_t)cfg.npad(l), whalf = cfg.w_half(l);
+    uint32_t accumulate = 0u;
+    // descriptors advance by (bytes >> 4) in their address field; shared memory < 256 KiB: no carry out of it
+    wg_fence();
+#pragma unroll (C::kStatic ? 4 : 1)
+    for (int kb = 0; kb < nfull; kb++) {
+        const uint64_t a_hi = wg_desc(abase + (uint32_t)kb * (2u * 128u * 128u) + (uint32_t)hf * (64u * 128u), 128);
+        const uint64_t b_hi = wg_desc(wbase + (uint32_t)kb * (npad * 128u) + (uint32_t)n0 * 128u, 128);
+        const uint64_t a_lo = a_hi + ((128u * 128u) >> 4), b_lo = b_hi + (whalf >> 4);
+#pragma unroll
+        for (int kin = 0; kin < 4; kin++) {
+            wg_mma3<W>(d, a_hi + 2 * kin, a_lo + 2 * kin, b_hi + 2 * kin, b_lo + 2 * kin, accumulate);
+            accumulate = 1u;
+        }
+    }
+    if (rbt) {
+        const uint64_t a_hi = wg_desc(abase + (uint32_t)nfull * (2u * 128u * 128u) + (uint32_t)hf * (64u * (uint32_t)rbt), rbt);
+        const uint64_t b_hi = wg_desc(wbase + (uint32_t)nfull * (npad * 128u) + (uint32_t)n0 * (uint32_t)rbt, rbt);
+        const uint64_t a_lo = a_hi + ((128u * (uint32_t)rbt) >> 4), b_lo = b_hi + (whalf >> 4);
+        const int nt = rbt == 128 ? 3 : (rbt >> 5);              // 16-wide k-steps of the tail block
+#pragma unroll (C::kStatic ? 3 : 1)
+        for (int kin = 0; kin < nt; kin++) {
+            wg_mma3<W>(d, a_hi + 2 * kin, a_lo + 2 * kin, b_hi + 2 * kin, b_lo + 2 * kin, accumulate);
+            accumulate = 1u;
+        }
+    }
+    wg_commit();
+    wg_wait<0>();
+    const int r0 = hf * 64 + wq * 16 + (lane >> 2), c = n0 + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < W / 8; j++) {
+        *reinterpret_cast<float2 *>(acc + r0 * pitch + c + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2 *>(acc + (r0 + 8) * pitch + c + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+}
+
 // SLOTS tiles in flight per CTA, WG warpgroups (128 threads) working on each: the warpgroups of a slot split the
 // 16-byte chunks of the gather and the 32-column chunks of every epilogue between them.  C: shape policy (above).
 template <class C, int SLOTS, int WG>
@@ -308,9 +319,10 @@ sa_fused_kernel(const SfParams p)
     uint8_t *wsm = smem + (size_t)SLOTS * cfg.abuf_bytes();  // weight images (1024-aligned: buffers are multiples of 1 KiB)
     float *ss = reinterpret_cast<float *>(wsm + cfg.w_total());
     float *wxs = ss + cfg.ss_total();                    // [3][kp0] hoisted mode: Wx * s1, zero beyond c
+    const int pitch = (int)cfg.acc_cols() + 4;           // staged accumulator row: +4 floats keep the accesses conflict-free
+    float *acc_all = wxs + 3 * cfg.kp(0);                // [SLOTS][128][pitch], 16-byte aligned (kp0 % 16 == 0)
 
-    __shared__ unsigned long long w_bar, mma_bar[SLOTS];
-    __shared__ uint32_t tmem_base_smem;
+    __shared__ unsigned long long w_bar;
     __shared__ float xs_all[SLOTS * WG][4 * 32];
 
     constexpr int NT = SF_THREADS * SLOTS * WG, ST = SF_THREADS * WG;     // threads per CTA / per slot
@@ -318,26 +330,19 @@ sa_fused_kernel(const SfParams p)
     const int tid = threadIdx.x, lane = tid & 31, q = (tid >> 5) & 3;
     const int slot = tid / ST, wg = (tid >> 7) % WG;
     const int r = tid & 127;                             // row of the slot's tile this thread works on
-    // the slot's first warp issues the MMAs; its index is made provably warp-uniform (shfl) so that descriptors are
-    // computed on the uniform datapath and tcgen05.mma takes them without a per-operand R2UR "waterfall" loop
-    const int slot_u = __shfl_sync(0xffffffffu, slot, 0);
-    const bool issuer_warp = __shfl_sync(0xffffffffu, (tid % ST) >> 5, 0) == 0;
+    // warp-uniform copies (shfl) so that descriptors are computed on the uniform datapath
+    const int slot_u = __shfl_sync(0xffffffffu, slot, 0), wg_u = __shfl_sync(0xffffffffu, wg, 0);
     const int slot_bar = 1 + slot, wg_bar = 1 + SLOTS + slot * WG + wg;
     uint8_t *buf = smem + (size_t)slot * cfg.abuf_bytes();   // the slot's operand buffer (every layer, in place)
     float *xs = xs_all[slot * WG + wg];
+    float *acc = acc_all + (size_t)slot * 128 * pitch;
     const int kp0 = cfg.kp(0);
 
     if (tid == 0) {
         mbar_init(smem_u32(&w_bar), 1);
-#pragma unroll
-        for (int i = 0; i < SLOTS; i++) mbar_init(smem_u32(&mma_bar[i]), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         mbar_arrive_expect_tx(smem_u32(&w_bar), cfg.w_total());
         bulk_g2s(smem_u32(wsm), p.w_blob, cfg.w_total(), smem_u32(&w_bar));
-    }
-    if (tid < 32) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"(p.tmem_alloc) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     for (uint32_t i = tid; i < cfg.ss_total(); i += NT) ss[i] = __ldg(p.ss_blob + i);
     if (cfg.hoist())
@@ -345,21 +350,18 @@ sa_fused_kernel(const SfParams p)
             const int a3 = i / kp0, k = i - a3 * kp0;
             wxs[i] = k < cfg.c() ? __ldg(p.wx + a3 * cfg.c() + k) : 0.0f;
         }
-    sf_fence_before();
+    // staged columns a layer narrower than acc_cols leaves unwritten are multiplied by a zero scale: keep them finite
+    for (int i = tid; i < SLOTS * 128 * pitch; i += NT) acc_all[i] = 0.0f;
     __syncthreads();
-    sf_fence_after();
-    const uint32_t tmem = tmem_base_smem + (uint32_t)slot * cfg.tmem_cols();
-    const uint32_t bar = smem_u32(&mma_bar[slot]);
-    mbar_wait_cta(smem_u32(&w_bar), 0);                  // weights landed (async proxy writes, read by UMMA only)
+    mbar_wait_cta(smem_u32(&w_bar), 0);                  // weights landed (async proxy writes, read by wgmma only)
 
 #ifdef SF_PROFILE
     const bool prof_on = blockIdx.x == 0 && (tid % ST) == 0 && slot == 0;
     long long t_prev = clock64();
 #endif
-    uint32_t mma_phase = 0;
     const int k0 = cfg.hoist() ? cfg.c() : cfg.c() + 3;  // valid operand columns
-    const int pitch = cfg.hoist() ? p.ldz : cfg.c();
-    const bool vec = (cfg.c() & 3) == 0 && (pitch & 3) == 0; // source rows are 16-byte aligned: float4 gathers
+    const int src_pitch = cfg.hoist() ? p.ldz : cfg.c();
+    const bool vec = (cfg.c() & 3) == 0 && (src_pitch & 3) == 0; // source rows are 16-byte aligned: float4 gathers
 
     const int tile0 = blockIdx.x * SLOTS + slot, tstep = gridDim.x * SLOTS;
     const int *units = p.units;
@@ -397,7 +399,7 @@ sa_fused_kernel(const SfParams p)
             const int a = a_next;
             my_group = (int)qi; my_ok = ok;
             fetch(tile + tstep, d_next, a_next);
-            const float *src_f = p.points + ((size_t)scene * p.n + a) * pitch;
+            const float *src_f = p.points + ((size_t)scene * p.n + a) * src_pitch;
             const float *src_x = p.xyz + ((size_t)scene * p.n + a) * 3;
             const float *ctr = p.new_xyz + (size_t)qi * 3;
             const int nchunk = kp0 >> 3;
@@ -458,64 +460,29 @@ sa_fused_kernel(const SfParams p)
         SF_T(0);                                                       // gather
 #pragma unroll (C::kStatic ? SF_MAX_LAYERS : 1)
         for (int l = 0; l < cfg.nl(); l++) {
-            // operand written with ordinary stores -> make it visible to the tensor-core (async) proxy
+            // operand written with ordinary stores -> make it visible to the tensor-core (async) proxy; the barrier also
+            // orders the previous layer's staged-accumulator reads before this layer's MMAs overwrite the staging
             sf_fence_async_smem();
-            sf_fence_before();
             sf_bar_sync(slot_bar, ST);
             SF_T(1 + 4 * l);                                           // barrier
-            if (issuer_warp) {
-                sf_fence_after();
-                // one MMA per k-step covers the whole layer width: a tcgen05.mma costs ~N/2 cycles plus a fixed
-                // per-instruction part, so narrower MMAs only add overhead (measured in round 1)
-                const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(cfg.npad(l) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-                const uint32_t tmem_u = tmem_base_smem + (uint32_t)slot_u * cfg.tmem_cols();
+            {
+                // work items (64-row half, <= 64-column chunk) of this layer, round robin over the slot's warpgroups: one
+                // wgmma per k-step covers the whole chunk width; chunk widths are 64 but for a 16 / 32 / 48 tail
                 const uint32_t abase = smem_u32(smem) + (uint32_t)slot_u * cfg.abuf_bytes();
                 const uint32_t wbase = smem_u32(wsm) + cfg.w_off(l);
-                const int nfull = cfg.nfull(l), rbt = cfg.rbt(l);
-                uint32_t acc = 0u;
-                // descriptors advance by (bytes >> 4) in their address field; shared memory < 256 KiB: no carry out of it
-#pragma unroll (C::kStatic ? 4 : 1)
-                for (int kb = 0; kb < nfull; kb++) {
-                    const uint64_t a_hi = sf_desc(abase + (uint32_t)kb * (2u * 128u * 128u), 128);
-                    const uint64_t b_hi = sf_desc(wbase + (uint32_t)kb * ((uint32_t)cfg.npad(l) * 128u), 128);
-                    const uint64_t a_lo = a_hi + ((128u * 128u) >> 4), b_lo = b_hi + (cfg.w_half(l) >> 4);
-#pragma unroll
-                    for (int kin = 0; kin < 4; kin++) {
-                        if (elect_one()) {
-                            sf_mma(tmem_u, a_hi + 2 * kin, b_hi + 2 * kin, idesc, acc);
-                            sf_mma(tmem_u, a_lo + 2 * kin, b_hi + 2 * kin, idesc, 1u);
-                            sf_mma(tmem_u, a_hi + 2 * kin, b_lo + 2 * kin, idesc, 1u);
-                        }
-                        acc = 1u;
-                    }
+                const int npad = cfg.npad(l), nch = (npad + 63) / 64;
+#pragma unroll (C::kStatic ? 8 : 1)
+                for (int item = wg_u; item < 2 * nch; item += WG) {
+                    const int hf = item & 1, n0 = (item >> 1) * 64, w = npad - n0 < 64 ? npad - n0 : 64;
+                    if (w == 64) sf_mma_chunk<64>(cfg, l, abase, wbase, hf, n0, acc, pitch, q, lane);
+                    else if (w == 48) sf_mma_chunk<48>(cfg, l, abase, wbase, hf, n0, acc, pitch, q, lane);
+                    else if (w == 32) sf_mma_chunk<32>(cfg, l, abase, wbase, hf, n0, acc, pitch, q, lane);
+                    else sf_mma_chunk<16>(cfg, l, abase, wbase, hf, n0, acc, pitch, q, lane);
                 }
-                if (rbt) {
-                    const uint64_t a_hi = sf_desc(abase + (uint32_t)nfull * (2u * 128u * 128u), rbt);
-                    const uint64_t b_hi = sf_desc(wbase + (uint32_t)nfull * ((uint32_t)cfg.npad(l) * 128u), rbt);
-                    const uint64_t a_lo = a_hi + ((128u * (uint32_t)rbt) >> 4), b_lo = b_hi + (cfg.w_half(l) >> 4);
-                    const int nt = rbt == 128 ? 3 : (rbt >> 5);              // 16-wide k-steps of the tail block
-#pragma unroll (C::kStatic ? 3 : 1)
-                    for (int kin = 0; kin < nt; kin++) {
-                        if (elect_one()) {
-                            sf_mma(tmem_u, a_hi + 2 * kin, b_hi + 2 * kin, idesc, acc);
-                            sf_mma(tmem_u, a_lo + 2 * kin, b_hi + 2 * kin, idesc, 1u);
-                            sf_mma(tmem_u, a_hi + 2 * kin, b_lo + 2 * kin, idesc, 1u);
-                        }
-                        acc = 1u;
-                    }
-                }
-                if (elect_one()) sf_commit(smem_u32(&mma_bar[slot_u]));
-                __syncwarp();
-                SF_T(2 + 4 * l);                                       // MMA issue
-                // ONE warp of the slot polls the mbarrier; the others sleep at the slot's named barrier (a hardware
-                // barrier costs no issue slots -- the all-warps poll loop was a quarter of the kernel's instructions)
-                mbar_wait_cta(bar, mma_phase);                       // MMAs done: accumulator ready, operand buffer free
-                sf_fence_before();
             }
-            sf_bar_sync(slot_bar, ST);
-            mma_phase ^= 1u;
+            SF_T(2 + 4 * l);                                           // MMAs
+            sf_bar_sync(slot_bar, ST);                                 // every MMA of the tile done: staging complete, buf free
             SF_T(3 + 4 * l);                                           // MMA wait
-            sf_fence_after();
             // ---- epilogue of layer l
             const float *sc = ss + cfg.ss_off(l);
             const float *sh = sc + cfg.sspad(l);
@@ -526,21 +493,25 @@ sa_fused_kernel(const SfParams p)
 #pragma unroll (C::kStatic ? 4 : 1)
             for (int ci = wg; ci < nchunks; ci += WG) {
                 const int c0 = ci * 32;
-                uint32_t rr[32];
-                sf_tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, rr);
+                float rr[32];
+#pragma unroll
+                for (int j4 = 0; j4 < 32; j4 += 4) {
+                    const float4 a4 = *reinterpret_cast<const float4 *>(acc + r * pitch + c0 + j4);
+                    rr[j4] = a4.x; rr[j4 + 1] = a4.y; rr[j4 + 2] = a4.z; rr[j4 + 3] = a4.w;
+                }
                 float v[32];
                 if (pool_first) {
 #pragma unroll
-                    for (int j = 0; j < 32; j++) v[j] = __uint_as_float(rr[j]);
+                    for (int j = 0; j < 32; j++) v[j] = rr[j];
                 } else {
 #pragma unroll
                     for (int j4 = 0; j4 < 32; j4 += 4) {              // scale/shift are zero-padded to 32-column chunks
                         const float4 s4 = *reinterpret_cast<const float4 *>(sc + c0 + j4);
                         const float4 h4 = *reinterpret_cast<const float4 *>(sh + c0 + j4);
-                        v[j4 + 0] = fmaxf(fmaf(__uint_as_float(rr[j4 + 0]), s4.x, h4.x), 0.0f);   // every conv has a ReLU
-                        v[j4 + 1] = fmaxf(fmaf(__uint_as_float(rr[j4 + 1]), s4.y, h4.y), 0.0f);
-                        v[j4 + 2] = fmaxf(fmaf(__uint_as_float(rr[j4 + 2]), s4.z, h4.z), 0.0f);
-                        v[j4 + 3] = fmaxf(fmaf(__uint_as_float(rr[j4 + 3]), s4.w, h4.w), 0.0f);
+                        v[j4 + 0] = fmaxf(fmaf(rr[j4 + 0], s4.x, h4.x), 0.0f);   // every conv has a ReLU
+                        v[j4 + 1] = fmaxf(fmaf(rr[j4 + 1], s4.y, h4.y), 0.0f);
+                        v[j4 + 2] = fmaxf(fmaf(rr[j4 + 2], s4.z, h4.z), 0.0f);
+                        v[j4 + 3] = fmaxf(fmaf(rr[j4 + 3], s4.w, h4.w), 0.0f);
                     }
                 }
                 if (!last) {
@@ -575,17 +546,10 @@ sa_fused_kernel(const SfParams p)
                     }
                 }
             }
-            sf_fence_before();                                         // TMEM reads done before the next MMAs overwrite it
             SF_T(4 + 4 * l);                                           // epilogue
         }
     }
 
-    sf_fence_before();
-    __syncthreads();
-    if (tid < 32) {
-        sf_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base_smem), "r"(p.tmem_alloc) : "memory");
-    }
 }
 
 }  // namespace ssd3d
@@ -613,7 +577,7 @@ static size_t sf_wimg_bytes(int kp, int npad)              // one half (hi or lo
     return (size_t)npad * (nfull * 128 + rbt);
 }
 
-struct SfPlan { size_t abuf, w, ssf; int maxn; };
+struct SfPlan { size_t abuf, acc, w, ssf; int maxn; };
 static bool sf_plan(int k_in, int nl, const int *nout, SfPlan *pl)      // k_in: columns of the first operand
 {
     if (nl < 1 || nl > SF_MAX_LAYERS) return false;
@@ -630,11 +594,12 @@ static bool sf_plan(int k_in, int nl, const int *nout, SfPlan *pl)      // k_in:
         if (npad > pl->maxn) pl->maxn = npad;
         kp = npad;
     }
+    pl->acc = (size_t)128 * ((pl->maxn + 31) / 32 * 32 + 4) * sizeof(float);   // staged accumulator of one slot
     return true;
 }
-static size_t sf_total(const SfPlan &pl, int slots) { return slots * pl.abuf + pl.w + pl.ssf * sizeof(float) + 1024; }
+static size_t sf_total(const SfPlan &pl, int slots) { return slots * (pl.abuf + pl.acc) + pl.w + pl.ssf * sizeof(float) + 1024; }
 constexpr size_t SF_SMEM_MAX = 226 * 1024;
-constexpr size_t SF_SMALL = 36 * 1024;                     // <= this: single-slot CTAs, up to 6 per SM
+constexpr size_t SF_SMALL = 72 * 1024;                     // <= this: single-slot, single-warpgroup CTAs, several per SM
 
 // Developer build only (-DSSD3D_DEV_HOOKS, csrc/ssd3d_dev.h): override the slot / warpgroup shape from a probe script.
 // The shipped library has no such state.
@@ -650,10 +615,9 @@ constexpr int g_sf_slots = 0, g_sf_wg = 0, g_sf_dynamic = 0;
 static int sf_slots(const SfPlan &pl)
 {
     if (sf_total(pl, 1) <= SF_SMALL) return 1;
-    int cols = 32;
-    while (cols < pl.maxn) cols *= 2;
     int s = g_sf_slots > 0 ? (g_sf_slots > 4 ? 4 : g_sf_slots) : 3;
-    while (s > 1 && (sf_total(pl, s) > SF_SMEM_MAX || s * cols > 512)) s--;
+    // the kernel's static shared memory (xs_all: 512 bytes per warpgroup, two per slot) counts against the same limit
+    while (s > 1 && sf_total(pl, s) + (size_t)s * 2 * 512 > SF_SMEM_MAX) s--;
     return s;
 }
 
@@ -689,9 +653,9 @@ static bool sf_launch_static(const SfParams &p, int slots, int wg, size_t smem, 
         if (k0 == 16 && n0 == 16 && n1 == 32 && ns == 32) { *e = sf_launch<SfStat<16, 16, 32, 32>, 1, 1>(p, smem, per_sm, st); return true; }
         if (k0 == 32 && n0 == 32 && n1 == 64 && ns == 64) { *e = sf_launch<SfStat<32, 32, 64, 64>, 1, 1>(p, smem, per_sm, st); return true; }
     }
-    if (slots == 3 && wg == 2) {
-        if (k0 == 64 && n0 == 64 && n1 == 128 && ns == 32) { *e = sf_launch<SfStat<64, 64, 128, 32>, 3, 2>(p, smem, per_sm, st); return true; }
-        if (k0 == 64 && n0 == 96 && n1 == 128 && ns == 64) { *e = sf_launch<SfStat<64, 96, 128, 64>, 3, 2>(p, smem, per_sm, st); return true; }
+    if (slots == 1 && wg == 2) {
+        if (k0 == 64 && n0 == 64 && n1 == 128 && ns == 32) { *e = sf_launch<SfStat<64, 64, 128, 32>, 1, 2>(p, smem, per_sm, st); return true; }
+        if (k0 == 64 && n0 == 96 && n1 == 128 && ns == 64) { *e = sf_launch<SfStat<64, 96, 128, 64>, 1, 2>(p, smem, per_sm, st); return true; }
     }
     return false;
 }
@@ -749,28 +713,24 @@ static int sa_mlp_fused_impl(int b, int n, int c, int m, int nsample, const floa
     p.w_total = woff; p.ss_total = ssoff;
     p.w_blob = (const uint8_t *)w_blob; p.ss_blob = ss_blob;
     p.abuf_bytes = (uint32_t)pl.abuf;
-    uint32_t cols = 32;
-    while ((int)cols < pl.maxn) cols *= 2;
-    p.tmem_cols = cols;
-    uint32_t alloc = 32;
-    while (alloc < cols * (uint32_t)slots) alloc *= 2;
-    p.tmem_alloc = alloc;
+    p.acc_cols = (uint32_t)(pl.maxn + 31) / 32 * 32;
     p.out_f32 = out_f32; p.ld_f32 = ld_f32;
     p.out_hi = (__nv_bfloat16 *)out_hi; p.out_lo = (__nv_bfloat16 *)out_lo; p.ld_split = ld_split;
 
-    // resident CTAs per SM: bounded by shared memory, TMEM columns (512 per SM) and, for single-slot CTAs, registers
+    // one warpgroup per slot for small stacks (several CTAs per SM), two when a slot needs most of an SM's shared memory
+    const bool small = slots == 1 && smem <= SF_SMALL;
+    const int wg = g_sf_wg > 0 ? g_sf_wg : (small ? 1 : 2);
+    // resident CTAs per SM: bounded by shared memory and, for single-warpgroup CTAs, registers
     int per_sm = 1;
-    if (slots == 1) {
+    if (slots == 1 && wg == 1) {
         per_sm = (int)((227 * 1024) / (smem + 1024));
-        if (per_sm > (int)(512 / alloc)) per_sm = 512 / alloc;
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 6) per_sm = 6;                                   // 6 x 128 threads x 80 registers
     }
-    const int wg = slots == 1 ? 1 : (g_sf_wg > 0 ? g_sf_wg : 2);
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaSuccess;
     if (g_sf_dynamic || !sf_launch_static(p, slots, wg, smem, per_sm, st, &e))
-        e = slots == 1 ? sf_launch<SfDyn, 1, 1>(p, smem, per_sm, st)
+        e = slots == 1 ? (wg == 1 ? sf_launch<SfDyn, 1, 1>(p, smem, per_sm, st) : sf_launch<SfDyn, 1, 2>(p, smem, per_sm, st))
           : slots == 2 ? (wg == 4 ? sf_launch<SfDyn, 2, 4>(p, smem, per_sm, st) : wg == 1 ? sf_launch<SfDyn, 2, 1>(p, smem, per_sm, st)
                                                                                            : sf_launch<SfDyn, 2, 2>(p, smem, per_sm, st))
           : slots == 3 ? (wg == 1 ? sf_launch<SfDyn, 3, 1>(p, smem, per_sm, st) : sf_launch<SfDyn, 3, 2>(p, smem, per_sm, st))

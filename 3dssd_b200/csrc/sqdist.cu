@@ -134,8 +134,7 @@ sqdist128_kernel(int n, int c, const float *__restrict__ a, float *__restrict__ 
     }
     __syncthreads();
     const int ty = tid / 16, tx = tid % 16;
-    // Packed fp32 FMAs (FFMA2, sm_100): two independent IEEE fmas per instruction -- bit-identical to the scalar
-    // chain, twice the throughput of the fp32 pipe.
+    // fp32 pairs: two independent IEEE fmas each -- bit-identical to the scalar chain.
     float2 acc2[8][4];
 #pragma unroll
     for (int y = 0; y < 8; y++)
@@ -152,7 +151,7 @@ sqdist128_kernel(int n, int c, const float *__restrict__ a, float *__restrict__ 
         for (int y = 0; y < 8; y++) {
             const float2 ap = make_float2(ar[y], ar[y]);
 #pragma unroll
-            for (int x = 0; x < 4; x++) acc2[y][x] = __ffma2_rn(ap, bp[x], acc2[y][x]);
+            for (int x = 0; x < 4; x++) acc2[y][x] = fma2_rn(ap, bp[x], acc2[y][x]);
         }
     }
     float acc[8][8];

@@ -1,4 +1,4 @@
-"""SA / FP / vote layers with the reference's signatures, on the B200 operators.
+"""SA / FP / vote layers with the reference's signatures, on the H100 operators.
 
 Mirrors /root/reference/lib/utils/layers_util.py: vote_layer :12-24, pointnet_sa_module :27-55,
 pointnet_sa_module_msg :59-189, pointnet_fp_module :192-225 -- same positional arguments and return values,

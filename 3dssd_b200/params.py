@@ -135,7 +135,7 @@ def _k_blocks(kp):
 
 
 def _swizzle_block(blk, rb):
-    """[npad, rb/2] bf16 -> canonical UMMA K-major image with swizzle span rb: 16-byte chunk j of row r is stored at
+    """[npad, rb/2] bf16 -> canonical K-major (wgmma / TMA) image with swizzle span rb: 16-byte chunk j of row r is stored at
     chunk j ^ ((r >> log2(128/rb)) & (rb/16 - 1)), i.e. SWIZZLE_128B / _64B / _32B for rb = 128 / 64 / 32."""
     npad = blk.shape[0]
     nc = rb // 16

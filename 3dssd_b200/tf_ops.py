@@ -267,7 +267,7 @@ BQ_GRID_MIN_N = 2048     # candidate sets at least this large take the spatially
 
 
 def query_ball_point_multi(min_radius_list, max_radius_list, nsample_list, xyz1, xyz2, dilated, grid=None, return_units=False):
-    """All radius shells of one SA layer in a single pass over the candidates (B200 fast path; same results
+    """All radius shells of one SA layer in a single pass over the candidates (fast path; same results
     as calling query_ball_point[_dilated] once per shell).  Returns lists (idx_list, pts_cnt_list).
     grid: None = automatic (the culled kernel for ndataset >= BQ_GRID_MIN_N), True / False = force / forbid it;
     the outputs are identical either way.
@@ -480,7 +480,7 @@ def linear_bn_relu(x, w, scale, shift, relu=True, pool=1, rowmask=None, cin=None
     return y
 
 
-# ---- tensor-core (tcgen05) path of the MLP: operands split in two bf16 terms ---------------------------------
+# ---- tensor-core (wgmma) path of the MLP: operands split in two bf16 terms ---------------------------------
 
 def round16(x):
     return (int(x) + 15) // 16 * 16

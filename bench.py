@@ -12,18 +12,21 @@ ends a step, inside the step's CUDA graph: this library's peer-memory kernel, `-
 value  : scenes/s, inputs resident in HBM.  Every step is one CUDA-graph replay; `--pipeline` (default 24) steps are in
          flight on separate streams with their own graphs and buffers (a step chains latency-bound sampling stages that
          keep a few SMs busy for milliseconds and short throughput-bound stages, so steps overlap).  Timing: after
-         max(W, 2*pipeline) warm-up steps, `--brackets` (5) brackets of K*reps steps each (reps chosen so a bracket lasts
-         >= 0.5 s), one CUDA-event pair per bracket, barrier + synchronize on both sides, L2 flushed before every step,
-         max over ranks per bracket, MEDIAN bracket reported; ms_per_step = that bracket / its steps.
-e2e    : the same brackets through the public API with HOST buffers: pinned H2D copy of the batch into the graph's
+         max(W, 2*pipeline) warm-up steps, exactly K timed steps in ONE window (one CUDA-event pair, barrier +
+         synchronize on both sides), the steps rotating over the pipelines so that min(K, pipeline) are in flight, L2
+         flushed before every step, max over ranks; ms_per_step = window / K.  The window starts and ends with an empty
+         pipeline, so K should be many times `--pipeline` (default K = 500: about a second on one H100).
+e2e    : the same window through the public API with HOST buffers: pinned H2D copy of the batch into the graph's
          input + the step + D2H read of the gathered detection blocks inside the timed region.
 config.latency_ms_single_step: one step at a time (sync after each), the library's latency mode (SABackbone
          latency_mode=True: layer-1 FPS cut into resumable launches whose samples are consumed while it continues).
 roofline: time-weighted tensor-pipe figure over ALL grouped-MLP kernels of one step (the kernels that dominate the
          step's SM-time), each timed live with CUDA events; roofline_fps: the layer-1 D-FPS chain (ns per round).
 cpu_baseline: the CPU restatement (oracle/, fp32 BLAS MLP) on a bounded sample of the same workload.
-clocks : sampled in-process through NVML from before the first bracket to after the last one (no nvidia-smi start-up
-         inside a bracket); median / reasons are over the samples that fall inside timed brackets.
+--dump-outputs DIR: after the timed steps, what the last timed step returned (detection blocks and counts, every
+         layer's xyz / features / sampled indices) as DIR/<name>.npy in float32 / float64, at most 64 MB in all.
+clocks : sampled in-process through NVML from before the first timed window to after the last one (no nvidia-smi
+         start-up inside a window); median / reasons are over the samples that fall inside timed windows.
 
 --impl reference: the reference's implementation of this path is CUDA (lib/utils/tf_ops/*_g.cu) -- it has no
 CPU code for sampling/grouping (SURVEY.md finding 4).  The arm therefore runs the reference's OWN kernels,
@@ -34,7 +37,6 @@ if that library is absent it falls back to the CPU port.  Its cpu_baseline objec
 import argparse
 import importlib
 import json
-import math
 import os
 import subprocess
 import sys
@@ -47,14 +49,14 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-METRIC = "KITTI-shape scenes/sec (B×16384 pts) full SA backbone, 1/2/4/8×B200"
+METRIC = "KITTI-shape scenes/sec (B×16384 pts) full SA backbone, 1/2/4/8×H100"
 UNIT = "scenes/s"
 SCENES_PER_GPU = 8
 NPOINTS = 16384
 # the SAME string in both arms (the driver compares them)
 WORKLOAD = ("configs[1]: full 3DSSD SA backbone (3dssd.yaml layer1-4 + vote) + detection head, decode and BEV NMS, "
             "synthetic KITTI 16384x4 clouds, batch 8 per GPU")
-DTYPE = "bf16x3-split/f32-acc"   # fp32 operands split in two bf16 terms, 3 tcgen05 MMAs per product, fp32 accumulation
+DTYPE = "bf16x3-split/f32-acc"   # fp32 operands split in two bf16 terms, 3 wgmma MMAs per product, fp32 accumulation
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -66,7 +68,7 @@ class ClockSampler:
     def __init__(self, index=0, period=0.05):
         self.index, self.period = index, period
         self.samples = []          # (t, sm_mhz, max_mhz, reason bits)
-        self.windows = []          # (t0, t1) of timed brackets
+        self.windows = []          # (t0, t1) of timed windows
         self.stop_flag = threading.Event()
         self.mode = None
         self.proc = None
@@ -146,7 +148,7 @@ class ClockSampler:
                 "sm_max_mhz": max(s[2] for s in use) if use else None,
                 "reasons": sorted(v for k, v in self.REASONS.items() if bits & k),
                 "samples": len(use), "samples_total": len(self.samples), "source": self.mode,
-                "note": "median over the samples taken inside the timed brackets (value and e2e)"}
+                "note": "median over the samples taken inside the timed windows (value and e2e)"}
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -189,19 +191,39 @@ def cpu_baseline(arch, params, head_params, pts_np, max_scenes=2):
                       % (sample.shape[0], pts_np.shape[0], dt)}
 
 
-def ncu_dram_bytes(name):
-    """dram read+write bytes per launch from a committed ncu export (profiles/<name>), or None."""
-    path = os.path.join(ROOT, "profiles", name)
-    if not os.path.exists(path):
-        return None
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    tot, seen = 0.0, 0
-    for line in open(path):
-        parts = line.split()
-        if len(parts) >= 3 and parts[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and parts[2] in unit:
-            tot += float(parts[1]) * unit[parts[2]]
-            seen += 1
-    return tot if seen == 2 else None
+DUMP_LIMIT = 64 * 1024 * 1024
+
+
+def dump_outputs(path, out, gather, np, torch):
+    """What one step returns to its caller -- the forward outputs (xyz, features and sampled indices of every layer)
+    and the detection block / count pair -- as <path>/<name>.npy: floating arrays as float32, integer arrays as float64
+    (exact).  If the arrays exceed DUMP_LIMIT in all, every array keeps a fixed, seeded sample of its leading-axis rows
+    after the scene axis, the same in every run."""
+    (xyz_l, feat_l, fps_l), _ = out
+    blk, cnt = gather.result()
+    arrays = {"detections_block": blk, "detections_count": cnt}
+    for i, (x, f) in enumerate(zip(xyz_l, feat_l)):
+        arrays["layer%d_xyz" % i] = x
+        if f is not None:
+            arrays["layer%d_features" % i] = f
+    for i, ix in enumerate(fps_l):
+        if ix is not None:
+            arrays["layer%d_sample_idx" % i] = ix
+    host = {}
+    for k, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        host[k] = a.astype(np.float32 if np.issubdtype(a.dtype, np.floating) else np.float64)
+    total = sum(a.nbytes for a in host.values())
+    if total > DUMP_LIMIT:
+        keep = DUMP_LIMIT / total
+        rng = np.random.default_rng(0)
+        for k, a in host.items():
+            if a.ndim >= 2 and a.shape[1] > 1:
+                rows = np.sort(rng.choice(a.shape[1], max(1, int(a.shape[1] * keep)), replace=False))
+                host[k] = np.ascontiguousarray(a[:, rows])
+    os.makedirs(path, exist_ok=True)
+    for k, a in host.items():
+        np.save(os.path.join(path, k + ".npy"), a)
 
 
 def nominal_mlp_flops(arch, in_channels, scenes, cfg):
@@ -306,11 +328,9 @@ class MlpTimer:
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=500, help="timed steps per leg, in one window")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--brackets", type=int, default=5, help="timed brackets per leg; the median is reported")
-    ap.add_argument("--min-bracket-s", type=float, default=0.5, help="a bracket runs K*reps steps with reps chosen to last this long")
     ap.add_argument("--ffps-mode", default="direct", choices=["direct", "matrix", "fused"])
     ap.add_argument("--mlp-mode", default="tc", choices=["tc", "fp32"])
     ap.add_argument("--gather-in-kernel", type=int, default=1, help="1: first conv of unfused SA scales gathers its operand itself")
@@ -327,6 +347,8 @@ def main():
                     help="N > 1: the per-step all-gather as this library's peer-memory kernel (default) or as ncclAllGather")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-scenes", type=int, default=2)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned as DIR/<name>.npy (float32 / float64, <= 64 MB)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -344,7 +366,7 @@ def main():
         raise SystemExit("bench.py needs a CUDA device: the product has no CPU path")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
-    sampler = ClockSampler(local).start() if rank == 0 else None      # runs from here to the end of the last bracket
+    sampler = ClockSampler(local).start() if rank == 0 else None      # runs from here to the end of the last timed window
     arch = pkg.config.ARCH_3DSSD
     params = pkg.params.init_params(arch, 1, seed=0)
     head_params = pkg.params.init_head_params(pkg.config.layer_channels(arch, 1)[-1], seed=1)
@@ -365,7 +387,7 @@ def main():
                          fps_packet=args.fps_packet, fps_bucket={"auto": None, "on": True, "off": False}[args.fps_bucket], **mk)
     net_lat = pkg.SABackbone(arch, params, fps_cluster=0, latency_mode=True, **mk)
     pts = torch.from_numpy(pts_np).to(dev)
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 50 MB L2
     total_scenes = SCENES_PER_GPU * world
 
     # ---- one eager step: launches per step (counted at the ctypes boundary: every C-ABI call below launches exactly
@@ -482,9 +504,11 @@ def main():
     host_in = torch.from_numpy(pts_np).pin_memory()
     host_out = [torch.empty((gathers[k].raw.numel(),), dtype=torch.uint8).pin_memory() for k in range(P)]
 
+    last = {}
+
     def one_step(i, e2e):
         k = i % P
-        runners[k](host_in if e2e else None)      # e2e: pinned H2D into the graph's static input first
+        last["out"], last["k"] = runners[k](host_in if e2e else None), k   # e2e: pinned H2D into the graph's static input first
         if e2e:
             host_out[k].copy_(gathers[k].raw, non_blocking=True)   # all ranks' detection blocks + counts
 
@@ -499,7 +523,7 @@ def main():
         for i in range(nsteps):
             s_ = streams[i % P]
             with torch.cuda.stream(s_):
-                flush.zero_()                                      # L2 flush before every step (inside the bracket)
+                flush.zero_()                                      # L2 flush before every step (inside the window)
                 one_step(i, e2e)
         for s_ in streams:
             main_s.wait_stream(s_)
@@ -516,17 +540,19 @@ def main():
         return ms
 
     warm = max(args.warmup, 2 * P)
+    in_flight = min(P, args.steps)                  # steps that overlap inside the timed window
+
     bracket(warm, False, timed=False)
-    est = bracket(args.steps, False, timed=False) / args.steps                 # ms per step, same on all ranks (max-reduced)
-    reps = max(1, int(math.ceil(args.min_bracket_s * 1e3 / (est * args.steps))))
-    nsteps = args.steps * reps
-    val_ms = sorted(bracket(nsteps, False) for _ in range(max(1, args.brackets)))
-    total_ms = val_ms[len(val_ms) // 2]
+    val_ms = bracket(args.steps, False)             # exactly --steps timed steps, one window
+    step_ms = val_ms / args.steps
+    if args.dump_outputs and rank == 0:             # ranks run different scenes: rank 0's step is the one dumped
+        torch.cuda.synchronize()
+        dump_outputs(args.dump_outputs, last["out"], gathers[last["k"]], np, torch)
 
     # ---- e2e: host buffers through the public API ---------------------------------------------------------
     bracket(warm, True, timed=False)
-    e2e_all = sorted(bracket(nsteps, True) for _ in range(max(1, args.brackets)))
-    e2e_ms = e2e_all[len(e2e_all) // 2]
+    e2e_ms = bracket(args.steps, True)
+    e2e_step_ms = e2e_ms / args.steps
     clocks = sampler.stop() if sampler else None
 
     # ---- single-step latency: one step at a time, sync after each, latency-mode network --------------------
@@ -586,15 +612,15 @@ def main():
         ppath = os.path.join(ROOT, "MEASURED_PEAKS.json")
         if os.path.exists(ppath):
             peaks = json.load(open(ppath))
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        tc_peak = float(peaks.get("bf16_tflops", 1700.0))
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))        # H100 SXM data sheet
+        tc_peak = float(peaks.get("bf16_tflops", 989.0))      # H100 SXM data sheet, dense BF16
         fps_bytes = SCENES_PER_GPU * (4096 - 1) * NPOINTS * 16          # B*(M-1)*N*(4c+4), SURVEY.md 8d
-        scenes = SCENES_PER_GPU * world * nsteps
+        scenes_per_step = SCENES_PER_GPU * world
         nominal = nominal_mlp_flops(arch, 1, SCENES_PER_GPU, pkg.config)
         ach_tc = mlp_flops / (mlp_ms * 1e-3) / 1e12
         line = {
-            "metric": METRIC, "value": scenes / (total_ms * 1e-3), "unit": UNIT, "n_gpus": world, "steps": args.steps,
-            "warmup": args.warmup, "ms_per_step": total_ms / nsteps, "higher_is_better": True, "scaling": "weak",
+            "metric": METRIC, "value": scenes_per_step / (step_ms * 1e-3), "unit": UNIT, "n_gpus": world, "steps": args.steps,
+            "warmup": args.warmup, "ms_per_step": step_ms, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": DTYPE, "data": "synthetic",
             "config": {"workload": WORKLOAD, "scenes_per_gpu": SCENES_PER_GPU,
                        "global_batch": SCENES_PER_GPU * world, "points": NPOINTS, "parallelism": "scene-sharded dp%d" % world,
@@ -608,43 +634,37 @@ def main():
                        "latency_ms_single_step_throughput_graph": latency_thr_ms,
                        "latency_note": "one step at a time with a sync after each (as the reference arm runs): latency-mode "
                                        "graph (SABackbone latency_mode=True) / the throughput graph used for `value`",
-                       "brackets": len(val_ms), "steps_per_bracket": nsteps, "warmup_effective": warm,
-                       "bracket_ms": val_ms, "e2e_bracket_ms": e2e_all,
-                       "timing": "median of %d brackets of %d steps (= steps x %d, >= %.1f s each); one CUDA-event pair per bracket "
-                                 "(L2 flushes included), barrier + synchronize on both sides, max over ranks per bracket; every step is "
-                                 "one CUDA-graph replay incl. the ncclAllGather, %d step pipelines on separate streams"
-                                 % (len(val_ms), nsteps, reps, args.min_bracket_s, P)},
-            "e2e": {"value": scenes / (e2e_ms * 1e-3), "unit": UNIT,
+                       "steps_in_flight_timed": in_flight, "warmup_effective": warm,
+                       "window_ms": val_ms, "e2e_window_ms": e2e_ms,
+                       "timing": "%d timed steps in one window of %.3f s; one CUDA-event pair (L2 flushes included), barrier + "
+                                 "synchronize on both sides, max over ranks; every step is one CUDA-graph replay incl. the exchange, "
+                                 "%d step pipelines on separate streams, %d of them in flight in the window"
+                                 % (args.steps, val_ms * 1e-3, P, in_flight)},
+            "e2e": {"value": scenes_per_step / (e2e_step_ms * 1e-3), "unit": UNIT,
                     "h2d_bytes_per_step": int(host_in.numel() * 4), "d2h_bytes_per_step": int(host_out[0].numel())},
             "gpu_launches": launches_per_step * args.steps,
             "gpu_launches_per_step": launches_per_step,
             "clocks": clocks,
             "roofline": {"bound": "tensor", "achieved": ach_tc, "peak": tc_peak, "unit": "TFLOP/s", "frac": ach_tc / tc_peak,
-                         "traffic": ncu_dram_bytes("r02_ncu_mlp_top.txt"),
                          "kernel": "time-weighted over ALL tensor-core MLP kernels of one step (%d launches: %s)"
                                    % (len(mt.rec), ", ".join("%s x%d" % (n, d["launches"]) for n, d in sorted(mlp_per.items()))),
                          "kernel_ms": mlp_ms, "per_kernel": mlp_per,
                          "algorithmic_gflop_per_step": nominal / 1e9,
                          "algorithmic_tflops_fp32_grade": nominal / (mlp_ms * 1e-3) / 1e12,
-                         "note": "achieved = bf16 tcgen05 flops ISSUED (3 MMAs per fp32-grade product, padded K/N) summed over the step's "
+                         "note": "achieved = bf16 wgmma flops ISSUED (3 MMAs per fp32-grade product, padded K/N) summed over the step's "
                                  "MLP launches / the sum of their CUDA-event times (one eager step, each launch timed on its stream); "
                                  "peak = MEASURED_PEAKS.json bf16_tflops (burst: kernels timed one at a time)"
-                                 + ("" if peaks else " [fallback 1700: file absent]")
+                                 + ("" if peaks else " [fallback 989, H100 SXM data sheet: file absent]")
                                  + "; algorithmic = 2*B*M*K*sum(Cin*Cout) unpadded incl. the hoisted first convs (SURVEY 8d), fp32-grade"},
             "roofline_fps": {"bound": "latency", "kernel": "fps3_direct_kernel (D-FPS layer 1, 16384->4096, B=8, 8 CTAs per scene: the latency-mode step), timed alone",
                              "throughput_kernel": {"kernel": "fps3_bucket_kernel (same sampling, ONE CTA per scene, spatial pruning: the throughput step)",
                                                    "kernel_ms": kb_ms, "ns_per_round": kb_ms * 1e6 / 4095, "sm_ms_per_batch": 8 * kb_ms,
                                                    "cluster_kernel_sm_ms_per_batch": 64 * k_ms},
                              "kernel_ms": k_ms, "rounds": 4095, "ns_per_round": k_ms * 1e6 / 4095,
-                             "floor_ns_per_round": 271.0,
-                             "floor_note": "critical path of one round at 1.965 GHz: 4 packed distance updates + compare chain (~60 cyc) "
-                                           "+ 2 redux.sync (~50) + st.async DSMEM one-way + mbarrier wake-up (~180, B300_MICROARCH DSMEM "
-                                           "latency) + LDS + 2 redux + LDS of the winner (~90) = ~533 cyc = 271 ns",
                              "effective_stream_gbs": fps_bytes / (k_ms * 1e-3) / 1e9, "hbm_peak_gbs": hbm_peak,
                              "effective_stream_frac": fps_bytes / (k_ms * 1e-3) / 1e9 / hbm_peak,
-                             "traffic": ncu_dram_bytes("r01_ncu_fps_l1.txt"),
                              "note": "effective-stream bytes B*(M-1)*N*16 = what the reference streams per round (SURVEY 8d); the kernel "
-                                     "keeps them on chip (DRAM traffic ~1.6 MB), so this is a latency chain, not an HBM-bound kernel"},
+                                     "keeps them on chip, so this is a latency chain, not an HBM-bound kernel"},
         }
         if not args.no_cpu_baseline:
             line["cpu_baseline"] = cpu_baseline(arch, params, head_params, pts_np, args.cpu_scenes)
@@ -708,8 +728,8 @@ def run_reference(args, torch, pkg, arch, params, head_params, pts_np, rank, wor
             "warmup": args.warmup, "ms_per_step": tot / steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": WORKLOAD,
-                       "reference_device": "B200: the reference's own CUDA kernels (oracle/_ref/libref_ops.so, unmodified "
-                                           "sources, nvcc -O2 sm_100) + PyTorch fp32 ops one-for-one for the TF stock ops + "
+                       "reference_device": "the reference's own CUDA kernels (oracle/_ref/libref_ops.so, unmodified "
+                                           "sources, nvcc -O2 sm_90) + PyTorch fp32 ops one-for-one for the TF stock ops + "
                                            "CPU NMS like tf.image.non_max_suppression; the reference has no CPU "
                                            "implementation of this path",
                        "l2": "flushed between timed steps",

@@ -1,5 +1,5 @@
 /*
- * ssd3d.h -- C ABI of libssd3d.so, the B200 (sm_100a) implementation of the set-abstraction
+ * ssd3d.h -- C ABI of libssd3d.so, the H100 (sm_90a) implementation of the set-abstraction
  * operators of dvlab-research/3DSSD.
  *
  * Drop-in boundary (SURVEY.md section 8b, seam iii): the reference's TF custom ops call free C++
@@ -118,7 +118,7 @@ int ssd3d_query_ball_point_dilated(int b, int n, int m, float min_radius, float 
                                    const float *xyz1, const float *xyz2, int *idx, int *pts_cnt,
                                    ssd3d_stream_t stream);
 
-/* B200 fast path used by pointnet_sa_module_msg: up to 4 (min_r,max_r,nsample) queries over the same
+/* Fast path used by pointnet_sa_module_msg: up to 4 (min_r,max_r,nsample) queries over the same
  * (xyz1,xyz2) answered in ONE pass over the candidates (the reference scans once per radius,
  * lib/utils/layers_util.py:134-147).  dilated!=0 selects the :308-357 predicate, else the :215-255 one
  * (min_radius ignored).  idx[s] / pts_cnt[s] are per-query outputs as above. */
@@ -184,9 +184,9 @@ int ssd3d_linear_bn_relu(long rows, int cin, int cout, const float *x, int ldx, 
                          const float *scale, const float *shift, int relu, int pool, const int *rowmask,
                          float *y, int ldy, ssd3d_stream_t stream);
 
-/* ---- tensor-core (tcgen05) path of the same layer -------------------------------------------------
+/* ---- tensor-core (wgmma) path of the same layer -------------------------------------------------
  * fp32 operands travel as TWO bf16 matrices (x = hi + lo, 16 mantissa bits); the product is evaluated as
- * hi.hi + lo.hi + hi.lo with fp32 accumulation in TMEM (error ~2^-16, inside the 1e-3 parity budget).
+ * hi.hi + lo.hi + hi.lo with fp32 accumulation (error ~2^-16, inside the 1e-3 parity budget).
  *   a_hi/a_lo [rows, kp] bf16 row-major (kp % 16 == 0, zero padded); b_hi/b_lo [n, kp] bf16 = W^T split;
  *   outputs (any subset): out_f32 [rows or rows/pool, ld_f32] and/or out_hi/out_lo [.., ld_split] bf16 for the
  *   next layer (columns n..ld_split-1 are written as zeros when pool == 1).  pool / rowmask as above. */

@@ -1,6 +1,6 @@
 """ctypes front-end of oracle/_ref/libref_ops.so: the REFERENCE's own CUDA kernels
-(/root/reference/lib/utils/tf_ops/{sampling/tf_sampling_g.cu, grouping/tf_grouping_g.cu,
-interpolation/tf_interpolate_g.cu}) compiled unmodified for sm_100 by oracle/Makefile (`make ref`).
+(lib/utils/tf_ops/{sampling/tf_sampling_g.cu, grouping/tf_grouping_g.cu,
+interpolation/tf_interpolate_g.cu}) compiled unmodified for sm_90 by oracle/Makefile (`make ref`).
 
 TEST INFRASTRUCTURE ONLY.  Used (a) as the bit-exactness oracle of the `-m gpu` tests, (b) to
 produce tests/golden/*.npz (make_golden.py), and (c) as the GPU leg of bench.py --impl reference.

@@ -12,7 +12,7 @@
  *
  * Parity pin: the reference has no golden vectors for this path (SURVEY.md section 8c); the pins
  * are tests/golden/*.npz, produced by running the reference's own kernels (oracle/_ref,
- * compiled unmodified from /root/reference) on a B200 -- see tests/golden/make_golden.py.
+ * compiled unmodified from the reference sources) on a GPU -- see tests/golden/make_golden.py.
  *
  * Citations are file:line under /root/reference/lib/utils/tf_ops/.
  */

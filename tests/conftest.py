@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -36,8 +36,16 @@ def cuda():
 
 @pytest.fixture(scope="session")
 def ref_ops(cuda):
-    """The reference's own kernels (oracle/_ref/libref_ops.so, built from /root/reference by `make -C oracle ref`)."""
-    from oracle import ref_ops
+    """Outputs of the reference's own kernels, replayed from tests/golden/ref_kernels.npz (oracle/ref_golden.py).
+    With SSD3D_RECORD_REF=<path> the live kernels (oracle/_ref/libref_ops.so, `make -C oracle ref`) run instead
+    and their outputs are written to <path> at the end of the session."""
+    from oracle import ref_golden, ref_ops
+    path = os.environ.get("SSD3D_RECORD_REF")
+    if not path:
+        yield ref_golden.Replay(os.path.join(ROOT, "tests", "golden", "ref_kernels.npz"))
+        return
     if not ref_ops.available():
-        pytest.skip("oracle/_ref/libref_ops.so not built")
-    return ref_ops
+        pytest.fail("SSD3D_RECORD_REF is set but oracle/_ref/libref_ops.so is not built")
+    rec = ref_golden.Recorder(ref_ops)
+    yield rec
+    rec.save(path)

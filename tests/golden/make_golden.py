@@ -1,8 +1,8 @@
 """Generates tests/golden/*.npz by running the REFERENCE's own CUDA kernels (oracle/_ref/libref_ops.so,
-compiled unmodified from /root/reference by `make -C oracle ref`) on seeded inputs.
+compiled unmodified from the reference sources by `make -C oracle ref`) on seeded inputs.
 
-Must run on a GPU box:   gpurun -- 'python tests/golden/make_golden.py gpurun_out/golden'
-then copy gpurun_out/golden/*.npz into tests/golden/ and commit.  The fixtures pin the CPU oracle
+Must run on a GPU:   python tests/golden/make_golden.py <dir>
+then copy <dir>/*.npz into tests/golden/ and commit.  The fixtures pin the CPU oracle
 (tests/test_oracle_cpu.py::test_oracle_against_reference_golden_vectors) -- the reference itself ships no
 golden vectors for this path (SURVEY.md section 8c).
 """
@@ -100,4 +100,4 @@ def main(out_dir):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "gpurun_out", "golden"))
+    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "golden_out"))

@@ -5,7 +5,7 @@ are pulled out of their source files with `ast` and executed as they are (nothin
   lib/utils/box_3d_utils.py   get_box3d_corners_helper_np
   lib/utils/kitti_util.py     project_to_image
   lib/utils/anchors_util.py   project_to_image_space_corners
-Runs in the build container only (needs /root/reference):   python tests/golden/make_golden_io.py
+Needs a reference checkout (path in $REFERENCE):   REFERENCE=<checkout> python tests/golden/make_golden_io.py
 """
 import ast
 import os
@@ -13,7 +13,7 @@ import types
 
 import numpy as np
 
-REF = "/root/reference/lib/utils"
+REF = os.path.join(os.environ.get("REFERENCE", "."), "lib", "utils")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

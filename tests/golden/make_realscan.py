@@ -1,16 +1,16 @@
 """Builds tests/golden/realscan_16384.npz from the reference's sample KITTI scan (SURVEY.md section 8d, distribution B).
 
-/root/reference/mayavi/kitti_sample_scan.txt holds 123 398 velodyne points (x forward, y left, z up).  They are mapped
+mayavi/kitti_sample_scan.txt of the reference holds 123 398 velodyne points (x forward, y left, z up).  They are mapped
 to the rect camera frame of configs/kitti/3dssd/3dssd.yaml:3 (x_r = -y_v, y_r = -z_v, z_r = x_v), cropped to the
 detection range x in (-40, 40), y in (-5, 3), z in (0, 70) and |x| < z (about 90 degrees of field of view), and a seeded
 choice of 16 384 of them is stored with a U(0,1) intensity: one real LiDAR scene in the loader's [16384, 4] layout.
-Runs in the build container only (needs /root/reference):   python tests/golden/make_realscan.py
+Needs a reference checkout (path in $REFERENCE):   REFERENCE=<checkout> python tests/golden/make_realscan.py
 """
 import os
 
 import numpy as np
 
-SRC = "/root/reference/mayavi/kitti_sample_scan.txt"
+SRC = os.path.join(os.environ.get("REFERENCE", "."), "mayavi", "kitti_sample_scan.txt")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

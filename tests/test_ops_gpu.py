@@ -517,7 +517,7 @@ def test_argument_validation(pkg, cuda):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# tensor-core path (tcgen05, bf16 hi/lo split, 3 MMAs): same 1e-3 budget, expected error ~1e-5
+# tensor-core path (wgmma, bf16 hi/lo split, 3 MMAs): same 1e-3 budget, expected error ~1e-5
 # ---------------------------------------------------------------------------------------------------------
 def _fold(pkg, cuda, rng, cin, cout, bn=True):
     P = importlib.import_module("3dssd_b200.params")

@@ -193,7 +193,7 @@ def _golden_files():
 @pytest.mark.parametrize("path", _golden_files() or [None])
 def test_oracle_against_reference_golden_vectors(oracle_ops, path):
     """Pins the oracle: outputs of the REFERENCE's own CUDA kernels (oracle/_ref, compiled unmodified from
-    /root/reference and run on a B200 by tests/golden/make_golden.py) must be reproduced bit-for-bit."""
+    the reference sources by tests/golden/make_golden.py and run on a GPU) must be reproduced bit-for-bit."""
     if path is None:
         pytest.skip("no golden vectors committed yet (parity unpinned)")
     z = np.load(path)

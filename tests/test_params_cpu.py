@@ -14,7 +14,7 @@ P = importlib.import_module("3dssd_b200.params")
 
 @pytest.mark.parametrize("rb", [128, 64, 32])
 def test_swizzle_block_is_the_canonical_xor_of_address_bits(rb):
-    """K-major UMMA / TMA shared-memory layouts SWIZZLE_128B / 64B / 32B XOR the 16-byte-chunk address bits [4, 4+B) with
+    """K-major wgmma / TMA shared-memory layouts SWIZZLE_128B / 64B / 32B XOR the 16-byte-chunk address bits [4, 4+B) with
     bits [7, 7+B) (B = 3 / 2 / 1): element (r, k) of a [rows, rb/2] bf16 block lives at byte a ^ (((a >> 7) & (2^B - 1)) << 4)
     with a = r * rb + 2k.  _swizzle_block is written in terms of chunks and row groups; this checks it address by address."""
     rows = 48

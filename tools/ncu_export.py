@@ -1,5 +1,5 @@
-"""Export the judged metrics of an .ncu-rep (ncu --set full) into a small text summary for profiles/.
-usage: python tools/ncu_export.py report.ncu-rep > profiles/rNN_<kernel>.txt"""
+"""Export the judged metrics of an .ncu-rep (ncu --set full) into a small text summary.
+usage: python tools/ncu_export.py report.ncu-rep > <kernel>.txt"""
 import csv
 import subprocess
 import sys

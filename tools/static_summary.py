@@ -1,7 +1,7 @@
 """Static evidence about the built library (no GPU needed): per-kernel registers / stack / static shared memory from
-`cuobjdump --dump-resource-usage`, and counts of the SASS mnemonics that prove the Blackwell paths are in the binary
-(B200_PROFILING.md: UTCHMMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st, UTMALDG/UTMASTG = TMA tensor copies, UBLKCP = bulk
-copy, CREDUX / REDUX = redux.sync, SYNCS = mbarrier, STAS = st.async).  Usage: python tools/static_summary.py > profiles/rNN_static_summary.txt"""
+`cuobjdump --dump-resource-usage`, and counts of the SASS mnemonics that show the Hopper paths are in the binary
+(HGMMA = wgmma, UTMALDG/UTMASTG = TMA tensor copies, UBLKCP = bulk copy, CREDUX / REDUX = redux.sync, SYNCS = mbarrier,
+STAS = st.async).  Usage: python tools/static_summary.py  (prints to stdout)"""
 import collections, os, re, subprocess, sys
 
 so = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "3dssd_b200", "libssd3d.so")
@@ -32,7 +32,7 @@ for ln in sass.splitlines():
     m = re.search(r"^\s+/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_]+)", ln)
     if m:
         op = m.group(1)
-        for key in ("UTCHMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "CREDUX", "REDUX", "SYNCS", "STAS", "FFMA2", "UTCATOMSWS", "UCGABAR", "ATOMG", "RED"):
+        for key in ("HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "CREDUX", "REDUX", "SYNCS", "STAS", "UCGABAR", "ATOMG", "RED"):
             if op.startswith(key):
                 cnt[key] += 1
                 per[key][fn] += 1

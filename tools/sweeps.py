@@ -1,5 +1,5 @@
 """BASELINE.json configs[2] and configs[3] (SURVEY.md 8d "Config 3" / "Config 4"), timed with CUDA events next to the
-reference's own kernels (oracle/_ref) on the same box.  JSON goes to profiles/ (commit it).
+reference's own kernels (oracle/_ref) on the same GPU.  Writes one JSON file.
 
   python tools/sweeps.py fps [out.json]   D-FPS (xyz) and F-FPS (xyz + 64 features ~N(0,1)) at N in {4096, 16384, 65536},
                                           M = N/4, B = 8: ms, ns per round, effective-stream GB/s, reference kernel ms.
@@ -9,7 +9,6 @@ reference's own kernels (oracle/_ref) on the same box.  JSON goes to profiles/ (
   python tools/sweeps.py bq [out.json]    N=16384 -> M=4096 D-FPS queries, r in {0.2,0.4,0.8} x K in {16,32,64}, C=64,
                                           MLP [64,64,128], B=8: ball query ms, fused gather+MLP+max ms, bf16 TFLOP/s issued,
                                           on synthetic-KITTI clouds and on U(0,1)^3 cubes (K saturates).
-ncu tensor-pipe % / DRAM bytes for the same shapes: profiles/r02_ncu_*.txt (captured with tools/fused_probe.py cases).
 """
 import importlib
 import json

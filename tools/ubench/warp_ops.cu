@@ -1,6 +1,6 @@
 // Dependent-chain latencies (cycles per operation, one warp unless noted) of the warp-collective and control operations the
 // pruned FPS round is made of (csrc/fps_bucket.cu): the numbers a redesign of that round has to be priced with.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench/warp_ops tools/ubench/warp_ops.cu && tools/ubench/warp_ops
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench/warp_ops tools/ubench/warp_ops.cu && tools/ubench/warp_ops
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
