@@ -5,6 +5,7 @@ from . import config, dist, head, kitti_io, layers_util, params, tf_ops  # noqa:
 from ._lib import EXPORTS, LIB_PATH, lib  # noqa: F401
 from .backbone import SABackbone  # noqa: F401
 from .head import DetectionHead  # noqa: F401
+from .params import TrainableParams  # noqa: F401
 from .layers_util import (pointnet_fp_module, pointnet_sa_module, pointnet_sa_module_msg,  # noqa: F401
                           vote_layer)
 from .tf_ops import (bev_nms, calc_square_dist, farthest_point_sample, farthest_point_sample_with_distance,  # noqa: F401

@@ -87,6 +87,16 @@ _SIGNATURES = {
     "ssd3d_vote_translate": [c_long, c_void_p, c_void_p, c_int, c_float, c_float, c_float, c_void_p, c_void_p],
     "ssd3d_decode_dist_anchor_free": [c_long, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                       c_void_p],
+    "ssd3d_linear_wgrad_workspace": [c_long, c_int, c_int],
+    "ssd3d_linear_wgrad": [c_long, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, ctypes.c_size_t, c_void_p, c_void_p,
+                           c_void_p],
+    "ssd3d_bn_train_grad_workspace": [c_int],
+    "ssd3d_bn_train_grad": [c_long, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                            c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p],
+    "ssd3d_rowgroup_max_grad": [c_long, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p],
+    "ssd3d_group_concat_grad": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                c_void_p],
+    "ssd3d_vote_translate_grad": [c_long, c_void_p, c_int, c_void_p, c_float, c_float, c_float, c_void_p, c_void_p],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["ssd3d_last_error"])
@@ -103,7 +113,8 @@ def lib():
         for name, argtypes in _SIGNATURES.items():
             fn = getattr(l, name)
             fn.argtypes = argtypes
-            fn.restype = ctypes.c_size_t if name in ("ssd3d_sa_fused_smem", "ssd3d_query_ball_point_workspace", "ssd3d_bn_train_workspace") else c_int
+            fn.restype = ctypes.c_size_t if name in ("ssd3d_sa_fused_smem", "ssd3d_query_ball_point_workspace", "ssd3d_bn_train_workspace",
+                                                   "ssd3d_linear_wgrad_workspace", "ssd3d_bn_train_grad_workspace") else c_int
             if name == "ssd3d_fps_temp_elems":
                 fn.restype = c_long
         l.ssd3d_last_error.restype = ctypes.c_char_p

@@ -16,7 +16,7 @@ import math
 import torch
 
 from . import tf_ops
-from .params import prepare
+from .params import TrainableParams, prepare
 
 ANGLE_CLS_NUM = 12          # MODEL.ANGLE_CLS_NUM (3dssd.yaml:38)
 REG_CHANNELS = 6            # 'Dist-Anchor-free': distances to the 6 faces (head_builder.py:49-55)
@@ -42,14 +42,21 @@ def _conv_chain(pp, hi, lo, scopes_bn_relu):
 def box_regression_head(feature_input, pred_cls_channel, pred_reg_base_num, pred_reg_channel_num, bn, is_training, *,
                         params, scope=''):
     """head_util.py:26-59 without the nuScenes attribute / velocity branches.  feature_input (bs, n, c) fp32.
-    Returns (pred_cls (bs,n,cls), pred_offset (bs,n,base,6), pred_angle_cls (bs,n,base,12), pred_angle_res (...))."""
-    if is_training:
-        raise NotImplementedError("inference only")
-    pp = prepare(params, feature_input.device)
+    Returns (pred_cls (bs,n,cls), pred_offset (bs,n,base,6), pred_angle_cls (bs,n,base,12), pred_angle_res (...)).
+    is_training=True needs params as a params.TrainableParams: both conv chains then run with batch-statistics BatchNorm
+    through the differentiable tf_ops.conv_train."""
     bs, n, _ = feature_input.shape
-    hi, lo = tf_ops.split_rows(feature_input)
-    pred_cls = _conv_chain(pp, hi, lo, [(_scope(scope, "pred_cls_base"), bn, True), (_scope(scope, "pred_cls"), False, False)])
-    pred_reg = _conv_chain(pp, hi, lo, [(_scope(scope, "pred_reg_base"), bn, True), (_scope(scope, "pred_reg"), False, False)])
+    if is_training:
+        if not isinstance(params, TrainableParams):
+            raise NotImplementedError("is_training=True needs params.TrainableParams (the inference forms are folded)")
+        chain = lambda base, pred: params.conv_train(_scope(scope, pred), params.conv_train(_scope(scope, base), feature_input, bn),
+                                                     False, relu=False)
+        pred_cls, pred_reg = chain("pred_cls_base", "pred_cls"), chain("pred_reg_base", "pred_reg")
+    else:
+        pp = prepare(params, feature_input.device)
+        hi, lo = tf_ops.split_rows(feature_input)
+        pred_cls = _conv_chain(pp, hi, lo, [(_scope(scope, "pred_cls_base"), bn, True), (_scope(scope, "pred_cls"), False, False)])
+        pred_reg = _conv_chain(pp, hi, lo, [(_scope(scope, "pred_reg_base"), bn, True), (_scope(scope, "pred_reg"), False, False)])
     pred_reg = pred_reg.view(bs, n, pred_reg_base_num, pred_reg_channel_num + ANGLE_CLS_NUM * 2)
     return (pred_cls, pred_reg[..., :pred_reg_channel_num],
             pred_reg[..., pred_reg_channel_num:pred_reg_channel_num + ANGLE_CLS_NUM],

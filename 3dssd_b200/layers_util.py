@@ -5,13 +5,15 @@ pointnet_sa_module_msg :59-189, pointnet_fp_module :192-225 -- same positional a
 torch CUDA tensors instead of TF tensors.  What TF resolved through variable scopes is passed explicitly as
 `params` (a dict keyed by the reference's variable names, or a params.PreparedParams).  is_training=True runs the
 convs with batch-statistics BatchNorm and updates the moving statistics in place (tf_util.py:424-444); the fused
-inference kernels fold BN and therefore serve is_training=False only.
+inference kernels fold BN and therefore serve is_training=False only.  With params a params.TrainableParams,
+is_training=True runs the same schedule through the differentiable operators of tf_ops (conv_train, group_max_train,
+group_concat_train, vote_translate_train): loss.backward() then reaches every weight, bias, gamma and beta.
 """
 import torch
 
 from . import config as _cfg
 from . import tf_ops
-from .params import prepare
+from .params import TrainableParams, prepare
 
 
 def _conv(pp, scope, x, bn=True, relu=True, pool=1, rowmask=None):
@@ -19,11 +21,18 @@ def _conv(pp, scope, x, bn=True, relu=True, pool=1, rowmask=None):
     return tf_ops.linear_bn_relu(x, f.w, f.scale, f.shift, relu=relu, pool=pool, rowmask=rowmask, cin=f.cin)
 
 
-def _conv_train(pp, scope, x, bn, bn_decay, relu=True):
+def _trainable(params, is_training):
+    return bool(is_training) and isinstance(params, TrainableParams)
+
+
+def _conv_train(pp, scope, x, bn, bn_decay, relu=True, debug=None):
     """conv (+bias) -> training-mode BatchNorm -> ReLU, tf_util.conv2d / conv1d with is_training=True
     (/root/reference/lib/utils/tf_util.py:51-124, :127-201, :424-444).  The contraction runs on the tensor-core path with
     the BN-less fold (scale = 1, shift = bias); the batch statistics, the normalisation and the in-place update of the
-    moving statistics are one ssd3d_bn_train call."""
+    moving statistics are one ssd3d_bn_train call.  A TrainableParams takes the differentiable twin (tf_ops.conv_train);
+    debug (a list) then receives the conv's (pre-BN, post-activation) tensors."""
+    if isinstance(pp, TrainableParams):
+        return pp.conv_train(scope, x, bn, bn_decay, relu, debug)
     hi, lo = tf_ops.split_rows(x)
     y, _ = tf_ops.linear_tc(hi, lo, pp.conv(scope, False), relu=bool(relu and not bn), want_f32=True, want_split=False)
     if not bn:
@@ -47,15 +56,19 @@ def _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_l
                     else tf_ops.query_ball_point(radius_list[i], nsample_list[i], xyz, new_xyz))
             idx_list.append(a); cnt_list.append(c)
     debug["idx"].append(idx_list); debug["cnt"].append(cnt_list)
+    trainable = isinstance(pp, TrainableParams)
+    group_concat = tf_ops.group_concat_train if trainable else tf_ops.group_concat
+    group_max = tf_ops.group_max_train if trainable else tf_ops.rowgroup_max
+    convs = debug.setdefault("convs", []) if trainable else None
     outs = []
     for i in range(nscale):
-        g = tf_ops.group_concat(xyz, points, new_xyz, idx_list[i])                                  # :160-165
+        g = group_concat(xyz, points, new_xyz, idx_list[i])                                         # :160-165
         for j in range(len(mlp_list[i])):
-            g = _conv_train(pp, "%s/conv%d_%d" % (scope, i, j), g, bn, bn_decay)                    # :167-176
-        outs.append(tf_ops.rowgroup_max(g, nsample_list[i], cnt_list[i]))                           # :178-180
+            g = _conv_train(pp, "%s/conv%d_%d" % (scope, i, j), g, bn, bn_decay, debug=convs)       # :167-176
+        outs.append(group_max(g, nsample_list[i], cnt_list[i]))                                     # :178-180
     new_points = outs[0] if len(outs) == 1 else torch.cat(outs, dim=-1)
     if use_agg:
-        new_points = _conv_train(pp, scope + "/ensemble", new_points, bn, bn_decay)                 # :183-185
+        new_points = _conv_train(pp, scope + "/ensemble", new_points, bn, bn_decay, debug=convs)    # :183-185
     return new_points
 
 
@@ -304,7 +317,8 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
         fps_parts = None                      # training takes the literal layer-by-layer schedule
     if mlp_mode not in ("tc", "fp32"):
         raise ValueError("mlp_mode must be 'tc' or 'fp32'")
-    pp = prepare(params, xyz.device)
+    trainable = _trainable(params, is_training)
+    pp = params if trainable else prepare(params, xyz.device)
     aggregation = _cfg.AGGREGATION_SA_FEATURE if aggregation is None else aggregation
     bs, n, _ = xyz.shape
     dev = xyz.device
@@ -316,7 +330,7 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
     # ---- hoisted first convs: the feature part of conv0 of every scale, once per POINT (independent of the sampling)
     c_feat = points.shape[-1]
     stacks = hoist = None
-    if nscale:
+    if nscale and not trainable:              # folded inference forms: not used by the differentiable path
         tc_ok = mlp_mode == "tc" and all(k in (8, 16, 32, 64, 128) for k in nsample_list) and all(m[-1] % 8 == 0 for m in mlp_list)
         stacks = [pp.fused_stack(["%s/conv%d_%d" % (scope, i, j) for j in range(len(mlp_list[i]))], bn, c_feat + 3)
                   if (fuse_scale and tc_ok) else None for i in range(nscale)]
@@ -431,7 +445,7 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
         if nscale and is_training:
             new_points = _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_list, mlp_list, bn,
                                               bn_decay, dilated_group, use_agg, debug)
-            debug = {"idx": debug["idx"][0], "cnt": debug["cnt"][0]}
+            debug = dict(debug, idx=debug["idx"][0], cnt=debug["cnt"][0])
         elif nscale:
             _compute_hoist(hoist, pp, scope, mlp_list, bn, points, stacks)
             new_points = _group_and_mlp(pp, scope, xyz, points, new_xyz, radius_list, nsample_list, mlp_list, bn,
@@ -476,17 +490,20 @@ _KEEPALIVE = []   # latency mode: the last layers' cross-stream temporaries (fre
 
 def pointnet_sa_module(xyz, points, mlp, is_training, bn_decay, bn, scope, *, params):
     """Global SA layer (layer type SA_Layer_SSG_Last): concat[xyz, points] -> MLP -> max over all points."""
-    pp = prepare(params, xyz.device)
+    trainable = _trainable(params, is_training)
+    pp = params if trainable else prepare(params, xyz.device)
     g = torch.cat([xyz, points], dim=-1).contiguous()              # xyz FIRST here (:42)
     n = g.shape[1]
     for j in range(len(mlp)):
         g = _conv_train(pp, "%s/conv%d" % (scope, j), g, bn, bn_decay) if is_training else _conv(pp, "%s/conv%d" % (scope, j), g, bn=bn)
+    if trainable and n:
+        return torch.amax(g, dim=1)                                # gradient split evenly among ties, like tf.reduce_max
     return g.max(dim=1).values if n else g
 
 
 def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay, scope, bn=True, *, params):
     """Feature propagation: inverse-distance interpolation from (xyz2, points2) onto xyz1, then an MLP."""
-    pp = prepare(params, xyz1.device)
+    pp = params if _trainable(params, is_training) else prepare(params, xyz1.device)
     dist, idx = tf_ops.three_nn(xyz1, xyz2)
     dist = torch.clamp_min(dist, 1e-10)                            # :207
     inv = 1.0 / dist
@@ -502,6 +519,11 @@ def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay,
 def vote_layer(xyz, points, mlp_list, is_training, bn_decay, bn, scope, *, params,
                max_translate_range=_cfg.MAX_TRANSLATE_RANGE, mlp_mode="tc"):
     """Vote layer: per-point MLP -> 3 offsets, clamped to +-max_translate_range (layers_util.py:12-24)."""
+    if _trainable(params, is_training):
+        for i in range(len(mlp_list)):
+            points = params.conv_train("%s/vote_layer_%d" % (scope, i), points, bn, bn_decay)
+        off = params.conv_train(scope + "/vote_offsets", points, False, bn_decay, relu=False)
+        return tf_ops.vote_translate_train(xyz, off, max_translate_range), points, off
     pp = prepare(params, xyz.device)
     if is_training:
         for i in range(len(mlp_list)):

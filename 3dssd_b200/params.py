@@ -279,5 +279,50 @@ class PreparedParams:
         return self
 
 
+class TrainableParams:
+    """The parameters of a params dict as device tensors for training (layers with is_training=True run their
+    differentiable path when given one of these): weights, biases, gamma and beta are leaf tensors with
+    requires_grad=True, the moving statistics plain tensors that training forwards update in place.  Keys are the TF
+    variable names.  Nothing folded is cached: every forward reads the live tensors, so an optimizer step is seen by the
+    next forward.  to_params() returns the numpy dict (moving statistics included) for prepare() / SABackbone."""
+
+    _STATS = ("/bn/moving_mean", "/bn/moving_variance")
+
+    def __init__(self, params, device="cuda"):
+        self.device = torch.device(device)
+        self.tensors = {}
+        for k, v in params.items():
+            t = torch.from_numpy(np.array(v, dtype=np.float32, copy=True)).to(self.device)
+            self.tensors[k] = t if k.endswith(self._STATS) else t.requires_grad_(True)
+
+    def named_parameters(self):
+        return [(k, t) for k, t in self.tensors.items() if t.requires_grad]
+
+    def parameters(self):
+        return [t for _, t in self.named_parameters()]
+
+    def grads(self):
+        """{TF name: gradient} of every trainable tensor (None where no gradient reached it)."""
+        return {k: t.grad for k, t in self.named_parameters()}
+
+    def to_params(self):
+        return {k: t.detach().cpu().numpy().copy() for k, t in self.tensors.items()}
+
+    def conv_train(self, scope, x, bn=True, bn_decay=None, relu=True, debug=None):
+        """One conv (+ training BatchNorm when bn) (+ ReLU) of `scope`, differentiable (tf_ops.conv_train)."""
+        from . import tf_ops
+        t = self.tensors
+        g = lambda k: t.get(scope + k)
+        b = g("/biases")
+        if b is None:
+            b = torch.zeros((t[scope + "/weights"].shape[1],), dtype=torch.float32, device=self.device)
+        return tf_ops.conv_train(x, t[scope + "/weights"], b, g("/bn/gamma"), g("/bn/beta"), g("/bn/moving_mean"),
+                                 g("/bn/moving_variance"), bn=bn, relu=relu, decay=0.9 if bn_decay is None else float(bn_decay),
+                                 debug=debug)
+
+
 def prepare(params, device="cuda"):
+    """Folded inference form of a params dict; a TrainableParams is folded from its current values."""
+    if isinstance(params, TrainableParams):
+        return PreparedParams(params.to_params(), device)
     return params if isinstance(params, PreparedParams) else PreparedParams(params, device)

@@ -946,3 +946,221 @@ def rowgroup_max(y, pool, rowmask=None):
     out = torch.empty(tuple(y.shape[:-2]) + (c,), dtype=torch.float32, device=y.device)
     check(lib().ssd3d_rowgroup_max(y.numel() // (c * pool), pool, c, _p(y), c, _p(rowmask), _p(out), _stream()), "rowgroup_max")
     return out
+
+
+# ---- backward of the training-mode layers (DESIGN.md "Backward") ---------------------------------------------------
+
+def _f32(t, name):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
+        raise ValueError("%s must be a float32 CUDA tensor" % name)
+    return t if t.is_contiguous() else t.contiguous()
+
+
+def linear_wgrad(x, dz, want_bias=True):
+    """Weight gradient of a 1x1 conv: x (..., cin), dz (..., cout) -> grad_w (cin, cout) = x^T dz over all rows and
+    grad_b (cout,) = column sums of dz (None unless want_bias).  Tensor cores, fixed-order split-K: same bits every run."""
+    x, dz = _f32(x, "x"), _f32(dz, "dz")
+    cin, cout = x.shape[-1], dz.shape[-1]
+    rows = x.numel() // cin if cin else 0
+    if cin == 0 or cout == 0 or dz.numel() // cout != rows or rows == 0:
+        raise ValueError("linear_wgrad: x %s and dz %s must share their rows" % (tuple(x.shape), tuple(dz.shape)))
+    ws_bytes = int(lib().ssd3d_linear_wgrad_workspace(rows, cin, cout))
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=x.device)
+    gw = torch.empty((cin, cout), dtype=torch.float32, device=x.device)
+    gb = torch.empty((cout,), dtype=torch.float32, device=x.device) if want_bias else None
+    check(lib().ssd3d_linear_wgrad(rows, cin, cout, _p(x), cin, _p(dz), cout, _p(ws), ws_bytes, _p(gw), _p(gb), _stream()),
+          "linear_wgrad")
+    return gw, gb
+
+
+def bn_train_grad(x, grad_out, scale, shift, batch_mean, batch_var, gamma, relu=True, eps=BN_EPS):
+    """Backward of bn_train (+ ReLU) from its input x (the pre-BN conv output) and its outputs (scale, shift, batch_mean,
+    batch_var) -> (grad_x, grad_gamma, grad_beta).  The moving statistics are not touched."""
+    x, grad_out = _f32(x, "x"), _f32(grad_out, "grad_out")
+    if grad_out.shape != x.shape:
+        raise ValueError("bn_train_grad: grad_out %s must have the shape of x %s" % (tuple(grad_out.shape), tuple(x.shape)))
+    c = x.shape[-1]
+    rows = x.numel() // c
+    for t, name in ((scale, "scale"), (shift, "shift"), (batch_mean, "batch_mean"), (batch_var, "batch_var"), (gamma, "gamma")):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or tuple(t.shape) != (c,) or not t.is_contiguous():
+            raise ValueError("%s must be a contiguous float32 CUDA tensor of shape (%d,)" % (name, c))
+    dev = x.device
+    gx = torch.empty_like(x)
+    gg, gbeta = (torch.empty((c,), dtype=torch.float32, device=dev) for _ in range(2))
+    ws = torch.empty((int(lib().ssd3d_bn_train_grad_workspace(c)),), dtype=torch.uint8, device=dev)
+    check(lib().ssd3d_bn_train_grad(rows, c, _p(x), c, _p(grad_out), c, _p(scale), _p(shift), _p(batch_mean), _p(batch_var),
+                                    _p(gamma), float(eps), 1 if relu else 0, _p(ws), _p(gg), _p(gbeta), _p(gx), c, _stream()),
+          "bn_train_grad")
+    return gx, gg, gbeta
+
+
+def rowgroup_max_grad(y, grad_out, pool, rowmask=None):
+    """Backward of rowgroup_max: y (..., pool, c), grad_out (..., c) -> grad_y (..., pool, c); the gradient of a group is
+    split evenly among its tied maxima and multiplied by (rowmask != 0)."""
+    y, grad_out = _f32(y, "y"), _f32(grad_out, "grad_out")
+    c, pool = y.shape[-1], int(pool)
+    if y.dim() < 2 or y.shape[-2] != pool or tuple(grad_out.shape) != tuple(y.shape[:-2]) + (c,):
+        raise ValueError("rowgroup_max_grad: y must be (..., pool, c) and grad_out (..., c)")
+    groups = grad_out.numel() // c
+    if rowmask is not None:
+        rowmask = _req(rowmask, "rowmask", torch.int32, rowmask.dim())
+        if rowmask.numel() != groups:
+            raise ValueError("rowmask must hold one entry per group")
+    gy = torch.empty_like(y)
+    check(lib().ssd3d_rowgroup_max_grad(groups, pool, c, _p(y), c, _p(rowmask), _p(grad_out), _p(gy), c, _stream()),
+          "rowgroup_max_grad")
+    return gy
+
+
+def group_concat_grad(grad_x, idx, n, c, want_points=True, want_xyz=True, want_new_xyz=True):
+    """Backward of group_concat: grad_x (b, m, nsample, ldx) -> (grad_points (b, n, c), grad_xyz (b, n, 3),
+    grad_new_xyz (b, m, 3)); an output not wanted is None."""
+    grad_x = _req(grad_x, "grad_x", torch.float32, 4)
+    idx = _req(idx, "idx", torch.int32, 3)
+    b, m, ns, ldx = grad_x.shape
+    if tuple(idx.shape) != (b, m, ns) or ldx < c + 3 or int(n) <= 0:
+        raise ValueError("group_concat_grad: grad_x %s does not match idx %s with c = %d" % (tuple(grad_x.shape), tuple(idx.shape), c))
+    dev = grad_x.device
+    gp = torch.empty((b, n, c), dtype=torch.float32, device=dev) if (want_points and c > 0) else None
+    gxyz = torch.empty((b, n, 3), dtype=torch.float32, device=dev) if want_xyz else None
+    gnew = torch.empty((b, m, 3), dtype=torch.float32, device=dev) if want_new_xyz else None
+    check(lib().ssd3d_group_concat_grad(b, int(n), int(c), m, ns, _p(idx), _p(grad_x), ldx, _p(gp), _p(gxyz), _p(gnew), _stream()),
+          "group_concat_grad")
+    return gp, gxyz, gnew
+
+
+def vote_translate_grad(offsets, grad_out, min_range):
+    """Backward of vote_translate w.r.t. the offsets (b, n, >= 3): grad_out (b, n, 3) where min <= offset <= -min
+    (inclusive), else 0 -> (b, n, 3)."""
+    offsets, grad_out = _req(offsets, "offsets", torch.float32, 3), _req(grad_out, "grad_out", torch.float32, 3, 3)
+    if offsets.shape[:2] != grad_out.shape[:2] or offsets.shape[2] < 3:
+        raise ValueError("offsets must be (b, n, >= 3) like grad_out")
+    g = torch.empty_like(grad_out)
+    check(lib().ssd3d_vote_translate_grad(grad_out.shape[0] * grad_out.shape[1], _p(offsets), offsets.shape[2], _p(grad_out),
+                                          float(min_range[0]), float(min_range[1]), float(min_range[2]), _p(g), _stream()),
+          "vote_translate_grad")
+    return g
+
+
+def _folded(w, scale, shift):
+    from .params import FoldedConv
+    return FoldedConv(w, scale, shift)
+
+
+class _ConvTrain(torch.autograd.Function):
+    """conv (+bias) -> [training BatchNorm] -> [ReLU] of one layer (tf_util.conv2d / conv1d with is_training=True).
+    Forward: split_rows -> linear_tc with the BN-less fold -> bn_train, the sequence of the non-trainable training path.
+    Backward: bn_train_grad -> split -> linear_tc with W^T (grad_x) and linear_wgrad (grad_w, grad_b)."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, gamma, beta, opts):
+        bn, relu, decay, moving, debug = opts
+        x = x if x.is_contiguous() else x.contiguous()
+        hi, lo = split_rows(x)
+        cout = w.shape[1]
+        ones = torch.ones((cout,), dtype=torch.float32, device=x.device)
+        y, _ = linear_tc(hi, lo, _folded(w.detach(), ones, b.detach()), relu=bool(relu and not bn), want_f32=True, want_split=False)
+        ctx.bn, ctx.relu = bn, relu
+        if bn:
+            out, scale, shift, bmean, bvar = bn_train(y, gamma.detach(), beta.detach(), moving[0], moving[1], decay=decay, relu=relu)
+            ctx.save_for_backward(x, w, y, scale, shift, bmean, bvar, gamma)
+        else:
+            out = y
+            ctx.save_for_backward(x, w, y)
+        if debug is not None:
+            debug.append((y, out))
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        g = g.contiguous()
+        x, w, y = ctx.saved_tensors[:3]
+        ggamma = gbeta = None
+        if ctx.bn:
+            scale, shift, bmean, bvar, gamma = ctx.saved_tensors[3:]
+            dz, ggamma, gbeta = bn_train_grad(y, g, scale, shift, bmean, bvar, gamma, relu=ctx.relu)
+        elif ctx.relu:
+            dz = torch.where(y > 0, g, torch.zeros((), dtype=g.dtype, device=g.device))   # ReluGrad: output > 0
+        else:
+            dz = g
+        cin, cout = w.shape
+        gx = None
+        if ctx.needs_input_grad[0]:
+            d_hi, d_lo = split_rows(dz)
+            wt = _folded(w.detach().t().contiguous(), torch.ones((cin,), dtype=torch.float32, device=dz.device),
+                         torch.zeros((cin,), dtype=torch.float32, device=dz.device))
+            gx, _ = linear_tc(d_hi, d_lo, wt, relu=False, want_f32=True, want_split=False)
+        gw, gb = linear_wgrad(x, dz, want_bias=True)
+        return gx, gw, gb, ggamma, gbeta, None
+
+
+def conv_train(x, w, b, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9, debug=None):
+    """Differentiable conv (+bias) -> training BatchNorm (bn=True; updates moving_mean / moving_var in place) -> ReLU of
+    one layer over the last axis of x, with the forward bits of the non-trainable training path.  x (..., cin),
+    w (cin, cout), b / gamma / beta (cout,).  debug: a list that receives (pre-BN conv output, layer output)."""
+    if not isinstance(x, torch.Tensor) or x.dtype != torch.float32:     # the device is checked by the kernels' wrappers
+        raise ValueError("x must be a float32 tensor")
+    if w.dim() != 2 or x.shape[-1] != w.shape[0] or tuple(b.shape) != (w.shape[1],):
+        raise ValueError("conv_train: x %s, w %s, b %s do not match" % (tuple(x.shape), tuple(w.shape), tuple(b.shape)))
+    if bn and (gamma is None or beta is None):
+        raise ValueError("conv_train: bn=True needs gamma and beta")
+    z = torch.zeros((0,), dtype=torch.float32, device=x.device)
+    return _ConvTrain.apply(x, w, b, gamma if bn else z, beta if bn else z,
+                            (bool(bn), bool(relu), float(decay), (moving_mean, moving_var), debug))
+
+
+class _GroupMax(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, y, pool, rowmask):
+        ctx.save_for_backward(y, rowmask)
+        ctx.pool = pool
+        return rowgroup_max(y, pool, rowmask)
+
+    @staticmethod
+    def backward(ctx, g):
+        y, rowmask = ctx.saved_tensors
+        return rowgroup_max_grad(y, g.contiguous(), ctx.pool, rowmask), None, None
+
+
+def group_max_train(y, pool, rowmask=None):
+    """Differentiable rowgroup_max (tf.reduce_max(axis=2) * mask): ties share the gradient evenly, as in TF."""
+    return _GroupMax.apply(y, int(pool), rowmask)
+
+
+class _GroupConcat(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, xyz, points, new_xyz, idx):
+        ctx.save_for_backward(idx)
+        ctx.n, ctx.c = xyz.shape[1], 0 if points is None else points.shape[2]
+        return group_concat(xyz, points, new_xyz, idx)
+
+    @staticmethod
+    def backward(ctx, g):
+        (idx,) = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        gp, gxyz, gnew = group_concat_grad(g.contiguous(), idx, ctx.n, ctx.c, need[1], need[0], need[2])
+        return gxyz, gp, gnew, None
+
+
+def group_concat_train(xyz, points, new_xyz, idx):
+    """Differentiable group_concat: gradients reach points, xyz and the query centres new_xyz."""
+    return _GroupConcat.apply(xyz, points, new_xyz, idx)
+
+
+class _VoteTranslate(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, xyz, offsets, min_range):
+        ctx.save_for_backward(offsets)
+        ctx.min_range = min_range
+        return vote_translate(xyz, offsets, min_range)
+
+    @staticmethod
+    def backward(ctx, g):
+        (offsets,) = ctx.saved_tensors
+        g = g.contiguous()
+        return g, vote_translate_grad(offsets, g, ctx.min_range), None
+
+
+def vote_translate_train(xyz, offsets, min_range):
+    """Differentiable vote_translate: identity for xyz, the clamp's gradient (inclusive bounds) for the offsets."""
+    return _VoteTranslate.apply(xyz, offsets, tuple(float(v) for v in min_range))

@@ -311,6 +311,44 @@ int ssd3d_bn_train(long rows, int c, const float *x, int ldx, const float *gamma
                    float *moving_var, float decay, float eps, void *workspace, float *scale, float *shift,
                    float *batch_mean, float *batch_var, int relu, float *out, int ldo, ssd3d_stream_t stream);
 
+/* ---- backward of the training-mode layers (csrc/train_grad.cu, csrc/bn.cu; DESIGN.md "Backward") ----------------
+ * The data gradient of a conv, grad_x = dz . W^T, needs no entry point of its own: it is ssd3d_linear_tc with the
+ * split of W^T as its weight (scale 1, shift 0, no ReLU). */
+
+/* Weight gradient of a 1x1 conv: grad_w[cin, cout] = sum_r x[r, 0:cin]^T dz[r, 0:cout], grad_b[cout] = sum_r dz[r, :]
+ * (grad_b may be NULL).  x [rows, ldx], dz [rows, lddz] fp32 row-major.  Tensor cores with the bf16 hi/lo split of
+ * ssd3d_linear_tc (hi.hi + lo.hi + hi.lo, fp32 accumulation), split over row ranges; the partial tiles are reduced in a
+ * fixed order through the workspace (ssd3d_linear_wgrad_workspace(rows, cin, cout) bytes, 8-byte aligned), so the
+ * result is the same bits from run to run. */
+size_t ssd3d_linear_wgrad_workspace(long rows, int cin, int cout);
+int ssd3d_linear_wgrad(long rows, int cin, int cout, const float *x, int ldx, const float *dz, int lddz, void *workspace,
+                       size_t workspace_bytes, float *grad_w, float *grad_b, ssd3d_stream_t stream);
+/* Backward of ssd3d_bn_train (+ its activation): x is the forward's input (the pre-BN conv output), scale / shift /
+ * batch_mean / batch_var its outputs.  The ReLU mask is the forward's decision fma(x, scale, shift) > 0.
+ * grad_beta = sum g, grad_gamma = sum g x^, grad_x = gamma r / N (N g - sum g - x^ sum g x^), r = rsqrt(var + eps),
+ * x^ = (x - mean) r; sums in double.  grad_gamma / grad_beta may be NULL.  The moving statistics are not touched.
+ * workspace: ssd3d_bn_train_grad_workspace(c) bytes, 8-byte aligned. */
+size_t ssd3d_bn_train_grad_workspace(int c);
+int ssd3d_bn_train_grad(long rows, int c, const float *x, int ldx, const float *grad_out, int ldg, const float *scale,
+                        const float *shift, const float *batch_mean, const float *batch_var, const float *gamma, float eps,
+                        int relu, void *workspace, float *grad_gamma, float *grad_beta, float *grad_x, int ldgx,
+                        ssd3d_stream_t stream);
+/* Backward of ssd3d_rowgroup_max: grad_y[g*pool + r, o] = (ind / num) * (grad_out[g, o] * (rowmask[g] != 0)) with
+ * ind = (y == max of the group), num = number of tied maxima (TF's reduce_max gradient); rowmask may be NULL.
+ * grad_out [groups, c] dense. */
+int ssd3d_rowgroup_max_grad(long groups, int pool, int c, const float *y, int ldy, const int *rowmask, const float *grad_out,
+                            float *grad_y, int ldgy, ssd3d_stream_t stream);
+/* Backward of ssd3d_group_concat from grad_x [b, m, nsample, ldx]: grad_points [b, n, c] (columns 0:c scattered through
+ * idx), grad_xyz [b, n, 3] (columns c:c+3 scattered), grad_new_xyz [b, m, 3] = -sum over the nsample rows of columns
+ * c:c+3.  Any output may be NULL; the scattered ones are zero-filled first and summed with fp32 atomics. */
+int ssd3d_group_concat_grad(int b, int n, int c, int m, int nsample, const int *idx, const float *grad_x, int ldx,
+                            float *grad_points, float *grad_xyz, float *grad_new_xyz, ssd3d_stream_t stream);
+/* Backward of ssd3d_vote_translate w.r.t. the offsets: grad_offsets[r, l] = grad_out[r, l] where
+ * min_l <= offsets[r, l] <= -min_l (both bounds inclusive, as tf.maximum / tf.minimum route ties), else 0.
+ * grad_out / grad_offsets [rows, 3]. */
+int ssd3d_vote_translate_grad(long rows, const float *offsets, int ld_offsets, const float *grad_out, float min_x, float min_y,
+                              float min_z, float *grad_offsets, ssd3d_stream_t stream);
+
 /* ---- the small elementwise stages of the path (csrc/misc.cu) --------------------------------- */
 
 /* points[rows, c] -> xyz[rows, 3], feat[rows, c-3]: the tf.slice pair of
