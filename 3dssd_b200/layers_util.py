@@ -9,6 +9,9 @@ inference kernels fold BN and therefore serve is_training=False only.  With para
 is_training=True runs the same schedule through the differentiable operators of tf_ops (conv_train, group_max_train,
 group_concat_train, vote_translate_train): loss.backward() then reaches every weight, bias, gamma and beta.
 """
+from functools import partial
+from types import SimpleNamespace
+
 import torch
 
 from . import config as _cfg
@@ -27,41 +30,46 @@ def _trainable(params, is_training):
 
 def _conv_train(pp, scope, x, bn, bn_decay, relu=True, debug=None):
     """conv (+bias) -> training-mode BatchNorm -> ReLU, tf_util.conv2d / conv1d with is_training=True
-    (/root/reference/lib/utils/tf_util.py:51-124, :127-201, :424-444).  The contraction runs on the tensor-core path with
-    the BN-less fold (scale = 1, shift = bias); the batch statistics, the normalisation and the in-place update of the
-    moving statistics are one ssd3d_bn_train call.  A TrainableParams takes the differentiable twin (tf_ops.conv_train);
-    debug (a list) then receives the conv's (pre-BN, post-activation) tensors."""
+    (/root/reference/lib/utils/tf_util.py:51-124, :127-201, :424-444): tf_ops.linear_bn_train with the cached BN-less
+    fold; the batch statistics, the normalisation and the in-place update of the moving statistics are one ssd3d_bn_train
+    call.  A TrainableParams takes the differentiable twin (tf_ops.conv_train); debug (a list) then receives the conv's
+    (pre-BN, post-activation) tensors."""
     if isinstance(pp, TrainableParams):
         return pp.conv_train(scope, x, bn, bn_decay, relu, debug)
-    hi, lo = tf_ops.split_rows(x)
-    y, _ = tf_ops.linear_tc(hi, lo, pp.conv(scope, False), relu=bool(relu and not bn), want_f32=True, want_split=False)
-    if not bn:
-        return y
-    st = pp.bn_state(scope)
-    return tf_ops.bn_train(y, st["gamma"], st["beta"], st["moving_mean"], st["moving_variance"],
-                           decay=0.9 if bn_decay is None else float(bn_decay), relu=relu)[0]
+    st = pp.bn_state(scope) if bn else {}
+    return tf_ops.linear_bn_train(x, pp.conv(scope, False), st.get("gamma"), st.get("beta"), st.get("moving_mean"),
+                                  st.get("moving_variance"), bn=bn, relu=relu,
+                                  decay=0.9 if bn_decay is None else float(bn_decay))[1][0]
+
+
+def _ball_query(xyz, new_xyz, radius_list, nsample_list, dilated_group, want_units=False):
+    """The ball queries of all scales (:137-145) -> (idx_list, cnt_list, units_list); units_list holds the unit lists of
+    query_ball_point_multi(return_units=True) when want_units (up to 4 scales), else None per scale."""
+    nscale = len(radius_list)
+    min_r = [0.0 if (i == 0 or not dilated_group) else radius_list[i - 1] for i in range(nscale)]   # :137-141
+    if nscale <= 4:   # one pass over the candidates for all shells
+        res = tf_ops.query_ball_point_multi(min_r, radius_list, nsample_list, xyz, new_xyz, dilated_group, return_units=want_units)
+        return res[0], res[1], res[2] if want_units else [None] * nscale
+    idx_list, cnt_list = [], []
+    for i in range(nscale):
+        a, c = (tf_ops.query_ball_point_dilated(min_r[i], radius_list[i], nsample_list[i], xyz, new_xyz) if dilated_group
+                else tf_ops.query_ball_point(radius_list[i], nsample_list[i], xyz, new_xyz))
+        idx_list.append(a); cnt_list.append(c)
+    return idx_list, cnt_list, [None] * nscale
 
 
 def _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_list, mlp_list, bn, bn_decay, dilated_group,
-                         use_agg, debug):
+                         use_agg):
     """Training-mode twin of _group_and_mlp: the literal op sequence of layers_util.py:137-185 (grouped tensor
-    materialised once, conv -> batch-norm -> relu per layer, reduce_max, mask, concat, aggregation)."""
-    nscale = len(radius_list)
-    min_r = [0.0 if (i == 0 or not dilated_group) else radius_list[i - 1] for i in range(nscale)]
-    idx_list, cnt_list = tf_ops.query_ball_point_multi(min_r, radius_list, nsample_list, xyz, new_xyz, dilated_group) \
-        if nscale <= 4 else ([], [])
-    if nscale > 4:
-        for i in range(nscale):
-            a, c = (tf_ops.query_ball_point_dilated(min_r[i], radius_list[i], nsample_list[i], xyz, new_xyz) if dilated_group
-                    else tf_ops.query_ball_point(radius_list[i], nsample_list[i], xyz, new_xyz))
-            idx_list.append(a); cnt_list.append(c)
-    debug["idx"].append(idx_list); debug["cnt"].append(cnt_list)
+    materialised once, conv -> batch-norm -> relu per layer, reduce_max, mask, concat, aggregation).
+    Returns (new_points, idx_list, cnt_list, convs): convs lists every conv's tensors with a TrainableParams, else None."""
+    idx_list, cnt_list, _ = _ball_query(xyz, new_xyz, radius_list, nsample_list, dilated_group)
     trainable = isinstance(pp, TrainableParams)
     group_concat = tf_ops.group_concat_train if trainable else tf_ops.group_concat
     group_max = tf_ops.group_max_train if trainable else tf_ops.rowgroup_max
-    convs = debug.setdefault("convs", []) if trainable else None
+    convs = [] if trainable else None
     outs = []
-    for i in range(nscale):
+    for i in range(len(radius_list)):
         g = group_concat(xyz, points, new_xyz, idx_list[i])                                         # :160-165
         for j in range(len(mlp_list[i])):
             g = _conv_train(pp, "%s/conv%d_%d" % (scope, i, j), g, bn, bn_decay, debug=convs)       # :167-176
@@ -69,18 +77,7 @@ def _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_l
     new_points = outs[0] if len(outs) == 1 else torch.cat(outs, dim=-1)
     if use_agg:
         new_points = _conv_train(pp, scope + "/ensemble", new_points, bn, bn_decay, debug=convs)    # :183-185
-    return new_points
-
-
-_CONSTS = {}
-
-
-def _const(values, device):
-    """Small device constants, created once (so that layer calls stay CUDA-graph capturable)."""
-    key = (values, str(device))
-    if key not in _CONSTS:
-        _CONSTS[key] = torch.tensor(values, dtype=torch.float32, device=device)
-    return _CONSTS[key]
+    return new_points, idx_list, cnt_list, convs
 
 
 _SIDE_STREAMS = {}
@@ -137,159 +134,135 @@ COMPACT_GROUPS = True      # fused SA scales convolve only the 8-row units that 
 HOIST_EXPAND_MIN_K = 256   # hoisted second convs at least this wide materialise their operand (tf_ops.hoist_expand_split)
 
 
-class _Hoisted:
-    """The per-point table of the hoisted first convs of a layer (see pointnet_sa_module_msg)."""
-    __slots__ = ("scales", "z", "zoffs", "wxs", "stacks")
+def _route_plan(pp, scope, nsample_list, mlp_list, bn, c_feat, use_agg, mlp_mode, fuse_scale, gather_in_kernel, hoist_first):
+    """Which kernels serve each scale of one SA layer at inference, decided from parameter shapes and options alone:
+      tc         the tensor-core route (nsample among the pooling widths of its epilogue, scale widths multiples of 8
+                 for 16-byte aligned column slices of the concat buffers), else the fp32 route;
+      hoisted    the scales whose first conv is hoisted (hoist_first: 0 off, 1 layer-by-layer scales only, 2 all): the
+                 feature part of those convs runs once per POINT into one table z (_hoist_table);
+      scales[i]  route: 'fused' (tf_ops.sa_mlp_fused) or 'fused_hoisted' (sa_mlp_fused_hoisted, the remaining convs in
+                 `stack`) run the whole scale in one kernel; layer by layer, the first operand is 'gather'ed in the
+                 kernel (linear_tc_gather), materialised by group_concat_split ('split'), built from z by the producer
+                 warps of linear_tc_hoisted ('hoisted') or materialised from z by hoist_expand_split ('expand', wide
+                 second convs).  zoff: its columns in z.  units: only the 8-row units of its unit list are convolved,
+                 and pooled into the zero-filled concat buffer;
+      compact    some scale uses its unit list;
+      split_out  the aggregation conv's split operand is written by the scales' epilogues (else split once afterwards)."""
+    tc = mlp_mode == "tc" and all(k in tf_ops.TC_POOL_WIDTHS for k in nsample_list) and all(m[-1] % 8 == 0 for m in mlp_list)
+    scopes = [["%s/conv%d_%d" % (scope, i, j) for j in range(len(m))] for i, m in enumerate(mlp_list)]
+    plan = SimpleNamespace(tc=tc, bn=bn, scopes=scopes, agg=scope + "/ensemble" if use_agg else None, hoisted=[], scales=[],
+                           compact=False, split_out=False)
+    if not tc:
+        return plan
+    stacks = [pp.fused_stack(names, bn, c_feat + 3) if fuse_scale else None for names in scopes]
+    # an xyz-only cloud (c_feat == 0) has no feature part to hoist: its first conv runs in the grouped domain
+    if gather_in_kernel and hoist_first and c_feat > 0:
+        plan.hoisted = [i for i, m in enumerate(mlp_list) if len(m) >= 2 and (int(hoist_first) >= 2 or stacks[i] is None)]
+    n1 = {i: pp.conv(scopes[i][0], bn).cout for i in plan.hoisted}
+    ldz = sum(n1.values())
+    for i, names in enumerate(scopes):
+        sc = SimpleNamespace(stack=stacks[i], zoff=None, units=COMPACT_GROUPS and len(mlp_list) <= 4)
+        if i in plan.hoisted:
+            sc.zoff = sum(n1[h] for h in plan.hoisted[:plan.hoisted.index(i)])
+        if sc.stack is not None:
+            hstack = pp.fused_stack(names[1:], bn, n1[i]) if i in n1 else None
+            sc.route, sc.stack = ("fused_hoisted", hstack) if hstack is not None else ("fused", sc.stack)
+        elif i in n1:
+            wide = pp.conv(names[1], bn).kp >= HOIST_EXPAND_MIN_K and sc.zoff % 4 == 0 and ldz % 4 == 0
+            sc.route = "expand" if wide else "hoisted"
+        else:
+            sc.route, sc.units = "gather" if gather_in_kernel else "split", False
+        plan.scales.append(sc)
+    plan.compact = any(sc.units for sc in plan.scales)
+    plan.split_out = use_agg and not plan.compact
+    return plan
 
 
-def _prepare_hoist(pp, scope, mlp_list, bn, c_feat, stacks, gather_in_kernel, hoist_first):
-    nscale = len(mlp_list)
-    h = _Hoisted()
-    # hoist_first: 0 off, 1 layer-by-layer scales only, 2 all.  An xyz-only cloud (c_feat == 0) has no feature part to
-    # hoist: the first conv then runs in the grouped domain (linear_tc_gather / sa_mlp_fused accept c = 0).
-    h.scales = [i for i in range(nscale) if len(mlp_list[i]) >= 2 and (int(hoist_first) >= 2 or stacks[i] is None)] \
-        if (gather_in_kernel and hoist_first and c_feat > 0) else []
-    h.z = h.zoffs = h.wxs = None
-    h.stacks = {}
-    return h
-
-
-def _compute_hoist(h, pp, scope, mlp_list, bn, points, stacks):
-    if not h.scales:
-        return
-    c_feat = points.shape[-1]
-    zconv, h.wxs, n1s = pp.hoisted(["%s/conv%d_0" % (scope, i) for i in h.scales], bn, c_feat)
+def _hoist_table(pp, plan, points):
+    """The table of the hoisted first convs (plan.hoisted): z = (features . [Wf_1 | Wf_2 | ...]) * s + t once per point,
+    and the xyz part wx of each of those convs.  None when nothing is hoisted."""
+    if not plan.hoisted:
+        return None
+    zconv, wxs, _ = pp.hoisted([plan.scopes[i][0] for i in plan.hoisted], plan.bn, points.shape[-1])
     p_hi, p_lo = tf_ops.split_rows(points)
-    h.z, _ = tf_ops.linear_tc(p_hi, p_lo, zconv, relu=False, want_f32=True, want_split=False)
-    h.zoffs = [sum(n1s[:t]) for t in range(len(h.scales))]
-    for t, i in enumerate(h.scales):
-        if stacks[i] is not None:    # remaining convs of a fused scale
-            h.stacks[i] = pp.fused_stack(["%s/conv%d_%d" % (scope, i, j) for j in range(1, len(mlp_list[i]))], bn, n1s[t])
+    z, _ = tf_ops.linear_tc(p_hi, p_lo, zconv, relu=False, want_f32=True, want_split=False)
+    return z, dict(zip(plan.hoisted, wxs))
 
 
-def _group_and_mlp(pp, scope, xyz, points, new_xyz, radius_list, nsample_list, mlp_list, bn, dilated_group, use_agg,
-                   mlp_mode, stacks, hoist, gather_in_kernel, debug):
-    """Everything of pointnet_sa_module_msg after the sampling, for one block of query points new_xyz (b, m_q, 3):
-    ball queries (:137-145), grouping + MLP + max-pool + mask per scale (:157-180), concat + aggregation (:182-185)."""
-    bs = xyz.shape[0]
-    nscale = len(radius_list)
-    min_r = [0.0 if (i == 0 or not dilated_group) else radius_list[i - 1] for i in range(nscale)]   # :137-141
-    units_list = [None] * nscale
-    tc_path = (mlp_mode == "tc" and all(k in (8, 16, 32, 64, 128) for k in nsample_list) and all(m[-1] % 8 == 0 for m in mlp_list))
-    if nscale <= 4:   # one pass over the candidates for all shells
-        want_units = COMPACT_GROUPS and tc_path and (any(st is not None for st in stacks) or bool(hoist.scales))
-        res = tf_ops.query_ball_point_multi(min_r, radius_list, nsample_list, xyz, new_xyz, dilated_group, return_units=want_units)
-        idx_list, cnt_list = res[0], res[1]
-        if want_units:
-            units_list = res[2]
-    else:
-        idx_list, cnt_list = [], []
-        for i in range(nscale):
-            if dilated_group:
-                a, c = tf_ops.query_ball_point_dilated(min_r[i], radius_list[i], nsample_list[i], xyz, new_xyz)
-            else:
-                a, c = tf_ops.query_ball_point(radius_list[i], nsample_list[i], xyz, new_xyz)
-            idx_list.append(a); cnt_list.append(c)
-    debug["idx"].append(idx_list); debug["cnt"].append(cnt_list)
-    # tensor-core path needs pooling widths the epilogue covers and 16-byte aligned column slices of the concat buffers
-    tc = tc_path
-    if tc:
-        # tensor-core path: every scale pools straight into its slice of the concat buffer (fp32 for the
-        # caller, split bf16 for the aggregation conv), activations stay split between layers
-        m_q = new_xyz.shape[1]
-        ctot = sum(m[-1] for m in mlp_list)
-        concat = torch.empty((bs, m_q, ctot), dtype=torch.float32, device=xyz.device)
-        # unit-list mode: the fused scales combine their 8-row units with atomicMax on the ZERO-FILLED fp32 concat buffer; the
-        # split copy the aggregation conv reads is then made once, from the finished buffer
-        # (layer-by-layer scales with a hoisted first conv take the same route through the *_units forms of their kernels)
-        use_units = [units_list[i] is not None and (stacks[i] is not None or i in hoist.scales) for i in range(nscale)]
-        compact = any(use_units)
-        if compact:
-            tf_ops.fill_zero(concat)
-        cat_hi = cat_lo = None
-        split_in_epilogue = use_agg and not compact
-        if split_in_epilogue:
-            ldc = tf_ops.round16(ctot)
-            mk = torch.zeros if ldc != ctot else torch.empty
-            cat_hi = mk((bs, m_q, ldc), dtype=torch.bfloat16, device=xyz.device)
-            cat_lo = mk((bs, m_q, ldc), dtype=torch.bfloat16, device=xyz.device)
-        off = 0
-        z, zoffs, wxs, hstacks, hscales = hoist.z, hoist.zoffs, hoist.wxs, hoist.stacks, hoist.scales
-        for i in range(nscale):
-            idx, cnt = idx_list[i], cnt_list[i]
-            nl = len(mlp_list[i])
-            stack = stacks[i]
-            if stack is not None:                                              # whole scale in one kernel
-                fkw = dict(out_f32=(concat, off), out_split=(cat_hi, cat_lo, off) if split_in_epilogue else None,
-                           units=units_list[i] if use_units[i] else None)
-                if hstacks.get(i) is not None:
-                    t = hscales.index(i)
-                    tf_ops.sa_mlp_fused_hoisted(xyz, z, zoffs[t], wxs[t], new_xyz, idx, cnt, hstacks[i], **fkw)
-                else:
-                    tf_ops.sa_mlp_fused(xyz, points, new_xyz, idx, cnt, stack, **fkw)
-                off += mlp_list[i][-1]
-                continue
-            hi = lo = None
-            for j in range(nl):
-                f = pp.conv("%s/conv%d_%d" % (scope, i, j), bn)
-                last_kw = dict(pool=nsample_list[i], rowmask=cnt, out_f32=(concat, off),
-                               out_split=(cat_hi, cat_lo, off) if split_in_epilogue else None)   # :167-180 conv+BN+ReLU+max+mask
-                ukw = {}
-                if use_units[i]:                  # compact rows; the last conv pools 8-row units into the zero-filled concat
-                    ukw = dict(units=units_list[i])
-                    last_kw = dict(out_f32=(concat, off), units=units_list[i], unit_pool=True)
-                if i in hscales:
-                    if j == 0:
-                        continue                  # folded into z and into the next conv's operand producer
-                    if j == 1:
-                        t = hscales.index(i)
-                        if f.kp >= HOIST_EXPAND_MIN_K and zoffs[t] % 4 == 0 and z.shape[2] % 4 == 0:
-                            # wide layer: materialise the operand once (elementwise, memory speed), plain TMA-fed GEMM
-                            hi, lo = tf_ops.hoist_expand_split(xyz, z, zoffs[t], wxs[t], new_xyz, idx, **ukw)
-                            if nl == 2:
-                                tf_ops.linear_tc(hi, lo, f, **last_kw)
-                            else:
-                                _, (hi, lo) = tf_ops.linear_tc(hi, lo, f, want_f32=False, want_split=True, **ukw)
-                            continue
-                        if nl == 2:
-                            tf_ops.linear_tc_hoisted(xyz, z, zoffs[t], wxs[t], new_xyz, idx, f, want_split=False, **last_kw)
-                        else:
-                            _, (hi, lo) = tf_ops.linear_tc_hoisted(xyz, z, zoffs[t], wxs[t], new_xyz, idx, f, **ukw)
-                        continue
-                if j == 0 and gather_in_kernel:   # :160-165 inside the kernel's operand load (no [B,M,K,C] tensor)
-                    if nl == 1:
-                        tf_ops.linear_tc_gather(xyz, points, new_xyz, idx, f, want_split=False, **last_kw)
-                    else:
-                        _, (hi, lo) = tf_ops.linear_tc_gather(xyz, points, new_xyz, idx, f)
-                    continue
-                if j == 0:                        # :160-165 fused with the split, materialised once in bf16 hi/lo
-                    hi, lo = tf_ops.group_concat_split(xyz, points, new_xyz, idx)
-                if j < nl - 1:
-                    _, (hi, lo) = tf_ops.linear_tc(hi, lo, f, want_f32=False, want_split=True, **ukw)
-                else:
-                    tf_ops.linear_tc(hi, lo, f, **last_kw)
-            off += mlp_list[i][-1]
-        new_points = concat
-        if use_agg:                                                            # :183-185
-            if not split_in_epilogue:
-                cat_hi, cat_lo = tf_ops.split_rows(concat)
-            new_points, _ = tf_ops.linear_tc(cat_hi, cat_lo, pp.conv(scope + "/ensemble", bn))
-        return new_points
-    outs = []
-    for i in range(nscale):
+def _fused_scale(sc, xyz, points, new_xyz, idx, cnt, hz, out):
+    """A whole scale in one kernel (:157-180); hz = (z, zoff, wx) of a hoisted first conv."""
+    kw = dict(out_f32=out["out_f32"], out_split=out.get("out_split"), units=out.get("units"))
+    if sc.route == "fused_hoisted":
+        return tf_ops.sa_mlp_fused_hoisted(xyz, *hz, new_xyz, idx, cnt, sc.stack, **kw)
+    return tf_ops.sa_mlp_fused(xyz, points, new_xyz, idx, cnt, sc.stack, **kw)
+
+
+def _layer_scale(sc, convs, xyz, points, new_xyz, idx, hz, units, out):
+    """A scale conv by conv (:160-180): the first kernel builds its operand from the neighbour lists as sc.route says,
+    each later conv is a linear_tc on the split activations of the one before, and the last writes as `out` says."""
+    mid = {} if units is None else dict(units=units)
+    if sc.route == "gather":         # :160-165 inside the kernel's operand load (no [B,M,K,C] tensor)
+        op = partial(tf_ops.linear_tc_gather, xyz, points, new_xyz, idx)
+    elif sc.route == "split":        # :160-165 fused with the split, materialised once in bf16 hi/lo
+        op = partial(tf_ops.linear_tc, *tf_ops.group_concat_split(xyz, points, new_xyz, idx))
+    elif sc.route == "hoisted":      # the first conv is in z; the second builds relu(z[idx] + rel-xyz . wx) in its loads
+        convs = convs[1:]
+        op = partial(tf_ops.linear_tc_hoisted, xyz, *hz, new_xyz, idx)
+    else:                            # 'expand', wide layer: materialise that operand once (elementwise, memory speed)
+        convs = convs[1:]
+        op = partial(tf_ops.linear_tc, *tf_ops.hoist_expand_split(xyz, *hz, new_xyz, idx, **mid))
+    for f in convs[:-1]:
+        _, (hi, lo) = op(f, want_f32=False, want_split=True, **mid)
+        op = partial(tf_ops.linear_tc, hi, lo)
+    op(convs[-1], want_split=False, **out)
+
+
+def _group_and_mlp(pp, plan, table, xyz, points, new_xyz, radius_list, nsample_list, mlp_list, dilated_group):
+    """Everything of pointnet_sa_module_msg after the sampling, for one block of query points new_xyz (b, m_q, 3), on
+    the routes of `plan`: ball queries (:137-145), grouping + MLP + max-pool + mask per scale (:157-180), concat +
+    aggregation (:182-185).  table: _hoist_table's.  Returns (new_points, idx_list, cnt_list)."""
+    idx_list, cnt_list, units_list = _ball_query(xyz, new_xyz, radius_list, nsample_list, dilated_group, plan.compact)
+    if not plan.tc:
+        outs = []
+        for i, scopes in enumerate(plan.scopes):
+            # rows with cnt == 0 come back zero-filled, which is what idx * (cnt > 0) produces (:157-159)
+            g = tf_ops.group_concat(xyz, points, new_xyz, idx_list[i])                # :160-165 fused
+            for j, s in enumerate(scopes):
+                last = j == len(scopes) - 1
+                g = _conv(pp, s, g, bn=plan.bn, pool=nsample_list[i] if last else 1, rowmask=cnt_list[i] if last else None)
+            outs.append(g)                                                             # :167-180
+        new_points = outs[0] if len(outs) == 1 else torch.cat(outs, dim=-1)
+        return (_conv(pp, plan.agg, new_points, bn=plan.bn) if plan.agg else new_points), idx_list, cnt_list   # :183-185
+    # every scale pools straight into its columns of the fp32 concat buffer (and, split_out, of the split bf16 copy the
+    # aggregation conv reads); activations stay split between layers
+    bs, m_q = new_xyz.shape[:2]
+    ctot = sum(m[-1] for m in mlp_list)
+    concat = torch.empty((bs, m_q, ctot), dtype=torch.float32, device=xyz.device)
+    if plan.compact:                 # unit lists combine their 8-row units with atomicMax on the ZERO-FILLED buffer
+        tf_ops.fill_zero(concat)
+    split = None
+    if plan.split_out:
+        ldc = tf_ops.round16(ctot)
+        mk = torch.zeros if ldc != ctot else torch.empty
+        split = tuple(mk((bs, m_q, ldc), dtype=torch.bfloat16, device=xyz.device) for _ in range(2))
+    off = 0
+    for i, sc in enumerate(plan.scales):
         idx, cnt = idx_list[i], cnt_list[i]
-        # rows with cnt == 0 come back zero-filled, which is what idx * (cnt > 0) produces (:157-159)
-        g = tf_ops.group_concat(xyz, points, new_xyz, idx)                    # :160-165 fused
-        nl = len(mlp_list[i])
-        for j in range(nl):
-            lastl = j == nl - 1
-            g = _conv(pp, "%s/conv%d_%d" % (scope, i, j), g, bn=bn,
-                      pool=nsample_list[i] if lastl else 1, rowmask=cnt if lastl else None)   # :167-180
-        outs.append(g)
-    new_points = outs[0] if len(outs) == 1 else torch.cat(outs, dim=-1)
-    if use_agg:
-        new_points = _conv(pp, scope + "/ensemble", new_points, bn=bn)        # :183-185
-    return new_points
+        units = units_list[i] if sc.units else None
+        if units is not None:        # the last conv pools every 8-row unit into its group's row
+            out = dict(out_f32=(concat, off), units=units, unit_pool=True)
+        else:                        # :167-180 conv + BN + ReLU + max + mask
+            out = dict(out_f32=(concat, off), out_split=None if split is None else split + (off,), pool=nsample_list[i], rowmask=cnt)
+        hz = None if sc.zoff is None else (table[0], sc.zoff, table[1][i])
+        if sc.route.startswith("fused"):
+            _fused_scale(sc, xyz, points, new_xyz, idx, cnt, hz, out)
+        else:
+            _layer_scale(sc, [pp.conv(s, plan.bn) for s in plan.scopes[i]], xyz, points, new_xyz, idx, hz, units, out)
+        off += mlp_list[i][-1]
+    if not plan.agg:
+        return concat, idx_list, cnt_list
+    cat_hi, cat_lo = split if split is not None else tf_ops.split_rows(concat)                 # :183-185
+    return tf_ops.linear_tc(cat_hi, cat_lo, pp.conv(plan.agg, plan.bn))[0], idx_list, cnt_list
 
 
 def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_training, bn_decay, bn,
@@ -326,20 +299,19 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
     main = torch.cuda.current_stream()
     in_parts = bool(fps_parts) and nscale > 0 and former_fps_idx is None
     keep = []                                  # temporaries shared between streams stay alive until the final join
+    use_agg = bool(aggregation and aggregation_channel is not None and aggregation_channel != -1)
 
-    # ---- hoisted first convs: the feature part of conv0 of every scale, once per POINT (independent of the sampling)
-    c_feat = points.shape[-1]
-    stacks = hoist = None
-    if nscale and not trainable:              # folded inference forms: not used by the differentiable path
-        tc_ok = mlp_mode == "tc" and all(k in (8, 16, 32, 64, 128) for k in nsample_list) and all(m[-1] % 8 == 0 for m in mlp_list)
-        stacks = [pp.fused_stack(["%s/conv%d_%d" % (scope, i, j) for j in range(len(mlp_list[i]))], bn, c_feat + 3)
-                  if (fuse_scale and tc_ok) else None for i in range(nscale)]
-        hoist = _prepare_hoist(pp, scope, mlp_list, bn, c_feat, stacks, gather_in_kernel and tc_ok, hoist_first)
-        if in_parts and hoist.scales:          # overlaps the first rounds of the sampling
+    # ---- inference: the kernels of every scale, and the hoisted first convs (the feature part of conv0 of every
+    # scale, once per POINT, independent of the sampling)
+    plan = table = None
+    if nscale and not is_training:
+        plan = _route_plan(pp, scope, nsample_list, mlp_list, bn, points.shape[-1], use_agg, mlp_mode, fuse_scale,
+                           gather_in_kernel, hoist_first)
+        if in_parts and plan.hoisted:          # overlaps the first rounds of the sampling
             zs = _side_stream(dev, 7)
             zs.wait_stream(main)
             with torch.cuda.stream(zs):
-                _compute_hoist(hoist, pp, scope, mlp_list, bn, points, stacks)
+                table = _hoist_table(pp, plan, points)
             z_ready = torch.cuda.Event()
             z_ready.record(zs)
 
@@ -432,7 +404,6 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
         col += width
 
     src_xyz = vote_ctr if vote_ctr is not None else xyz
-    use_agg = bool(aggregation and aggregation_channel is not None and aggregation_channel != -1)
     debug = {"idx": [], "cnt": []}
 
     if not in_parts:
@@ -443,31 +414,31 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
             fps_idx = torch.cat([fps_idx, former_fps_idx], dim=-1).contiguous()    # :113-114
         new_xyz = tf_ops.gather_point(src_xyz, fps_idx)                            # :116-119
         if nscale and is_training:
-            new_points = _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_list, mlp_list, bn,
-                                              bn_decay, dilated_group, use_agg, debug)
-            debug = dict(debug, idx=debug["idx"][0], cnt=debug["cnt"][0])
+            new_points, idx, cnt, convs = _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_list,
+                                                               mlp_list, bn, bn_decay, dilated_group, use_agg)
+            debug = {"idx": idx, "cnt": cnt} if convs is None else {"idx": idx, "cnt": cnt, "convs": convs}
         elif nscale:
-            _compute_hoist(hoist, pp, scope, mlp_list, bn, points, stacks)
-            new_points = _group_and_mlp(pp, scope, xyz, points, new_xyz, radius_list, nsample_list, mlp_list, bn,
-                                        dilated_group, use_agg, mlp_mode, stacks, hoist, gather_in_kernel, debug)
-            debug = {"idx": debug["idx"][0], "cnt": debug["cnt"][0]}
+            table = _hoist_table(pp, plan, points)
+            new_points, idx, cnt = _group_and_mlp(pp, plan, table, xyz, points, new_xyz, radius_list, nsample_list,
+                                                  mlp_list, dilated_group)
+            debug = {"idx": idx, "cnt": cnt}
         else:
             new_points = tf_ops.gather_point(points.contiguous(), fps_idx)         # :186-187
     else:
         # ---- one consumer chain per part, each on its own stream, joined at the end
-        xyz_parts, pts_parts, done = [], [], []
+        xyz_parts, pts_parts, found, done = [], [], [], []
         for pi, (c0, c1, ev) in enumerate(parts):
             st = _side_stream(dev, 8 + pi)
             st.wait_event(ev)
-            if hoist.scales:
+            if plan.hoisted:
                 st.wait_event(z_ready)
             with torch.cuda.stream(st):
                 nx = tf_ops.gather_point(src_xyz, fps_idx[:, c0:c1])
-                npnts = _group_and_mlp(pp, scope, xyz, points, nx, radius_list, nsample_list, mlp_list, bn, dilated_group,
-                                       use_agg, mlp_mode, stacks, hoist, gather_in_kernel, debug)
+                npnts, idx, cnt = _group_and_mlp(pp, plan, table, xyz, points, nx, radius_list, nsample_list, mlp_list,
+                                                 dilated_group)
                 e2 = torch.cuda.Event()
                 e2.record(st)
-            xyz_parts.append(nx); pts_parts.append(npnts); done.append(e2)
+            xyz_parts.append(nx); pts_parts.append(npnts); found.append((idx, cnt)); done.append(e2)
         for e2 in done:
             main.wait_event(e2)
         for i in range(nside):
@@ -476,9 +447,9 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
         new_points = tf_ops.concat_rows(pts_parts)
         keep.extend(xyz_parts + pts_parts)
         if return_debug:
-            debug = {"idx": [torch.cat([d[i] for d in debug["idx"]], dim=1) for i in range(nscale)],
-                     "cnt": [torch.cat([d[i] for d in debug["cnt"]], dim=1) for i in range(nscale)]}
-        _KEEPALIVE.append((keep, debug if not return_debug else None, hoist))
+            debug = {"idx": [torch.cat([f[0][i] for f in found], dim=1) for i in range(nscale)],
+                     "cnt": [torch.cat([f[1][i] for f in found], dim=1) for i in range(nscale)]}
+        _KEEPALIVE.append((keep, found if not return_debug else None, table))
         del _KEEPALIVE[:-8]
     if return_debug:
         return new_xyz, new_points, fps_idx, debug
@@ -519,12 +490,8 @@ def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay,
 def vote_layer(xyz, points, mlp_list, is_training, bn_decay, bn, scope, *, params,
                max_translate_range=_cfg.MAX_TRANSLATE_RANGE, mlp_mode="tc"):
     """Vote layer: per-point MLP -> 3 offsets, clamped to +-max_translate_range (layers_util.py:12-24)."""
-    if _trainable(params, is_training):
-        for i in range(len(mlp_list)):
-            points = params.conv_train("%s/vote_layer_%d" % (scope, i), points, bn, bn_decay)
-        off = params.conv_train(scope + "/vote_offsets", points, False, bn_decay, relu=False)
-        return tf_ops.vote_translate_train(xyz, off, max_translate_range), points, off
-    pp = prepare(params, xyz.device)
+    trainable = _trainable(params, is_training)
+    pp = params if trainable else prepare(params, xyz.device)
     if is_training:
         for i in range(len(mlp_list)):
             points = _conv_train(pp, "%s/vote_layer_%d" % (scope, i), points, bn, bn_decay)
@@ -538,4 +505,5 @@ def vote_layer(xyz, points, mlp_list, is_training, bn_decay, bn, scope, *, param
         for i in range(len(mlp_list)):
             points = _conv(pp, "%s/vote_layer_%d" % (scope, i), points, bn=bn)
         off = _conv(pp, scope + "/vote_offsets", points, bn=False, relu=False)
-    return tf_ops.vote_translate(xyz, off, max_translate_range), points, off                       # :20-23
+    translate = tf_ops.vote_translate_train if trainable else tf_ops.vote_translate
+    return translate(xyz, off, max_translate_range), points, off                                    # :20-23

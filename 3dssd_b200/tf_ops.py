@@ -482,6 +482,9 @@ def linear_bn_relu(x, w, scale, shift, relu=True, pool=1, rowmask=None, cin=None
 
 # ---- tensor-core (wgmma) path of the MLP: operands split in two bf16 terms ---------------------------------
 
+TC_POOL_WIDTHS = (8, 16, 32, 64, 128)   # group sizes the max-pool epilogue of the tensor-core kernels covers
+
+
 def round16(x):
     return (int(x) + 15) // 16 * 16
 
@@ -580,8 +583,8 @@ def linear_tc(a_hi, a_lo, f, relu=True, pool=1, rowmask=None, want_f32=True, wan
     pool = int(pool)
     lead = tuple(a_hi.shape[:-1])
     if pool > 1:
-        if lead[-1] != pool or pool not in (8, 16, 32, 64, 128):
-            raise ValueError("pool must equal the second-to-last dimension and be one of 8, 16, 32, 64, 128")
+        if lead[-1] != pool or pool not in TC_POOL_WIDTHS:
+            raise ValueError("pool must equal the second-to-last dimension and be one of %s" % (TC_POOL_WIDTHS,))
         lead = lead[:-1]
     n = f.cout
     y, pf, ldf, sp, ph, pl, lds = _tc_outputs(lead, n, pool, a_hi.device, want_f32, want_split, out_f32, out_split)
@@ -614,8 +617,8 @@ def linear_tc_gather(xyz, points, new_xyz, idx, f, relu=True, pool=1, rowmask=No
         raise ValueError("layer input width %d does not match c+3 = %d" % (f.cin, c + 3))
     _, m, ns = idx.shape
     pool = int(pool)
-    if pool > 1 and (pool != ns or pool not in (8, 16, 32, 64, 128)):
-        raise ValueError("pool must equal nsample and be one of 8, 16, 32, 64, 128")
+    if pool > 1 and (pool != ns or pool not in TC_POOL_WIDTHS):
+        raise ValueError("pool must equal nsample and be one of %s" % (TC_POOL_WIDTHS,))
     lead = (b, m) if pool > 1 else (b, m, ns)
     y, pf, ldf, sp, ph, pl, lds = _tc_outputs(lead, f.cout, pool, xyz.device, want_f32, want_split, out_f32, out_split)
     vp = ctypes.c_void_p
@@ -645,8 +648,8 @@ def linear_tc_hoisted(xyz, z, zoff, wx, new_xyz, idx, f, relu=True, pool=1, rowm
         raise ValueError("second conv expects %d inputs, the hoisted first conv has %d outputs" % (f.cin, n1))
     _, m, ns = idx.shape
     pool = int(pool)
-    if pool > 1 and (pool != ns or pool not in (8, 16, 32, 64, 128)):
-        raise ValueError("pool must equal nsample and be one of 8, 16, 32, 64, 128")
+    if pool > 1 and (pool != ns or pool not in TC_POOL_WIDTHS):
+        raise ValueError("pool must equal nsample and be one of %s" % (TC_POOL_WIDTHS,))
     lead = (b, m) if pool > 1 else (b, m, ns)
     y, pf, ldf, sp, ph, pl, lds = _tc_outputs(lead, f.cout, pool, xyz.device, want_f32, want_split, out_f32, out_split)
     vp = ctypes.c_void_p
@@ -1047,25 +1050,35 @@ def _folded(w, scale, shift):
     return FoldedConv(w, scale, shift)
 
 
+def linear_bn_train(x, f, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9):
+    """Forward of one training-mode layer: split_rows -> linear_tc with the BN-less fold f (params.FoldedConv with
+    scale = 1, shift = bias) -> bn_train (bn=True: batch statistics, moving statistics updated in place) -> ReLU.
+    Returns (y, r): y the conv output before BatchNorm, r bn_train's (out, scale, shift, batch_mean, batch_var), or (y,)
+    when bn=False."""
+    hi, lo = split_rows(x)
+    y, _ = linear_tc(hi, lo, f, relu=bool(relu and not bn), want_f32=True, want_split=False)
+    if not bn:
+        return y, (y,)
+    return y, bn_train(y, gamma, beta, moving_mean, moving_var, decay=decay, relu=relu)
+
+
 class _ConvTrain(torch.autograd.Function):
     """conv (+bias) -> [training BatchNorm] -> [ReLU] of one layer (tf_util.conv2d / conv1d with is_training=True).
-    Forward: split_rows -> linear_tc with the BN-less fold -> bn_train, the sequence of the non-trainable training path.
+    Forward: linear_bn_train with a fold of the live weights, the sequence of the non-trainable training path.
     Backward: bn_train_grad -> split -> linear_tc with W^T (grad_x) and linear_wgrad (grad_w, grad_b)."""
 
     @staticmethod
     def forward(ctx, x, w, b, gamma, beta, opts):
         bn, relu, decay, moving, debug = opts
         x = x if x.is_contiguous() else x.contiguous()
-        hi, lo = split_rows(x)
-        cout = w.shape[1]
-        ones = torch.ones((cout,), dtype=torch.float32, device=x.device)
-        y, _ = linear_tc(hi, lo, _folded(w.detach(), ones, b.detach()), relu=bool(relu and not bn), want_f32=True, want_split=False)
+        ones = torch.ones((w.shape[1],), dtype=torch.float32, device=x.device)
+        y, r = linear_bn_train(x, _folded(w.detach(), ones, b.detach()), gamma.detach(), beta.detach(), moving[0], moving[1],
+                               bn=bn, relu=relu, decay=decay)
+        out = r[0]
         ctx.bn, ctx.relu = bn, relu
         if bn:
-            out, scale, shift, bmean, bvar = bn_train(y, gamma.detach(), beta.detach(), moving[0], moving[1], decay=decay, relu=relu)
-            ctx.save_for_backward(x, w, y, scale, shift, bmean, bvar, gamma)
+            ctx.save_for_backward(x, w, y, *r[1:], gamma)       # scale, shift, batch_mean, batch_var
         else:
-            out = y
             ctx.save_for_backward(x, w, y)
         if debug is not None:
             debug.append((y, out))

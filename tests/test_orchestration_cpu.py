@@ -5,29 +5,53 @@ resumable rounds, the latency-mode part schedule and its joins -- runs here with
 oracle's own layer code.  (The kernels themselves are covered by the -m gpu tests.)"""
 import copy
 import importlib
+import inspect
+import json
+import os
 
 import numpy as np
 import pytest
 import torch
 
+_SYNC = {}   # state of the stream / event stand-ins: creation counters, the torch.cuda.stream stack, the trace (list or None)
+
+
+def _reset_sync(trace=None):
+    _SYNC.clear()
+    _SYNC.update(s=0, e=0, trace=trace)
+    main = _Inert(kind="s")
+    main.name = "main"
+    _SYNC["stack"] = [main]
+
+
+def _log(line):
+    if _SYNC["trace"] is not None:
+        _SYNC["trace"].append(line)
+
 
 class _Inert:
-    def __init__(self, *a, **k):
-        pass
+    """Stream / event stand-in with an identity: streams s1, s2, ... and events e1, e2, ... in creation order; the
+    stream outside every torch.cuda.stream block is 'main'.  What they are asked to do goes to the trace."""
 
-    def wait_stream(self, *a):
-        pass
+    def __init__(self, *a, kind="s", **k):
+        _SYNC[kind] += 1
+        self.name = "%s%d" % (kind, _SYNC[kind])
 
-    def wait_event(self, *a):
-        pass
+    def wait_stream(self, s):
+        _log("%s.wait_stream(%s)" % (self.name, s.name))
 
-    def record(self, *a):
-        pass
+    def wait_event(self, e):
+        _log("%s.wait_event(%s)" % (self.name, e.name))
+
+    def record(self, s=None):
+        _log("%s.record(%s)" % (self.name, (s or _SYNC["stack"][-1]).name))
 
     def __enter__(self):
+        _SYNC["stack"].append(self)
         return self
 
     def __exit__(self, *a):
+        _SYNC["stack"].pop()
         return False
 
 
@@ -204,6 +228,22 @@ def dry(monkeypatch, oracle_ops):
         assert wx.shape[1] == stack.cin
         return fused(hoisted_operand(xyz, z, zoff, wx, new_xyz, idx), cnt, stack, out_f32, out_split, idx.shape[-1], units)
 
+    # ---- training mode: float64 batch-statistics BatchNorm and the masked row-group max
+    def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=True, eps=1e-3):
+        flat = x.reshape(-1, x.shape[-1]).double()
+        mean = flat.mean(0)
+        var = ((flat - mean) ** 2).mean(0)
+        inv = gamma.double() / torch.sqrt(var + eps)
+        y = x.double() * inv + (beta.double() - mean * inv)
+        if moving_mean is not None:                                  # in place, like updates_collections=None
+            moving_mean.sub_(((moving_mean.double() - mean) * (1.0 - decay)).float())
+            moving_var.sub_(((moving_var.double() - var) * (1.0 - decay)).float())
+        return (torch.relu(y) if relu else y).float(), inv.float(), (beta.double() - mean * inv).float(), mean.float(), var.float()
+
+    def rowgroup_max(y, pool, rowmask=None):
+        out = y.max(dim=-2).values
+        return out * (rowmask > 0).unsqueeze(-1).to(out.dtype) if rowmask is not None else out
+
     fakes = dict(
         fill_zero=lambda x: x.zero_(),
         split_rows=split_rows, linear_tc=linear_tc, linear_tc_gather=linear_tc_gather, linear_tc_hoisted=linear_tc_hoisted,
@@ -220,13 +260,15 @@ def dry(monkeypatch, oracle_ops):
         fps_supports_rounds=lambda nn, c=3: True, ffps_supported=lambda nn, c: c <= 68,
         fps_temp_elems=lambda nn, c=3, npoint=0, **kw: 2 * nn,
         vote_translate=lambda xyz, off, rng: xyz + torch.minimum(torch.maximum(off[..., :3], torch.tensor(rng)), -torch.tensor(rng)),
+        bn_train=bn_train, rowgroup_max=rowgroup_max,
     )
     for k, v in fakes.items():
         monkeypatch.setattr(T, k, v)
-    monkeypatch.setattr(torch.cuda, "current_stream", lambda *a, **k: _Inert())
-    monkeypatch.setattr(torch.cuda, "Stream", _Inert)
-    monkeypatch.setattr(torch.cuda, "Event", _Inert)
-    monkeypatch.setattr(torch.cuda, "stream", lambda s: _Inert())
+    _reset_sync()
+    monkeypatch.setattr(torch.cuda, "current_stream", lambda *a, **k: _SYNC["stack"][-1])
+    monkeypatch.setattr(torch.cuda, "Stream", lambda *a, **k: _Inert(kind="s"))
+    monkeypatch.setattr(torch.cuda, "Event", lambda *a, **k: _Inert(kind="e"))
+    monkeypatch.setattr(torch.cuda, "stream", lambda s: s)
     monkeypatch.setattr(L, "_SIDE_STREAMS", {})
     return pkg
 
@@ -239,9 +281,13 @@ def _scaled(pkg, div):
     return arch
 
 
-@pytest.mark.parametrize("mlp_mode,gather,hoist,fuse", [("fp32", True, 2, True), ("tc", True, 2, True), ("tc", True, 1, True),
-                                                        ("tc", True, 0, True), ("tc", False, 0, False), ("tc", True, 2, False)])
-@pytest.mark.parametrize("latency,parts", [(False, None), (True, 2), (True, [0.5, 0.25, 0.25])])
+_ROUTES = [("fp32", True, 2, True), ("tc", True, 2, True), ("tc", True, 1, True), ("tc", True, 0, True), ("tc", False, 0, False),
+           ("tc", True, 2, False)]
+_LATENCY = [(False, None), (True, 2), (True, [0.5, 0.25, 0.25])]
+
+
+@pytest.mark.parametrize("mlp_mode,gather,hoist,fuse", _ROUTES)
+@pytest.mark.parametrize("latency,parts", _LATENCY)
 def test_backbone_orchestration_dry_run_matches_oracle_layers(dry, oracle_ops, latency, parts, mlp_mode, gather, hoist, fuse):
     pkg = dry
     from oracle import layers as olayers
@@ -309,32 +355,13 @@ def test_head_orchestration_dry_run_writes_into_gather_buffers(dry, oracle_ops, 
 
 
 @pytest.mark.parametrize("decay", [None, 0.5])
-def test_training_mode_orchestration_dry_run_matches_oracle(dry, oracle_ops, monkeypatch, decay):
+def test_training_mode_orchestration_dry_run_matches_oracle(dry, oracle_ops, decay):
     """is_training=True through pointnet_sa_module_msg on the CPU (SURVEY 8f row f3): the literal conv -> batch-norm -> relu
-    schedule with ssd3d_bn_train / ssd3d_rowgroup_max replaced by a few float64 lines, against the oracle's restatement of
-    tf_util.py:424-444; the moving statistics are updated in place, commit_bn() writes them back and inference then folds
-    the NEW statistics."""
+    schedule with ssd3d_bn_train / ssd3d_rowgroup_max replaced by a few float64 lines (the dry fixture), against the
+    oracle's restatement of tf_util.py:424-444; the moving statistics are updated in place, commit_bn() writes them back
+    and inference then folds the NEW statistics."""
     pkg = dry
     from oracle import layers as olayers
-    T = pkg.tf_ops
-
-    def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=True, eps=1e-3):
-        flat = x.reshape(-1, x.shape[-1]).double()
-        mean = flat.mean(0)
-        var = ((flat - mean) ** 2).mean(0)
-        inv = gamma.double() / torch.sqrt(var + eps)
-        y = x.double() * inv + (beta.double() - mean * inv)
-        if moving_mean is not None:                                  # in place, like updates_collections=None
-            moving_mean.sub_(((moving_mean.double() - mean) * (1.0 - decay)).float())
-            moving_var.sub_(((moving_var.double() - var) * (1.0 - decay)).float())
-        return (torch.relu(y) if relu else y).float(), inv.float(), (beta.double() - mean * inv).float(), mean.float(), var.float()
-
-    def rowgroup_max(y, pool, rowmask=None):
-        out = y.max(dim=-2).values
-        return out * (rowmask > 0).unsqueeze(-1).to(out.dtype) if rowmask is not None else out
-
-    monkeypatch.setattr(T, "bn_train", bn_train)
-    monkeypatch.setattr(T, "rowgroup_max", rowgroup_max)
     rng = np.random.default_rng(11)
     synth = importlib.import_module("3dssd_b200.synth")
     pts = synth.kitti_like(2, 512, seed=61)
@@ -368,3 +395,74 @@ def test_training_mode_orchestration_dry_run_matches_oracle(dry, oracle_ops, mon
     got_i = pkg.pointnet_sa_module_msg(torch.from_numpy(xyz), torch.from_numpy(feats), *args_inf, aggregation_channel=64, params=pp)
     exp_i = olayers.pointnet_sa_module_msg(xyz, feats, *args_inf, aggregation_channel=64, params=params_ref)
     assert np.abs(got_i[1].numpy() - exp_i[1]).max() <= 1e-4 * np.abs(exp_i[1]).max()
+
+
+TRACE_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "launch_trace.json")
+
+
+def _describe(v):
+    if isinstance(v, torch.Tensor):
+        return "%s%s" % (str(v.dtype).replace("torch.", ""), list(v.shape))
+    if isinstance(v, (list, tuple)):
+        return "(%s)" % ",".join(_describe(x) for x in v)
+    if isinstance(v, dict):
+        return "{%s}" % ",".join("%s:%s" % (k, _describe(x)) for k, x in sorted(v.items()))
+    if hasattr(v, "w_blob"):                                      # params.FusedStack
+        return "stack(%d->%s)" % (v.cin, v.nout)
+    if hasattr(v, "b_hi"):                                        # params.FoldedConv
+        return "conv(%d->%d)" % (v.cin, v.cout)
+    if v is None or isinstance(v, (bool, int, float, str)):
+        return repr(v)
+    return type(v).__name__
+
+
+def _traced(name, fn):
+    sig = inspect.signature(fn)
+
+    def call(*a, **k):
+        b = sig.bind(*a, **k)
+        b.apply_defaults()
+        _log("%s@%s %s" % (name, _SYNC["stack"][-1].name, " ".join("%s=%s" % (p, _describe(v)) for p, v in b.arguments.items())))
+        return fn(*a, **k)
+    return call
+
+
+def test_launch_trace_matches_recording(dry, oracle_ops, monkeypatch):
+    """Which kernel serves each scale, where its output goes and on which stream, pinned call by call.  A route that
+    falls back (a FusedStack that no longer fits, a scale that loses its unit list) gives the same numbers but a
+    different trace.  Every tf_ops stand-in of the dry fixture logs its name, stream, tensor shapes and scalar and
+    keyword arguments; the streams and events log their waits and records.  The dry runs are the 18 route / latency
+    combinations of the backbone test and the training-mode layer.  SSD3D_RECORD_TRACE=<file> writes the traces to
+    <file> instead of comparing them with tests/golden/launch_trace.json."""
+    T = dry.tf_ops
+    for k, v in list(vars(T).items()):
+        if inspect.isfunction(v) and v.__module__ == __name__:
+            monkeypatch.setattr(T, k, _traced(k, v))
+    runs = {}
+    for latency, parts in _LATENCY:
+        for route in _ROUTES:
+            runs["backbone-%s-gather%d-hoist%d-fuse%d-latency%d-parts%s" % (route + (latency, parts))] = \
+                lambda r=route, lt=latency, p=parts: test_backbone_orchestration_dry_run_matches_oracle_layers(dry, oracle_ops, lt, p, *r)
+    for decay in (None, 0.5):
+        runs["training-decay%s" % decay] = lambda d=decay: test_training_mode_orchestration_dry_run_matches_oracle(dry, oracle_ops, d)
+    got = {}
+    for key, run in runs.items():
+        monkeypatch.setattr(dry.layers_util, "_SIDE_STREAMS", {})
+        _reset_sync(trace=[])
+        run()
+        got[key] = _SYNC["trace"]
+        _reset_sync()
+    record = os.environ.get("SSD3D_RECORD_TRACE")
+    if record:
+        with open(record, "w") as fh:
+            json.dump(got, fh, indent=0)
+            fh.write("\n")
+        return
+    with open(TRACE_GOLDEN) as fh:
+        exp = json.load(fh)
+    assert sorted(got) == sorted(exp)
+    for key in exp:
+        g, e = got[key], exp[key]
+        first = next((i for i in range(min(len(g), len(e))) if g[i] != e[i]), min(len(g), len(e)))
+        assert g == e, "%s: call %d differs\n got: %s\n exp: %s" % (key, first, g[first] if first < len(g) else "<end>",
+                                                                   e[first] if first < len(e) else "<end>")
