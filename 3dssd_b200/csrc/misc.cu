@@ -93,7 +93,9 @@ __global__ void decode_kernel(long rows, int nbins, const float *__restrict__ ct
     o[4] = fmaxf(__fmul_rn(hy, 2.0f), 0.1f);
     o[5] = fmaxf(__fmul_rn(hz, 2.0f), 0.1f);
     o[6] = angle;
-    scores[r] = 1.0f / (1.0f + expf(-cls[r * ldcls]));
+    // the sigmoid in double, rounded once: in float, expf's own 2-ulp error plus the rounding of the add and the divide
+    // put some scores more than 2 ulp away from the exact sigmoid
+    scores[r] = (float)(1.0 / (1.0 + exp(-(double)cls[r * ldcls])));
 }
 
 // out[s, off_i + q, :] = src_i[s, q, :] for the (up to 8) row blocks of a scene: tf.concat(axis=1) of per-part results
