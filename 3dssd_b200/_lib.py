@@ -97,6 +97,13 @@ _SIGNATURES = {
     "ssd3d_group_concat_grad": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                 c_void_p],
     "ssd3d_vote_translate_grad": [c_long, c_void_p, c_int, c_void_p, c_float, c_float, c_float, c_void_p, c_void_p],
+    "ssd3d_det_assign": [c_int, c_int, c_int, c_int, c_int] + [c_void_p] * 15,
+    "ssd3d_det_loss_workspace": [c_int],
+    "ssd3d_det_loss": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
+                       c_void_p, c_int] + [c_void_p] * 12,
+    "ssd3d_det_loss_grad": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                            c_int, c_void_p, c_int] + [c_void_p] * 11 + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
+                                                                         c_void_p, c_int, c_void_p, c_void_p],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["ssd3d_last_error"])
@@ -114,7 +121,8 @@ def lib():
             fn = getattr(l, name)
             fn.argtypes = argtypes
             fn.restype = ctypes.c_size_t if name in ("ssd3d_sa_fused_smem", "ssd3d_query_ball_point_workspace", "ssd3d_bn_train_workspace",
-                                                   "ssd3d_linear_wgrad_workspace", "ssd3d_bn_train_grad_workspace") else c_int
+                                                   "ssd3d_linear_wgrad_workspace", "ssd3d_bn_train_grad_workspace",
+                                                   "ssd3d_det_loss_workspace") else c_int
             if name == "ssd3d_fps_temp_elems":
                 fn.restype = c_long
         l.ssd3d_last_error.restype = ctypes.c_char_p

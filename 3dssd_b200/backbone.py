@@ -5,6 +5,8 @@ Follows SingleStageDetector.network_forward's backbone loop
 (/root/reference/lib/builder/layer_builder.py:45-101): xyz_list / feature_list / fps_idx_list grow by one
 entry per layer, layers address their inputs by index.
 """
+from typing import NamedTuple
+
 import torch
 
 from . import config as _cfg
@@ -164,3 +166,36 @@ class SABackbone:
             return out, blk
 
         return replay
+
+
+class TrainOutputs(NamedTuple):
+    """What the loss of a training step needs: head = (pred_cls, pred_offset, pred_angle_cls, pred_angle_res) of
+    head.box_regression_head; vote_offsets = the raw offsets of each vote layer; base_xyz = the centres of the last SA
+    layer (the candidate points of the head); vote_base = the input points of the last vote layer."""
+    head: tuple
+    vote_offsets: list
+    base_xyz: torch.Tensor
+    vote_base: torch.Tensor
+
+
+def train_forward(arch, tp, xyz, feat):
+    """The backbone loop of SABackbone.forward in training mode (SA and vote layers, batch-statistics BatchNorm) with
+    params.TrainableParams, then conv1d_0 and the box-regression head of the 3DSSD head on the last layer's features
+    (single_stage_detector.py:115-125, head_builder.py:81-114).  Everything is differentiable w.r.t. tp's parameters."""
+    from . import head as _head
+    xyz_l, feat_l, fps_l, offs, vote_base = [xyz], [feat], [None], [], None
+    for spec in arch:
+        (xyz_i, feat_i, radius, nsample, mlps, bn, rng, method, npoint, former, attn, ltype, scope, dilated, vote_idx, agg) = spec
+        if ltype == "SA_Layer":
+            r = L.pointnet_sa_module_msg(xyz_l[xyz_i[0]], feat_l[feat_i[0]], radius, nsample, mlps, True, None, bn, rng, method,
+                                         npoint, fps_l[former] if former != -1 else None, attn, scope, dilated,
+                                         xyz_l[vote_idx] if vote_idx != -1 else None, agg, params=tp)
+            xyz_l.append(r[0]); feat_l.append(r[1]); fps_l.append(r[2])
+        elif ltype == "Vote_Layer":
+            vote_base = xyz_l[xyz_i[0]]                                 # PRED_VOTE_BASE (layer_builder.py:96)
+            nx, nf, off = L.vote_layer(vote_base, feat_l[feat_i[0]], mlps, True, None, bn, scope, params=tp)
+            xyz_l.append(nx); feat_l.append(nf); fps_l.append(None); offs.append(off)
+        else:
+            raise ValueError("layer type %r has no training driver here" % (ltype,))
+    f = tp.conv_train("conv1d_0", feat_l[-1], True)
+    return TrainOutputs(_head.box_regression_head(f, 1, 1, 6, True, True, params=tp), offs, xyz_l[-1], vote_base)

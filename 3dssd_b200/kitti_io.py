@@ -180,3 +180,21 @@ def params_from_tf_variables(variables):
                 if v is not None and v.shape != (cout,):
                     raise ValueError("%s/%s: shape %s does not match %d output channels" % (scope, leaf, v.shape, cout))
     return out
+
+
+def make_label_batch(samples):
+    """The labels of a batch of frames padded with zeros to the batch's largest count, as the reference's data provider
+    concatenates them (lib/dataset/data_provider/data_provider.py:610-626): (gt_boxes [B, G, 7] fp32, gt_labels [B, G]
+    int32), G = max over the frames (0 when no frame has a label).  Rows of zeros are the padding the target assigner
+    skips."""
+    boxes = [np.asarray(s[KEY_LABEL_BOXES_3D], np.float32).reshape(-1, 7) for s in samples]
+    classes = [np.asarray(s[KEY_LABEL_CLASSES]).reshape(-1).astype(np.int32) for s in samples]
+    g = max((len(b) for b in boxes), default=0)
+    out_b = np.zeros((len(samples), g, 7), np.float32)
+    out_c = np.zeros((len(samples), g), np.int32)
+    for i, (b, c) in enumerate(zip(boxes, classes)):
+        if len(b) != len(c):
+            raise ValueError("frame %d has %d boxes but %d classes" % (i, len(b), len(c)))
+        out_b[i, :len(b)] = b
+        out_c[i, :len(c)] = c
+    return out_b, out_c

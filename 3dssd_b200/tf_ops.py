@@ -1177,3 +1177,122 @@ class _VoteTranslate(torch.autograd.Function):
 def vote_translate_train(xyz, offsets, min_range):
     """Differentiable vote_translate: identity for xyz, the clamp's gradient (inclusive bounds) for the offsets."""
     return _VoteTranslate.apply(xyz, offsets, tuple(float(v) for v in min_range))
+
+
+# ---- training targets and detection losses (DESIGN.md section 3.8) --------------------------------------------------
+
+DET_TARGETS = ("assigned_idx", "assigned_box", "pmask", "nmask", "cls_label", "angle_bin", "angle_res", "offset_target",
+               "vote_mask", "vote_target")
+_LOSS_TARGETS = ("assigned_box", "pmask", "nmask", "cls_label", "angle_bin", "angle_res", "vote_mask", "vote_target")
+
+
+def det_assign(base_xyz, vote_base, gt_boxes, gt_labels, angle_bins=12):
+    """'Mask' assignment + vote targets (ssd3d_det_assign): base_xyz (b, n, 3), vote_base (b, nv, 3), gt_boxes (b, g, 7)
+    zero-padded, gt_labels (b, g) int32 -> dict of the DET_TARGETS tensors."""
+    base_xyz = _req(base_xyz, "base_xyz", torch.float32, 3, 3)
+    vote_base = _req(vote_base, "vote_base", torch.float32, 3, 3)
+    gt_boxes = _req(gt_boxes, "gt_boxes", torch.float32, 3, 7)
+    gt_labels = _req(gt_labels, "gt_labels", torch.int32, 2)
+    b, n, _ = base_xyz.shape
+    nv, g = vote_base.shape[1], gt_boxes.shape[1]
+    if vote_base.shape[0] != b or gt_boxes.shape[0] != b or tuple(gt_labels.shape) != (b, g):
+        raise ValueError("det_assign: base_xyz %s, vote_base %s, gt_boxes %s, gt_labels %s do not share the batch"
+                         % (tuple(base_xyz.shape), tuple(vote_base.shape), tuple(gt_boxes.shape), tuple(gt_labels.shape)))
+    dev = base_xyz.device
+    f = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
+    i = lambda *s: torch.empty(s, dtype=torch.int32, device=dev)
+    t = dict(assigned_idx=i(b, n), assigned_box=f(b, n, 7), pmask=f(b, n), nmask=f(b, n), cls_label=f(b, n),
+             angle_bin=i(b, n), angle_res=f(b, n), offset_target=f(b, n, 6), vote_mask=f(b, nv), vote_target=f(b, nv, 3))
+    check(lib().ssd3d_det_assign(b, n, nv, g, int(angle_bins), _p(base_xyz), _p(vote_base), _p(gt_boxes), _p(gt_labels),
+                                 *[_p(t[k]) for k in DET_TARGETS], _stream()), "det_assign")
+    return t
+
+
+def _rows(t, name, b, n, width):
+    """(b, n, [1,] width) float32 CUDA tensor, read in place when its last axis is dense and its rows evenly strided (a
+    column block of a wider tensor, e.g. the head's [b, n, 1, 30] regression output) -> (tensor, row stride in floats)."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
+        raise ValueError("%s must be a float32 CUDA tensor" % name)
+    if t.dim() < 3 or tuple(t.shape[:2]) != (b, n) or t.shape[-1] != width or any(s != 1 for s in t.shape[2:-1]):
+        raise ValueError("%s must be (%d, %d, [1,] %d), got %s" % (name, b, n, width, tuple(t.shape)))
+    ld = t.stride(1)
+    if t.stride(-1) != 1 or ld < width or (b > 1 and t.stride(0) != n * ld):
+        t, ld = t.contiguous(), width
+    return t, ld
+
+
+def _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins):
+    base_xyz = _req(base_xyz, "base_xyz", torch.float32, 3, 3)
+    b, n, _ = base_xyz.shape
+    nv = tg["vote_mask"].shape[1]
+    ins = [(base_xyz,)]
+    for t, name, w in ((pred_cls, "pred_cls", 1), (pred_offset, "pred_offset", 6), (pred_angle_cls, "pred_angle_cls", angle_bins),
+                       (pred_angle_res, "pred_angle_res", angle_bins)):
+        ins.append(_rows(t, name, b, n, w))
+    ins.append(_rows(vote_offset, "vote_offset", b, nv, 3))
+    for k in _LOSS_TARGETS:
+        if tg[k].shape[:2] != (b, nv if k.startswith("vote") else n):
+            raise ValueError("target %s %s does not match the inputs" % (k, tuple(tg[k].shape)))
+    return b, n, nv, ins
+
+
+def _det_args(ins, tg):
+    args = [_p(ins[0][0])]
+    for t, ld in ins[1:]:
+        args += [_p(t), ld]
+    return args + [_p(tg[k]) for k in _LOSS_TARGETS]
+
+
+def det_loss(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins=12):
+    """The six detection losses (ssd3d_det_loss) -> (loss (6,) = cls, offset, angle bin, angle residual, corner, vote;
+    norm (3,) = the classification, positive and vote normalisers).  The head outputs are read in place."""
+    b, n, nv, ins = _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins)
+    dev = ins[0][0].device
+    ws = torch.empty((int(lib().ssd3d_det_loss_workspace(b)),), dtype=torch.uint8, device=dev)
+    loss = torch.empty((6,), dtype=torch.float32, device=dev)
+    norm = torch.empty((3,), dtype=torch.float32, device=dev)
+    check(lib().ssd3d_det_loss(b, n, nv, int(angle_bins), *_det_args(ins, tg), _p(ws), _p(loss), _p(norm), _stream()), "det_loss")
+    return loss, norm
+
+
+def det_loss_grad(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, grad_loss, norm, angle_bins=12):
+    """Backward of det_loss from grad_loss (6,) -> (grad_base_xyz (b, n, 3), grad_cls (b, n, 1), grad_reg (b, n, 6 + 2 *
+    angle_bins) laid out as the head's [offset | angle logits | angle residuals], grad_vote_offset (b, nv, 3))."""
+    b, n, nv, ins = _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins)
+    grad_loss, norm = _req(grad_loss, "grad_loss", torch.float32, 1, 6), _req(norm, "norm", torch.float32, 1, 3)
+    dev = ins[0][0].device
+    ldr = 6 + 2 * angle_bins
+    gbase = torch.empty((b, n, 3), dtype=torch.float32, device=dev)
+    gcls = torch.empty((b, n, 1), dtype=torch.float32, device=dev)
+    greg = torch.empty((b, n, ldr), dtype=torch.float32, device=dev)
+    gvote = torch.empty((b, nv, 3), dtype=torch.float32, device=dev)
+    check(lib().ssd3d_det_loss_grad(b, n, nv, int(angle_bins), *_det_args(ins, tg), _p(grad_loss), _p(norm), _p(gbase), _p(gcls), 1,
+                                    _p(greg), ldr, ctypes.c_void_p(greg.data_ptr() + 4 * 6), ldr,
+                                    ctypes.c_void_p(greg.data_ptr() + 4 * (6 + angle_bins)), ldr, _p(gvote), _stream()),
+          "det_loss_grad")
+    return gbase, gcls, greg, gvote
+
+
+class _DetLoss(torch.autograd.Function):
+    """det_loss forward; det_loss_grad backward (one kernel for every input's gradient)."""
+
+    @staticmethod
+    def forward(ctx, base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins):
+        loss, norm = det_loss(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins)
+        ctx.save_for_backward(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, norm)
+        ctx.tg, ctx.angle_bins = tg, angle_bins
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, norm = ctx.saved_tensors
+        nb = ctx.angle_bins
+        gbase, gcls, greg, gvote = det_loss_grad(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset,
+                                                 ctx.tg, g.contiguous(), norm, nb)
+        return (gbase, gcls.reshape(pred_cls.shape), greg[..., :6].reshape(pred_offset.shape),
+                greg[..., 6:6 + nb].reshape(pred_angle_cls.shape), greg[..., 6 + nb:].reshape(pred_angle_res.shape), gvote, None, None)
+
+
+def det_loss_train(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins=12):
+    """Differentiable det_loss -> loss (6,); gradients reach base_xyz, the four head outputs and vote_offset."""
+    return _DetLoss.apply(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, int(angle_bins))

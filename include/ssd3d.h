@@ -376,6 +376,67 @@ int ssd3d_vote_translate(long rows, const float *xyz, const float *offsets, int 
 int ssd3d_decode_dist_anchor_free(long rows, int angle_bins, const float *center_xyz, const float *pred_reg, int ld_reg,
                                   const float *pred_cls, int ld_cls, float *boxes, float *scores, ssd3d_stream_t stream);
 
+/* ---- training targets and detection losses (csrc/det_loss.cu, DESIGN.md section 3.8) -------- */
+
+/* 'Mask' target assignment and vote targets of the shipped 3DSSD configuration in one launch, one CTA per scene:
+ * TargetAssigner.assign + mask_assign_targets_anchors_np + vote_targets_np (lib/builder/target_assigner.py:147,
+ * lib/np_functions/gt_sampler.py:168-259, :28-61) with the encode step of the regression targets.
+ * gt_boxes [b, g, 7] (x, y, z, l, h, w, ry; a row of seven zeros is padding and is skipped, any g >= 0),
+ * gt_labels [b, g] int32.  For each candidate point base_xyz [b, n, 3]:
+ *   inside        the face-plane test of check_inside_points (lib/utils/voxelnet_aug.py:318-342, :532-567): a point
+ *                 is outside a box as soon as one face gives sign >= 0, so a point on a face is outside;
+ *   assigned_idx  [b, n] int32: the first valid box that contains the point, else the first valid box;
+ *   assigned_box  [b, n, 7]: that box;
+ *   pmask [b, n]  inside && |base_xyz - box[:3]| <= 10;  nmask [b, n] = !inside (inside but beyond 10 m: neither);
+ *   cls_label     [b, n]: the centre-ness label (lib/builder/loss_builder.py:99-137) of a positive whose box has
+ *                 label 1, else 0 (the label one_hot(label - 1) * centre-ness of the one class);
+ *   angle_bin     [b, n] int32, angle_res [b, n]: encode_angle2class of the box's ry with float32 floor-mods
+ *                 (lib/utils/anchor_encoder.py:9-33; a bin that rounds to angle_bins is clamped to angle_bins - 1);
+ *   offset_target [b, n, 6]: encode_dist_anchor_free (anchor_encoder.py:151-173): box centre moved up by h/2 minus
+ *                 base_xyz, then l/2, h/2, w/2.
+ * For each vote base point vote_base [b, nv, 3], against the boxes grown by 0.1 in l, h and w (gt_sampler.py:28-61):
+ *   vote_mask [b, nv], vote_target [b, nv, 3] = (x, y - h/2, z) of the first (unexpanded) box whose expansion holds the
+ *   point, else of the first valid box, minus the point.
+ * A scene without a valid box: every point is a negative, assigned_idx / assigned_box / cls_label / angle_bin /
+ * angle_res / offset_target / vote_mask / vote_target are 0.  float32 targets made of + - * / are the bits of the
+ * reference's float32 numpy / TF arithmetic; the centre-ness label is evaluated in double and rounded once. */
+int ssd3d_det_assign(int b, int n, int nv, int g, int angle_bins, const float *base_xyz, const float *vote_base,
+                     const float *gt_boxes, const int *gt_labels, int *assigned_idx, float *assigned_box, float *pmask,
+                     float *nmask, float *cls_label, int *angle_bin, float *angle_res, float *offset_target, float *vote_mask,
+                     float *vote_target, ssd3d_stream_t stream);
+/* The six losses of LossBuilder.forward (loss_builder.py) for 'Center-ness' sigmoid classification, 'Dist-Anchor-free'
+ * regression, the corner loss and the vote loss, from the head outputs read in place through row strides
+ * (pred_cls [b, n, ld_cls] column 0, pred_offset [.., ld_offset] columns 0:6, pred_angle_cls / pred_angle_res columns
+ * 0:angle_bins), the raw vote offsets vote_offset [b, nv, ld_vote] and the targets of ssd3d_det_assign.  The
+ * regression target is encoded again from assigned_box and base_xyz (the bits of offset_target for the same points), so
+ * the loss is a function of the base_xyz it differentiates.
+ * loss[6] = cls, offset, angle bin, angle residual, corner, vote; norm[3] = max(1, sum) of the classification mask
+ * (pmask + nmask), of pmask and of vote_mask over the whole batch.  The corner loss decodes the predicted box with the
+ * GT angle bin (single_stage_detector.py:173-177).  Each term is summed per scene, then over the scenes in order, in
+ * double; transcendentals and loss arithmetic run in double and each result is rounded once.
+ * workspace: ssd3d_det_loss_workspace(b) bytes, 8-byte aligned. */
+size_t ssd3d_det_loss_workspace(int b);
+int ssd3d_det_loss(int b, int n, int nv, int angle_bins, const float *base_xyz, const float *pred_cls, int ld_cls,
+                   const float *pred_offset, int ld_offset, const float *pred_angle_cls, int ld_angle_cls,
+                   const float *pred_angle_res, int ld_angle_res, const float *vote_offset, int ld_vote,
+                   const float *assigned_box, const float *pmask, const float *nmask, const float *cls_label,
+                   const int *angle_bin, const float *angle_res, const float *vote_mask, const float *vote_target,
+                   void *workspace, float *loss, float *norm, ssd3d_stream_t stream);
+/* Backward of ssd3d_det_loss from grad_loss[6] (device) and the norm[3] it wrote: grad_base_xyz [b, n, 3] (through the
+ * offset target and the corner loss's decoded box; none through the centre-ness label, which TF stops),
+ * grad_cls / grad_offset / grad_angle_cls / grad_angle_res with row strides ldg_* (the residual gradient only at the
+ * GT bin; lhw = max(2 * half, 0.1) routes a tie to 2 * half), grad_vote_offset [b, nv, 3].  Rows no term touches get
+ * exactly 0.  One thread per row, no atomics. */
+int ssd3d_det_loss_grad(int b, int n, int nv, int angle_bins, const float *base_xyz, const float *pred_cls, int ld_cls,
+                        const float *pred_offset, int ld_offset, const float *pred_angle_cls, int ld_angle_cls,
+                        const float *pred_angle_res, int ld_angle_res, const float *vote_offset, int ld_vote,
+                        const float *assigned_box, const float *pmask, const float *nmask, const float *cls_label,
+                        const int *angle_bin, const float *angle_res, const float *vote_mask, const float *vote_target,
+                        const float *grad_loss, const float *norm, float *grad_base_xyz,
+                        float *grad_cls, int ldg_cls, float *grad_offset, int ldg_offset, float *grad_angle_cls,
+                        int ldg_angle_cls, float *grad_angle_res, int ldg_angle_res, float *grad_vote_offset,
+                        ssd3d_stream_t stream);
+
 /* ---- sharded step: exchange over NVLink peer memory ---------------------------------------- */
 
 /* All-gather of one slice per rank as ONE kernel (csrc/peer_gather.cu): no reference counterpart (the reference's

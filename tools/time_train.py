@@ -2,9 +2,11 @@
 (params.TrainableParams, is_training=True) on one GPU, timed with CUDA events after warm-up; then every launch of the
 backward kernels (linear_wgrad, bn_train_grad, rowgroup_max_grad, group_concat_grad) of one step timed with its own
 event pair, and the issued / algorithmic MMA rate of linear_wgrad against the 989 TFLOP/s BF16 data-sheet figure of the
-H100 SXM.  Prints the card name and its power limit, then one JSON line.
+H100 SXM.  The loss is the mean of the squared head outputs and vote offsets, a stand-in; --loss det trains against the
+3DSSD detection loss (loss.assign_targets + loss.detection_loss) on synth.kitti_like_with_boxes scenes and also times
+each launch of det_assign, det_loss and det_loss_grad.  Prints the card name and its power limit, then one JSON line.
 
-    python tools/time_train.py [--batch 8] [--points 16384] [--steps 5] [--warmup 2]
+    python tools/time_train.py [--batch 8] [--points 16384] [--steps 5] [--warmup 2] [--loss squares|det]
 """
 import argparse
 import importlib
@@ -24,23 +26,9 @@ PEAK_BF16 = 989e12            # H100 SXM data sheet, dense BF16
 
 
 def train_forward(arch, tp, xyz, feat):
-    """The backbone loop of SABackbone.forward in training mode (SA and vote layers), then conv1d_0 and the
-    box-regression head of the 3DSSD head on the last layer's features.  Returns (outputs of the head, offsets)."""
-    xyz_l, feat_l, fps_l, offs = [xyz], [feat], [None], []
-    for spec in arch:
-        (xyz_i, feat_i, radius, nsample, mlps, bn, rng, method, npoint, former, attn, ltype, scope, dilated, vote_idx, agg) = spec
-        if ltype == "SA_Layer":
-            r = pkg.pointnet_sa_module_msg(xyz_l[xyz_i[0]], feat_l[feat_i[0]], radius, nsample, mlps, True, None, bn, rng, method,
-                                           npoint, fps_l[former] if former != -1 else None, attn, scope, dilated,
-                                           xyz_l[vote_idx] if vote_idx != -1 else None, agg, params=tp)
-            xyz_l.append(r[0]); feat_l.append(r[1]); fps_l.append(r[2])
-        elif ltype == "Vote_Layer":
-            nx, nf, off = pkg.vote_layer(xyz_l[xyz_i[0]], feat_l[feat_i[0]], mlps, True, None, bn, scope, params=tp)
-            xyz_l.append(nx); feat_l.append(nf); fps_l.append(None); offs.append(off)
-        else:
-            raise ValueError("layer type %r has no training driver here" % (ltype,))
-    f = tp.conv_train("conv1d_0", feat_l[-1], True)
-    return pkg.head.box_regression_head(f, 1, 1, 6, True, True, params=tp), offs
+    """backbone.train_forward: returns (outputs of the head, raw vote offsets)."""
+    o = pkg.backbone.train_forward(arch, tp, xyz, feat)
+    return o.head, o.vote_offsets
 
 
 def trainable(arch, device, seed=0):
@@ -54,6 +42,15 @@ def step(arch, tp, xyz, feat):
     loss = sum((o.float() ** 2).mean() for o in outs) + sum((o ** 2).mean() for o in offs)
     loss.backward()
     return loss
+
+
+def det_step(arch, tp, xyz, feat, gt_boxes, gt_labels):
+    """One step with the real 3DSSD objective: train_forward -> assign_targets -> detection_loss -> backward."""
+    o = pkg.backbone.train_forward(arch, tp, xyz, feat)
+    tg = pkg.loss.assign_targets(o.base_xyz, o.vote_base, gt_boxes, gt_labels)
+    losses = pkg.loss.detection_loss(o.base_xyz, *o.head, o.vote_offsets[-1], tg)
+    losses["total"].backward()
+    return losses
 
 
 class _Timed:
@@ -72,7 +69,8 @@ class _Timed:
                 s.record()
                 r = _f(*a, **k)
                 e.record()
-                shape = (a[0].numel() // a[0].shape[-1], a[0].shape[-1], a[1].shape[-1]) if _n == "linear_wgrad" else tuple(a[0].shape)
+                shape = (a[0].numel() // a[0].shape[-1], a[0].shape[-1], a[1].shape[-1]) if _n == "linear_wgrad" else \
+                    (tuple(a[0].shape) + ((a[2].shape[1],) if _n == "det_assign" else ()))
                 self.rec.append((_n, shape, s, e))
                 return r
             setattr(T, n, wrap)
@@ -89,6 +87,10 @@ def main():
     ap.add_argument("--points", type=int, default=16384)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--loss", choices=("squares", "det"), default="squares",
+                    help="squares: mean of squared head outputs and vote offsets (a stand-in); det: the 3DSSD detection "
+                         "loss on synth.kitti_like_with_boxes scenes, with the target and loss launches timed as well")
+    ap.add_argument("--max-boxes", type=int, default=40, help="GT rows per scene of --loss det")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("time_train.py measures on a CUDA device; none is available")
@@ -102,23 +104,32 @@ def main():
     print("card: %s, power limit / max SM clock: %s" % (card, power))
     arch = pkg.config.ARCH_3DSSD
     synth = importlib.import_module("3dssd_b200.synth")
-    pts = torch.from_numpy(synth.kitti_like(a.batch, a.points, seed=1)).to(dev)
+    timed = ["linear_wgrad", "bn_train_grad", "rowgroup_max_grad", "group_concat_grad"]
+    if a.loss == "det":
+        p, boxes, labels = synth.kitti_like_with_boxes(a.batch, a.points, a.max_boxes, seed=1)
+        pts = torch.from_numpy(p).to(dev)
+        gb, gl = torch.from_numpy(boxes).to(dev), torch.from_numpy(labels).to(dev)
+        run = lambda: det_step(arch, tp, xyz, feat, gb, gl)
+        timed += ["det_assign", "det_loss", "det_loss_grad"]
+    else:
+        pts = torch.from_numpy(synth.kitti_like(a.batch, a.points, seed=1)).to(dev)
+        run = lambda: step(arch, tp, xyz, feat)
     xyz, feat = T.split_points(pts)
     tp = trainable(arch, dev)
     for _ in range(a.warmup):
-        step(arch, tp, xyz, feat)
+        run()
         tp_zero(tp)
     torch.cuda.synchronize()
     s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     s.record()
     for _ in range(a.steps):
-        step(arch, tp, xyz, feat)
+        run()
         tp_zero(tp)
     e.record()
     torch.cuda.synchronize()
     step_ms = s.elapsed_time(e) / a.steps
-    with _Timed(["linear_wgrad", "bn_train_grad", "rowgroup_max_grad", "group_concat_grad"]) as tm:
-        step(arch, tp, xyz, feat)
+    with _Timed(timed) as tm:
+        run()
         tp_zero(tp)
     torch.cuda.synchronize()
     per = {}
@@ -136,13 +147,15 @@ def main():
         print("%-18s %3d launches %8.3f ms" % (n, len(lst), sum(ms for _, ms in lst)))
         for shape, ms in lst:
             print("    %-28s %8.4f ms" % (shape, ms))
-    res = {"card": card, "power_limit_max_sm_clock": power, "batch": a.batch, "points": a.points,
+    res = {"card": card, "power_limit_max_sm_clock": power, "batch": a.batch, "points": a.points, "loss": a.loss,
            "train_step_ms": round(step_ms, 3),
-           "backward_kernels_ms": {n: round(sum(ms for _, ms in lst), 3) for n, lst in per.items()},
+           "backward_kernels_ms": {n: round(sum(ms for _, ms in lst), 3) for n, lst in per.items() if not n.startswith("det_")},
            "linear_wgrad_issued_bf16_tflops": round(wg_issued / (wg_ms * 1e-3) / 1e12, 2),
            "linear_wgrad_issued_share_of_989": round(wg_issued / (wg_ms * 1e-3) / PEAK_BF16, 4),
            "linear_wgrad_algorithmic_tflops": round(wg_alg / (wg_ms * 1e-3) / 1e12, 2),
            "linear_wgrad_algorithmic_share_of_989": round(wg_alg / (wg_ms * 1e-3) / PEAK_BF16, 4)}
+    if a.loss == "det":
+        res["det_kernels_ms"] = {n: round(sum(ms for _, ms in lst), 4) for n, lst in per.items() if n.startswith("det_")}
     print(json.dumps(res))
 
 
