@@ -11,10 +11,12 @@ checks mirror the reference's OP_REQUIRES (InvalidArgument -> ValueError); outpu
 TF's allocate_output, and the kernels run on torch's current stream (CUDA-graph capturable).
 """
 import ctypes
+import math
 
 import torch
 
 from ._lib import check, lib
+from .params import BN_EPS, FoldedConv, round16
 
 
 def _stream():
@@ -25,38 +27,44 @@ def _p(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
 
 
-def _req(t, name, dtype, rank, last=None):
+def _req(t, name, dtype, rank=None, last=None, copy=True):
+    """The one operand check: a CUDA tensor of `dtype`, of rank `rank` (None: any) and last dimension `last` (None: any).
+    copy=True: an input, returned contiguous (copied if it is not); copy=False: used in place (caller-supplied outputs,
+    workspaces, state updated in place), so it must already be contiguous; copy=None: returned as it is, for callers
+    that read its strides."""
     if not isinstance(t, torch.Tensor):
         raise ValueError("%s must be a torch.Tensor" % name)
     if not t.is_cuda:
         raise ValueError("%s must be a CUDA tensor (there is no CPU path)" % name)
     if t.dtype != dtype:
         raise ValueError("%s must be %s, got %s" % (name, dtype, t.dtype))
-    if t.dim() != rank:
+    if rank is not None and t.dim() != rank:
         raise ValueError("%s must have rank %d, got shape %s" % (name, rank, tuple(t.shape)))
     if last is not None and t.shape[-1] != last:
         raise ValueError("%s must have last dimension %d, got shape %s" % (name, last, tuple(t.shape)))
-    return t if t.is_contiguous() else t.contiguous()
+    if copy is None or t.is_contiguous():
+        return t
+    if not copy:
+        raise ValueError("%s is written or kept in place and must be contiguous" % name)
+    return t.contiguous()
 
 
-def _scene_strided(t, name, rank=3, last=None):
+def _vec(t, name, c):
+    """A per-channel float32 vector of length c, read or updated in place."""
+    t = _req(t, name, torch.float32, 1, copy=False)
+    if t.shape[0] != c:
+        raise ValueError("%s must have shape (%d,), got %s" % (name, c, tuple(t.shape)))
+    return t
+
+
+def _scene_strided(t, name):
     """A float32 CUDA tensor (b, n, c) whose rows are dense but whose scenes may be strided (a [:, a:b] slice of a
     dense tensor): returns (tensor, scene stride in floats) without copying; anything else is made contiguous."""
-    if not isinstance(t, torch.Tensor):
-        raise ValueError("%s must be a torch.Tensor" % name)
-    if not t.is_cuda:
-        raise ValueError("%s must be a CUDA tensor (there is no CPU path)" % name)
-    if t.dtype != torch.float32:
-        raise ValueError("%s must be %s, got %s" % (name, torch.float32, t.dtype))
-    if t.dim() != rank:
-        raise ValueError("%s must have rank %d, got shape %s" % (name, rank, tuple(t.shape)))
-    if last is not None and t.shape[-1] != last:
-        raise ValueError("%s must have last dimension %d, got shape %s" % (name, last, tuple(t.shape)))
+    t = _req(t, name, torch.float32, 3, copy=None)
     b, n, c = t.shape
     if c > 0 and n > 0 and t.stride(2) == 1 and t.stride(1) == c and (b <= 1 or t.stride(0) >= n * c):
         return t, (t.stride(0) if b > 1 else n * c)
-    t = t.contiguous()
-    return t, n * c
+    return t.contiguous(), n * c
 
 
 def _idx_out(out, b, npoint, device):
@@ -65,9 +73,18 @@ def _idx_out(out, b, npoint, device):
         o = torch.empty((b, npoint), dtype=torch.int32, device=device)
         return o, o.data_ptr(), npoint
     buf, col = out
-    if buf.dtype != torch.int32 or buf.dim() != 2 or not buf.is_contiguous() or buf.shape[0] != b or col < 0 or col + npoint > buf.shape[1]:
+    buf = _req(buf, "out", torch.int32, 2, copy=False)
+    if buf.shape[0] != b or col < 0 or col + npoint > buf.shape[1]:
         raise ValueError("out must be (int32 contiguous (b, >= col + npoint) buffer, col)")
     return buf[:, col:col + npoint], buf.data_ptr() + 4 * col, buf.shape[1]
+
+
+def _temp(temp, elems):
+    """The caller's FPS state buffer: contiguous float32 of at least `elems` elements, used in place."""
+    temp = _req(temp, "temp", torch.float32, copy=False)
+    if temp.numel() < elems:
+        raise ValueError("temp must hold at least %d elements, got %d" % (elems, temp.numel()))
+    return temp
 
 
 def _fps_flags(packet_kernel, bucket_kernel):
@@ -107,8 +124,8 @@ def farthest_point_sample(npoint, inp, *, out=None, idx_offset=0, rounds=None, t
         if (j0, j1) != (0, npoint):
             raise ValueError("a partial range of rounds needs the caller's temp (batch, fps_temp_elems(...)) float32 buffer")
         temp = torch.empty((b, elems), dtype=torch.float32, device=inp.device)
-    if temp is not None and (temp.dtype != torch.float32 or not temp.is_contiguous() or temp.numel() < b * elems):
-        raise ValueError("temp must be a contiguous float32 buffer of at least batch * fps_temp_elems(n, c, npoint) elements")
+    if temp is not None:
+        temp = _temp(temp, b * elems)
     check(lib().ssd3d_farthest_point_sample_ex(b, n, c, npoint, _p(inp), stride, _p(temp), ctypes.c_void_p(optr), ldo,
                                                int(idx_offset), j0, j1, int(cluster), flags, _stream()),
           "farthest_point_sample")
@@ -161,8 +178,10 @@ def farthest_point_sample_features(npoint, xyz, points=None, *, out=None, idx_of
     npoint = int(npoint)
     o, optr, ldo = _idx_out(out, b, npoint, xyz.device)
     j0, j1 = (0, npoint) if rounds is None else (int(rounds[0]), int(rounds[1]))
-    if (j0, j1) != (0, npoint) and (temp is None or temp.dtype != torch.float32 or not temp.is_contiguous() or temp.numel() < b * n):
-        raise ValueError("a partial range of rounds needs a contiguous float32 temp buffer of batch * n elements")
+    if (j0, j1) != (0, npoint):
+        if temp is None:
+            raise ValueError("a partial range of rounds needs a contiguous float32 temp buffer of batch * n elements")
+        temp = _temp(temp, b * n)
     check(lib().ssd3d_farthest_point_sample_features_ex(b, n, ca, cb, npoint, _p(xyz), sa, _p(points), sb, _p(temp),
                                                         ctypes.c_void_p(optr), ldo, int(idx_offset), j0, j1, _stream()),
           "farthest_point_sample_features")
@@ -206,9 +225,9 @@ def gather_point(inp, idx):
     """inp (batch, ndataset, c) float32, idx (batch, npoints) int32 -> (batch, npoints, c).  tf_sampling.py:24-32.
     Differentiable w.r.t. inp (the reference registers GatherPoint's gradient, tf_sampling.py:37-42)."""
     inp = _req(inp, "inp", torch.float32, 3)
-    if not (isinstance(idx, torch.Tensor) and idx.is_cuda and idx.dtype == torch.int32 and idx.dim() == 2
-            and idx.stride(1) == 1 and idx.stride(0) >= idx.shape[1]):
-        idx = _req(idx, "idx", torch.int32, 2)
+    idx = _req(idx, "idx", torch.int32, 2, copy=None)
+    if not (idx.stride(1) == 1 and idx.stride(0) >= idx.shape[1]):
+        idx = idx.contiguous()
     if idx.shape[0] != inp.shape[0]:
         raise ValueError("GatherPoint expects (batch_size,num_result) idx shape")
     if inp.requires_grad and torch.is_grad_enabled():
@@ -224,43 +243,38 @@ def _bq_shapes(xyz1, xyz2):
     return xyz1, xyz2
 
 
-def query_ball_point(radius, nsample, xyz1, xyz2):
-    """xyz1 (batch, ndataset, 3), xyz2 (batch, npoint, 3) -> idx (batch, npoint, nsample) int32,
-    pts_cnt (batch, npoint) int32.  tf_grouping.py:53-65."""
+def _query_ball(op, min_radius, max_radius, nsample, xyz1, xyz2, dilated):
+    """The body of query_ball_point (dilated=False, min_radius unused) and query_ball_point_dilated; op names the
+    reference op in the error texts."""
     xyz1, xyz2 = _bq_shapes(xyz1, xyz2)
-    if not radius > 0:
-        raise ValueError("QueryBallPoint expects positive radius")      # tf_grouping.cpp:275
+    if not max_radius > 0:
+        raise ValueError("%s expects positive radius" % op)      # tf_grouping.cpp:275
     if not int(nsample) > 0:
-        raise ValueError("QueryBallPoint expects positive nsample")     # tf_grouping.cpp:278
+        raise ValueError("%s expects positive nsample" % op)     # tf_grouping.cpp:278
     b, n, _ = xyz1.shape
     m = xyz2.shape[1]
     if n >= BQ_GRID_MIN_N and lib().ssd3d_query_ball_point_workspace(b, n):
-        i, c = query_ball_point_multi([0.0], [radius], [nsample], xyz1, xyz2, False)
+        i, c = query_ball_point_multi([min_radius], [max_radius], [nsample], xyz1, xyz2, dilated)
         return i[0], c[0]
     idx = torch.empty((b, m, int(nsample)), dtype=torch.int32, device=xyz1.device)
     cnt = torch.empty((b, m), dtype=torch.int32, device=xyz1.device)
-    check(lib().ssd3d_query_ball_point(b, n, m, float(radius), int(nsample), _p(xyz1), _p(xyz2), _p(idx), _p(cnt),
-                                       _stream()), "query_ball_point")
+    tail = (int(nsample), _p(xyz1), _p(xyz2), _p(idx), _p(cnt), _stream())
+    if dilated:
+        check(lib().ssd3d_query_ball_point_dilated(b, n, m, float(min_radius), float(max_radius), *tail), "query_ball_point_dilated")
+    else:
+        check(lib().ssd3d_query_ball_point(b, n, m, float(max_radius), *tail), "query_ball_point")
     return idx, cnt
+
+
+def query_ball_point(radius, nsample, xyz1, xyz2):
+    """xyz1 (batch, ndataset, 3), xyz2 (batch, npoint, 3) -> idx (batch, npoint, nsample) int32,
+    pts_cnt (batch, npoint) int32.  tf_grouping.py:53-65."""
+    return _query_ball("QueryBallPoint", 0.0, radius, nsample, xyz1, xyz2, False)
 
 
 def query_ball_point_dilated(min_radius, max_radius, nsample, xyz1, xyz2):
     """Shell query  d == 0 or min_radius <= d < max_radius.  tf_grouping.py:68-81."""
-    xyz1, xyz2 = _bq_shapes(xyz1, xyz2)
-    if not max_radius > 0:
-        raise ValueError("QueryBallPointDilated expects positive radius")
-    if not int(nsample) > 0:
-        raise ValueError("QueryBallPointDilated expects positive nsample")
-    b, n, _ = xyz1.shape
-    m = xyz2.shape[1]
-    if n >= BQ_GRID_MIN_N and lib().ssd3d_query_ball_point_workspace(b, n):
-        i, c = query_ball_point_multi([min_radius], [max_radius], [nsample], xyz1, xyz2, True)
-        return i[0], c[0]
-    idx = torch.empty((b, m, int(nsample)), dtype=torch.int32, device=xyz1.device)
-    cnt = torch.empty((b, m), dtype=torch.int32, device=xyz1.device)
-    check(lib().ssd3d_query_ball_point_dilated(b, n, m, float(min_radius), float(max_radius), int(nsample), _p(xyz1),
-                                               _p(xyz2), _p(idx), _p(cnt), _stream()), "query_ball_point_dilated")
-    return idx, cnt
+    return _query_ball("QueryBallPointDilated", min_radius, max_radius, nsample, xyz1, xyz2, True)
 
 
 BQ_GRID_MIN_N = 2048     # candidate sets at least this large take the spatially culled kernel (csrc/ball_query_grid.cu)
@@ -429,18 +443,111 @@ def calc_square_dist(a):
     return out
 
 
-def group_concat(xyz, points, new_xyz, idx, ldx=None):
-    """concat[group_point(points, idx), group_point(xyz, idx) - new_xyz] (layers_util.py:160-165) in one kernel.
-    Returns x (b, m, nsample, ldx) with zero padding beyond c+3."""
+def _grouping(xyz, points, new_xyz, idx, cnt=None):
+    """The operands of a grouping kernel: xyz (b, n, 3), points (b, n, c) or None, new_xyz (b, m, 3), idx (b, m, nsample)
+    int32 and, when given, cnt (b, m) int32 -> (xyz, points, new_xyz, idx, b, n, c, m, nsample)."""
     xyz = _req(xyz, "xyz", torch.float32, 3, 3)
     new_xyz = _req(new_xyz, "new_xyz", torch.float32, 3, 3)
     idx = _req(idx, "idx", torch.int32, 3)
     b, n, _ = xyz.shape
+    _, m, ns = idx.shape
+    if tuple(new_xyz.shape) != (b, m, 3) or idx.shape[0] != b:
+        raise ValueError("new_xyz %s and idx %s must be (b, m, 3) and (b, m, nsample) with xyz %s"
+                         % (tuple(new_xyz.shape), tuple(idx.shape), tuple(xyz.shape)))
     c = 0
     if points is not None:
         points = _req(points, "points", torch.float32, 3)
         c = points.shape[2]
-    _, m, ns = idx.shape
+        if points.shape[:2] != (b, n):
+            raise ValueError("points %s must be (b, n, c) like xyz %s" % (tuple(points.shape), tuple(xyz.shape)))
+    if cnt is not None and tuple(_req(cnt, "cnt", torch.int32, 2, copy=False).shape) != (b, m):
+        raise ValueError("cnt must be (%d, %d), got %s" % (b, m, tuple(cnt.shape)))
+    return xyz, points, new_xyz, idx, b, n, c, m, ns
+
+
+def _hoisted_table(z, zoff, wx, b, n):
+    """The per-point table of a hoisted first conv: z (b, n, ldz) fp32 whose columns [zoff, zoff + n1) belong to this
+    scale, wx (3, n1) fp32 -> (pointer to column zoff, ldz, wx, n1)."""
+    z = _req(z, "z", torch.float32, 3)
+    wx = _req(wx, "wx", torch.float32, 2)
+    n1 = wx.shape[1]
+    if z.shape[:2] != (b, n) or wx.shape[0] != 3 or zoff < 0 or zoff + n1 > z.shape[2]:
+        raise ValueError("z must be (b, n, ldz) with zoff + n1 <= ldz and wx (3, n1)")
+    return ctypes.c_void_p(z.data_ptr() + 4 * zoff), z.shape[2], wx, n1
+
+
+def _placed(out, name, dtype, lead, n):
+    """A caller's output slot for n columns, (buffer, col) or (hi, lo, col): contiguous `dtype` buffers (*lead, ld) with
+    0 <= col and col + n <= ld -> ([buffers], [pointers to their column col], ld)."""
+    buf, col = out[:-1], int(out[-1])
+    bufs = [_req(t, name, dtype, copy=False) for t in buf]
+    ld = bufs[0].shape[-1]
+    if any(tuple(t.shape) != tuple(lead) + (ld,) for t in bufs) or col < 0 or col + n > ld:
+        raise ValueError("%s must be (%s buffer (%s, ld), col) with 0 <= col and col + %d <= ld, got shape %s and col %d"
+                         % (name, dtype, ", ".join(map(str, lead)), n, tuple(bufs[0].shape), col))
+    return bufs, [ctypes.c_void_p(t.data_ptr() + t.element_size() * col) for t in bufs], ld
+
+
+def _outputs(lead, n, dev, want_f32, want_split, out_f32, out_split, pooled):
+    """The fp32 and split-bf16 outputs of the tensor-core and fused kernels: the caller's (buffer, col) /
+    (hi, lo, col) slots, else fresh tensors (*lead, n) / (*lead, round16(n)) when wanted.  A pooled split output is
+    zero-filled so that its padding columns are 0.  -> (y, (hi, lo) or None, [pf, ldf, phi, plo, lds])."""
+    y, sp = None, None
+    pf, ldf = ctypes.c_void_p(0), 0
+    if out_f32 is not None:
+        (y,), (pf,), ldf = _placed(out_f32, "out_f32", torch.float32, lead, n)
+    elif want_f32:
+        y = torch.empty(lead + (n,), dtype=torch.float32, device=dev)
+        pf, ldf = _p(y), n
+    ph = pl = ctypes.c_void_p(0)
+    lds = 0
+    if out_split is not None:
+        sp, (ph, pl), lds = _placed(out_split, "out_split", torch.bfloat16, lead, n)
+        sp = tuple(sp)
+    elif want_split:
+        lds = round16(n)
+        alloc = torch.zeros if (pooled and lds != n) else torch.empty
+        sp = tuple(alloc(lead + (lds,), dtype=torch.bfloat16, device=dev) for _ in range(2))
+        ph, pl = _p(sp[0]), _p(sp[1])
+    return y, sp, [pf, ldf, ph, pl, lds]
+
+
+def _units_check(units, unit_pool, pool=1, rowmask=None, relu=True, out_f32=None, out_split=None, want_split=False):
+    """A unit list (query_ball_point_multi(return_units=True)) replaces pool / rowmask; with unit_pool the listed 8-row
+    units are max-pooled into the caller's zero-filled out_f32 by atomicMax, so there is no split output."""
+    if units is None:
+        if unit_pool:
+            raise ValueError("unit_pool needs a unit list")
+        return
+    _req(units, "units", torch.int32, copy=False)
+    if int(pool) != 1 or rowmask is not None:
+        raise ValueError("a unit list replaces pool / rowmask (unit_pool=True pools the listed 8-row units)")
+    if unit_pool and (not relu or out_f32 is None or out_split is not None or want_split):
+        raise ValueError("a pooled unit list needs relu, out_f32=(zero-filled buffer, col_offset) and no split output")
+
+
+def _pool(pool, group):
+    """The max-pool width of a tensor-core kernel: 1, or the group size `group` when that is one of TC_POOL_WIDTHS."""
+    pool = int(pool)
+    if pool > 1 and (pool != group or pool not in TC_POOL_WIDTHS):
+        raise ValueError("pool must equal nsample (the second-to-last dimension) and be one of %s" % (TC_POOL_WIDTHS,))
+    return pool
+
+
+def _rowmask(rowmask, groups):
+    """A pooled output's mask: int32 with one entry per pooled group, or None."""
+    if rowmask is None:
+        return None
+    rowmask = _req(rowmask, "rowmask", torch.int32)
+    if rowmask.numel() != groups:
+        raise ValueError("rowmask must hold one entry per group (%d), got shape %s" % (groups, tuple(rowmask.shape)))
+    return rowmask
+
+
+def group_concat(xyz, points, new_xyz, idx, ldx=None):
+    """concat[group_point(points, idx), group_point(xyz, idx) - new_xyz] (layers_util.py:160-165) in one kernel.
+    Returns x (b, m, nsample, ldx) with zero padding beyond c+3."""
+    xyz, points, new_xyz, idx, b, n, c, m, ns = _grouping(xyz, points, new_xyz, idx)
     ldx = c + 3 if ldx is None else int(ldx)
     x = torch.empty((b, m, ns, ldx), dtype=torch.float32, device=xyz.device)
     check(lib().ssd3d_group_concat(b, n, c, m, ns, _p(xyz), _p(points), _p(new_xyz), _p(idx), _p(x), ldx, _stream()),
@@ -451,9 +558,7 @@ def group_concat(xyz, points, new_xyz, idx, ldx=None):
 def linear_bn_relu(x, w, scale, shift, relu=True, pool=1, rowmask=None, cin=None):
     """act((x[..., :cin] @ w) * scale + shift) over the last axis; pool > 1 max-pools runs of `pool` rows and
     multiplies by rowmask != 0 (layers_util.py:178-180).  x (..., ldx), w (cin, cout)."""
-    if x.dtype != torch.float32 or not x.is_cuda:
-        raise ValueError("x must be a float32 CUDA tensor")
-    x = x if x.is_contiguous() else x.contiguous()
+    x = _req(x, "x", torch.float32)
     w = _req(w, "w", torch.float32, 2)
     wcin, cout = w.shape
     cin = wcin if cin is None else cin
@@ -463,18 +568,15 @@ def linear_bn_relu(x, w, scale, shift, relu=True, pool=1, rowmask=None, cin=None
     rows = x.numel() // ldx
     pool = int(pool)
     lead = tuple(x.shape[:-1])
-    if pool > 1:
-        if lead[-1] != pool:
-            raise ValueError("pool must equal the second-to-last dimension of x")
-        if 128 % pool != 0:
-            y = linear_bn_relu(x, w, scale, shift, relu, 1, None, cin)
-            out = torch.empty(lead[:-1] + (cout,), dtype=torch.float32, device=x.device)
-            check(lib().ssd3d_rowgroup_max(rows // pool, pool, cout, _p(y), cout, _p(rowmask), _p(out), _stream()),
-                  "rowgroup_max")
-            return out
-        y = torch.empty(lead[:-1] + (cout,), dtype=torch.float32, device=x.device)
-    else:
-        y = torch.empty(lead + (cout,), dtype=torch.float32, device=x.device)
+    if pool > 1 and lead[-1] != pool:
+        raise ValueError("pool must equal the second-to-last dimension of x")
+    olead = lead[:-1] if pool > 1 else lead
+    rowmask = _rowmask(rowmask, math.prod(olead))
+    y = torch.empty(olead + (cout,), dtype=torch.float32, device=x.device)
+    if pool > 1 and 128 % pool != 0:
+        r = linear_bn_relu(x, w, scale, shift, relu, 1, None, cin)
+        check(lib().ssd3d_rowgroup_max(rows // pool, pool, cout, _p(r), cout, _p(rowmask), _p(y), _stream()), "rowgroup_max")
+        return y
     check(lib().ssd3d_linear_bn_relu(rows, cin, cout, _p(x), ldx, _p(w), _p(scale), _p(shift), 1 if relu else 0, pool,
                                      _p(rowmask), _p(y), cout, _stream()), "linear_bn_relu")
     return y
@@ -485,15 +587,9 @@ def linear_bn_relu(x, w, scale, shift, relu=True, pool=1, rowmask=None, cin=None
 TC_POOL_WIDTHS = (8, 16, 32, 64, 128)   # group sizes the max-pool epilogue of the tensor-core kernels covers
 
 
-def round16(x):
-    return (int(x) + 15) // 16 * 16
-
-
 def split_rows(x, kp=None):
     """fp32 (..., c) -> (hi, lo) bf16 (..., kp) with hi + lo ~= x (16 mantissa bits), zero padded to kp."""
-    if x.dtype != torch.float32 or not x.is_cuda:
-        raise ValueError("x must be a float32 CUDA tensor")
-    x = x if x.is_contiguous() else x.contiguous()
+    x = _req(x, "x", torch.float32)
     c = x.shape[-1]
     kp = round16(c) if kp is None else int(kp)
     rows = x.numel() // c
@@ -505,15 +601,7 @@ def split_rows(x, kp=None):
 
 def group_concat_split(xyz, points, new_xyz, idx, kp=None):
     """group_concat + split in one kernel: (hi, lo) bf16 (b, m, nsample, kp)."""
-    xyz = _req(xyz, "xyz", torch.float32, 3, 3)
-    new_xyz = _req(new_xyz, "new_xyz", torch.float32, 3, 3)
-    idx = _req(idx, "idx", torch.int32, 3)
-    b, n, _ = xyz.shape
-    c = 0
-    if points is not None:
-        points = _req(points, "points", torch.float32, 3)
-        c = points.shape[2]
-    _, m, ns = idx.shape
+    xyz, points, new_xyz, idx, b, n, c, m, ns = _grouping(xyz, points, new_xyz, idx)
     kp = round16(c + 3) if kp is None else int(kp)
     hi = torch.empty((b, m, ns, kp), dtype=torch.bfloat16, device=xyz.device)
     lo = torch.empty_like(hi)
@@ -522,47 +610,16 @@ def group_concat_split(xyz, points, new_xyz, idx, kp=None):
     return hi, lo
 
 
-def _tc_outputs(lead, n, pool, dev, want_f32, want_split, out_f32, out_split):
-    """Resolve the output arguments shared by linear_tc / linear_tc_gather -> (y, pf, ldf, sp, ph, pl, lds)."""
-    y = None
-    pf, ldf = 0, 0
-    if out_f32 is not None:
-        buf, off = out_f32
-        ldf = buf.shape[-1]
-        pf = buf.data_ptr() + 4 * off
-        y = buf
-    elif want_f32:
-        y = torch.empty(lead + (n,), dtype=torch.float32, device=dev)
-        pf, ldf = y.data_ptr(), n
-    sp = None
-    ph = pl = 0
-    lds = 0
-    if out_split is not None:
-        hb, lb, off = out_split
-        lds = hb.shape[-1]
-        ph, pl = hb.data_ptr() + 2 * off, lb.data_ptr() + 2 * off
-        sp = (hb, lb)
-    elif want_split:
-        lds = round16(n)
-        alloc = torch.zeros if (pool > 1 and lds != n) else torch.empty
-        hb = alloc(lead + (lds,), dtype=torch.bfloat16, device=dev)
-        lb = alloc(lead + (lds,), dtype=torch.bfloat16, device=dev)
-        ph, pl = hb.data_ptr(), lb.data_ptr()
-        sp = (hb, lb)
-    return y, pf, ldf, sp, ph, pl, lds
-
-
-def _tc_units_check(units, unit_pool, pool, rowmask, relu, out_f32, out_split, want_split):
-    if units is None:
-        if unit_pool:
-            raise ValueError("unit_pool needs a unit list")
-        return
-    if units.dtype != torch.int32 or not units.is_cuda or not units.is_contiguous():
-        raise ValueError("units must be the int32 CUDA unit list returned by query_ball_point_multi(return_units=True)")
-    if int(pool) != 1 or rowmask is not None:
-        raise ValueError("a unit list replaces pool / rowmask (unit_pool=True pools the listed 8-row units)")
-    if unit_pool and (not relu or out_f32 is None or out_split is not None or want_split):
-        raise ValueError("unit_pool needs relu, out_f32=(zero-filled buffer, col_offset) and no split output")
+def _tc_epilogue(f, relu, pool, rowmask, lead, ns, dev, want_f32, want_split, out_f32, out_split, units, unit_pool):
+    """Checks and output placement shared by the linear_tc* wrappers, for an operand of leading shape `lead` in groups
+    of ns rows -> (y, (hi, lo) or None, pool, rowmask, the layer's arguments, the output arguments)."""
+    _units_check(units, unit_pool, pool, rowmask, relu, out_f32, out_split, want_split)
+    pool = _pool(pool, ns)
+    pooled = pool > 1 or unit_pool
+    olead = lead[:-1] if pooled else lead
+    rowmask = _rowmask(rowmask, math.prod(olead))
+    y, sp, out = _outputs(olead, f.cout, dev, want_f32, want_split, out_f32, out_split, pooled)
+    return y, sp, pool, rowmask, [_p(f.b_hi), _p(f.b_lo), _p(f.scale), _p(f.shift), 1 if relu else 0], out
 
 
 def linear_tc(a_hi, a_lo, f, relu=True, pool=1, rowmask=None, want_f32=True, want_split=False, out_f32=None,
@@ -573,30 +630,20 @@ def linear_tc(a_hi, a_lo, f, relu=True, pool=1, rowmask=None, want_f32=True, wan
     units: the operand holds COMPACT rows (8 per listed unit, include/ssd3d.h ssd3d_linear_tc_units) in its first
     units[0] * 8 rows; outputs are compact likewise, or -- unit_pool=True, the last conv of a scale -- every unit is
     max-pooled and combined into out_f32[group] by atomicMax (buffer zero-filled by the caller)."""
-    _tc_units_check(units, unit_pool, pool, rowmask, relu, out_f32, out_split, want_split)
-    if a_hi.dtype != torch.bfloat16 or a_lo.dtype != torch.bfloat16 or a_hi.shape != a_lo.shape:
+    a_hi, a_lo = _req(a_hi, "a_hi", torch.bfloat16), _req(a_lo, "a_lo", torch.bfloat16)
+    if a_hi.shape != a_lo.shape:
         raise ValueError("a_hi / a_lo must be bfloat16 tensors of the same shape")
     kp = a_hi.shape[-1]
     if kp != f.kp:
         raise ValueError("operand K (%d) does not match the layer's padded K (%d)" % (kp, f.kp))
-    rows = a_hi.numel() // kp
-    pool = int(pool)
     lead = tuple(a_hi.shape[:-1])
-    if pool > 1:
-        if lead[-1] != pool or pool not in TC_POOL_WIDTHS:
-            raise ValueError("pool must equal the second-to-last dimension and be one of %s" % (TC_POOL_WIDTHS,))
-        lead = lead[:-1]
-    n = f.cout
-    y, pf, ldf, sp, ph, pl, lds = _tc_outputs(lead, n, pool, a_hi.device, want_f32, want_split, out_f32, out_split)
-    vp = ctypes.c_void_p
+    y, sp, pool, rowmask, head, out = _tc_epilogue(f, relu, pool, rowmask, lead, lead[-1] if lead else 1, a_hi.device,
+                                                   want_f32, want_split, out_f32, out_split, units, unit_pool)
+    args = [a_hi.numel() // kp, kp, f.cout, _p(a_hi), _p(a_lo)] + head
     if units is not None:
-        check(lib().ssd3d_linear_tc_units(rows, kp, n, _p(a_hi), _p(a_lo), _p(f.b_hi), _p(f.b_lo), _p(f.scale), _p(f.shift),
-                                          1 if relu else 0, _p(units), 1 if unit_pool else 0, vp(pf), ldf, vp(ph), vp(pl), lds,
-                                          _stream()), "linear_tc_units")
-        return y, sp
-    check(lib().ssd3d_linear_tc(rows, kp, n, _p(a_hi), _p(a_lo), _p(f.b_hi), _p(f.b_lo), _p(f.scale), _p(f.shift),
-                                1 if relu else 0, pool, _p(rowmask), vp(pf), ldf, vp(ph), vp(pl), lds, _stream()),
-          "linear_tc")
+        check(lib().ssd3d_linear_tc_units(*args, _p(units), 1 if unit_pool else 0, *out, _stream()), "linear_tc_units")
+    else:
+        check(lib().ssd3d_linear_tc(*args, pool, _p(rowmask), *out, _stream()), "linear_tc")
     return y, sp
 
 
@@ -605,26 +652,13 @@ def linear_tc_gather(xyz, points, new_xyz, idx, f, relu=True, pool=1, rowmask=No
     """First conv layer of an SA scale with the gather / centre-subtract / concat of layers_util.py:160-165 fused
     into the tensor-core kernel's operand load (no [B,M,K,C] tensor in HBM).  Outputs as linear_tc, leading shape
     (b, m, nsample) or (b, m) when pooled."""
-    xyz = _req(xyz, "xyz", torch.float32, 3, 3)
-    new_xyz = _req(new_xyz, "new_xyz", torch.float32, 3, 3)
-    idx = _req(idx, "idx", torch.int32, 3)
-    b, n, _ = xyz.shape
-    c = 0
-    if points is not None:
-        points = _req(points, "points", torch.float32, 3)
-        c = points.shape[2]
+    xyz, points, new_xyz, idx, b, n, c, m, ns = _grouping(xyz, points, new_xyz, idx)
     if round16(c + 3) != f.kp or c + 3 != f.cin:
         raise ValueError("layer input width %d does not match c+3 = %d" % (f.cin, c + 3))
-    _, m, ns = idx.shape
-    pool = int(pool)
-    if pool > 1 and (pool != ns or pool not in TC_POOL_WIDTHS):
-        raise ValueError("pool must equal nsample and be one of %s" % (TC_POOL_WIDTHS,))
-    lead = (b, m) if pool > 1 else (b, m, ns)
-    y, pf, ldf, sp, ph, pl, lds = _tc_outputs(lead, f.cout, pool, xyz.device, want_f32, want_split, out_f32, out_split)
-    vp = ctypes.c_void_p
-    check(lib().ssd3d_linear_tc_gather(b, n, c, m, ns, _p(xyz), _p(points), _p(new_xyz), _p(idx), f.cout, _p(f.b_hi),
-                                       _p(f.b_lo), _p(f.scale), _p(f.shift), 1 if relu else 0, pool, _p(rowmask), vp(pf),
-                                       ldf, vp(ph), vp(pl), lds, _stream()), "linear_tc_gather")
+    y, sp, pool, rowmask, head, out = _tc_epilogue(f, relu, pool, rowmask, (b, m, ns), ns, xyz.device, want_f32,
+                                                   want_split, out_f32, out_split, None, False)
+    check(lib().ssd3d_linear_tc_gather(b, n, c, m, ns, _p(xyz), _p(points), _p(new_xyz), _p(idx), f.cout, *head, pool,
+                                       _p(rowmask), *out, _stream()), "linear_tc_gather")
     return y, sp
 
 
@@ -634,34 +668,18 @@ def linear_tc_hoisted(xyz, z, zoff, wx, new_xyz, idx, f, relu=True, pool=1, rowm
     z: (b, n, ldz) fp32 per-point table = (features . Wf) * s1 + t1 for all scales of the layer, this scale's
     columns start at zoff; wx: (3, n1) fp32 = Wx * s1; f: params.FoldedConv of the second conv (cin == n1).
     units / unit_pool: as linear_tc (the source rows are looked up through the list, outputs are compact)."""
-    _tc_units_check(units, unit_pool, pool, rowmask, relu, out_f32, out_split, want_split)
-    xyz = _req(xyz, "xyz", torch.float32, 3, 3)
-    new_xyz = _req(new_xyz, "new_xyz", torch.float32, 3, 3)
-    idx = _req(idx, "idx", torch.int32, 3)
-    z = _req(z, "z", torch.float32, 3)
-    wx = _req(wx, "wx", torch.float32, 2)
-    b, n, _ = xyz.shape
-    n1 = wx.shape[1]
-    if z.shape[:2] != (b, n) or wx.shape[0] != 3 or zoff < 0 or zoff + n1 > z.shape[2]:
-        raise ValueError("z must be (b, n, ldz) with zoff + n1 <= ldz and wx (3, n1)")
+    xyz, _, new_xyz, idx, b, n, _, m, ns = _grouping(xyz, None, new_xyz, idx)
+    zp, ldz, wx, n1 = _hoisted_table(z, zoff, wx, b, n)
     if f.cin != n1:
         raise ValueError("second conv expects %d inputs, the hoisted first conv has %d outputs" % (f.cin, n1))
-    _, m, ns = idx.shape
-    pool = int(pool)
-    if pool > 1 and (pool != ns or pool not in TC_POOL_WIDTHS):
-        raise ValueError("pool must equal nsample and be one of %s" % (TC_POOL_WIDTHS,))
-    lead = (b, m) if pool > 1 else (b, m, ns)
-    y, pf, ldf, sp, ph, pl, lds = _tc_outputs(lead, f.cout, pool, xyz.device, want_f32, want_split, out_f32, out_split)
-    vp = ctypes.c_void_p
+    y, sp, pool, rowmask, head, out = _tc_epilogue(f, relu, pool, rowmask, (b, m, ns), ns, xyz.device, want_f32,
+                                                   want_split, out_f32, out_split, units, unit_pool)
+    args = [b, n, n1, m, ns, _p(xyz), zp, ldz, _p(wx), _p(new_xyz), _p(idx)]
     if units is not None:
-        check(lib().ssd3d_linear_tc_hoisted_units(b, n, n1, m, ns, _p(xyz), vp(z.data_ptr() + 4 * zoff), z.shape[2], _p(wx),
-                                                  _p(new_xyz), _p(idx), _p(units), f.cout, _p(f.b_hi), _p(f.b_lo), _p(f.scale),
-                                                  _p(f.shift), 1 if relu else 0, 1 if unit_pool else 0, vp(pf), ldf, vp(ph),
-                                                  vp(pl), lds, _stream()), "linear_tc_hoisted_units")
-        return y, sp
-    check(lib().ssd3d_linear_tc_hoisted(b, n, n1, m, ns, _p(xyz), vp(z.data_ptr() + 4 * zoff), z.shape[2], _p(wx), _p(new_xyz),
-                                        _p(idx), f.cout, _p(f.b_hi), _p(f.b_lo), _p(f.scale), _p(f.shift), 1 if relu else 0,
-                                        pool, _p(rowmask), vp(pf), ldf, vp(ph), vp(pl), lds, _stream()), "linear_tc_hoisted")
+        check(lib().ssd3d_linear_tc_hoisted_units(*args, _p(units), f.cout, *head, 1 if unit_pool else 0, *out, _stream()),
+              "linear_tc_hoisted_units")
+    else:
+        check(lib().ssd3d_linear_tc_hoisted(*args, f.cout, *head, pool, _p(rowmask), *out, _stream()), "linear_tc_hoisted")
     return y, sp
 
 
@@ -670,37 +688,40 @@ def hoist_expand_split(xyz, z, zoff, wx, new_xyz, idx, units=None):
     split(relu(z[idx] + (xyz[idx] - new_xyz) . wx)).  Followed by the plain linear_tc this is the faster route for wide
     layers (K >= 256), where the resident operand of the in-kernel route leaves the weight ring two narrow stages.
     units: only the listed 8-row units are built, as compact rows at the start of the buffers."""
-    xyz = _req(xyz, "xyz", torch.float32, 3, 3)
-    new_xyz = _req(new_xyz, "new_xyz", torch.float32, 3, 3)
-    idx = _req(idx, "idx", torch.int32, 3)
-    z = _req(z, "z", torch.float32, 3)
-    wx = _req(wx, "wx", torch.float32, 2)
-    b, n, _ = xyz.shape
-    n1 = wx.shape[1]
-    if z.shape[:2] != (b, n) or wx.shape[0] != 3 or zoff < 0 or zoff + n1 > z.shape[2] or zoff % 4 or z.shape[2] % 4:
+    xyz, _, new_xyz, idx, b, n, _, m, ns = _grouping(xyz, None, new_xyz, idx)
+    zp, ldz, wx, n1 = _hoisted_table(z, zoff, wx, b, n)
+    if zoff % 4 or ldz % 4:                         # the kernel reads the table in 16-byte vectors
         raise ValueError("z must be (b, n, ldz) with ldz, zoff multiples of 4, zoff + n1 <= ldz, and wx (3, n1)")
-    _, m, ns = idx.shape
+    _units_check(units, False)
     kp = round16(n1)
     hi = torch.empty((b, m, ns, kp), dtype=torch.bfloat16, device=xyz.device)
     lo = torch.empty_like(hi)
+    args = [b, n, n1, m, ns, _p(xyz), zp, ldz, _p(wx), _p(new_xyz), _p(idx)]
     if units is not None:
-        _tc_units_check(units, False, 1, None, True, None, None, False)
-        check(lib().ssd3d_hoist_expand_split_units(b, n, n1, m, ns, _p(xyz), ctypes.c_void_p(z.data_ptr() + 4 * zoff), z.shape[2],
-                                                   _p(wx), _p(new_xyz), _p(idx), _p(units), _p(hi), _p(lo), kp, _stream()),
-              "hoist_expand_split_units")
-        return hi, lo
-    check(lib().ssd3d_hoist_expand_split(b, n, n1, m, ns, _p(xyz), ctypes.c_void_p(z.data_ptr() + 4 * zoff), z.shape[2], _p(wx),
-                                         _p(new_xyz), _p(idx), _p(hi), _p(lo), kp, _stream()), "hoist_expand_split")
+        check(lib().ssd3d_hoist_expand_split_units(*args, _p(units), _p(hi), _p(lo), kp, _stream()), "hoist_expand_split_units")
+    else:
+        check(lib().ssd3d_hoist_expand_split(*args, _p(hi), _p(lo), kp, _stream()), "hoist_expand_split")
     return hi, lo
 
 
-def _units_check(units, out_f32, out_split):
-    if units is None:
-        return
-    if units.dtype != torch.int32 or not units.is_cuda or not units.is_contiguous():
-        raise ValueError("units must be the int32 CUDA unit list returned by query_ball_point_multi(return_units=True)")
-    if out_f32 is None or out_split is not None:
-        raise ValueError("a unit list needs out_f32=(zero-filled buffer, col_offset) and no out_split (results combine through atomicMax)")
+def _sa_fused(xyz, points, table, new_xyz, idx, cnt, stack, out_f32, out_split, units):
+    """The body of sa_mlp_fused (points, table None) and sa_mlp_fused_hoisted (table = (z, zoff, wx)) up to the entry
+    point -> (y, the entry point's arguments without the stream)."""
+    _units_check(units, units is not None, out_f32=out_f32, out_split=out_split)
+    xyz, points, new_xyz, idx, b, n, c, m, ns = _grouping(xyz, points, new_xyz, idx, cnt)
+    if table is None:
+        if c + 3 != stack.cin:
+            raise ValueError("feature channels (%d) do not match the stack's input width (%d)" % (c, stack.cin - 3))
+        src = [c, m, ns, _p(xyz), _p(points)]
+    else:
+        zp, ldz, wx, n1 = _hoisted_table(*table, b, n)
+        if n1 != stack.cin:
+            raise ValueError("hoisted width (%d) does not match the stack's input width (%d)" % (n1, stack.cin))
+        src = [n1, m, ns, _p(xyz), zp, ldz, _p(wx)]
+    y, _, out = _outputs((b, m), stack.nout[-1], xyz.device, out_split is None, False, out_f32, out_split, True)
+    nout = (ctypes.c_int * len(stack.nout))(*stack.nout)
+    return y, [b, n] + src + [_p(new_xyz), _p(idx), _p(cnt), _p(units), len(stack.nout), ctypes.cast(nout, ctypes.c_void_p),
+                              _p(stack.w_blob), _p(stack.ss_blob), 1 if stack.last_scale_nonneg else 0] + out
 
 
 def sa_mlp_fused(xyz, points, new_xyz, idx, cnt, stack, out_f32=None, out_split=None, units=None):
@@ -710,74 +731,16 @@ def sa_mlp_fused(xyz, points, new_xyz, idx, cnt, stack, out_f32=None, out_split=
     units: the scale's unit list (query_ball_point_multi(return_units=True)): only the listed 8-row units are convolved
     -- the skipped rows repeat a group's first neighbour and cannot change the max-pool -- and results are combined with
     atomicMax into out_f32, which must be zero-filled (fill_zero)."""
-    _units_check(units, out_f32, out_split)
-    xyz = _req(xyz, "xyz", torch.float32, 3, 3)
-    new_xyz = _req(new_xyz, "new_xyz", torch.float32, 3, 3)
-    idx = _req(idx, "idx", torch.int32, 3)
-    b, n, _ = xyz.shape
-    c = 0
-    if points is not None:
-        points = _req(points, "points", torch.float32, 3)
-        c = points.shape[2]
-    if c + 3 != stack.cin:
-        raise ValueError("feature channels (%d) do not match the stack's input width (%d)" % (c, stack.cin - 3))
-    _, m, ns = idx.shape
-    n3 = stack.nout[-1]
-    y = None
-    pf, ldf = 0, 0
-    if out_f32 is not None:
-        buf, off = out_f32
-        ldf, pf, y = buf.shape[-1], buf.data_ptr() + 4 * off, buf
-    elif out_split is None:
-        y = torch.empty((b, m, n3), dtype=torch.float32, device=xyz.device)
-        pf, ldf = y.data_ptr(), n3
-    ph = pl = lds = 0
-    if out_split is not None:
-        hb, lb, off = out_split
-        lds, ph, pl = hb.shape[-1], hb.data_ptr() + 2 * off, lb.data_ptr() + 2 * off
-    nout = (ctypes.c_int * len(stack.nout))(*stack.nout)
-    vp = ctypes.c_void_p
-    check(lib().ssd3d_sa_mlp_fused(b, n, c, m, ns, _p(xyz), _p(points), _p(new_xyz), _p(idx), _p(cnt), _p(units), len(stack.nout),
-                                   ctypes.cast(nout, vp), _p(stack.w_blob), _p(stack.ss_blob), 1 if stack.last_scale_nonneg else 0,
-                                   vp(pf), ldf, vp(ph), vp(pl), lds, _stream()), "sa_mlp_fused")
+    y, args = _sa_fused(xyz, points, None, new_xyz, idx, cnt, stack, out_f32, out_split, units)
+    check(lib().ssd3d_sa_mlp_fused(*args, _stream()), "sa_mlp_fused")
     return y
 
 
 def sa_mlp_fused_hoisted(xyz, z, zoff, wx, new_xyz, idx, cnt, stack, out_f32=None, out_split=None, units=None):
     """sa_mlp_fused with the scale's first conv hoisted into the per-point table z (see linear_tc_hoisted): `stack` is the
     params.FusedStack of the REMAINING convs (its input width == wx.shape[1]).  units: as sa_mlp_fused."""
-    _units_check(units, out_f32, out_split)
-    xyz = _req(xyz, "xyz", torch.float32, 3, 3)
-    new_xyz = _req(new_xyz, "new_xyz", torch.float32, 3, 3)
-    idx = _req(idx, "idx", torch.int32, 3)
-    z = _req(z, "z", torch.float32, 3)
-    wx = _req(wx, "wx", torch.float32, 2)
-    b, n, _ = xyz.shape
-    n1 = wx.shape[1]
-    if z.shape[:2] != (b, n) or wx.shape[0] != 3 or zoff < 0 or zoff + n1 > z.shape[2]:
-        raise ValueError("z must be (b, n, ldz) with zoff + n1 <= ldz and wx (3, n1)")
-    if n1 != stack.cin:
-        raise ValueError("hoisted width (%d) does not match the stack's input width (%d)" % (n1, stack.cin))
-    _, m, ns = idx.shape
-    n3 = stack.nout[-1]
-    y = None
-    pf, ldf = 0, 0
-    if out_f32 is not None:
-        buf, off = out_f32
-        ldf, pf, y = buf.shape[-1], buf.data_ptr() + 4 * off, buf
-    elif out_split is None:
-        y = torch.empty((b, m, n3), dtype=torch.float32, device=xyz.device)
-        pf, ldf = y.data_ptr(), n3
-    ph = pl = lds = 0
-    if out_split is not None:
-        hb, lb, off = out_split
-        lds, ph, pl = hb.shape[-1], hb.data_ptr() + 2 * off, lb.data_ptr() + 2 * off
-    nout = (ctypes.c_int * len(stack.nout))(*stack.nout)
-    vp = ctypes.c_void_p
-    check(lib().ssd3d_sa_mlp_fused_hoisted(b, n, n1, m, ns, _p(xyz), vp(z.data_ptr() + 4 * zoff), z.shape[2], _p(wx), _p(new_xyz),
-                                           _p(idx), _p(cnt), _p(units), len(stack.nout), ctypes.cast(nout, vp), _p(stack.w_blob),
-                                           _p(stack.ss_blob), 1 if stack.last_scale_nonneg else 0, vp(pf), ldf, vp(ph), vp(pl),
-                                           lds, _stream()), "sa_mlp_fused_hoisted")
+    y, args = _sa_fused(xyz, None, (z, zoff, wx), new_xyz, idx, cnt, stack, out_f32, out_split, units)
+    check(lib().ssd3d_sa_mlp_fused_hoisted(*args, _stream()), "sa_mlp_fused_hoisted")
     return y
 
 
@@ -794,9 +757,8 @@ def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
         block = torch.empty((b, int(max_output), 9), dtype=torch.float32, device=boxes.device)
         cnt = torch.empty((b,), dtype=torch.int32, device=boxes.device)
     else:
-        block, cnt = out
-        if (block.dtype != torch.float32 or tuple(block.shape) != (b, int(max_output), 9) or not block.is_contiguous()
-                or cnt.dtype != torch.int32 or tuple(cnt.shape) != (b,) or not cnt.is_contiguous()):
+        block, cnt = _req(out[0], "out block", torch.float32, 3, 9, copy=False), _req(out[1], "out count", torch.int32, 1, copy=False)
+        if tuple(block.shape) != (b, int(max_output), 9) or tuple(cnt.shape) != (b,):
             raise ValueError("out must be (float32 (b, max_output, 9), int32 (b,)) contiguous tensors")
     check(lib().ssd3d_bev_nms(b, n, _p(boxes), _p(scores), float(iou_threshold), int(max_output), int(cls_id),
                               _p(block), _p(cnt), _stream()), "bev_nms")
@@ -807,8 +769,7 @@ def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
 
 def fill_zero(t):
     """t[...] = 0 for a contiguous float32 CUDA tensor, as a kernel of this library."""
-    if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
-        raise ValueError("fill_zero takes a contiguous float32 CUDA tensor")
+    t = _req(t, "t", torch.float32, copy=False)
     check(lib().ssd3d_fill_zero(_p(t), t.numel(), _stream()), "fill_zero")
     return t
 
@@ -819,8 +780,7 @@ def peer_allgather(send, peers, world, rank, slice_bytes, recv_off, flag_off, st
     process; state: int32 [>= 3] zero-initialised, owned by this exchange (state[2] counts waits that timed out); out: uint8
     [world * slice_bytes]."""
     for name, t, dt in (("send", send, torch.uint8), ("peers", peers, torch.int64), ("state", state, torch.int32), ("out", out, torch.uint8)):
-        if t.dtype != dt or not t.is_cuda or not t.is_contiguous():
-            raise ValueError("%s must be a contiguous CUDA tensor of %s" % (name, dt))
+        _req(t, name, dt, copy=False)
     if send.numel() < slice_bytes or out.numel() < world * slice_bytes or peers.numel() < world or state.numel() < 3:
         raise ValueError("peer_allgather: buffers smaller than world=%d slices of %d bytes" % (world, slice_bytes))
     check(lib().ssd3d_peer_allgather(_p(send), int(slice_bytes), _p(peers), int(world), int(rank), int(recv_off[0]), int(recv_off[1]),
@@ -911,21 +871,16 @@ def concat_rows(parts):
 
 # ---- training-mode BatchNorm (SURVEY.md 8f row f3) -----------------------------------------------------------------
 
-BN_EPS = 1e-3   # tf.contrib.layers.batch_norm default epsilon
-
-
 def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=True, eps=BN_EPS):
     """Batch-statistics BatchNorm + activation over the last axis of x (tf_util.py:424-444, is_training=True);
     moving_mean / moving_var (float32 CUDA tensors [c]) are updated IN PLACE like updates_collections=None does.
     Returns (y, scale, shift, batch_mean, batch_var); (scale, shift) is the folded per-channel form."""
-    if x.dtype != torch.float32 or not x.is_cuda:
-        raise ValueError("x must be a float32 CUDA tensor")
-    x = x if x.is_contiguous() else x.contiguous()
+    x = _req(x, "x", torch.float32)
     c = x.shape[-1]
     rows = x.numel() // c
     for t, name in ((gamma, "gamma"), (beta, "beta"), (moving_mean, "moving_mean"), (moving_var, "moving_var")):
-        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or tuple(t.shape) != (c,) or not t.is_contiguous()):
-            raise ValueError("%s must be a contiguous float32 CUDA tensor of shape (%d,)" % (name, c))
+        if t is not None:
+            _vec(t, name, c)
     if (moving_mean is None) != (moving_var is None):
         raise ValueError("moving_mean and moving_var go together")
     dev = x.device
@@ -940,12 +895,11 @@ def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=
 
 def rowgroup_max(y, pool, rowmask=None):
     """tf.reduce_max over runs of `pool` rows times (rowmask != 0) (layers_util.py:178-180): y (..., pool, c) -> (..., c)."""
-    if y.dtype != torch.float32 or not y.is_cuda:
-        raise ValueError("y must be a float32 CUDA tensor")
-    y = y if y.is_contiguous() else y.contiguous()
+    y = _req(y, "y", torch.float32)
     c, pool = y.shape[-1], int(pool)
     if y.shape[-2] != pool:
         raise ValueError("pool must equal the second-to-last dimension")
+    rowmask = _rowmask(rowmask, y.numel() // (c * pool))
     out = torch.empty(tuple(y.shape[:-2]) + (c,), dtype=torch.float32, device=y.device)
     check(lib().ssd3d_rowgroup_max(y.numel() // (c * pool), pool, c, _p(y), c, _p(rowmask), _p(out), _stream()), "rowgroup_max")
     return out
@@ -953,16 +907,10 @@ def rowgroup_max(y, pool, rowmask=None):
 
 # ---- backward of the training-mode layers (DESIGN.md "Backward") ---------------------------------------------------
 
-def _f32(t, name):
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
-        raise ValueError("%s must be a float32 CUDA tensor" % name)
-    return t if t.is_contiguous() else t.contiguous()
-
-
 def linear_wgrad(x, dz, want_bias=True):
     """Weight gradient of a 1x1 conv: x (..., cin), dz (..., cout) -> grad_w (cin, cout) = x^T dz over all rows and
     grad_b (cout,) = column sums of dz (None unless want_bias).  Tensor cores, fixed-order split-K: same bits every run."""
-    x, dz = _f32(x, "x"), _f32(dz, "dz")
+    x, dz = _req(x, "x", torch.float32), _req(dz, "dz", torch.float32)
     cin, cout = x.shape[-1], dz.shape[-1]
     rows = x.numel() // cin if cin else 0
     if cin == 0 or cout == 0 or dz.numel() // cout != rows or rows == 0:
@@ -979,14 +927,13 @@ def linear_wgrad(x, dz, want_bias=True):
 def bn_train_grad(x, grad_out, scale, shift, batch_mean, batch_var, gamma, relu=True, eps=BN_EPS):
     """Backward of bn_train (+ ReLU) from its input x (the pre-BN conv output) and its outputs (scale, shift, batch_mean,
     batch_var) -> (grad_x, grad_gamma, grad_beta).  The moving statistics are not touched."""
-    x, grad_out = _f32(x, "x"), _f32(grad_out, "grad_out")
+    x, grad_out = _req(x, "x", torch.float32), _req(grad_out, "grad_out", torch.float32)
     if grad_out.shape != x.shape:
         raise ValueError("bn_train_grad: grad_out %s must have the shape of x %s" % (tuple(grad_out.shape), tuple(x.shape)))
     c = x.shape[-1]
     rows = x.numel() // c
     for t, name in ((scale, "scale"), (shift, "shift"), (batch_mean, "batch_mean"), (batch_var, "batch_var"), (gamma, "gamma")):
-        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or tuple(t.shape) != (c,) or not t.is_contiguous():
-            raise ValueError("%s must be a contiguous float32 CUDA tensor of shape (%d,)" % (name, c))
+        _vec(t, name, c)
     dev = x.device
     gx = torch.empty_like(x)
     gg, gbeta = (torch.empty((c,), dtype=torch.float32, device=dev) for _ in range(2))
@@ -1000,15 +947,12 @@ def bn_train_grad(x, grad_out, scale, shift, batch_mean, batch_var, gamma, relu=
 def rowgroup_max_grad(y, grad_out, pool, rowmask=None):
     """Backward of rowgroup_max: y (..., pool, c), grad_out (..., c) -> grad_y (..., pool, c); the gradient of a group is
     split evenly among its tied maxima and multiplied by (rowmask != 0)."""
-    y, grad_out = _f32(y, "y"), _f32(grad_out, "grad_out")
+    y, grad_out = _req(y, "y", torch.float32), _req(grad_out, "grad_out", torch.float32)
     c, pool = y.shape[-1], int(pool)
     if y.dim() < 2 or y.shape[-2] != pool or tuple(grad_out.shape) != tuple(y.shape[:-2]) + (c,):
         raise ValueError("rowgroup_max_grad: y must be (..., pool, c) and grad_out (..., c)")
     groups = grad_out.numel() // c
-    if rowmask is not None:
-        rowmask = _req(rowmask, "rowmask", torch.int32, rowmask.dim())
-        if rowmask.numel() != groups:
-            raise ValueError("rowmask must hold one entry per group")
+    rowmask = _rowmask(rowmask, groups)
     gy = torch.empty_like(y)
     check(lib().ssd3d_rowgroup_max_grad(groups, pool, c, _p(y), c, _p(rowmask), _p(grad_out), _p(gy), c, _stream()),
           "rowgroup_max_grad")
@@ -1045,11 +989,6 @@ def vote_translate_grad(offsets, grad_out, min_range):
     return g
 
 
-def _folded(w, scale, shift):
-    from .params import FoldedConv
-    return FoldedConv(w, scale, shift)
-
-
 def linear_bn_train(x, f, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9):
     """Forward of one training-mode layer: split_rows -> linear_tc with the BN-less fold f (params.FoldedConv with
     scale = 1, shift = bias) -> bn_train (bn=True: batch statistics, moving statistics updated in place) -> ReLU.
@@ -1072,7 +1011,7 @@ class _ConvTrain(torch.autograd.Function):
         bn, relu, decay, moving, debug = opts
         x = x if x.is_contiguous() else x.contiguous()
         ones = torch.ones((w.shape[1],), dtype=torch.float32, device=x.device)
-        y, r = linear_bn_train(x, _folded(w.detach(), ones, b.detach()), gamma.detach(), beta.detach(), moving[0], moving[1],
+        y, r = linear_bn_train(x, FoldedConv(w.detach(), ones, b.detach()), gamma.detach(), beta.detach(), moving[0], moving[1],
                                bn=bn, relu=relu, decay=decay)
         out = r[0]
         ctx.bn, ctx.relu = bn, relu
@@ -1100,7 +1039,7 @@ class _ConvTrain(torch.autograd.Function):
         gx = None
         if ctx.needs_input_grad[0]:
             d_hi, d_lo = split_rows(dz)
-            wt = _folded(w.detach().t().contiguous(), torch.ones((cin,), dtype=torch.float32, device=dz.device),
+            wt = FoldedConv(w.detach().t().contiguous(), torch.ones((cin,), dtype=torch.float32, device=dz.device),
                          torch.zeros((cin,), dtype=torch.float32, device=dz.device))
             gx, _ = linear_tc(d_hi, d_lo, wt, relu=False, want_f32=True, want_split=False)
         gw, gb = linear_wgrad(x, dz, want_bias=True)
@@ -1211,8 +1150,7 @@ def det_assign(base_xyz, vote_base, gt_boxes, gt_labels, angle_bins=12):
 def _rows(t, name, b, n, width):
     """(b, n, [1,] width) float32 CUDA tensor, read in place when its last axis is dense and its rows evenly strided (a
     column block of a wider tensor, e.g. the head's [b, n, 1, 30] regression output) -> (tensor, row stride in floats)."""
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
-        raise ValueError("%s must be a float32 CUDA tensor" % name)
+    t = _req(t, name, torch.float32, copy=None)
     if t.dim() < 3 or tuple(t.shape[:2]) != (b, n) or t.shape[-1] != width or any(s != 1 for s in t.shape[2:-1]):
         raise ValueError("%s must be (%d, %d, [1,] %d), got %s" % (name, b, n, width, tuple(t.shape)))
     ld = t.stride(1)
