@@ -14,9 +14,9 @@
 //
 // Kernel shape: 640 threads = 5 warpgroups; warp 0 = TMA producer (warps 1-3 idle), warps 4-11 = operand producers of
 // the gather modes, warps 12-19 = two consumer warpgroups.  Consumer warpgroup g owns rows 64g..64g+63 of the tile: it
-// issues the wgmma chain into its registers, stages the fp32 accumulator in shared memory (row-per-thread order), then
-// runs the epilogue (scale/shift/ReLU -> fp32 / split-bf16 through TMA tensor stores, or max-pool as a shuffle
-// reduce-and-transpose butterfly; two warps per 32-row quarter share the 32-column chunks).
+// issues the wgmma chain into its registers and runs the epilogue on the accumulator fragments where they are
+// (scale/shift/ReLU in place -> fp32 / split-bf16 through per-warp TMA tensor stores, or max-pool as a shuffle
+// reduce-and-transpose butterfly over the fragment rows; only pools of 32-128 rows meet other warps, in a 2 KiB exchange).
 // Tile 128 rows x BN<=64 columns (BN = 32 or 64, a template parameter: the wgmma width is part of the
 // instruction), K streamed in 64-element blocks through a multi-stage mbarrier ring; a stage is released as soon as
 // the wgmma group that read it has retired, so the TMA loads of the next k-blocks overlap the MMAs.
@@ -26,14 +26,13 @@
 // Unit-list mode (TcParams::units, round 2): the grouped matrix holds only the 8-row units the ball query listed (rows
 // that repeat a group's first neighbour cannot change the max-pool); the row count comes from the list at run time, the
 // gather producers look their source up through it, and the last conv of a scale pools each unit and combines the units
-// of a group with atomicMax (pooled_units_chunk).  Same bits as the dense schedule.
+// of a group with atomicMax (the unit_pool branch of the epilogue).  Same bits as the dense schedule.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdio>
 #include <cstring>
 
 #include "common.cuh"
-#include "pool.cuh"
 #include "wgmma.cuh"
 
 namespace ssd3d {
@@ -45,12 +44,19 @@ constexpr int TC_PROD_WARPS = 8;          // builds 4 of the 8 16-byte chunks of
 constexpr int TC_EPI_WARP0 = TC_PROD_WARP0 + TC_PROD_WARPS;   // warps 12..19: the two consumer warpgroups (MMA + epilogue)
 constexpr int TC_EPI_WARPS = 8;
 constexpr int TC_THREADS = (TC_EPI_WARP0 + TC_EPI_WARPS) * 32;
-// 640 threads leave 96 registers per thread: at BN = 64 the consumer already spills 68 bytes (stores) / 76 bytes (loads)
-// per thread to local memory, at BN = 128 about 1 KB, so tiles stop at 64 columns.
+// 640 threads leave 96 registers per thread: at BN = 64 the consumer's 32 accumulator registers and the fragment epilogue
+// fit without spills, a BN = 128 accumulator would not, so tiles stop at 64 columns.
 constexpr int TC_MAX_BN = 64;
 constexpr int TC_MAX_STAGES = 4;
 constexpr int TC_MAX_AKB = 4;            // A-stationary mode: k-blocks of an m-tile resident at once (K <= 256)
 constexpr uint32_t TC_A_BYTES = TC_BM * TC_BK * 2;   // one A tile (hi or lo): 16 KiB
+// Shared memory per CTA: the planner hands out at most TC_DYN_SMEM of dynamic shared memory (1 KiB of it is the
+// alignment slack of the carve); the kernel's static __shared__ (mbarriers + pool_xs, allocated in 1 KiB granules) takes
+// the rest of the 227 KiB opt-in limit.  At BN = 64 that is 3 KiB, so the limit is met exactly: anything added to the
+// static footprint must come out of TC_DYN_SMEM.
+constexpr size_t TC_DYN_SMEM = 224 * 1024;
+constexpr size_t TC_STATIC_SMEM = (2 * TC_MAX_STAGES + 4 * TC_MAX_AKB) * 8 + TC_EPI_WARPS * TC_MAX_BN * sizeof(float);
+static_assert(TC_DYN_SMEM + (TC_STATIC_SMEM + 1023) / 1024 * 1024 <= 227 * 1024, "linear_tc: shared memory over the opt-in limit");
 
 struct TcParams {
     long rows;
@@ -109,16 +115,6 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ---- epilogue helpers ---------------------------------------------------------------------------------------
-// order-preserving float <-> uint map (so that an unsigned redux.max is a float max, also for negative values)
-__device__ __forceinline__ uint32_t f2ord(float x)
-{
-    const uint32_t b = __float_as_uint(x);
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float ord2f(uint32_t u)
-{
-    return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
 __device__ __forceinline__ void split_pair(float x0, float x1, uint32_t &hw, uint32_t &lw)
 {
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hw) : "f"(x1), "f"(x0));       // {x1 : x0} like two adjacent bf16
@@ -126,55 +122,61 @@ __device__ __forceinline__ void split_pair(float x0, float x1, uint32_t &hw, uin
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lw) : "f"(x1 - h1), "f"(x0 - h0));
 }
 
-// Max-pool of one 32-column chunk over runs of POOL rows (tf.reduce_max(axis=2), layers_util.py:178) + mask (:180).
-// A thread holds one row; the rows of a group are lanes of a warp (POOL <= 32) or of 2-4 warps (64, 128).
-template <int POOL>
-__device__ __forceinline__ void pooled_chunk(const TcParams &p, float (&v)[32], int lane, int q, int h, int mt,
-                                             int col0, float *xs /* [2 halves][4 quarters][32] */)
+// ---- epilogue on the accumulator fragment ---------------------------------------------------------------------
+// Thread t of warp w (of its warpgroup) holds tile rows 64g + 16w + t/4 in d[4j], d[4j+1] and the row 8 below in
+// d[4j+2], d[4j+3], columns 8j + 2(t%4) + {0, 1} (wgmma.cuh).  The max-pools reduce these fragments where they are.
+//
+// Reduce-and-transpose over the 8 lanes of a column quad (lane bits 2-4, i.e. the 8 rows t/4 of a fragment half): on
+// return lane t owns, in v[i], the maximum of value slot i + (N/8)(t/4) over those 8 lanes.  3 steps, N - N/8 shuffles.
+// (Each step is its own fully unrolled loop: any index the compiler cannot resolve would move the accumulator fragment
+// to local memory for the whole kernel.)
+template <int HALF, int O, int N>
+__device__ __forceinline__ void quad_rowmax_step(float (&v)[N], int lane)
 {
-    constexpr int GP = POOL >= 32 ? 32 : POOL;       // lanes per group inside a warp
-    constexpr int KEEP = 32 / GP;                    // columns a lane ends up owning
-    warp_colmax_transpose<GP>(v, lane);              // lane owns columns (lane % GP) * KEEP + k in v[k]
-    if (POOL > 32) {                                 // combine the 2 (4) warps that share a group
-        constexpr int WPG = POOL > 32 ? POOL / 32 : 1;
-        xs[(h * 4 + q) * 32 + lane] = v[0];
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + h) : "memory");      // the 4 quarter-warps of this column half
-        if ((q % WPG) == 0) {
+    const bool up = (lane & O) != 0;
 #pragma unroll
-            for (int w = 1; w < WPG; w++) v[0] = fmaxf(v[0], xs[(h * 4 + q + w) * 32 + lane]);
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + h) : "memory");      // xs reusable by the next chunk
-        if ((q % WPG) != 0) return;
-    }
-    const long gg = (long)mt * (TC_BM / POOL) + (q * 32 + lane) / POOL;
-    if (gg * POOL >= p.rows) return;
-    const bool masked = p.rowmask && p.rowmask[gg] == 0;
-#pragma unroll
-    for (int k = 0; k < KEEP; k++) {
-        const int col = col0 + (lane % GP) * KEEP + k;
-        if (col >= p.n) continue;
-        const float mx = masked ? 0.0f : v[k];
-        if (p.out_f32) p.out_f32[(size_t)gg * p.ld_f32 + col] = mx;
-        if (p.out_hi) {
-            const __nv_bfloat16 hb = __float2bfloat16_rn(mx);
-            p.out_hi[(size_t)gg * p.ld_split + col] = hb;
-            p.out_lo[(size_t)gg * p.ld_split + col] = __float2bfloat16_rn(mx - __bfloat162float(hb));
-        }
+    for (int i = 0; i < HALF; i++) {
+        const float send = up ? v[i] : v[i + HALF];
+        const float keep = up ? v[i + HALF] : v[i];
+        v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, O));
     }
 }
-
-// Unit-list twin of pooled_chunk<8>: lanes 8u' .. 8u'+7 of a warp hold one unit; its column maxima go to the unit's GROUP row.
-__device__ __forceinline__ void pooled_units_chunk(const TcParams &p, float (&v)[32], int lane, int q, int mt, int col0, int nunits)
+template <int N>
+__device__ __forceinline__ void quad_rowmax_transpose(float (&v)[N], int lane)
 {
-    warp_colmax_transpose<8>(v, lane);               // lane owns columns (lane % 8) * 4 + k of its unit in v[k]
-    const int ui = mt * (TC_BM / 8) + ((q * 32 + lane) >> 3);
-    if (ui >= nunits) return;
-    const int group = __ldg(p.units + 1 + ui) >> 4;
+    quad_rowmax_step<N / 2, 16>(v, lane);
+    quad_rowmax_step<N / 4, 8>(v, lane);
+    quad_rowmax_step<N / 8, 4>(v, lane);
+}
+
+// 8-row max-pool of a warp's fragment (dense pool == 8 or the unit-list pool): the two 8-row halves stay apart.  On return
+// lane t owns slots s = i + (BN/16)(t/4), i < BN/16, of d: column 8(s/4) + 2(t%4) + (s%2) of row half (s/2)%2.
+template <int BN>
+__device__ __forceinline__ void frag_pool8(float (&d)[BN / 2], int lane) { quad_rowmax_transpose<BN / 2>(d, lane); }
+
+// 16-row max-pool of a warp's fragment: halves combined first, then the quad butterfly.  On return u[i], i < BN/32, holds
+// column 8(s/2) + 2(t%4) + (s%2), s = i + (BN/32)(t/4), over the warp's 16 rows.
+template <int BN>
+__device__ __forceinline__ void frag_pool16(const float (&d)[BN / 2], float (&u)[BN / 4], int lane)
+{
 #pragma unroll
-    for (int k = 0; k < 4; k++) {
-        const int col = col0 + (lane & 7) * 4 + k;
-        if (col >= p.n) continue;
-        atomicMax(reinterpret_cast<unsigned int *>(p.out_f32 + (size_t)group * p.ld_f32 + col), __float_as_uint(v[k]) & 0x7fffffffu);
+    for (int j = 0; j < BN / 8; j++) {
+        u[2 * j] = fmaxf(d[4 * j], d[4 * j + 2]);
+        u[2 * j + 1] = fmaxf(d[4 * j + 1], d[4 * j + 3]);
+    }
+    quad_rowmax_transpose<BN / 4>(u, lane);
+}
+
+// pooled row gg (group of POOL rows) of columns `col`: mask (layers_util.py:180), fp32 and / or split bf16 outputs
+__device__ __forceinline__ void store_pooled(const TcParams &p, long gg, int col, float mx)
+{
+    if (col >= p.n) return;
+    if (p.rowmask && p.rowmask[gg] == 0) mx = 0.0f;
+    if (p.out_f32) p.out_f32[(size_t)gg * p.ld_f32 + col] = mx;
+    if (p.out_hi) {
+        const __nv_bfloat16 hb = __float2bfloat16_rn(mx);
+        p.out_hi[(size_t)gg * p.ld_split + col] = hb;
+        p.out_lo[(size_t)gg * p.ld_split + col] = __float2bfloat16_rn(mx - __bfloat162float(hb));
     }
 }
 
@@ -190,11 +192,6 @@ __device__ long long tc_prof[16];
 #define TCP(i) do { } while (0)
 #endif
 
-// Accumulator staging of one consumer warpgroup: 64 rows x (BN + 4) fp32 (the pad keeps both the fragment writes
-// and the row-per-thread float4 reads free of bank conflicts)
-template <int BN> __host__ __device__ constexpr int tc_acc_pitch() { return BN + 4; }
-static size_t tc_acc_bytes(int bn) { return (size_t)TC_BM * (bn + 4) * sizeof(float); }
-
 // ---------------------------------------------------------------------------------------------------------
 template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -204,8 +201,8 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                  const __grid_constant__ CUtensorMap map_of32, const TcParams p)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [resident A tiles] [stages] x { A_hi | A_lo | B_hi | B_lo }, per-warp output blocks (4 KiB each),
-    // accumulator staging, then scale/shift
+    // carve: [resident A tiles] [stages] x { A_hi | A_lo | B_hi | B_lo }, per-warp output blocks (4 KiB each), then
+    // scale/shift
     const uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;
     const int nkb = (p.kp + TC_BK - 1) / TC_BK;
     const uint32_t a_tile = (uint32_t)nkb * 2u * TC_A_BYTES;                        // one resident A tile: [nkb] x { A_hi | A_lo }
@@ -218,14 +215,13 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
     const int ncov = p.n_tiles * p.bn + 32;
     uint8_t *ring = smem + a_region;
     uint8_t *out_stage = ring + (size_t)p.stages * stage_bytes;          // [8 warps][4 KiB], 4 KiB aligned
-    float *s_acc = reinterpret_cast<float *>(out_stage + (p.tma_store ? TC_EPI_WARPS * 4096 : 0));   // [2 wg][64][BN+4]
-    float *s_scale = s_acc + TC_BM * tc_acc_pitch<BN>();
+    float *s_scale = reinterpret_cast<float *>(out_stage + (p.tma_store ? TC_EPI_WARPS * 4096 : 0));
     float *s_shift = s_scale + ncov;
     float *s_wx = s_shift + ncov;                                        // [3][kp] (hoisted mode only)
 
     __shared__ unsigned long long full_bar[TC_MAX_STAGES], empty_bar[TC_MAX_STAGES];
     __shared__ unsigned long long afull_bar[2 * TC_MAX_AKB], aempty_bar[2 * TC_MAX_AKB];   // [A buffer][k-block]
-    __shared__ float pool_xs[2 * 4 * 32];
+    __shared__ __align__(16) float pool_xs[TC_EPI_WARPS * BN];          // 32-128-row pools: per-warp 16-row maxima (TC_STATIC_SMEM)
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // provably warp-uniform
     // unit-list mode: the row count comes from the list (written earlier on this stream), p.rows is the buffers' capacity
@@ -389,15 +385,11 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
         }
     } else if (warp >= TC_EPI_WARP0) {
         // ===== consumers: warpgroup g = rows 64g..64g+63 of the tile.  MMAs: the whole warpgroup issues the wgmma chain
-        // of every k-block into its registers.  Epilogue: warp w of the group handles the 32-row quarter q = 2g + (w & 1)
-        // and the 32-column chunks of parity h = w >> 1, one row per thread, from the staged accumulator.
-        constexpr int PITCH = tc_acc_pitch<BN>();
-        const int g = (warp - TC_EPI_WARP0) >> 2, w = warp & 3;
-        const int q = 2 * g + (w & 1);
-        const int h = w >> 1;
-        const int wg_bar = 4 + g;                                        // named barrier of this warpgroup (2, 3: pooling)
-        float *acc_g = s_acc + g * 64 * PITCH;
-        constexpr int nchunks = BN / 32;
+        // of every k-block into its registers.  Epilogue: each warp works on its own fragment (16 rows x BN columns, see
+        // quad_rowmax_transpose) in registers; only the 32-128-row pools meet other warps, through pool_xs.
+        const int g = (warp - TC_EPI_WARP0) >> 2;
+        const int we = warp - TC_EPI_WARP0;                              // consumer warp 0..7 = 16-row slab of the tile
+        const int cq = 2 * (lane & 3);                                   // this thread's column pair inside each 8 columns
         int it = 0, mi = 0, mt, nt;
         TCP_DECL;
         for (int i = 0; tile_at(i, mt, nt); i++) {
@@ -438,110 +430,145 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
             release(prev_s, prev_kb);
             if (last_nt) mi++;
             if (warp == TC_EPI_WARP0) TCP(8);
-            // stage the accumulator: fragment rows 16w + lane/4 (+8), columns 8j + 2(lane%4)
-            named_bar_sync(wg_bar, 128);                                 // the previous tile's epilogue has read the buffer
-            {
-                const int r0 = w * 16 + (lane >> 2), c = 2 * (lane & 3);
+            // epilogue on the fragment: folded bias/BN scale/shift, ReLU, then store or pool
+            const int col_t = nt * p.bn;
 #pragma unroll
-                for (int j = 0; j < BN / 8; j++) {
-                    *reinterpret_cast<float2 *>(acc_g + r0 * PITCH + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
-                    *reinterpret_cast<float2 *>(acc_g + (r0 + 8) * PITCH + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
-                }
+            for (int j = 0; j < BN / 8; j++) {
+                const float2 sc = *reinterpret_cast<const float2 *>(s_scale + col_t + 8 * j + cq);
+                const float2 sh = *reinterpret_cast<const float2 *>(s_shift + col_t + 8 * j + cq);
+                d[4 * j] = fmaf(d[4 * j], sc.x, sh.x);
+                d[4 * j + 1] = fmaf(d[4 * j + 1], sc.y, sh.y);
+                d[4 * j + 2] = fmaf(d[4 * j + 2], sc.x, sh.x);
+                d[4 * j + 3] = fmaf(d[4 * j + 3], sc.y, sh.y);
             }
-            named_bar_sync(wg_bar, 128);
-            const long row = (long)mt * TC_BM + q * 32 + lane;
-            const bool row_ok = row < rows;
-            const float *acc_row = acc_g + ((w & 1) * 32 + lane) * PITCH;
-            for (int ci = h; ci < nchunks; ci += 2) {
-                const int c0 = ci * 32;
-                const int col0 = nt * p.bn + c0;
-                float v[32];
+            if (p.relu) {
 #pragma unroll
-                for (int j4 = 0; j4 < 32; j4 += 4) {
-                    const float4 a4 = *reinterpret_cast<const float4 *>(acc_row + c0 + j4);
-                    const float4 sc = *reinterpret_cast<const float4 *>(s_scale + col0 + j4);
-                    const float4 sh = *reinterpret_cast<const float4 *>(s_shift + col0 + j4);
-                    v[j4 + 0] = fmaf(a4.x, sc.x, sh.x);
-                    v[j4 + 1] = fmaf(a4.y, sc.y, sh.y);
-                    v[j4 + 2] = fmaf(a4.z, sc.z, sh.z);
-                    v[j4 + 3] = fmaf(a4.w, sc.w, sh.w);
-                }
-                if (p.relu) {
+                for (int j = 0; j < BN / 2; j++) d[j] = fmaxf(d[j], 0.0f);
+            }
+            const int row0 = mt * TC_BM + 16 * we;                       // first row of this warp's fragment
+            const int rq = lane >> 2;                                    // fragment row of d[4j], d[4j+1]; +8 for the others
+            if (p.pool <= 1 && p.tma_store) {
+                // Each warp owns a 4 KiB block: its [16 rows x 32 columns] pieces are laid out in the TMA swizzle and one
+                // bulk tensor store per piece writes whole 64/128-byte row segments (rows / columns beyond the tensor are
+                // clipped by the hardware); the block is reused once the previous stores have read it.
+                uint8_t *blk = out_stage + we * 4096;
+                if (lane == 0) tma_store_wait_read();
+                __syncwarp();
 #pragma unroll
-                    for (int j = 0; j < 32; j++) v[j] = fmaxf(v[j], 0.0f);
-                }
-                if (p.pool <= 1 && p.tma_store) {
-                    // Each warp owns a [32 rows x 32 columns] block: stage it in shared memory in the TMA swizzle and
-                    // let one bulk tensor store write whole 64/128-byte row segments (rows / columns beyond the tensor
-                    // are clipped by the hardware); the block is reused once the previous store has read it.
-                    uint8_t *blk = out_stage + (warp - TC_EPI_WARP0) * 4096;
-                    if (lane == 0) tma_store_wait_read();
-                    __syncwarp();
-                    const int row0 = mt * TC_BM + q * 32;
-                    if (p.out_f32) {                                   // 128-byte rows, SWIZZLE_128B
+                for (int c32 = 0; c32 < BN / 32; c32++) {
+                    uint8_t *piece = blk + c32 * 2048;
+                    if (p.out_f32) {                                     // 128-byte rows, SWIZZLE_128B: 2 KiB
 #pragma unroll
-                        for (int c = 0; c < 8; c++)
-                            *reinterpret_cast<float4 *>(blk + lane * 128 + ((c ^ (lane & 7)) << 4)) =
-                                make_float4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-                        fence_async_smem();
-                        __syncwarp();
-                        if (lane == 0) { tma_store_2d(&map_of32, smem_u32(blk), col0, row0); tma_store_commit(); }
-                    } else {                                           // two 64-byte-row blocks (hi, lo), SWIZZLE_64B
-#pragma unroll
-                        for (int c = 0; c < 4; c++) {
-                            uint32_t hw[4], lw[4];
-#pragma unroll
-                            for (int t = 0; t < 4; t++) split_pair(v[8 * c + 2 * t], v[8 * c + 2 * t + 1], hw[t], lw[t]);
-                            const uint32_t off = (uint32_t)lane * 64u + (uint32_t)((c ^ ((lane >> 1) & 3)) << 4);
-                            *reinterpret_cast<uint4 *>(blk + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                            *reinterpret_cast<uint4 *>(blk + 2048 + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                        for (int jj = 0; jj < 4; jj++) {
+                            const int j = 4 * c32 + jj;
+                            const uint32_t off = (uint32_t)rq * 128u + (uint32_t)(((2 * jj + (cq >> 2)) ^ rq) << 4) + (uint32_t)(cq & 2) * 4u;
+                            *reinterpret_cast<float2 *>(piece + off) = make_float2(d[4 * j], d[4 * j + 1]);
+                            *reinterpret_cast<float2 *>(piece + 1024 + off) = make_float2(d[4 * j + 2], d[4 * j + 3]);
                         }
-                        fence_async_smem();
-                        __syncwarp();
-                        if (lane == 0) {
-                            tma_store_2d(&map_ohi, smem_u32(blk), col0, row0);
-                            tma_store_2d(&map_olo, smem_u32(blk + 2048), col0, row0);
-                            tma_store_commit();
+                    } else {                                             // 64-byte rows (hi | lo), SWIZZLE_64B: 1 KiB each
+#pragma unroll
+                        for (int jj = 0; jj < 4; jj++) {
+                            const int j = 4 * c32 + jj;
+                            const uint32_t off = (uint32_t)rq * 64u + (uint32_t)((jj ^ ((rq >> 1) & 3)) << 4) + (uint32_t)cq * 2u;
+                            uint32_t hw, lw;
+                            split_pair(d[4 * j], d[4 * j + 1], hw, lw);
+                            *reinterpret_cast<uint32_t *>(piece + off) = hw;
+                            *reinterpret_cast<uint32_t *>(piece + 1024 + off) = lw;
+                            split_pair(d[4 * j + 2], d[4 * j + 3], hw, lw);
+                            *reinterpret_cast<uint32_t *>(piece + 512 + off) = hw;
+                            *reinterpret_cast<uint32_t *>(piece + 1536 + off) = lw;
                         }
                     }
-                } else if (p.pool <= 1) {
-                    if (row_ok) {
+                }
+                fence_async_smem();
+                __syncwarp();
+                if (lane == 0) {
+#pragma unroll
+                    for (int c32 = 0; c32 < BN / 32; c32++) {
+                        const uint32_t piece = smem_u32(blk + c32 * 2048);
                         if (p.out_f32) {
-                            float *dst = p.out_f32 + (size_t)row * p.ld_f32 + col0;
-                            if (col0 + 32 <= p.n && ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0)) {
-#pragma unroll
-                                for (int j4 = 0; j4 < 32; j4 += 4)
-                                    *reinterpret_cast<float4 *>(dst + j4) = make_float4(v[j4], v[j4 + 1], v[j4 + 2], v[j4 + 3]);
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 32; j++)
-                                    if (col0 + j < p.n) dst[j] = v[j];
-                            }
+                            tma_store_2d(&map_of32, piece, col_t + 32 * c32, row0);
+                        } else {
+                            tma_store_2d(&map_ohi, piece, col_t + 32 * c32, row0);
+                            tma_store_2d(&map_olo, piece + 1024, col_t + 32 * c32, row0);
                         }
-                        if (p.out_hi) {
-                            // x = hi + lo (bf16 each); columns n..ld_split-1 come out as exact zeros (next layer's K padding)
-                            __nv_bfloat16 *dh = p.out_hi + (size_t)row * p.ld_split + col0;
-                            __nv_bfloat16 *dl = p.out_lo + (size_t)row * p.ld_split + col0;
+                    }
+                    tma_store_commit();
+                }
+            } else if (p.pool <= 1) {
 #pragma unroll
-                            for (int j8 = 0; j8 < 32; j8 += 8) {
-                                if (col0 + j8 >= p.ld_split) break;
-                                uint32_t hw[4], lw[4];
+                for (int hf = 0; hf < 2; hf++) {
+                    const long row = (long)row0 + rq + 8 * hf;
+                    if (row >= rows) continue;
 #pragma unroll
-                                for (int t = 0; t < 4; t++) split_pair(v[j8 + 2 * t], v[j8 + 2 * t + 1], hw[t], lw[t]);
-                                *reinterpret_cast<uint4 *>(dh + j8) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                                *reinterpret_cast<uint4 *>(dl + j8) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                    for (int j = 0; j < BN / 8; j++) {
+                        const int col = col_t + 8 * j + cq;
+                        const float x0 = d[4 * j + 2 * hf], x1 = d[4 * j + 2 * hf + 1];
+                        if (p.out_f32) {
+                            float *dst = p.out_f32 + (size_t)row * p.ld_f32 + col;
+                            if (col < p.n) dst[0] = x0;
+                            if (col + 1 < p.n) dst[1] = x1;
+                        }
+                        // x = hi + lo (bf16 each); columns n..ld_split-1 come out as exact zeros (next layer's K padding)
+                        if (p.out_hi && col < p.ld_split) {
+                            uint32_t hw, lw;
+                            split_pair(x0, x1, hw, lw);
+                            *reinterpret_cast<uint32_t *>(p.out_hi + (size_t)row * p.ld_split + col) = hw;
+                            *reinterpret_cast<uint32_t *>(p.out_lo + (size_t)row * p.ld_split + col) = lw;
+                        }
+                    }
+                }
+            } else if (p.unit_pool) {
+                // each 8-row fragment half is one listed unit; its column maxima go to the unit's GROUP row by atomicMax
+                frag_pool8<BN>(d, lane);
+#pragma unroll
+                for (int i = 0; i < BN / 16; i++) {
+                    const int s = i + (BN / 16) * rq;
+                    const int ui = mt * (TC_BM / 8) + 2 * we + ((s >> 1) & 1);
+                    const int col = col_t + 8 * (s >> 2) + cq + (s & 1);
+                    if (ui >= nunits || col >= p.n) continue;
+                    const int group = __ldg(p.units + 1 + ui) >> 4;
+                    atomicMax(reinterpret_cast<unsigned int *>(p.out_f32 + (size_t)group * p.ld_f32 + col), __float_as_uint(d[i]) & 0x7fffffffu);
+                }
+            } else if (p.pool == 8) {
+                frag_pool8<BN>(d, lane);
+#pragma unroll
+                for (int i = 0; i < BN / 16; i++) {
+                    const int s = i + (BN / 16) * rq;
+                    const long gg = (long)mt * (TC_BM / 8) + 2 * we + ((s >> 1) & 1);
+                    if (gg * 8 < p.rows) store_pooled(p, gg, col_t + 8 * (s >> 2) + cq + (s & 1), d[i]);
+                }
+            } else {
+                // pools of 16-128 rows: 16-row maxima per warp, then (32-128) the warps of a group combine through pool_xs
+                float u[BN / 4];
+                frag_pool16<BN>(d, u, lane);
+                const int wpg = p.pool / 16;                             // warps per pooling group
+                if (wpg > 1) {
+#pragma unroll
+                    for (int i = 0; i < BN / 32; i++) {
+                        const int s = i + (BN / 32) * rq;
+                        pool_xs[we * BN + 8 * (s >> 1) + cq + (s & 1)] = u[i];
+                    }
+                    if (wpg == 8) named_bar_sync(2, 256);
+                    else named_bar_sync(4 + g, 128);
+                    if (we % wpg == 0) {
+                        for (int k = 1; k < wpg; k++) {
+#pragma unroll
+                            for (int i = 0; i < BN / 32; i++) {
+                                const int s = i + (BN / 32) * rq;
+                                u[i] = fmaxf(u[i], pool_xs[(we + k) * BN + 8 * (s >> 1) + cq + (s & 1)]);
                             }
                         }
                     }
-                } else if (p.unit_pool) {
-                    pooled_units_chunk(p, v, lane, q, mt, col0, nunits);
-                } else {
-                    switch (p.pool) {
-                        case 8: pooled_chunk<8>(p, v, lane, q, h, mt, col0, pool_xs); break;
-                        case 16: pooled_chunk<16>(p, v, lane, q, h, mt, col0, pool_xs); break;
-                        case 32: pooled_chunk<32>(p, v, lane, q, h, mt, col0, pool_xs); break;
-                        case 64: pooled_chunk<64>(p, v, lane, q, h, mt, col0, pool_xs); break;
-                        default: pooled_chunk<128>(p, v, lane, q, h, mt, col0, pool_xs); break;
+                    if (wpg == 8) named_bar_sync(2, 256);                 // pool_xs reusable by the next tile
+                    else named_bar_sync(4 + g, 128);
+                }
+                if (we % wpg == 0) {
+                    const long gg = ((long)mt * TC_BM + 16 * we) / p.pool;
+#pragma unroll
+                    for (int i = 0; i < BN / 32; i++) {
+                        const int s = i + (BN / 32) * rq;
+                        if (gg * p.pool < p.rows) store_pooled(p, gg, col_t + 8 * (s >> 1) + cq + (s & 1), u[i]);
                     }
                 }
             }
@@ -768,7 +795,7 @@ static int make_map(CUtensorMap *map, const void *ptr, long nrows, int kp, int b
     return 0;
 }
 
-// output matrix [nrows x ncols] (row pitch ld elements) -> 2D map with a [32 x 32] box for the per-warp stores
+// output matrix [nrows x ncols] (row pitch ld elements) -> 2D map with a [16 rows x 32 columns] box for the per-warp stores
 static int make_out_map(CUtensorMap *map, const void *ptr, long nrows, int ncols, int ld, bool f32)
 {
     EncodeTiledFn enc = get_encode_fn();
@@ -776,7 +803,7 @@ static int make_out_map(CUtensorMap *map, const void *ptr, long nrows, int ncols
     const int esz = f32 ? 4 : 2;
     cuuint64_t dims[2] = {(cuuint64_t)ncols, (cuuint64_t)nrows};
     cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
-    cuuint32_t box[2] = {32, 32};
+    cuuint32_t box[2] = {32, 16};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(ptr),
                      dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -837,12 +864,12 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     bool tma_store = pool <= 1 && (want_f32 != want_split);
     if (tma_store && want_f32) tma_store = (ld_f32 % 4 == 0) && ((reinterpret_cast<uintptr_t>(out_f32) & 15u) == 0);
     p.tma_store = tma_store ? 1 : 0;
-    const size_t budget = 224 * 1024 - 1024;   // 227 KiB per CTA minus static barriers and the 1 KiB alignment slack
+    const size_t budget = TC_DYN_SMEM - 1024;  // the 1 KiB alignment slack is added back at the launch
     const int nkb = (kp + TC_BK - 1) / TC_BK;
-    auto misc_bytes = [&](int bn) {            // scale/shift (+ hoisted Wx) + per-warp store blocks + accumulator staging
+    auto misc_bytes = [&](int bn) {            // scale/shift (+ hoisted Wx) + per-warp store blocks
         const int nt = (ncover + bn - 1) / bn;
         return 2 * ((size_t)nt * bn + 32) * sizeof(float) + (tma_store ? TC_EPI_WARPS * 4096 : 0) +
-               (g && g->wx ? (size_t)3 * kp * sizeof(float) : 0) + tc_acc_bytes(bn);
+               (g && g->wx ? (size_t)3 * kp * sizeof(float) : 0);
     };
     // Tile widths are multiples of 32 (columns beyond the weight rows come in as TMA zero fill and are never stored),
     // widest first: every wgmma re-reads its 64-row A slab from shared memory, so a wide tile reads A fewer times.
