@@ -33,6 +33,8 @@
 #include <cstring>
 
 #include "common.cuh"
+#include "operand.cuh"
+#include "pool.cuh"
 #include "wgmma.cuh"
 
 namespace ssd3d {
@@ -55,7 +57,7 @@ constexpr uint32_t TC_A_BYTES = TC_BM * TC_BK * 2;   // one A tile (hi or lo): 1
 // the rest of the 227 KiB opt-in limit.  At BN = 64 that is 3 KiB, so the limit is met exactly: anything added to the
 // static footprint must come out of TC_DYN_SMEM.
 constexpr size_t TC_DYN_SMEM = 224 * 1024;
-constexpr size_t TC_STATIC_SMEM = (2 * TC_MAX_STAGES + 4 * TC_MAX_AKB) * 8 + TC_EPI_WARPS * TC_MAX_BN * sizeof(float);
+constexpr size_t TC_STATIC_SMEM = (2 * TC_MAX_STAGES + 2 * TC_MAX_AKB) * 8 + TC_EPI_WARPS * TC_MAX_BN * sizeof(float);
 static_assert(TC_DYN_SMEM + (TC_STATIC_SMEM + 1023) / 1024 * 1024 <= 227 * 1024, "linear_tc: shared memory over the opt-in limit");
 
 struct TcParams {
@@ -79,8 +81,7 @@ struct TcParams {
     // astat ("A-stationary", gather modes): the produced A tile of an m-tile (all its k-blocks) stays in shared memory
     // while the CTA sweeps that m-tile's n-tiles, so the producers build it once instead of once per n-tile; only the
     // weights travel through the ring.  Tiles are then enumerated m-major per CTA.
-    int astat;       // 0: A through the ring; 1: one resident A tile; 2: TWO resident A tiles (the producers build m-tile
-                     // i+1 while the MMAs of m-tile i run -- with one buffer the two strictly alternate)
+    int astat;       // 0: A through the ring; 1: the resident A tile
     int gather, g_n, g_c, g_m, g_ns, g_ldz;
     const float *g_xyz, *g_points, *g_new_xyz, *g_wx;
     const int *g_idx;
@@ -99,10 +100,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(dst), "l"(map), "r"(bar), "r"(x), "r"(y) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, uint32_t src, int x, int y)
 {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
@@ -111,43 +108,11 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, uint32_t sr
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-
-// ---- epilogue helpers ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void split_pair(float x0, float x1, uint32_t &hw, uint32_t &lw)
-{
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hw) : "f"(x1), "f"(x0));       // {x1 : x0} like two adjacent bf16
-    const float h0 = __uint_as_float(hw << 16), h1 = __uint_as_float(hw & 0xffff0000u);
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lw) : "f"(x1 - h1), "f"(x0 - h0));
-}
 
 // ---- epilogue on the accumulator fragment ---------------------------------------------------------------------
 // Thread t of warp w (of its warpgroup) holds tile rows 64g + 16w + t/4 in d[4j], d[4j+1] and the row 8 below in
-// d[4j+2], d[4j+3], columns 8j + 2(t%4) + {0, 1} (wgmma.cuh).  The max-pools reduce these fragments where they are.
-//
-// Reduce-and-transpose over the 8 lanes of a column quad (lane bits 2-4, i.e. the 8 rows t/4 of a fragment half): on
-// return lane t owns, in v[i], the maximum of value slot i + (N/8)(t/4) over those 8 lanes.  3 steps, N - N/8 shuffles.
-// (Each step is its own fully unrolled loop: any index the compiler cannot resolve would move the accumulator fragment
-// to local memory for the whole kernel.)
-template <int HALF, int O, int N>
-__device__ __forceinline__ void quad_rowmax_step(float (&v)[N], int lane)
-{
-    const bool up = (lane & O) != 0;
-#pragma unroll
-    for (int i = 0; i < HALF; i++) {
-        const float send = up ? v[i] : v[i + HALF];
-        const float keep = up ? v[i + HALF] : v[i];
-        v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, O));
-    }
-}
-template <int N>
-__device__ __forceinline__ void quad_rowmax_transpose(float (&v)[N], int lane)
-{
-    quad_rowmax_step<N / 2, 16>(v, lane);
-    quad_rowmax_step<N / 4, 8>(v, lane);
-    quad_rowmax_step<N / 8, 4>(v, lane);
-}
+// d[4j+2], d[4j+3], columns 8j + 2(t%4) + {0, 1} (wgmma.cuh).  The max-pools reduce these fragments where they are
+// (quad_rowmax_transpose, pool.cuh).
 
 // 8-row max-pool of a warp's fragment (dense pool == 8 or the unit-list pool): the two 8-row halves stay apart.  On return
 // lane t owns slots s = i + (BN/16)(t/4), i < BN/16, of d: column 8(s/4) + 2(t%4) + (s%2) of row half (s/2)%2.
@@ -171,13 +136,7 @@ __device__ __forceinline__ void frag_pool16(const float (&d)[BN / 2], float (&u)
 __device__ __forceinline__ void store_pooled(const TcParams &p, long gg, int col, float mx)
 {
     if (col >= p.n) return;
-    if (p.rowmask && p.rowmask[gg] == 0) mx = 0.0f;
-    if (p.out_f32) p.out_f32[(size_t)gg * p.ld_f32 + col] = mx;
-    if (p.out_hi) {
-        const __nv_bfloat16 hb = __float2bfloat16_rn(mx);
-        p.out_hi[(size_t)gg * p.ld_split + col] = hb;
-        p.out_lo[(size_t)gg * p.ld_split + col] = __float2bfloat16_rn(mx - __bfloat162float(hb));
-    }
+    store_pooled_value(mx, p.rowmask && p.rowmask[gg] == 0, (size_t)gg, col, p.out_f32, p.ld_f32, p.out_hi, p.out_lo, p.ld_split);
 }
 
 // Developer instrumentation (nvcc -DTC_PROFILE): CTA 0 accumulates, per role, the cycles spent waiting on each barrier
@@ -205,8 +164,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
     // scale/shift
     const uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;
     const int nkb = (p.kp + TC_BK - 1) / TC_BK;
-    const uint32_t a_tile = (uint32_t)nkb * 2u * TC_A_BYTES;                        // one resident A tile: [nkb] x { A_hi | A_lo }
-    const uint32_t a_region = (uint32_t)p.astat * a_tile;
+    const uint32_t a_region = p.astat ? (uint32_t)nkb * 2u * TC_A_BYTES : 0u;       // resident A tile: [nkb] x { A_hi | A_lo }
     const uint32_t stage_bytes = (p.astat ? 0u : 2 * TC_A_BYTES) + 2 * b_bytes;     // ring stage
     const uint32_t b_off = p.astat ? 0u : 2 * TC_A_BYTES;                           // B_hi inside a stage
     // 1 KiB alignment by pointer arithmetic on the __shared__ array (an integer round-trip would demote every access
@@ -220,7 +178,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
     float *s_wx = s_shift + ncov;                                        // [3][kp] (hoisted mode only)
 
     __shared__ unsigned long long full_bar[TC_MAX_STAGES], empty_bar[TC_MAX_STAGES];
-    __shared__ unsigned long long afull_bar[2 * TC_MAX_AKB], aempty_bar[2 * TC_MAX_AKB];   // [A buffer][k-block]
+    __shared__ unsigned long long afull_bar[TC_MAX_AKB], aempty_bar[TC_MAX_AKB];   // per k-block of the resident A tile
     __shared__ __align__(16) float pool_xs[TC_EPI_WARPS * BN];          // 32-128-row pools: per-warp 16-row maxima (TC_STATIC_SMEM)
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // provably warp-uniform
@@ -245,8 +203,8 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
         // full barrier: the TMA thread's expect_tx arrival (+ one arrival per producer warp in gather mode);
         // empty barriers: one arrival per consumer warp once its wgmma group reading the slot has retired
         for (int s = 0; s < p.stages; s++) { mbar_init(smem_u32(&full_bar[s]), (p.gather && !p.astat) ? 1 + TC_PROD_WARPS : 1); mbar_init(smem_u32(&empty_bar[s]), TC_EPI_WARPS); }
-        for (int k = 0; k < 2 * TC_MAX_AKB; k++) { mbar_init(smem_u32(&afull_bar[k]), TC_PROD_WARPS); mbar_init(smem_u32(&aempty_bar[k]), TC_EPI_WARPS); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int k = 0; k < TC_MAX_AKB; k++) { mbar_init(smem_u32(&afull_bar[k]), TC_PROD_WARPS); mbar_init(smem_u32(&aempty_bar[k]), TC_EPI_WARPS); }
+        fence_mbar_init_cluster();
     }
     for (int i = threadIdx.x; i < ncov; i += TC_THREADS) {      // columns >= n: scale = shift = 0 -> exact zeros
         s_scale[i] = i < p.n ? __ldg(p.scale + i) : 0.0f;
@@ -299,7 +257,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
             const bool hoisted = p.gather == 2;
             const int src_pitch = hoisted ? p.g_ldz : p.g_c;
             const bool vec4 = (p.g_c % 4 == 0) && (src_pitch % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.g_points) & 15u) == 0);
-            const uint32_t row_off = (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u;
+            const int kend = hoisted ? p.g_c : p.g_c + 3;        // operand columns read from the sources
             int it = 0, mi = 0, mt, nt;
             TCP_DECL;
             for (int i = 0; tile_at(i, mt, nt); i++) {
@@ -307,10 +265,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                 const uint32_t row = (uint32_t)mt * TC_BM + (uint32_t)r;
                 const bool ok = (long)row < rows;
                 uint32_t rr = ok ? row : 0u;                      // position of this row's neighbour in idx[]
-                if (p.units && ok) {
-                    const uint32_t desc = (uint32_t)__ldg(p.units + 1 + (row >> 3));
-                    rr = (desc >> 4) * (uint32_t)p.g_ns + ((desc & 15u) << 3) + (row & 7u);
-                }
+                if (p.units && ok) rr = unit_slot((uint32_t)__ldg(p.units + 1 + (row >> 3)), (uint32_t)p.g_ns, row & 7u);
                 const uint32_t scene = rr / rps, q = rr / (uint32_t)p.g_ns;
                 const int a = __ldg(p.g_idx + rr);
                 const float *src_f = p.g_points + ((size_t)scene * p.g_n + a) * src_pitch;
@@ -324,61 +279,25 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                     const int s = it % p.stages;
                     float f[4][8];
 #pragma unroll
-                    for (int cc = 0; cc < 4; cc++) {
-                        const int k0 = kb * TC_BK + (c16_0 + cc) * 8;
-                        if (vec4 && ok && k0 + 8 <= p.g_c) {
-                            const float4 u0 = __ldg(reinterpret_cast<const float4 *>(src_f + k0));
-                            const float4 u1 = __ldg(reinterpret_cast<const float4 *>(src_f + k0 + 4));
-                            f[cc][0] = u0.x; f[cc][1] = u0.y; f[cc][2] = u0.z; f[cc][3] = u0.w;
-                            f[cc][4] = u1.x; f[cc][5] = u1.y; f[cc][6] = u1.z; f[cc][7] = u1.w;
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 8; e++) {
-                                const int k = k0 + e;
-                                float val = 0.0f;
-                                if (ok && k < p.kp) {
-                                    if (k < p.g_c) val = __ldg(src_f + k);
-                                    else if (!hoisted && k < p.g_c + 3) val = __ldg(src_x + (k - p.g_c)) - __ldg(ctr + (k - p.g_c));
-                                }
-                                f[cc][e] = val;
-                            }
-                        }
-                    }
+                    for (int cc = 0; cc < 4; cc++) load_concat8(f[cc], src_f, src_x, ctr, p.g_c, kend, kb * TC_BK + (c16_0 + cc) * 8, vec4, ok);
                     // (loads already in flight) wait for the slot: ring stage, or this k-block of the resident A tile
                     if (warp == TC_PROD_WARP0) TCP(7);
-                    const int ab = p.astat == 2 ? (mi & 1) : 0;
-                    const uint32_t aph = (uint32_t)(p.astat == 2 ? (mi >> 1) : mi) & 1u;
-                    if (p.astat) mbar_wait_cta(smem_u32(&aempty_bar[ab * TC_MAX_AKB + kb]), aph ^ 1u);
+                    if (p.astat) mbar_wait_cta(smem_u32(&aempty_bar[kb]), ((uint32_t)mi & 1u) ^ 1u);
                     else mbar_wait_cta(smem_u32(&empty_bar[s]), ((uint32_t)(it / p.stages) & 1u) ^ 1u);
                     if (warp == TC_PROD_WARP0) TCP(6);
-                    uint8_t *rowp = (p.astat ? smem + (size_t)ab * a_tile + (size_t)kb * 2 * TC_A_BYTES : ring + (size_t)s * stage_bytes) + row_off;
+                    uint8_t *blk = p.astat ? smem + (size_t)kb * 2 * TC_A_BYTES : ring + (size_t)s * stage_bytes;
 #pragma unroll
                     for (int cc = 0; cc < 4; cc++) {
                         const int c16 = c16_0 + cc;
                         const int k0 = kb * TC_BK + c16 * 8;
                         if (k0 >= p.kp) break;
-                        if (hoisted) {                                   // relu(z + d . Wx'); rows beyond the tensor stay 0
-#pragma unroll
-                            for (int e4 = 0; e4 < 8; e4 += 4) {
-                                const float4 w0 = *reinterpret_cast<const float4 *>(s_wx + k0 + e4);
-                                const float4 w1 = *reinterpret_cast<const float4 *>(s_wx + p.kp + k0 + e4);
-                                const float4 w2 = *reinterpret_cast<const float4 *>(s_wx + 2 * p.kp + k0 + e4);
-                                f[cc][e4 + 0] = fmaxf(fmaf(dz, w2.x, fmaf(dy, w1.x, fmaf(dx, w0.x, f[cc][e4 + 0]))), 0.0f);
-                                f[cc][e4 + 1] = fmaxf(fmaf(dz, w2.y, fmaf(dy, w1.y, fmaf(dx, w0.y, f[cc][e4 + 1]))), 0.0f);
-                                f[cc][e4 + 2] = fmaxf(fmaf(dz, w2.z, fmaf(dy, w1.z, fmaf(dx, w0.z, f[cc][e4 + 2]))), 0.0f);
-                                f[cc][e4 + 3] = fmaxf(fmaf(dz, w2.w, fmaf(dy, w1.w, fmaf(dx, w0.w, f[cc][e4 + 3]))), 0.0f);
-                            }
-                        }
-                        uint32_t hw[4], lw[4];
-#pragma unroll
-                        for (int t = 0; t < 4; t++) split_pair(f[cc][2 * t], f[cc][2 * t + 1], hw[t], lw[t]);
-                        const uint32_t off = (uint32_t)((c16 ^ (r & 7)) << 4);
-                        *reinterpret_cast<uint4 *>(rowp + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        *reinterpret_cast<uint4 *>(rowp + TC_A_BYTES + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                        if (hoisted) hoisted_row8(f[cc], s_wx + k0, p.kp, dx, dy, dz);   // rows beyond the tensor stay 0
+                        const uint32_t off = sw128_chunk((uint32_t)r, (uint32_t)c16);
+                        split_store8(blk + off, blk + TC_A_BYTES + off, f[cc]);
                     }
                     fence_async_smem();                                   // generic-proxy stores -> visible to the tensor core
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(smem_u32(p.astat ? &afull_bar[ab * TC_MAX_AKB + kb] : &full_bar[s]));
+                    if (lane == 0) mbar_arrive(smem_u32(p.astat ? &afull_bar[kb] : &full_bar[s]));
                 }
                 mi++;
             }
@@ -396,24 +315,22 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
             const bool last_nt = nt == p.n_tiles - 1;
             float d[BN / 2];
             int prev_s = -1, prev_kb = 0;
-            const int ab = p.astat == 2 ? (mi & 1) : 0;                  // resident A buffer of this m-tile
-            const uint32_t aph = (uint32_t)(p.astat == 2 ? (mi >> 1) : mi) & 1u;   // how often it has been used before
             // a ring stage (and, after the last n-tile, a resident A k-block) is free once the wgmma group reading it retired
             auto release = [&](int s, int kb) {
                 if (lane == 0) {
                     mbar_arrive(smem_u32(&empty_bar[s]));
-                    if (p.astat && last_nt) mbar_arrive(smem_u32(&aempty_bar[ab * TC_MAX_AKB + kb]));
+                    if (p.astat && last_nt) mbar_arrive(smem_u32(&aempty_bar[kb]));
                 }
             };
             for (int kb = 0; kb < nkb; kb++, it++) {
                 const int s = it % p.stages;
                 if (warp == TC_EPI_WARP0) TCP(5);
-                if (p.astat && nt == 0) mbar_wait_cta(smem_u32(&afull_bar[ab * TC_MAX_AKB + kb]), aph);   // this m-tile's A k-block
+                if (p.astat && nt == 0) mbar_wait_cta(smem_u32(&afull_bar[kb]), (uint32_t)mi & 1u);   // this m-tile's A k-block
                 if (warp == TC_EPI_WARP0) TCP(2);
                 mbar_wait_cta(smem_u32(&full_bar[s]), (uint32_t)(it / p.stages) & 1u);
                 if (warp == TC_EPI_WARP0) TCP(3);
                 const uint32_t base = smem_u32(ring + (size_t)s * stage_bytes);
-                const uint32_t abase = (p.astat ? smem_u32(smem) + (uint32_t)ab * a_tile + (uint32_t)kb * 2u * TC_A_BYTES : base) +
+                const uint32_t abase = (p.astat ? smem_u32(smem) + (uint32_t)kb * 2u * TC_A_BYTES : base) +
                                        (uint32_t)g * (64u * 128u);        // this warpgroup's 64 rows (8 swizzle atoms)
                 const int ksteps = min(TC_BK, p.kp - kb * TC_BK) / 16;
                 const uint64_t a_hi = wg_desc(abase, 128), a_lo = wg_desc(abase + TC_A_BYTES, 128);
@@ -527,8 +444,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                     const int ui = mt * (TC_BM / 8) + 2 * we + ((s >> 1) & 1);
                     const int col = col_t + 8 * (s >> 2) + cq + (s & 1);
                     if (ui >= nunits || col >= p.n) continue;
-                    const int group = __ldg(p.units + 1 + ui) >> 4;
-                    atomicMax(reinterpret_cast<unsigned int *>(p.out_f32 + (size_t)group * p.ld_f32 + col), __float_as_uint(d[i]) & 0x7fffffffu);
+                    atomic_max_nonneg(p.out_f32 + (size_t)unit_group((uint32_t)__ldg(p.units + 1 + ui)) * p.ld_f32 + col, d[i]);
                 }
             } else if (p.pool == 8) {
                 frag_pool8<BN>(d, lane);
@@ -579,13 +495,6 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
 }
 
 // ---- fp32 -> split bf16 producers -------------------------------------------------------------------------
-__device__ __forceinline__ void split_store(float x, __nv_bfloat16 *hi, __nv_bfloat16 *lo)
-{
-    const __nv_bfloat16 h = __float2bfloat16_rn(x);
-    *hi = h;
-    *lo = __float2bfloat16_rn(x - __bfloat162float(h));
-}
-
 // hi/lo[row, 0:kp] = split(x[row, 0:c]) zero-padded
 __global__ void split_rows_kernel(long rows, int c, const float *__restrict__ x, int ldx, __nv_bfloat16 *__restrict__ hi,
                                   __nv_bfloat16 *__restrict__ lo, int kp)
@@ -616,12 +525,8 @@ split_rows_v8_kernel(unsigned nchunks, int c, const float *__restrict__ x, int l
 #pragma unroll
             for (int e = 0; e < 8; e++) f[e] = k0 + e < c ? __ldg(src + e) : 0.0f;
         }
-        uint32_t hw[4], lw[4];
-#pragma unroll
-        for (int t = 0; t < 4; t++) split_pair(f[2 * t], f[2 * t + 1], hw[t], lw[t]);
         const size_t off = (size_t)row * kp + k0;
-        *reinterpret_cast<uint4 *>(hi + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-        *reinterpret_cast<uint4 *>(lo + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+        split_store8(hi + off, lo + off, f);
     }
 }
 
@@ -709,7 +614,8 @@ group_concat_split_kernel(long rows, int n, int c, int m, int ns, const float *_
 // For wide layers (K >= 256, 3DSSD layer 4) the A-stationary in-kernel producers starve the tensor pipe -- 128 KiB of
 // resident operand leave room for two narrow weight stages -- while this elementwise pass runs at memory speed on the whole
 // machine and the GEMM then takes the plain TMA-fed path.  One warp per row, one 8-column chunk per lane per step.
-__global__ void __launch_bounds__(256)
+// (6 CTAs per SM: without the bound ptxas spends 48 registers on the unrolled chunk and only 5 fit.)
+__global__ void __launch_bounds__(256, 6)
 hoist_expand_split_kernel(long rows, int n, int n1, int m, int ns, const float *__restrict__ xyz, const float *__restrict__ z,
                           int ldz, const float *__restrict__ wx, const float *__restrict__ new_xyz,
                           const int *__restrict__ idx, const int *__restrict__ units, __nv_bfloat16 *__restrict__ hi,
@@ -728,10 +634,7 @@ hoist_expand_split_kernel(long rows, int n, int n1, int m, int ns, const float *
     const int nchunk = kp >> 3;
     for (long row = warp0; row < rows; row += nwarps) {
         long src = row;                                                  // position of this row's neighbour in idx[]
-        if (units) {
-            const unsigned desc = (unsigned)__ldg(units + 1 + (row >> 3));
-            src = (long)(desc >> 4) * ns + ((desc & 15u) << 3) + (row & 7);
-        }
+        if (units) src = unit_slot((uint32_t)__ldg(units + 1 + (row >> 3)), (uint32_t)ns, (uint32_t)row & 7u);
         const long scene = src / rps, q = src / ns;
         const int a = __ldg(idx + src);
         const float *px = xyz + ((size_t)scene * n + a) * 3, *pc = new_xyz + (size_t)q * 3;
@@ -747,16 +650,8 @@ hoist_expand_split_kernel(long rows, int n, int n1, int m, int ns, const float *
 #pragma unroll
                 for (int e = 0; e < 8; e++) f[e] = k0 + e < n1 ? __ldg(zr + k0 + e) : 0.0f;
             }
-            uint32_t hw[4], lw[4];
-#pragma unroll
-            for (int e = 0; e < 8; e++) {
-                const float v = fmaf(dz, hx_wx[2 * kp + k0 + e], fmaf(dy, hx_wx[kp + k0 + e], fmaf(dx, hx_wx[k0 + e], f[e])));
-                f[e] = k0 + e < n1 ? fmaxf(v, 0.0f) : 0.0f;
-            }
-#pragma unroll
-            for (int t = 0; t < 4; t++) split_pair(f[2 * t], f[2 * t + 1], hw[t], lw[t]);
-            *reinterpret_cast<uint4 *>(hi + (size_t)row * kp + k0) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-            *reinterpret_cast<uint4 *>(lo + (size_t)row * kp + k0) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+            hoisted_row8(f, hx_wx + k0, kp, dx, dy, dz);
+            split_store8(hi + (size_t)row * kp + k0, lo + (size_t)row * kp + k0, f);
         }
     }
 }
@@ -878,8 +773,7 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     int bn = 0, stages = 0;
     p.astat = 0;
     // gather modes keep the produced A tile resident (A-stationary) when all its k-blocks fit next to a >= 2-stage
-    // weight ring: the producers then build it once per m-tile, not once per (m, n) tile.  (The kernel can also
-    // alternate between two resident tiles, TcParams::astat == 2; this planner does not choose it.)
+    // weight ring: the producers then build it once per m-tile, not once per (m, n) tile.
     if (g && nkb <= TC_MAX_AKB) {
         const size_t a_tile = (size_t)nkb * 2 * TC_A_BYTES;
         for (int ci = 0; ci < 2 && !bn; ci++) {

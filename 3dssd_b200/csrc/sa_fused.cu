@@ -34,6 +34,7 @@
 #include <cstring>
 
 #include "common.cuh"
+#include "operand.cuh"
 #include "pool.cuh"
 #include "wgmma.cuh"
 
@@ -77,27 +78,18 @@ struct SfParams {
     int pool_first;                  // caller guarantees scale >= 0 in the LAST layer: pool raw accumulators, affine after
 };
 
-__device__ __forceinline__ void sf_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// x = hi + lo with hi = bf16(x), lo = bf16(x - hi); two values per call, packed {x1 : x0} like two adjacent bf16
-__device__ __forceinline__ void sf_split_pair(float x0, float x1, uint32_t &hw, uint32_t &lw)
-{
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hw) : "f"(x1), "f"(x0));
-    const float h0 = __uint_as_float(hw << 16), h1 = __uint_as_float(hw & 0xffff0000u);
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lw) : "f"(x1 - h1), "f"(x0 - h0));
-}
 // Where row r of a 128-row operand tile lives.  An A buffer is laid out as k-blocks of { hi tile | lo tile }
 // (128 rows x rb bytes each), each tile in the canonical K-major swizzled layout of span rb: 16-byte chunk j of
-// row r sits at chunk j ^ ((r >> log2(128/rb)) & (rb/16 - 1)).  The first nfull blocks are 64 wide (rb = 128),
-// the tail block is rbt bytes wide.  Built once per (thread, layer); chunk() is then a handful of integer ops.
+// row r sits at chunk j ^ ((r >> log2(128/rb)) & (rb/16 - 1)).  The first nfull blocks are 64 wide (rb = 128,
+// sw128_chunk), the tail block is rbt bytes wide.  Built once per (thread, layer); chunk() is then a handful of integer ops.
 struct SfRowMap {
-    uint32_t row_f, xor_f;            // full blocks: byte offset of the row inside a tile, swizzle mask
+    uint32_t row;                     // the row (full blocks)
     uint32_t base_t, row_t, xor_t;    // tail block: byte offset of the block, of the row, swizzle mask
     uint32_t lo_t;                    // hi -> lo tile distance in the tail block (full blocks: 16 KiB)
     int full8;                        // nfull * 8: first 16-byte chunk index of the tail block
     __device__ __forceinline__ SfRowMap(int r, int nfull, int rbt)
     {
-        row_f = (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u;
-        xor_f = (uint32_t)(r & 7);
+        row = (uint32_t)r;
         const int sh = rbt == 128 ? 0 : (rbt == 64 ? 1 : 2);
         base_t = (uint32_t)nfull * (2u * 128u * 128u);
         row_t = (uint32_t)(r >> 3) * (uint32_t)(8 * rbt) + (uint32_t)(r & 7) * (uint32_t)rbt;
@@ -110,19 +102,12 @@ struct SfRowMap {
     {
         if (c16g < full8) {
             *lo_off = 128u * 128u;
-            return (uint32_t)(c16g >> 3) * (2u * 128u * 128u) + row_f + ((((uint32_t)c16g & 7u) ^ xor_f) << 4);
+            return (uint32_t)(c16g >> 3) * (2u * 128u * 128u) + sw128_chunk(row, (uint32_t)c16g & 7u);
         }
         *lo_off = lo_t;
         return base_t + row_t + (((uint32_t)(c16g - full8) ^ xor_t) << 4);
     }
 };
-__device__ __forceinline__ void sf_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-__device__ __forceinline__ uint32_t sf_f2ord(float x)
-{
-    const uint32_t b = __float_as_uint(x);
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float sf_ord2f(uint32_t u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
 
 // ---- shape policies -------------------------------------------------------------------------------------------------
 // The kernel body is written once against a policy C that answers every shape question (layer count, padded K / N of a
@@ -132,11 +117,17 @@ __device__ __forceinline__ float sf_ord2f(uint32_t u) { return __uint_as_float((
 // literal (integer / branch / uniform-register bookkeeping of exactly these questions is otherwise a large share of the
 // kernel's issued instructions).
 __host__ __device__ constexpr int sf_r16(int x) { return (x + 15) / 16 * 16; }
-__host__ __device__ constexpr int sf_rbt_of(int kp) { return kp % 64 == 0 ? 0 : (kp % 64 <= 16 ? 32 : (kp % 64 <= 32 ? 64 : 128)); }
-__host__ __device__ constexpr uint32_t sf_abuf_of(int kp)
+// Operand layout of a layer with padded K = kp: nfull 64-wide k-blocks of 128-byte rows + a tail block whose rows are
+// 32 / 64 / 128 bytes for a remainder of 16 / 32 / 48 columns (must match params._k_blocks)
+__host__ __device__ constexpr int sf_nfull(int kp) { return kp / 64; }
+__host__ __device__ constexpr int sf_rbt(int kp) { return kp % 64 == 0 ? 0 : (kp % 64 <= 16 ? 32 : (kp % 64 <= 32 ? 64 : 128)); }
+// operand buffer: { hi | lo } tiles of 128 rows per block, 1 KiB granular
+__host__ __device__ constexpr uint32_t sf_abuf_bytes(int kp)
 {
-    return (uint32_t)(((kp / 64) * 2 * 128 * 128 + 2 * 128 * sf_rbt_of(kp) + 1023) / 1024 * 1024);
+    return (uint32_t)((sf_nfull(kp) * 2 * 128 * 128 + 2 * 128 * sf_rbt(kp) + 1023) / 1024 * 1024);
 }
+// one half (hi or lo) of a layer's weight image
+__host__ __device__ constexpr uint32_t sf_wimg_bytes(int kp, int npad) { return (uint32_t)(npad * (sf_nfull(kp) * 128 + sf_rbt(kp))); }
 
 struct SfDyn {
     static constexpr bool kStatic = false;
@@ -175,15 +166,15 @@ struct SfStat {
     __device__ __forceinline__ constexpr int kp(int l) const { return l == 0 ? KP0 : NP0; }
     __device__ __forceinline__ constexpr int npad(int l) const { return l == 0 ? NP0 : NP1; }
     __device__ __forceinline__ constexpr int nout(int l) const { return l == 0 ? N0 : N1; }
-    __device__ __forceinline__ constexpr int nfull(int l) const { return kp(l) / 64; }
-    __device__ __forceinline__ constexpr int rbt(int l) const { return sf_rbt_of(kp(l)); }
-    __device__ __forceinline__ constexpr uint32_t w_half(int l) const { return (uint32_t)(npad(l) * (nfull(l) * 128 + rbt(l))); }
+    __device__ __forceinline__ constexpr int nfull(int l) const { return sf_nfull(kp(l)); }
+    __device__ __forceinline__ constexpr int rbt(int l) const { return sf_rbt(kp(l)); }
+    __device__ __forceinline__ constexpr uint32_t w_half(int l) const { return sf_wimg_bytes(kp(l), npad(l)); }
     __device__ __forceinline__ constexpr uint32_t w_off(int l) const { return l == 0 ? 0u : 2u * w_half(0); }
     __device__ __forceinline__ constexpr int sspad(int l) const { return (npad(l) + 31) / 32 * 32; }
     __device__ __forceinline__ constexpr uint32_t ss_off(int l) const { return l == 0 ? 0u : 2u * (uint32_t)sspad(0); }
     __device__ __forceinline__ constexpr uint32_t w_total() const { return 2u * w_half(0) + 2u * w_half(1); }
     __device__ __forceinline__ constexpr uint32_t ss_total() const { return 2u * (uint32_t)sspad(0) + 2u * (uint32_t)sspad(1); }
-    __device__ __forceinline__ constexpr uint32_t abuf_bytes() const { return sf_abuf_of(KP0) > sf_abuf_of(NP0) ? sf_abuf_of(KP0) : sf_abuf_of(NP0); }
+    __device__ __forceinline__ constexpr uint32_t abuf_bytes() const { return sf_abuf_bytes(KP0) > sf_abuf_bytes(NP0) ? sf_abuf_bytes(KP0) : sf_abuf_bytes(NP0); }
     __device__ __forceinline__ constexpr uint32_t acc_cols() const { return (uint32_t)((NP0 > NP1 ? NP0 : NP1) + 31) / 32 * 32; }
 };
 
@@ -207,12 +198,12 @@ __device__ __forceinline__ void sf_pool_store(const SfParams &p, float (&v)[32],
     warp_colmax_transpose<GP>(v, lane);                   // lane owns columns (lane % GP) * KEEP + k in v[k]
     if (POOL > 32) {                                      // groups spanning 2 or 4 warps: combine through shared memory
         xs[q * 32 + lane] = v[0];
-        sf_bar_sync(wg_bar, 128);
+        named_bar_sync(wg_bar, 128);
         if ((q % WPG) == 0) {
 #pragma unroll
             for (int w = 1; w < WPG; w++) v[0] = fmaxf(v[0], xs[(q + w) * 32 + lane]);
         }
-        sf_bar_sync(wg_bar, 128);
+        named_bar_sync(wg_bar, 128);
         if ((q % WPG) != 0) return;
     }
     const int gg = tile * (128 / POOL) + (q * 32 + lane) / POOL;
@@ -225,20 +216,12 @@ __device__ __forceinline__ void sf_pool_store(const SfParams &p, float (&v)[32],
         if (col >= nout) continue;
         float mx = v[k];
         if (AFTER) mx = fmaxf(fmaf(mx, sc[col0 + cc], sh[col0 + cc]), 0.0f);
-        mx = masked ? 0.0f : mx;
-        if (p.out_f32) asm volatile("st.global.f32 [%0], %1;" ::"l"(p.out_f32 + (size_t)gg * p.ld_f32 + col), "f"(mx) : "memory");
-        if (p.out_hi) {
-            const __nv_bfloat16 hb = __float2bfloat16_rn(mx);
-            const __nv_bfloat16 lb = __float2bfloat16_rn(mx - __bfloat162float(hb));
-            asm volatile("st.global.b16 [%0], %1;" ::"l"(p.out_hi + (size_t)gg * p.ld_split + col), "h"(__bfloat16_as_ushort(hb)) : "memory");
-            asm volatile("st.global.b16 [%0], %1;" ::"l"(p.out_lo + (size_t)gg * p.ld_split + col), "h"(__bfloat16_as_ushort(lb)) : "memory");
-        }
+        store_pooled_value(mx, masked, (size_t)gg, col, p.out_f32, p.ld_f32, p.out_hi, p.out_lo, p.ld_split);
     }
 }
 
-// Unit-list mode: a unit is 8 rows = 8 consecutive lanes.  Max over the unit, then atomicMax into out[group]: post-ReLU
-// values are >= 0, where the unsigned order of the bit patterns is the float order (a -0.0 is folded to +0.0), and the
-// caller zero-fills the output, which is also the result of a group without hits (the mask of layers_util.py:180).
+// Unit-list mode: a unit is 8 rows = 8 consecutive lanes.  Max over the unit, then atomicMax into out[group] (post-ReLU
+// values; the caller's zero fill is also the result of a group without hits, the mask of layers_util.py:180).
 template <bool AFTER>
 __device__ __forceinline__ void sf_pool_atomic8(const SfParams &p, float (&v)[32], int lane, int col0, int nout, const float *sc,
                                                 const float *sh, int group, bool ok)
@@ -252,7 +235,7 @@ __device__ __forceinline__ void sf_pool_atomic8(const SfParams &p, float (&v)[32
         if (col >= nout) continue;
         float mx = v[k];
         if (AFTER) mx = fmaxf(fmaf(mx, sc[col0 + cc], sh[col0 + cc]), 0.0f);
-        atomicMax(reinterpret_cast<unsigned int *>(p.out_f32 + (size_t)group * p.ld_f32 + col), __float_as_uint(mx) & 0x7fffffffu);
+        atomic_max_nonneg(p.out_f32 + (size_t)group * p.ld_f32 + col, mx);
     }
 }
 
@@ -340,7 +323,7 @@ sa_fused_kernel(const SfParams p)
 
     if (tid == 0) {
         mbar_init(smem_u32(&w_bar), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        fence_mbar_init_cluster();
         mbar_arrive_expect_tx(smem_u32(&w_bar), cfg.w_total());
         bulk_g2s(smem_u32(wsm), p.w_blob, cfg.w_total(), smem_u32(&w_bar));
     }
@@ -378,7 +361,7 @@ sa_fused_kernel(const SfParams p)
             const int ui = t * 16 + (r >> 3);
             if (ui < nunits) {
                 desc = __ldg(units + 1 + ui);
-                a = __ldg(p.idx + (size_t)(desc >> 4) * (uint32_t)cfg.ns() + (uint32_t)(((desc & 15) << 3) + (r & 7)));
+                a = __ldg(p.idx + unit_slot((uint32_t)desc, (uint32_t)cfg.ns(), (uint32_t)r & 7u));
             }
         } else if ((long)t * 128 + r < p.rows) {
             desc = 0;
@@ -394,7 +377,7 @@ sa_fused_kernel(const SfParams p)
         {
             const uint32_t row = (uint32_t)tile * 128u + (uint32_t)r;
             const bool ok = d_next >= 0;
-            const uint32_t qi = !ok ? 0u : (compact ? (uint32_t)(d_next >> 4) : row / (uint32_t)cfg.ns());    // == scene*m + query
+            const uint32_t qi = !ok ? 0u : (compact ? unit_group((uint32_t)d_next) : row / (uint32_t)cfg.ns());    // == scene*m + query
             const uint32_t scene = qi / (uint32_t)p.m;
             const int a = a_next;
             my_group = (int)qi; my_ok = ok;
@@ -412,48 +395,17 @@ sa_fused_kernel(const SfParams p)
             for (int cg0 = wg * U; cg0 < nchunk; cg0 += WG * U) {     // U chunks of 8 columns in flight per thread
                 float f[U][8];
 #pragma unroll
-                for (int u = 0; u < U; u++) {
-                    const int kb = (cg0 + u) * 8;
-                    if (vec && ok && kb + 8 <= cfg.c()) {
-                        const float4 lo4 = __ldg(reinterpret_cast<const float4 *>(src_f + kb));
-                        const float4 hi4 = __ldg(reinterpret_cast<const float4 *>(src_f + kb + 4));
-                        f[u][0] = lo4.x; f[u][1] = lo4.y; f[u][2] = lo4.z; f[u][3] = lo4.w;
-                        f[u][4] = hi4.x; f[u][5] = hi4.y; f[u][6] = hi4.z; f[u][7] = hi4.w;
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 8; e++) {
-                            const int k = kb + e;
-                            float val = 0.0f;
-                            if (ok) {
-                                if (k < cfg.c()) val = __ldg(src_f + k);
-                                else if (k < k0) val = __ldg(src_x + (k - cfg.c())) - __ldg(ctr + (k - cfg.c()));   // never in hoisted mode
-                            }
-                            f[u][e] = val;
-                        }
-                    }
-                }
+                for (int u = 0; u < U; u++) load_concat8(f[u], src_f, src_x, ctr, cfg.c(), k0, (cg0 + u) * 8, vec, ok);
 #pragma unroll
                 for (int u = 0; u < U; u++) {
                     if (cg0 + u >= nchunk) break;
-                    if (cfg.hoist()) {                                 // relu(z + d . Wx'); padded columns and rows stay 0
-                        const float *w = wxs + (cg0 + u) * 8;
-#pragma unroll
-                        for (int e4 = 0; e4 < 8; e4 += 4) {
-                            const float4 w0 = *reinterpret_cast<const float4 *>(w + e4);
-                            const float4 w1 = *reinterpret_cast<const float4 *>(w + kp0 + e4);
-                            const float4 w2 = *reinterpret_cast<const float4 *>(w + 2 * kp0 + e4);
-                            f[u][e4 + 0] = fmaxf(fmaf(dz, w2.x, fmaf(dy, w1.x, fmaf(dx, w0.x, f[u][e4 + 0]))), 0.0f);
-                            f[u][e4 + 1] = fmaxf(fmaf(dz, w2.y, fmaf(dy, w1.y, fmaf(dx, w0.y, f[u][e4 + 1]))), 0.0f);
-                            f[u][e4 + 2] = fmaxf(fmaf(dz, w2.z, fmaf(dy, w1.z, fmaf(dx, w0.z, f[u][e4 + 2]))), 0.0f);
-                            f[u][e4 + 3] = fmaxf(fmaf(dz, w2.w, fmaf(dy, w1.w, fmaf(dx, w0.w, f[u][e4 + 3]))), 0.0f);
-                        }
-                    }
-                    uint32_t hw[4], lw[4], lo_off;
-#pragma unroll
-                    for (int t = 0; t < 4; t++) sf_split_pair(f[u][2 * t], f[u][2 * t + 1], hw[t], lw[t]);
+                    if (cfg.hoist()) hoisted_row8(f[u], wxs + (cg0 + u) * 8, kp0, dx, dy, dz);   // padded columns and rows stay 0
+                    uint4 h, l;
+                    uint32_t lo_off;
+                    split8(f[u], 0, h, l);
                     const uint32_t off = map0.chunk(cg0 + u, &lo_off);
-                    *reinterpret_cast<uint4 *>(buf + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                    *reinterpret_cast<uint4 *>(buf + off + lo_off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                    *reinterpret_cast<uint4 *>(buf + off) = h;
+                    *reinterpret_cast<uint4 *>(buf + off + lo_off) = l;
                 }
             }
         }
@@ -462,8 +414,8 @@ sa_fused_kernel(const SfParams p)
         for (int l = 0; l < cfg.nl(); l++) {
             // operand written with ordinary stores -> make it visible to the tensor-core (async) proxy; the barrier also
             // orders the previous layer's staged-accumulator reads before this layer's MMAs overwrite the staging
-            sf_fence_async_smem();
-            sf_bar_sync(slot_bar, ST);
+            fence_async_smem();
+            named_bar_sync(slot_bar, ST);
             SF_T(1 + 4 * l);                                           // barrier
             {
                 // work items (64-row half, <= 64-column chunk) of this layer, round robin over the slot's warpgroups: one
@@ -481,7 +433,7 @@ sa_fused_kernel(const SfParams p)
                 }
             }
             SF_T(2 + 4 * l);                                           // MMAs
-            sf_bar_sync(slot_bar, ST);                                 // every MMA of the tile done: staging complete, buf free
+            named_bar_sync(slot_bar, ST);                              // every MMA of the tile done: staging complete, buf free
             SF_T(3 + 4 * l);                                           // MMA wait
             // ---- epilogue of layer l
             const float *sc = ss + cfg.ss_off(l);
@@ -518,12 +470,12 @@ sa_fused_kernel(const SfParams p)
 #pragma unroll
                     for (int j8 = 0; j8 < 32; j8 += 8) {
                         if (c0 + j8 >= cfg.kp(l + 1)) break;
-                        uint32_t hw[4], lw[4], lo_off;
-#pragma unroll
-                        for (int t = 0; t < 4; t++) sf_split_pair(v[j8 + 2 * t], v[j8 + 2 * t + 1], hw[t], lw[t]);
+                        uint4 h, l;
+                        uint32_t lo_off;
+                        split8(v, j8, h, l);
                         const uint32_t off = mapn.chunk((c0 + j8) >> 3, &lo_off);
-                        *reinterpret_cast<uint4 *>(buf + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        *reinterpret_cast<uint4 *>(buf + off + lo_off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                        *reinterpret_cast<uint4 *>(buf + off) = h;
+                        *reinterpret_cast<uint4 *>(buf + off + lo_off) = l;
                     }
                 } else if (compact) {
                     if (pool_first) sf_pool_atomic8<true>(p, v, lane, c0, cfg.nout(l), sc, sh, my_group, my_ok);
@@ -555,27 +507,6 @@ sa_fused_kernel(const SfParams p)
 }  // namespace ssd3d
 
 using namespace ssd3d;
-
-// Operand layout of a layer with padded K = kp: nfull 64-wide k-blocks of 128-byte rows + a tail block whose rows
-// are 32 / 64 / 128 bytes for a remainder of 16 / 32 / 48 columns (must match params._k_blocks).
-static void sf_k_blocks(int kp, int *nfull, int *rbt)
-{
-    *nfull = kp / 64;
-    const int rem = kp % 64;
-    *rbt = rem == 0 ? 0 : (rem <= 16 ? 32 : (rem <= 32 ? 64 : 128));
-}
-static size_t sf_abuf_bytes(int kp)                       // { hi | lo } tiles of 128 rows per block, 1 KiB granular
-{
-    int nfull, rbt;
-    sf_k_blocks(kp, &nfull, &rbt);
-    return ((size_t)nfull * 2 * 128 * 128 + (size_t)2 * 128 * rbt + 1023) / 1024 * 1024;
-}
-static size_t sf_wimg_bytes(int kp, int npad)              // one half (hi or lo) of a layer's weight image
-{
-    int nfull, rbt;
-    sf_k_blocks(kp, &nfull, &rbt);
-    return (size_t)npad * (nfull * 128 + rbt);
-}
 
 struct SfPlan { size_t abuf, acc, w, ssf; int maxn; };
 static bool sf_plan(int k_in, int nl, const int *nout, SfPlan *pl)      // k_in: columns of the first operand
@@ -701,9 +632,10 @@ static int sa_mlp_fused_impl(int b, int n, int c, int m, int nsample, const floa
         p.kp[l] = kprev;
         p.nout[l] = nout[l];
         p.npad[l] = (nout[l] + 15) / 16 * 16;
-        sf_k_blocks(p.kp[l], &p.nfull[l], &p.rbt[l]);
+        p.nfull[l] = sf_nfull(p.kp[l]);
+        p.rbt[l] = sf_rbt(p.kp[l]);
         p.w_off[l] = woff;
-        p.w_half[l] = (uint32_t)sf_wimg_bytes(p.kp[l], p.npad[l]);
+        p.w_half[l] = sf_wimg_bytes(p.kp[l], p.npad[l]);
         woff += 2 * p.w_half[l];
         p.ss_off[l] = ssoff;
         p.sspad[l] = (p.npad[l] + 31) / 32 * 32;

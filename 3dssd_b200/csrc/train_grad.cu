@@ -17,6 +17,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "operand.cuh"
 #include "wgmma.cuh"
 
 namespace ssd3d {
@@ -39,26 +40,6 @@ static void wgrad_plan(long rows, int cin, int cout, long &rps, int &splits)
     rps = ((chunks + s - 1) / s) * WG_BK;
     splits = (int)((rows + rps - 1) / rps);
     if (splits < 1) splits = 1;
-}
-
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-__device__ __forceinline__ void split_pair_bf16(float x0, float x1, uint32_t &hw, uint32_t &lw)
-{
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hw) : "f"(x1), "f"(x0));       // {x1 : x0}: x0 at the lower k index
-    const float h0 = __uint_as_float(hw << 16), h1 = __uint_as_float(hw & 0xffff0000u);
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lw) : "f"(x1 - h1), "f"(x0 - h0));
-}
-
-// 8 consecutive rows of one channel -> one 16-byte chunk (k = 8 c16 .. 8 c16 + 7) of smem row `ch`, hi and lo images
-__device__ __forceinline__ void store_chunk(uint8_t *img_hi, uint32_t lo_off, int ch, int c16, const float (&f)[8])
-{
-    uint32_t hw[4], lw[4];
-#pragma unroll
-    for (int t = 0; t < 4; t++) split_pair_bf16(f[2 * t], f[2 * t + 1], hw[t], lw[t]);
-    const uint32_t off = (uint32_t)ch * 128u + (uint32_t)((c16 ^ (ch & 7)) << 4);
-    *reinterpret_cast<uint4 *>(img_hi + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-    *reinterpret_cast<uint4 *>(img_hi + lo_off + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
 }
 
 template <int BN>
@@ -110,17 +91,22 @@ linear_wgrad_kernel(long rows, int cin, int cout, const float *__restrict__ x, i
     for (int i = 0; i < nch; i++) {
         uint8_t *st = smem + (size_t)(i & 1) * STAGE;
         __syncthreads();                                     // every warp retired the wgmma group that read this stage
+        // 8 consecutive rows of one channel -> one 16-byte chunk (k = 8 c16 .. 8 c16 + 7) of smem row `ch`, hi and lo images
 #pragma unroll
-        for (int j = 0; j < 4; j++) store_chunk(st, A_BYTES, a_ch, a_c0 + 2 * j, fa[j]);
+        for (int j = 0; j < 4; j++) {
+            const uint32_t off = sw128_chunk((uint32_t)a_ch, (uint32_t)(a_c0 + 2 * j));
+            split_store8(st + off, st + A_BYTES + off, fa[j]);
+        }
 #pragma unroll
         for (int j = 0; j < BJ; j++) {
-            store_chunk(st + 2 * A_BYTES, B_BYTES, b_ch, b_c0 + j * (WG_THREADS / BN), fb[j]);
+            const uint32_t off = 2 * A_BYTES + sw128_chunk((uint32_t)b_ch, (uint32_t)(b_c0 + j * (WG_THREADS / BN)));
+            split_store8(st + off, st + B_BYTES + off, fb[j]);
             if (want_b) {
 #pragma unroll
                 for (int e = 0; e < 8; e++) sb += (double)fb[j][e];
             }
         }
-        fence_proxy_async();
+        fence_async_smem();
         __syncthreads();
         const uint32_t base = smem_u32(st);
         const uint64_t a_hi = wg_desc(base, 128), a_lo = wg_desc(base + A_BYTES, 128);

@@ -857,7 +857,7 @@ def test_hoisted_first_conv_matches_oracle_and_gather_path(pkg, oracle_ops, cuda
     else:
         _, (hi2, lo2) = pkg.linear_tc(ehi, elo, f1, want_f32=False, want_split=True)
         y2, _ = pkg.linear_tc(hi2, lo2, pp.conv(scopes[2], True), pool=k, rowmask=tc, want_f32=True, want_split=False)
-    assert rel_err(N(y2), N(y)) < 1e-6
+    assert torch.equal(y2, y)
 
 
 @pytest.mark.parametrize("b,n,c,m,k,mlp", [
@@ -897,6 +897,14 @@ def test_sa_mlp_fused_hoisted_vs_oracle(pkg, oracle_ops, cuda, b, n, c, m, k, ml
     y = pkg.sa_mlp_fused_hoisted(tx, z, 0, wxs[0], tn, ti, tc, stack)
     # absolute coordinates up to 70 m: |(x_j - c_i) . Wx| is compared on the scale of the layer's outputs
     assert y.shape == (b, m, mlp[-1]) and rel_err(N(y), exp) < 1e-4
+    # the same scale layer by layer (the hoisted operand built by linear_tc's producer warps): the same bits
+    f1 = pp.conv(scopes[1], True)
+    if len(mlp) == 2:
+        y1, _ = pkg.linear_tc_hoisted(tx, z, 0, wxs[0], tn, ti, f1, pool=k, rowmask=tc, want_f32=True, want_split=False)
+    else:
+        _, (hi, lo) = pkg.linear_tc_hoisted(tx, z, 0, wxs[0], tn, ti, f1)
+        y1, _ = pkg.linear_tc(hi, lo, pp.conv(scopes[2], True), pool=k, rowmask=tc, want_f32=True, want_split=False)
+    assert torch.equal(y1, y)
 
 
 @pytest.mark.parametrize("c,ks,mlps,hoist", [

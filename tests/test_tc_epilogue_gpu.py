@@ -121,8 +121,8 @@ def test_dense_outputs(pkg, cuda, rows, cout, outputs):
 def test_gather_route_resident_operand(pkg, cuda, pool):
     """The two operand routes of linear_tc_kernel on the same rows.  linear_tc streams A through the TMA ring (astat 0);
     linear_tc_gather with K = 16 (one k-block, 32 KiB) always fits the planner's A-stationary plan, so its producer
-    warps build each m-tile once and it stays resident while the CTA sweeps the three 64-column n-tiles (astat 1).  (The
-    two-buffer mode, astat 2, has no entry point: the planner does not choose it.)  Both must give the float64 result."""
+    warps build each m-tile once and it stays resident while the CTA sweeps the three 64-column n-tiles (astat 1).
+    Both must give the float64 result."""
     rng = np.random.default_rng(pool)
     b, n, c, m, ns, cout = 2, 300, 13, 37, 16 if pool == 1 else pool, 160
     xyz = torch.tensor(rng.integers(0, 33, (b, n, 3)) / 8.0, dtype=torch.float32, device=cuda)
