@@ -4,20 +4,20 @@
 // the conv2d/bias/BN/ReLU stack, reduce_max, mask multiply -- ~25 TF kernels per scale, each streaming [B,M,K,C]
 // through HBM) for the layers whose weights fit in shared memory (3DSSD layer1/layer2: 93% of the grouped rows).
 // Nothing but the neighbour indices, the gathered source rows (L2-resident) and the pooled [B,M,C3] result touches
-// global memory; activations go wgmma registers -> fp32 staging in shared memory -> registers -> shared memory (already
-// split in bf16 hi/lo and already in the swizzled K-major layout the next layer's wgmma descriptors expect).
+// global memory; activations go wgmma registers -> epilogue on the accumulator fragments -> shared memory (already split
+// in bf16 hi/lo and already in the swizzled K-major layout the next layer's wgmma descriptors expect).
 //
-// Per CTA: S "slots" of 128*WG threads (a slot works on one 128-row tile = 128/K neighbour groups; its WG warpgroups
-// split the 16-byte chunks of the gather and the 32-column chunks of every epilogue):
+// Per CTA: S "slots" of 128*WG threads, each working on one 128-row tile (= 128/K neighbour groups) at a time:
 //   weights of all layers (hi+lo images, pre-swizzled on the host) are bulk-copied to shared memory once and shared
-//   by the slots; each slot owns ONE operand buffer and one fp32 accumulator staging buffer and loops over tiles:
-//   gather+split -> [fence.proxy.async] -> layer-0 MMAs (the slot's warpgroups split the 64-row halves of the tile and
-//   the <= 64-column chunks of the layer; each chunk is one wgmma chain into registers, staged row-major) -> epilogue
-//   (scale/shift/ReLU, split) written IN PLACE over the operand the finished MMAs no longer need -> ... -> last layer:
-//   max-pool.
-// Small stacks (layer1) run S=1 with several CTAs per SM; stacks whose weights fill most of shared memory (layer2) run
-// one CTA per SM with as many slots as fit, each of two warpgroups -- one slot for the layer-2 stacks, whose staged
-// accumulator (128 x 132 fp32) and weights leave no room for a second, so their tiles overlap only across SMs.
+//   by the slots; each slot owns ONE operand buffer and loops over tiles.  The buffer keeps the two 64-row halves of the
+//   tile in separate byte ranges for every layer (SfRowMap), so a row half is a pipeline of its own:
+//   gather+split of the half -> [fence.proxy.async + warpgroup barrier] -> the layer's MMAs for the half (one wgmma chain
+//   per <= 64-column chunk, all chunks held in registers) -> epilogue on the fragments (scale/shift/ReLU, split) written
+//   IN PLACE over the half's operand, which its retired MMAs no longer need -> ... -> last layer: one chunk at a time,
+//   max-pooled on the fragment (8-row units by a shuffle butterfly; wider groups meet in a 4 KiB per-slot exchange).
+// Small stacks (layer1) run S=1 with one warpgroup that takes the two halves in turn, several CTAs per SM; larger
+// stacks (layer2) run one CTA per SM with two slots of two warpgroups, each warpgroup owning one row half, so that no
+// barrier wider than a warpgroup separates the layers (only a pool of 128 rows meets the other half).
 // Hoisted mode (SfParams::hoist): the scale's first conv has been moved to a per-point table z (include/ssd3d.h,
 // ssd3d_sa_mlp_fused_hoisted); the gather then builds relu(z[idx] + (xyz[idx] - centre) . Wx') and the stack starts at
 // the second conv.
@@ -32,6 +32,7 @@
 #include <cuda_bf16.h>
 #include <cstdio>
 #include <cstring>
+#include <type_traits>
 
 #include "common.cuh"
 #include "operand.cuh"
@@ -42,6 +43,8 @@ namespace ssd3d {
 
 constexpr int SF_THREADS = 128;
 constexpr int SF_MAX_LAYERS = 3;
+constexpr int SF_MAX_NCH = 4;                // <= 64-column chunks of a layer (npad <= 256)
+constexpr int SF_XS_FLOATS = 16 * 64;        // pooled-value exchange of a slot: [8-row slab][chunk column]
 
 struct SfParams {
     int n, c, m, ns;                 // points per scene, feature channels, queries per scene, neighbours per query
@@ -72,37 +75,40 @@ struct SfParams {
     int nfull[SF_MAX_LAYERS];        // layer l's K = nfull 64-wide k-blocks (128-byte rows) + one tail block
     int rbt[SF_MAX_LAYERS];          // bytes per row of the tail block: 0 (none), 32 (16 wide), 64 (32), 128 (48)
     uint32_t abuf_bytes;             // operand buffer of one slot
-    uint32_t acc_cols;               // staged accumulator columns of one slot (widest layer, rounded up to 32)
     float *out_f32; int ld_f32;
     __nv_bfloat16 *out_hi, *out_lo; int ld_split;
     int pool_first;                  // caller guarantees scale >= 0 in the LAST layer: pool raw accumulators, affine after
 };
 
-// Where row r of a 128-row operand tile lives.  An A buffer is laid out as k-blocks of { hi tile | lo tile }
-// (128 rows x rb bytes each), each tile in the canonical K-major swizzled layout of span rb: 16-byte chunk j of
-// row r sits at chunk j ^ ((r >> log2(128/rb)) & (rb/16 - 1)).  The first nfull blocks are 64 wide (rb = 128,
-// sw128_chunk), the tail block is rbt bytes wide.  Built once per (thread, layer); chunk() is then a handful of integer ops.
+// Where row r of a 128-row operand tile lives.  The buffer holds the two 64-row halves of the tile one after the other,
+// half_bytes (half the buffer of the widest layer) apart, so that rows 64h .. 64h+63 of EVERY layer stay inside half h's
+// bytes and the warpgroup running a half can overwrite them with the next layer's operand as soon as its own MMAs have
+// retired.  A half is laid out as k-blocks of { hi tile | lo tile } (64 rows x rb bytes each), each tile in the canonical
+// K-major swizzled layout of span rb: 16-byte chunk j of row r sits at chunk j ^ ((r >> log2(128/rb)) & (rb/16 - 1)).
+// The first nfull blocks are 64 wide (rb = 128, sw128_chunk), the tail block is rbt bytes wide.  Built once per
+// (thread, row, layer); chunk() is then a handful of integer ops.
 struct SfRowMap {
-    uint32_t row;                     // the row (full blocks)
+    uint32_t half, row;               // byte offset of the row's half, row within the half
     uint32_t base_t, row_t, xor_t;    // tail block: byte offset of the block, of the row, swizzle mask
-    uint32_t lo_t;                    // hi -> lo tile distance in the tail block (full blocks: 16 KiB)
+    uint32_t lo_t;                    // hi -> lo tile distance in the tail block (full blocks: 8 KiB)
     int full8;                        // nfull * 8: first 16-byte chunk index of the tail block
-    __device__ __forceinline__ SfRowMap(int r, int nfull, int rbt)
+    __device__ __forceinline__ SfRowMap(int r, int nfull, int rbt, uint32_t half_bytes)
     {
-        row = (uint32_t)r;
+        half = (uint32_t)(r >> 6) * half_bytes;
+        row = (uint32_t)r & 63u;
         const int sh = rbt == 128 ? 0 : (rbt == 64 ? 1 : 2);
-        base_t = (uint32_t)nfull * (2u * 128u * 128u);
-        row_t = (uint32_t)(r >> 3) * (uint32_t)(8 * rbt) + (uint32_t)(r & 7) * (uint32_t)rbt;
+        base_t = half + (uint32_t)nfull * (2u * 64u * 128u);
+        row_t = row * (uint32_t)rbt;
         xor_t = (uint32_t)((r >> sh) & ((rbt >> 4) - 1));
-        lo_t = 128u * (uint32_t)rbt;
+        lo_t = 64u * (uint32_t)rbt;
         full8 = nfull * 8;
     }
     // byte offset of the 16-byte chunk holding columns [8*c16g, 8*c16g+8); *lo_off = distance to the lo tile
     __device__ __forceinline__ uint32_t chunk(int c16g, uint32_t *lo_off) const
     {
         if (c16g < full8) {
-            *lo_off = 128u * 128u;
-            return (uint32_t)(c16g >> 3) * (2u * 128u * 128u) + sw128_chunk(row, (uint32_t)c16g & 7u);
+            *lo_off = 64u * 128u;
+            return half + (uint32_t)(c16g >> 3) * (2u * 64u * 128u) + sw128_chunk(row, (uint32_t)c16g & 7u);
         }
         *lo_off = lo_t;
         return base_t + row_t + (((uint32_t)(c16g - full8) ^ xor_t) << 4);
@@ -115,17 +121,14 @@ struct SfRowMap {
 // time (any stack the planner accepts); SfStat<...> answers at COMPILE time for the stacks of the shipped 3DSSD
 // configuration, so that after unrolling the layer loop every address computation, chunk bound and pooling width is a
 // literal (integer / branch / uniform-register bookkeeping of exactly these questions is otherwise a large share of the
-// kernel's issued instructions).
+// kernel's issued instructions) and every accumulator fragment index is resolved at compile time.
 __host__ __device__ constexpr int sf_r16(int x) { return (x + 15) / 16 * 16; }
 // Operand layout of a layer with padded K = kp: nfull 64-wide k-blocks of 128-byte rows + a tail block whose rows are
 // 32 / 64 / 128 bytes for a remainder of 16 / 32 / 48 columns (must match params._k_blocks)
 __host__ __device__ constexpr int sf_nfull(int kp) { return kp / 64; }
 __host__ __device__ constexpr int sf_rbt(int kp) { return kp % 64 == 0 ? 0 : (kp % 64 <= 16 ? 32 : (kp % 64 <= 32 ? 64 : 128)); }
-// operand buffer: { hi | lo } tiles of 128 rows per block, 1 KiB granular
-__host__ __device__ constexpr uint32_t sf_abuf_bytes(int kp)
-{
-    return (uint32_t)((sf_nfull(kp) * 2 * 128 * 128 + 2 * 128 * sf_rbt(kp) + 1023) / 1024 * 1024);
-}
+// operand buffer: { hi | lo } tiles of 128 rows per block (a multiple of 8 KiB, so each row half is 1 KiB aligned)
+__host__ __device__ constexpr uint32_t sf_abuf_bytes(int kp) { return (uint32_t)(sf_nfull(kp) * 2 * 128 * 128 + 2 * 128 * sf_rbt(kp)); }
 // one half (hi or lo) of a layer's weight image
 __host__ __device__ constexpr uint32_t sf_wimg_bytes(int kp, int npad) { return (uint32_t)(npad * (sf_nfull(kp) * 128 + sf_rbt(kp))); }
 
@@ -149,7 +152,6 @@ struct SfDyn {
     __device__ __forceinline__ uint32_t w_total() const { return p.w_total; }
     __device__ __forceinline__ uint32_t ss_total() const { return p.ss_total; }
     __device__ __forceinline__ uint32_t abuf_bytes() const { return p.abuf_bytes; }
-    __device__ __forceinline__ uint32_t acc_cols() const { return p.acc_cols; }
 };
 
 // Hoisted stacks of two convs (the shipped configuration): operand width K0 = n1 of the hoisted first conv, then
@@ -175,7 +177,6 @@ struct SfStat {
     __device__ __forceinline__ constexpr uint32_t w_total() const { return 2u * w_half(0) + 2u * w_half(1); }
     __device__ __forceinline__ constexpr uint32_t ss_total() const { return 2u * (uint32_t)sspad(0) + 2u * (uint32_t)sspad(1); }
     __device__ __forceinline__ constexpr uint32_t abuf_bytes() const { return sf_abuf_bytes(KP0) > sf_abuf_bytes(NP0) ? sf_abuf_bytes(KP0) : sf_abuf_bytes(NP0); }
-    __device__ __forceinline__ constexpr uint32_t acc_cols() const { return (uint32_t)((NP0 > NP1 ? NP0 : NP1) + 31) / 32 * 32; }
 };
 
 #ifdef SF_PROFILE
@@ -185,68 +186,24 @@ __device__ long long sf_prof[16];
 #define SF_T(i) do { } while (0)
 #endif
 
-// Max-pool of one 32-column chunk over runs of POOL rows + mask + store.  AFTER: v holds RAW accumulators and the folded
-// affine + ReLU is applied to the pooled values only (valid when the layer's scale is >= 0: fma(x, s, t) is then monotone
-// non-decreasing in x, so max_i relu(fma(x_i, s, t)) == relu(fma(max_i x_i, s, t)) exactly) -- 1/POOL of the epilogue math.
-template <int POOL, bool AFTER>
-__device__ __forceinline__ void sf_pool_store(const SfParams &p, float (&v)[32], int lane, int q, int tile,
-                                              int col0, int nout, float *xs, int wg_bar, const float *sc, const float *sh)
+// Calls f(std::integral_constant<int, W>()) for the width w of a column chunk: 64, or the 16 / 32 / 48 remainder of a layer
+// (the wgmma width is part of the instruction)
+template <class F>
+__device__ __forceinline__ void sf_with_width(int w, F &&f)
 {
-    constexpr int GP = POOL >= 32 ? 32 : POOL;
-    constexpr int KEEP = 32 / GP;
-    constexpr int WPG = POOL > 32 ? POOL / 32 : 1;
-    warp_colmax_transpose<GP>(v, lane);                   // lane owns columns (lane % GP) * KEEP + k in v[k]
-    if (POOL > 32) {                                      // groups spanning 2 or 4 warps: combine through shared memory
-        xs[q * 32 + lane] = v[0];
-        named_bar_sync(wg_bar, 128);
-        if ((q % WPG) == 0) {
-#pragma unroll
-            for (int w = 1; w < WPG; w++) v[0] = fmaxf(v[0], xs[(q + w) * 32 + lane]);
-        }
-        named_bar_sync(wg_bar, 128);
-        if ((q % WPG) != 0) return;
-    }
-    const int gg = tile * (128 / POOL) + (q * 32 + lane) / POOL;
-    if ((long)gg * POOL >= p.rows) return;
-    const bool masked = p.cnt && p.cnt[gg] == 0;
-#pragma unroll
-    for (int k = 0; k < KEEP; k++) {
-        const int cc = (lane % GP) * KEEP + k;
-        const int col = col0 + cc;
-        if (col >= nout) continue;
-        float mx = v[k];
-        if (AFTER) mx = fmaxf(fmaf(mx, sc[col0 + cc], sh[col0 + cc]), 0.0f);
-        store_pooled_value(mx, masked, (size_t)gg, col, p.out_f32, p.ld_f32, p.out_hi, p.out_lo, p.ld_split);
-    }
+    if (w == 64) f(std::integral_constant<int, 64>());
+    else if (w == 48) f(std::integral_constant<int, 48>());
+    else if (w == 32) f(std::integral_constant<int, 32>());
+    else f(std::integral_constant<int, 16>());
 }
 
-// Unit-list mode: a unit is 8 rows = 8 consecutive lanes.  Max over the unit, then atomicMax into out[group] (post-ReLU
-// values; the caller's zero fill is also the result of a group without hits, the mask of layers_util.py:180).
-template <bool AFTER>
-__device__ __forceinline__ void sf_pool_atomic8(const SfParams &p, float (&v)[32], int lane, int col0, int nout, const float *sc,
-                                                const float *sh, int group, bool ok)
-{
-    warp_colmax_transpose<8>(v, lane);                    // lane owns columns (lane % 8) * 4 + k of its unit in v[k]
-    if (!ok) return;
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        const int cc = (lane & 7) * 4 + k;
-        const int col = col0 + cc;
-        if (col >= nout) continue;
-        float mx = v[k];
-        if (AFTER) mx = fmaxf(fmaf(mx, sc[col0 + cc], sh[col0 + cc]), 0.0f);
-        atomic_max_nonneg(p.out_f32 + (size_t)group * p.ld_f32 + col, mx);
-    }
-}
-
-// One work item of a layer's MMAs: rows 64*hf .. 64*hf+63 of the slot's tile, output columns n0 .. n0+W-1, over the
-// whole K of layer l (full 64-wide blocks + the tail block), issued by one warpgroup as a single wgmma chain; the fp32
-// result is staged row-major in acc (pitch floats per row), where the row-per-thread epilogue reads it.
+// The MMAs of one column chunk: rows of the row half at abase (64 rows), output columns n0 .. n0+W-1, over the whole K of
+// layer l (full 64-wide blocks + the tail block), issued by one warpgroup as a single wgmma chain into d and committed;
+// the caller waits.  Thread t of warp w holds rows 16w + t/4 (d[4j], d[4j+1]) and +8 (d[4j+2], d[4j+3]) of columns
+// n0 + 8j + 2(t%4) + {0, 1} (wgmma.cuh).
 template <int W, class C>
-__device__ __forceinline__ void sf_mma_chunk(const C &cfg, int l, uint32_t abase, uint32_t wbase, int hf, int n0, float *acc,
-                                             int pitch, int wq, int lane)
+__device__ __forceinline__ void sf_mma_chain(const C &cfg, int l, uint32_t abase, uint32_t wbase, int n0, float (&d)[W / 2])
 {
-    float d[W / 2];
     const int nfull = cfg.nfull(l), rbt = cfg.rbt(l);
     const uint32_t npad = (uint32_t)cfg.npad(l), whalf = cfg.w_half(l);
     uint32_t accumulate = 0u;
@@ -254,9 +211,9 @@ __device__ __forceinline__ void sf_mma_chunk(const C &cfg, int l, uint32_t abase
     wg_fence();
 #pragma unroll (C::kStatic ? 4 : 1)
     for (int kb = 0; kb < nfull; kb++) {
-        const uint64_t a_hi = wg_desc(abase + (uint32_t)kb * (2u * 128u * 128u) + (uint32_t)hf * (64u * 128u), 128);
+        const uint64_t a_hi = wg_desc(abase + (uint32_t)kb * (2u * 64u * 128u), 128);
         const uint64_t b_hi = wg_desc(wbase + (uint32_t)kb * (npad * 128u) + (uint32_t)n0 * 128u, 128);
-        const uint64_t a_lo = a_hi + ((128u * 128u) >> 4), b_lo = b_hi + (whalf >> 4);
+        const uint64_t a_lo = a_hi + ((64u * 128u) >> 4), b_lo = b_hi + (whalf >> 4);
 #pragma unroll
         for (int kin = 0; kin < 4; kin++) {
             wg_mma3<W>(d, a_hi + 2 * kin, a_lo + 2 * kin, b_hi + 2 * kin, b_lo + 2 * kin, accumulate);
@@ -264,9 +221,9 @@ __device__ __forceinline__ void sf_mma_chunk(const C &cfg, int l, uint32_t abase
         }
     }
     if (rbt) {
-        const uint64_t a_hi = wg_desc(abase + (uint32_t)nfull * (2u * 128u * 128u) + (uint32_t)hf * (64u * (uint32_t)rbt), rbt);
+        const uint64_t a_hi = wg_desc(abase + (uint32_t)nfull * (2u * 64u * 128u), rbt);
         const uint64_t b_hi = wg_desc(wbase + (uint32_t)nfull * (npad * 128u) + (uint32_t)n0 * (uint32_t)rbt, rbt);
-        const uint64_t a_lo = a_hi + ((128u * (uint32_t)rbt) >> 4), b_lo = b_hi + (whalf >> 4);
+        const uint64_t a_lo = a_hi + ((64u * (uint32_t)rbt) >> 4), b_lo = b_hi + (whalf >> 4);
         const int nt = rbt == 128 ? 3 : (rbt >> 5);              // 16-wide k-steps of the tail block
 #pragma unroll (C::kStatic ? 3 : 1)
         for (int kin = 0; kin < nt; kin++) {
@@ -275,21 +232,31 @@ __device__ __forceinline__ void sf_mma_chunk(const C &cfg, int l, uint32_t abase
         }
     }
     wg_commit();
-    wg_wait<0>();
-    const int r0 = hf * 64 + wq * 16 + (lane >> 2), c = n0 + 2 * (lane & 3);
-#pragma unroll
-    for (int j = 0; j < W / 8; j++) {
-        *reinterpret_cast<float2 *>(acc + r0 * pitch + c + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
-        *reinterpret_cast<float2 *>(acc + (r0 + 8) * pitch + c + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+}
+
+// Calls f(std::integral_constant<int, c>()) for c = 0 .. n-1 (n <= SF_MAX_NCH): the chunk index is a literal before any
+// loop unrolling, so the accumulator arrays it selects stay in registers
+template <int C0 = 0, class F>
+__device__ __forceinline__ void sf_for_chunks(int n, F &&f)
+{
+    if constexpr (C0 < SF_MAX_NCH) {
+        if (C0 < n) {
+            f(std::integral_constant<int, C0>());
+            sf_for_chunks<C0 + 1>(n, f);
+        }
     }
 }
 
-// SLOTS tiles in flight per CTA, WG warpgroups (128 threads) working on each: the warpgroups of a slot split the
-// 16-byte chunks of the gather and the 32-column chunks of every epilogue between them.  C: shape policy (above).
+// Width of column chunk c of a layer with npad columns
+__device__ __forceinline__ int sf_chunk_w(int npad, int c) { return npad - 64 * c < 64 ? npad - 64 * c : 64; }
+
+// SLOTS tiles in flight per CTA, WG warpgroups (128 threads) working on each: WG == 1 runs the two row halves of its tile
+// in turn, WG == 2 gives each warpgroup one row half for the whole tile (gather, every layer, pool).  C: shape policy.
 template <class C, int SLOTS, int WG>
 __global__ void __launch_bounds__(SF_THREADS * SLOTS * WG, SLOTS * WG == 1 ? 6 : 1)
 sa_fused_kernel(const SfParams p)
 {
+    static_assert(WG == 1 || WG == 2, "sa_fused: one warpgroup per slot or one per row half");
     const C cfg(p);
     // pointers inside the by-value parameter struct carry no address space: tell the compiler they are global
     __builtin_assume(__isGlobal(p.xyz)); __builtin_assume(__isGlobal(p.new_xyz)); __builtin_assume(__isGlobal(p.idx));
@@ -302,23 +269,25 @@ sa_fused_kernel(const SfParams p)
     uint8_t *wsm = smem + (size_t)SLOTS * cfg.abuf_bytes();  // weight images (1024-aligned: buffers are multiples of 1 KiB)
     float *ss = reinterpret_cast<float *>(wsm + cfg.w_total());
     float *wxs = ss + cfg.ss_total();                    // [3][kp0] hoisted mode: Wx * s1, zero beyond c
-    const int pitch = (int)cfg.acc_cols() + 4;           // staged accumulator row: +4 floats keep the accesses conflict-free
-    float *acc_all = wxs + 3 * cfg.kp(0);                // [SLOTS][128][pitch], 16-byte aligned (kp0 % 16 == 0)
+    float *xs_all = wxs + 3 * cfg.kp(0);                 // [SLOTS][SF_XS_FLOATS] pooled-value exchange
 
     __shared__ unsigned long long w_bar;
-    __shared__ float xs_all[SLOTS * WG][4 * 32];
 
     constexpr int NT = SF_THREADS * SLOTS * WG, ST = SF_THREADS * WG;     // threads per CTA / per slot
-    constexpr int U = WG == 1 ? 4 : (WG == 2 ? 3 : 2);   // gather chunks in flight per thread
-    const int tid = threadIdx.x, lane = tid & 31, q = (tid >> 5) & 3;
+    constexpr int U = WG == 1 ? 4 : 3;                   // gather chunks in flight per thread
+    const int tid = threadIdx.x, lane = tid & 31, q = (tid >> 5) & 3, t = tid & 127;
     const int slot = tid / ST, wg = (tid >> 7) % WG;
-    const int r = tid & 127;                             // row of the slot's tile this thread works on
+    // gather: WG == 1: thread t builds row t; WG == 2: warpgroup wg builds row half wg, two threads per row (`phase`)
+    const int r = WG == 1 ? t : 64 * wg + (t & 63);
+    const int phase = WG == 1 ? 0 : t >> 6;
+    const int cq = 2 * (lane & 3);                       // this thread's column pair inside each 8 columns of a fragment
     // warp-uniform copies (shfl) so that descriptors are computed on the uniform datapath
     const int slot_u = __shfl_sync(0xffffffffu, slot, 0), wg_u = __shfl_sync(0xffffffffu, wg, 0);
     const int slot_bar = 1 + slot, wg_bar = 1 + SLOTS + slot * WG + wg;
     uint8_t *buf = smem + (size_t)slot * cfg.abuf_bytes();   // the slot's operand buffer (every layer, in place)
-    float *xs = xs_all[slot * WG + wg];
-    float *acc = acc_all + (size_t)slot * 128 * pitch;
+    float *xs = xs_all + (size_t)slot * SF_XS_FLOATS;
+    const uint32_t half_bytes = cfg.abuf_bytes() / 2;
+    const uint32_t abuf_u = smem_u32(smem) + (uint32_t)slot_u * cfg.abuf_bytes();
     const int kp0 = cfg.kp(0);
 
     if (tid == 0) {
@@ -333,8 +302,6 @@ sa_fused_kernel(const SfParams p)
             const int a3 = i / kp0, k = i - a3 * kp0;
             wxs[i] = k < cfg.c() ? __ldg(p.wx + a3 * cfg.c() + k) : 0.0f;
         }
-    // staged columns a layer narrower than acc_cols leaves unwritten are multiplied by a zero scale: keep them finite
-    for (int i = tid; i < SLOTS * 128 * pitch; i += NT) acc_all[i] = 0.0f;
     __syncthreads();
     mbar_wait_cta(smem_u32(&w_bar), 0);                  // weights landed (async proxy writes, read by wgmma only)
 
@@ -354,24 +321,22 @@ sa_fused_kernel(const SfParams p)
     const int tiles = compact ? (nunits + 15) >> 4 : p.tiles;
     // neighbour index (and, in unit-list mode, unit descriptor) of this thread's row, fetched one tile ahead
     // (rows < 2^31: checked by the launcher)
-    auto fetch = [&](int t, int &desc, int &a) {
+    auto fetch = [&](int tl, int &desc, int &a) {
         desc = -1; a = 0;
-        if (t >= tiles) return;
+        if (tl >= tiles) return;
         if (compact) {
-            const int ui = t * 16 + (r >> 3);
+            const int ui = tl * 16 + (r >> 3);
             if (ui < nunits) {
                 desc = __ldg(units + 1 + ui);
                 a = __ldg(p.idx + unit_slot((uint32_t)desc, (uint32_t)cfg.ns(), (uint32_t)r & 7u));
             }
-        } else if ((long)t * 128 + r < p.rows) {
+        } else if ((long)tl * 128 + r < p.rows) {
             desc = 0;
-            a = __ldg(p.idx + (size_t)t * 128u + r);
+            a = __ldg(p.idx + (size_t)tl * 128u + r);
         }
     };
     int d_next, a_next;
     fetch(tile0, d_next, a_next);
-    int my_group = 0;                                                  // unit-list mode: the group this thread's row belongs to
-    bool my_ok = false;
     for (int tile = tile0; tile < tiles; tile += tstep) {
         // ---- gather + centre-subtract + concat + split -> buf (layers_util.py:157-165)
         {
@@ -380,19 +345,18 @@ sa_fused_kernel(const SfParams p)
             const uint32_t qi = !ok ? 0u : (compact ? unit_group((uint32_t)d_next) : row / (uint32_t)cfg.ns());    // == scene*m + query
             const uint32_t scene = qi / (uint32_t)p.m;
             const int a = a_next;
-            my_group = (int)qi; my_ok = ok;
             fetch(tile + tstep, d_next, a_next);
             const float *src_f = p.points + ((size_t)scene * p.n + a) * src_pitch;
             const float *src_x = p.xyz + ((size_t)scene * p.n + a) * 3;
             const float *ctr = p.new_xyz + (size_t)qi * 3;
             const int nchunk = kp0 >> 3;
-            const SfRowMap map0(r, cfg.nfull(0), cfg.rbt(0));
+            const SfRowMap map0(r, cfg.nfull(0), cfg.rbt(0), half_bytes);
             float dx = 0.0f, dy = 0.0f, dz = 0.0f;
             if (cfg.hoist() && ok) {
                 dx = __ldg(src_x) - __ldg(ctr); dy = __ldg(src_x + 1) - __ldg(ctr + 1); dz = __ldg(src_x + 2) - __ldg(ctr + 2);
             }
 #pragma unroll (C::kStatic ? 4 : 1)
-            for (int cg0 = wg * U; cg0 < nchunk; cg0 += WG * U) {     // U chunks of 8 columns in flight per thread
+            for (int cg0 = phase * U; cg0 < nchunk; cg0 += WG * U) {  // U chunks of 8 columns in flight per thread
                 float f[U][8];
 #pragma unroll
                 for (int u = 0; u < U; u++) load_concat8(f[u], src_f, src_x, ctr, cfg.c(), k0, (cg0 + u) * 8, vec, ok);
@@ -412,125 +376,162 @@ sa_fused_kernel(const SfParams p)
         SF_T(0);                                                       // gather
 #pragma unroll (C::kStatic ? SF_MAX_LAYERS : 1)
         for (int l = 0; l < cfg.nl(); l++) {
-            // operand written with ordinary stores -> make it visible to the tensor-core (async) proxy; the barrier also
-            // orders the previous layer's staged-accumulator reads before this layer's MMAs overwrite the staging
+            // the half's operand was written with ordinary stores by this warpgroup -> visible to the tensor-core (async) proxy
             fence_async_smem();
-            named_bar_sync(slot_bar, ST);
-            SF_T(1 + 4 * l);                                           // barrier
-            {
-                // work items (64-row half, <= 64-column chunk) of this layer, round robin over the slot's warpgroups: one
-                // wgmma per k-step covers the whole chunk width; chunk widths are 64 but for a 16 / 32 / 48 tail
-                const uint32_t abase = smem_u32(smem) + (uint32_t)slot_u * cfg.abuf_bytes();
-                const uint32_t wbase = smem_u32(wsm) + cfg.w_off(l);
-                const int npad = cfg.npad(l), nch = (npad + 63) / 64;
-#pragma unroll (C::kStatic ? 8 : 1)
-                for (int item = wg_u; item < 2 * nch; item += WG) {
-                    const int hf = item & 1, n0 = (item >> 1) * 64, w = npad - n0 < 64 ? npad - n0 : 64;
-                    if (w == 64) sf_mma_chunk<64>(cfg, l, abase, wbase, hf, n0, acc, pitch, q, lane);
-                    else if (w == 48) sf_mma_chunk<48>(cfg, l, abase, wbase, hf, n0, acc, pitch, q, lane);
-                    else if (w == 32) sf_mma_chunk<32>(cfg, l, abase, wbase, hf, n0, acc, pitch, q, lane);
-                    else sf_mma_chunk<16>(cfg, l, abase, wbase, hf, n0, acc, pitch, q, lane);
-                }
-            }
-            SF_T(2 + 4 * l);                                           // MMAs
-            named_bar_sync(slot_bar, ST);                              // every MMA of the tile done: staging complete, buf free
-            SF_T(3 + 4 * l);                                           // MMA wait
-            // ---- epilogue of layer l
+            named_bar_sync(wg_bar, 128);
+            const uint32_t wbase = smem_u32(wsm) + cfg.w_off(l);
+            const int npad = cfg.npad(l), nch = (npad + 63) / 64;
             const float *sc = ss + cfg.ss_off(l);
-            const float *sh = sc + cfg.sspad(l);
-            const bool last = l == cfg.nl() - 1;
-            const bool pool_first = last && p.pool_first;              // last layer with scale >= 0: pool raw accumulators
-            const SfRowMap mapn(r, last ? 0 : cfg.nfull(l + 1), last ? 32 : cfg.rbt(l + 1));
-            const int nchunks = (cfg.npad(l) + 31) / 32;
-#pragma unroll (C::kStatic ? 4 : 1)
-            for (int ci = wg; ci < nchunks; ci += WG) {
-                const int c0 = ci * 32;
-                float rr[32];
+            const float *sh = sc + cfg.sspad(l);                       // scale/shift are zero-padded to 32-column chunks
+            if (l < cfg.nl() - 1) {
+                // ---- a hidden layer: every chunk of the half into registers, then scale/shift/ReLU/split IN PLACE
 #pragma unroll
-                for (int j4 = 0; j4 < 32; j4 += 4) {
-                    const float4 a4 = *reinterpret_cast<const float4 *>(acc + r * pitch + c0 + j4);
-                    rr[j4] = a4.x; rr[j4 + 1] = a4.y; rr[j4 + 2] = a4.z; rr[j4 + 3] = a4.w;
+                for (int hi = 0; hi < 2 / WG; hi++) {
+                    const int hf = WG == 1 ? hi : wg_u;
+                    const uint32_t abase = abuf_u + (uint32_t)hf * half_bytes;
+                    float d[SF_MAX_NCH][32];
+                    sf_for_chunks(nch, [&](auto cc) {
+                        constexpr int c = decltype(cc)::value;
+                        sf_with_width(sf_chunk_w(npad, c), [&](auto wc) {
+                            constexpr int W = decltype(wc)::value;
+                            sf_mma_chain<W>(cfg, l, abase, wbase, 64 * c, *reinterpret_cast<float(*)[W / 2]>(&d[c][0]));
+                        });
+                    });
+                    wg_wait<0>();                                      // the half's operand is free from here on
+                    const int r0 = 64 * hf + 16 * q + (lane >> 2);
+                    const SfRowMap m0(r0, cfg.nfull(l + 1), cfg.rbt(l + 1), half_bytes);
+                    const SfRowMap m1(r0 + 8, cfg.nfull(l + 1), cfg.rbt(l + 1), half_bytes);
+                    sf_for_chunks(nch, [&](auto cc) {
+                        constexpr int c = decltype(cc)::value;
+                        sf_with_width(sf_chunk_w(npad, c), [&](auto wc) {
+                            constexpr int W = decltype(wc)::value;
+#pragma unroll
+                            for (int j = 0; j < W / 8; j++) {
+                                const int col = 64 * c + 8 * j + cq;
+                                const float2 s2 = *reinterpret_cast<const float2 *>(sc + col);
+                                const float2 h2 = *reinterpret_cast<const float2 *>(sh + col);
+                                // every conv has a ReLU; a column pair is 4 bytes of one 16-byte chunk of the next operand
+                                uint32_t hw, lw, lo_off;
+                                split_pair(fmaxf(fmaf(d[c][4 * j], s2.x, h2.x), 0.0f), fmaxf(fmaf(d[c][4 * j + 1], s2.y, h2.y), 0.0f), hw, lw);
+                                uint32_t off = m0.chunk(8 * c + j, &lo_off) + 2u * (uint32_t)cq;
+                                *reinterpret_cast<uint32_t *>(buf + off) = hw;
+                                *reinterpret_cast<uint32_t *>(buf + off + lo_off) = lw;
+                                split_pair(fmaxf(fmaf(d[c][4 * j + 2], s2.x, h2.x), 0.0f), fmaxf(fmaf(d[c][4 * j + 3], s2.y, h2.y), 0.0f), hw, lw);
+                                off = m1.chunk(8 * c + j, &lo_off) + 2u * (uint32_t)cq;
+                                *reinterpret_cast<uint32_t *>(buf + off) = hw;
+                                *reinterpret_cast<uint32_t *>(buf + off + lo_off) = lw;
+                            }
+                        });
+                    });
                 }
-                float v[32];
-                if (pool_first) {
+            } else {
+                // ---- the last layer: one chunk at a time (nothing is written in place), max-pooled on the fragment.
+                // pool_first (scale >= 0): fma(x, s, t) is then monotone non-decreasing in x, so max_i relu(fma(x_i, s, t))
+                // == relu(fma(max_i x_i, s, t)) exactly -- the affine + ReLU runs on the pooled values only.
+                const bool pool_first = p.pool_first != 0;
+                const int ns = cfg.ns(), nout = cfg.nout(l);
+                auto finish = [&](float mx, int col) { return pool_first ? fmaxf(fmaf(mx, sc[col], sh[col]), 0.0f) : mx; };
+#pragma unroll (C::kStatic ? SF_MAX_NCH : 1)
+                for (int c = 0; c < nch; c++)
+                    sf_with_width(sf_chunk_w(npad, c), [&](auto wc) {
+                        constexpr int W = decltype(wc)::value;
 #pragma unroll
-                    for (int j = 0; j < 32; j++) v[j] = rr[j];
-                } else {
+                        for (int hi = 0; hi < 2 / WG; hi++) {
+                            const int hf = WG == 1 ? hi : wg_u;
+                            float d[W / 2];
+                            sf_mma_chain<W>(cfg, l, abuf_u + (uint32_t)hf * half_bytes, wbase, 64 * c, d);
+                            wg_wait<0>();
+                            if (!pool_first) {
 #pragma unroll
-                    for (int j4 = 0; j4 < 32; j4 += 4) {              // scale/shift are zero-padded to 32-column chunks
-                        const float4 s4 = *reinterpret_cast<const float4 *>(sc + c0 + j4);
-                        const float4 h4 = *reinterpret_cast<const float4 *>(sh + c0 + j4);
-                        v[j4 + 0] = fmaxf(fmaf(rr[j4 + 0], s4.x, h4.x), 0.0f);   // every conv has a ReLU
-                        v[j4 + 1] = fmaxf(fmaf(rr[j4 + 1], s4.y, h4.y), 0.0f);
-                        v[j4 + 2] = fmaxf(fmaf(rr[j4 + 2], s4.z, h4.z), 0.0f);
-                        v[j4 + 3] = fmaxf(fmaf(rr[j4 + 3], s4.w, h4.w), 0.0f);
-                    }
-                }
-                if (!last) {
+                                for (int j = 0; j < W / 8; j++) {
+                                    const float2 s2 = *reinterpret_cast<const float2 *>(sc + 64 * c + 8 * j + cq);
+                                    const float2 h2 = *reinterpret_cast<const float2 *>(sh + 64 * c + 8 * j + cq);
+                                    d[4 * j] = fmaxf(fmaf(d[4 * j], s2.x, h2.x), 0.0f);
+                                    d[4 * j + 1] = fmaxf(fmaf(d[4 * j + 1], s2.y, h2.y), 0.0f);
+                                    d[4 * j + 2] = fmaxf(fmaf(d[4 * j + 2], s2.x, h2.x), 0.0f);
+                                    d[4 * j + 3] = fmaxf(fmaf(d[4 * j + 3], s2.y, h2.y), 0.0f);
+                                }
+                            }
+                            // 8-row maxima: lane owns slots s = i + (W/16)(lane/4) of d, column 8(s/4) + cq + (s%2) of the
+                            // 8-row slab (s/2)%2 of its warp's 16 rows
+                            quad_rowmax_transpose<W / 2>(d, lane);
 #pragma unroll
-                    for (int j8 = 0; j8 < 32; j8 += 8) {
-                        if (c0 + j8 >= cfg.kp(l + 1)) break;
-                        uint4 h, l;
-                        uint32_t lo_off;
-                        split8(v, j8, h, l);
-                        const uint32_t off = mapn.chunk((c0 + j8) >> 3, &lo_off);
-                        *reinterpret_cast<uint4 *>(buf + off) = h;
-                        *reinterpret_cast<uint4 *>(buf + off + lo_off) = l;
-                    }
-                } else if (compact) {
-                    if (pool_first) sf_pool_atomic8<true>(p, v, lane, c0, cfg.nout(l), sc, sh, my_group, my_ok);
-                    else sf_pool_atomic8<false>(p, v, lane, c0, cfg.nout(l), sc, sh, my_group, my_ok);
-                } else if (pool_first) {
-                    switch (cfg.ns()) {
-                        case 8: sf_pool_store<8, true>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                        case 16: sf_pool_store<16, true>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                        case 32: sf_pool_store<32, true>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                        case 64: sf_pool_store<64, true>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                        default: sf_pool_store<128, true>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                    }
-                } else {
-                    switch (cfg.ns()) {
-                        case 8: sf_pool_store<8, false>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                        case 16: sf_pool_store<16, false>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                        case 32: sf_pool_store<32, false>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                        case 64: sf_pool_store<64, false>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                        default: sf_pool_store<128, false>(p, v, lane, q, tile, c0, cfg.nout(l), xs, wg_bar, sc, sh); break;
-                    }
-                }
+                            for (int i = 0; i < W / 16; i++) {
+                                const int s = i + (W / 16) * (lane >> 2);
+                                const int slab = 8 * hf + 2 * q + ((s >> 1) & 1);      // 8-row slab of the tile
+                                const int cl = 8 * (s >> 2) + cq + (s & 1), col = 64 * c + cl;
+                                if (compact) {                         // a slab is one listed unit: atomicMax into its group
+                                    const int ui = tile * 16 + slab;
+                                    if (ui < nunits && col < nout)
+                                        atomic_max_nonneg(p.out_f32 + (size_t)unit_group((uint32_t)__ldg(units + 1 + ui)) * p.ld_f32 + col,
+                                                          finish(d[i], col));
+                                } else if (ns == 8) {
+                                    const long gg = (long)tile * 16 + slab;
+                                    if (gg * 8 < p.rows && col < nout)
+                                        store_pooled_value(finish(d[i], col), p.cnt && p.cnt[gg] == 0, (size_t)gg, col, p.out_f32,
+                                                           p.ld_f32, p.out_hi, p.out_lo, p.ld_split);
+                                } else {
+                                    xs[slab * 64 + cl] = d[i];
+                                }
+                            }
+                        }
+                        if (!compact && ns > 8) {
+                            // groups of 16-128 rows: the slabs of a group meet in xs.  A team is the threads whose slabs
+                            // they are: the slot's warpgroup (WG == 1), the half's warpgroup, or both halves (128 rows, WG == 2)
+                            const bool both = WG == 2 && ns == 128;
+                            const int bar = both ? slot_bar : wg_bar, nthr = both ? ST : 128, tt = both ? tid % ST : t;
+                            const int slab0 = WG == 2 && !both ? 8 * wg : 0, per = ns / 8;
+                            const int outs = ((WG == 1 || both ? 16 : 8) / per) * W;
+                            named_bar_sync(bar, nthr);
+                            for (int o = tt; o < outs; o += nthr) {
+                                const int gl = o / W, cl = o - gl * W, col = 64 * c + cl;
+                                const float *x = xs + (slab0 + gl * per) * 64 + cl;
+                                float mx = x[0];
+                                for (int k = 1; k < per; k++) mx = fmaxf(mx, x[k * 64]);
+                                const long gg = (long)tile * (128 / ns) + slab0 * 8 / ns + gl;
+                                if (gg * ns < p.rows && col < nout)
+                                    store_pooled_value(finish(mx, col), p.cnt && p.cnt[gg] == 0, (size_t)gg, col, p.out_f32,
+                                                       p.ld_f32, p.out_hi, p.out_lo, p.ld_split);
+                            }
+                            named_bar_sync(bar, nthr);                         // xs reusable by the next chunk
+                        }
+                    });
             }
-            SF_T(4 + 4 * l);                                           // epilogue
+            SF_T(1 + l);                                               // layer l
         }
     }
-
 }
 
 }  // namespace ssd3d
 
 using namespace ssd3d;
 
-struct SfPlan { size_t abuf, acc, w, ssf; int maxn; };
+struct SfPlan { size_t abuf, w, ssf; };
 static bool sf_plan(int k_in, int nl, const int *nout, SfPlan *pl)      // k_in: columns of the first operand
 {
     if (nl < 1 || nl > SF_MAX_LAYERS) return false;
-    pl->abuf = 0; pl->w = 0; pl->ssf = 0; pl->maxn = 32;
+    pl->abuf = 0; pl->w = 0; pl->ssf = 0;
     int kp = (k_in + 15) / 16 * 16;
     pl->ssf = 3 * (size_t)kp;                               // room for the hoisted mode's Wx table
     for (int l = 0; l < nl; l++) {
         const int npad = (nout[l] + 15) / 16 * 16;
-        if (npad > 256) return false;
+        if (npad > 64 * SF_MAX_NCH) return false;
         const size_t a = sf_abuf_bytes(kp);
         if (a > pl->abuf) pl->abuf = a;
         pl->w += 2 * sf_wimg_bytes(kp, npad);
         pl->ssf += (size_t)2 * ((npad + 31) / 32 * 32);
-        if (npad > pl->maxn) pl->maxn = npad;
         kp = npad;
     }
-    pl->acc = (size_t)128 * ((pl->maxn + 31) / 32 * 32 + 4) * sizeof(float);   // staged accumulator of one slot
     return true;
 }
-static size_t sf_total(const SfPlan &pl, int slots) { return slots * (pl.abuf + pl.acc) + pl.w + pl.ssf * sizeof(float) + 1024; }
+// per slot: the operand buffer and the pooled-value exchange; per CTA: weights, scale/shift, Wx table, alignment slack
+static size_t sf_total(const SfPlan &pl, int slots) { return slots * (pl.abuf + SF_XS_FLOATS * sizeof(float)) + pl.w + pl.ssf * sizeof(float) + 1024; }
 constexpr size_t SF_SMEM_MAX = 226 * 1024;
 constexpr size_t SF_SMALL = 72 * 1024;                     // <= this: single-slot, single-warpgroup CTAs, several per SM
+// Slots of larger stacks: two slots of two warpgroups (512 threads) leave 128 registers per thread, which hold a hidden
+// layer's accumulators (up to 48 per thread in the shipped stacks) and the fragment epilogue without spills; a third slot
+// would cut that to 80.
+constexpr int SF_MAX_SLOTS = 2;
 
 // Developer build only (-DSSD3D_DEV_HOOKS, csrc/ssd3d_dev.h): override the slot / warpgroup shape from a probe script.
 // The shipped library has no such state.
@@ -542,13 +543,12 @@ extern "C" void ssd3d_dev_set_fused_dynamic(int on) { g_sf_dynamic = on; }   // 
 constexpr int g_sf_slots = 0, g_sf_wg = 0, g_sf_dynamic = 0;
 #endif
 
-// Slots per CTA for a stack: 1 for small stacks (several CTAs per SM), else as many as fit one SM (<= 3).
+// Slots per CTA for a stack: 1 for small stacks (several CTAs per SM), else as many as fit one SM (<= SF_MAX_SLOTS).
 static int sf_slots(const SfPlan &pl)
 {
     if (sf_total(pl, 1) <= SF_SMALL) return 1;
-    int s = g_sf_slots > 0 ? (g_sf_slots > 4 ? 4 : g_sf_slots) : 3;
-    // the kernel's static shared memory (xs_all: 512 bytes per warpgroup, two per slot) counts against the same limit
-    while (s > 1 && sf_total(pl, s) + (size_t)s * 2 * 512 > SF_SMEM_MAX) s--;
+    int s = g_sf_slots > 0 && g_sf_slots < SF_MAX_SLOTS ? g_sf_slots : SF_MAX_SLOTS;
+    while (s > 1 && sf_total(pl, s) > SF_SMEM_MAX) s--;
     return s;
 }
 
@@ -584,9 +584,9 @@ static bool sf_launch_static(const SfParams &p, int slots, int wg, size_t smem, 
         if (k0 == 16 && n0 == 16 && n1 == 32 && ns == 32) { *e = sf_launch<SfStat<16, 16, 32, 32>, 1, 1>(p, smem, per_sm, st); return true; }
         if (k0 == 32 && n0 == 32 && n1 == 64 && ns == 64) { *e = sf_launch<SfStat<32, 32, 64, 64>, 1, 1>(p, smem, per_sm, st); return true; }
     }
-    if (slots == 1 && wg == 2) {
-        if (k0 == 64 && n0 == 64 && n1 == 128 && ns == 32) { *e = sf_launch<SfStat<64, 64, 128, 32>, 1, 2>(p, smem, per_sm, st); return true; }
-        if (k0 == 64 && n0 == 96 && n1 == 128 && ns == 64) { *e = sf_launch<SfStat<64, 96, 128, 64>, 1, 2>(p, smem, per_sm, st); return true; }
+    if (slots == 2 && wg == 2) {
+        if (k0 == 64 && n0 == 64 && n1 == 128 && ns == 32) { *e = sf_launch<SfStat<64, 64, 128, 32>, 2, 2>(p, smem, per_sm, st); return true; }
+        if (k0 == 64 && n0 == 96 && n1 == 128 && ns == 64) { *e = sf_launch<SfStat<64, 96, 128, 64>, 2, 2>(p, smem, per_sm, st); return true; }
     }
     return false;
 }
@@ -645,13 +645,12 @@ static int sa_mlp_fused_impl(int b, int n, int c, int m, int nsample, const floa
     p.w_total = woff; p.ss_total = ssoff;
     p.w_blob = (const uint8_t *)w_blob; p.ss_blob = ss_blob;
     p.abuf_bytes = (uint32_t)pl.abuf;
-    p.acc_cols = (uint32_t)(pl.maxn + 31) / 32 * 32;
     p.out_f32 = out_f32; p.ld_f32 = ld_f32;
     p.out_hi = (__nv_bfloat16 *)out_hi; p.out_lo = (__nv_bfloat16 *)out_lo; p.ld_split = ld_split;
 
-    // one warpgroup per slot for small stacks (several CTAs per SM), two when a slot needs most of an SM's shared memory
+    // one warpgroup per slot for small stacks (several CTAs per SM), else one per row half
     const bool small = slots == 1 && smem <= SF_SMALL;
-    const int wg = g_sf_wg > 0 ? g_sf_wg : (small ? 1 : 2);
+    const int wg = slots == 1 && g_sf_wg > 0 ? (g_sf_wg == 1 ? 1 : 2) : (small ? 1 : 2);
     // resident CTAs per SM: bounded by shared memory and, for single-warpgroup CTAs, registers
     int per_sm = 1;
     if (slots == 1 && wg == 1) {
@@ -662,11 +661,8 @@ static int sa_mlp_fused_impl(int b, int n, int c, int m, int nsample, const floa
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaSuccess;
     if (g_sf_dynamic || !sf_launch_static(p, slots, wg, smem, per_sm, st, &e))
-        e = slots == 1 ? (wg == 1 ? sf_launch<SfDyn, 1, 1>(p, smem, per_sm, st) : sf_launch<SfDyn, 1, 2>(p, smem, per_sm, st))
-          : slots == 2 ? (wg == 4 ? sf_launch<SfDyn, 2, 4>(p, smem, per_sm, st) : wg == 1 ? sf_launch<SfDyn, 2, 1>(p, smem, per_sm, st)
-                                                                                           : sf_launch<SfDyn, 2, 2>(p, smem, per_sm, st))
-          : slots == 3 ? (wg == 1 ? sf_launch<SfDyn, 3, 1>(p, smem, per_sm, st) : sf_launch<SfDyn, 3, 2>(p, smem, per_sm, st))
-                       : sf_launch<SfDyn, 4, 1>(p, smem, per_sm, st);
+        e = slots == 2 ? sf_launch<SfDyn, 2, 2>(p, smem, per_sm, st)
+          : wg == 1 ? sf_launch<SfDyn, 1, 1>(p, smem, per_sm, st) : sf_launch<SfDyn, 1, 2>(p, smem, per_sm, st);
     if (e != cudaSuccess) return cuda_status(e, "sa_mlp_fused attr");
 #ifdef SF_PROFILE
     {
@@ -674,7 +670,7 @@ static int sa_mlp_fused_impl(int b, int n, int c, int m, int nsample, const floa
         cudaDeviceSynchronize();
         cudaMemcpyFromSymbol(h, sf_prof, sizeof(h));
         fprintf(stderr, "sf_prof slots=%d tiles=%d:", slots, p.tiles);
-        for (int i = 0; i < 13; i++) fprintf(stderr, " %lld", h[i]);
+        for (int i = 0; i < 1 + SF_MAX_LAYERS; i++) fprintf(stderr, " %lld", h[i]);
         fprintf(stderr, "\n");
         memset(h, 0, sizeof(h));
         cudaMemcpyToSymbol(sf_prof, h, sizeof(h));
