@@ -23,7 +23,6 @@
 
 namespace ssd3d {
 
-constexpr int FPS_T = 256;  // threads per CTA
 constexpr int FPS_NW = FPS_T / 32;
 // Ownership map: slot i of global thread g (g = cta_rank*256 + tid, TT = CL*256 threads per scene).
 // Each thread owns points of one residue class mod 1024 (or 1024/TT classes when TT < 1024), visited
@@ -64,7 +63,7 @@ template <int CL>
 struct FpsShared {
     FpsPacket warp_pk[2][FPS_NW];
     FpsPacket cl_pk[2][CL];
-    unsigned long long mbar[2];
+    FpsRing ring;
 };
 
 // pf_rows != nullptr (with-distance kernel): while the CTA's candidate travels to the peers, warp 0 prefetches that
@@ -77,11 +76,11 @@ __device__ __forceinline__ void fps_exchange(FpsShared<CL> &sh, int j, uint32_t 
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int par = j & 1;
-    const uint32_t u = __float_as_uint(fmaxf(best, 0.0f));
+    const uint2 cd = fps_candidate(best, my_key);
     uint32_t mx, kmin;
-    warp_argmax(u, best >= 0.0f ? my_key : KEY_INVALID, mx, kmin);
+    warp_argmax(cd.x, cd.y, mx, kmin);
     {
-        const uint32_t bal = __ballot_sync(0xffffffffu, (u == mx) && ((best >= 0.0f ? my_key : KEY_INVALID) == kmin));
+        const uint32_t bal = __ballot_sync(0xffffffffu, cd.x == mx && cd.y == kmin);
         if (lane == __ffs(bal) - 1) {
             uint4 *dst = reinterpret_cast<uint4 *>(&sh.warp_pk[par][warp]);
             dst[0] = make_uint4(mx, kmin, __float_as_uint(cx), __float_as_uint(cy));
@@ -106,12 +105,12 @@ __device__ __forceinline__ void fps_exchange(FpsShared<CL> &sh, int j, uint32_t 
             return;
         }
         constexpr int PIECES = WITH_XYZ ? 2 : 1;
-        if (lane == 0) mbar_arrive_expect_tx(smem_u32(&sh.mbar[par]), CL * PIECES * 16);
+        if (lane == 0) sh.ring.expect(j, CL * PIECES * 16);
         if (lane < PIECES * CL) {
             const int piece = WITH_XYZ ? (lane & 1) : 0;
             const uint32_t peer = WITH_XYZ ? (lane >> 1) : lane;
             const uint4 v4 = reinterpret_cast<const uint4 *>(&sh.warp_pk[par][ww])[piece];
-            st_async_v4(mapa(smem_u32(&sh.cl_pk[par][rank]) + piece * 16, peer), mapa(smem_u32(&sh.mbar[par]), peer), v4);
+            st_async_v4(mapa(smem_u32(&sh.cl_pk[par][rank]) + piece * 16, peer), mapa(sh.ring.at(j), peer), v4);
         }
         if (pf_rows != nullptr && k2 != KEY_INVALID) {
             const float *row = pf_rows + (size_t)fps_key_to_k(k2) * pf_n;
@@ -120,7 +119,7 @@ __device__ __forceinline__ void fps_exchange(FpsShared<CL> &sh, int j, uint32_t 
         }
     }
     if (CL > 1) {
-        mbar_wait_cta(smem_u32(&sh.mbar[par]), ((j - 1) >> 1) & 1);
+        sh.ring.wait(j);
         const uint32_t v = lane < CL ? sh.cl_pk[par][lane].val : 0u;
         const uint32_t kk = lane < CL ? sh.cl_pk[par][lane].key : KEY_INVALID;
         uint32_t m3, k3;
@@ -136,18 +135,6 @@ __device__ __forceinline__ void fps_exchange(FpsShared<CL> &sh, int j, uint32_t 
     }
 }
 
-template <int CL>
-__device__ __forceinline__ void fps_shared_init(FpsShared<CL> &sh)
-{
-    if (threadIdx.x == 0) {
-        mbar_init(smem_u32(&sh.mbar[0]), 1);
-        mbar_init(smem_u32(&sh.mbar[1]), 1);
-        fence_mbar_init_cluster();
-    }
-    __syncthreads();
-    if (CL > 1) cluster_sync_all();  // every CTA's barriers exist before any peer st.async targets them
-}
-
 // ---------------------------------------------------------------------------------------------------
 // D-FPS on xyz (c == 3): points + running distances live in registers.
 // ---------------------------------------------------------------------------------------------------
@@ -158,18 +145,14 @@ fps3_cluster_kernel(int n, int m, const float *__restrict__ inp, int *__restrict
     using Map = FpsMap<CL * FPS_T, P>;
     extern __shared__ float4 own_pts[];  // [P][FPS_T] xyz of this CTA's points (lookup by the round winner)
     __shared__ FpsShared<CL> sh;
-
-    const int tid = threadIdx.x;
-    const uint32_t rank = CL > 1 ? cluster_ctarank() : 0u;
-    const int scene = blockIdx.x / CL;
-    const int g = (int)rank * FPS_T + tid;
-    const float *data = inp + (size_t)scene * io.sa;
-    int *idxs = out + (size_t)scene * io.ldo;
+    const FpsScene<CL> s;
+    const float *data = s.in(inp, io.sa);
+    int *idxs = s.row(out, io);
 
     float px[P], py[P], pz[P], td[P];
 #pragma unroll
     for (int i = 0; i < P; i++) {
-        const int k = Map::k_of(g, i);
+        const int k = Map::k_of(s.g, i);
         if (k < n) {
             px[i] = data[3 * k]; py[i] = data[3 * k + 1]; pz[i] = data[3 * k + 2];
             td[i] = 1e38f;  // tf_sampling_g.cu:136
@@ -177,30 +160,24 @@ fps3_cluster_kernel(int n, int m, const float *__restrict__ inp, int *__restrict
             px[i] = py[i] = pz[i] = 0.0f;
             td[i] = -1.0f;  // padding slot: can never win (min(d,-1) stays -1, valid values are >= 0)
         }
-        own_pts[i * FPS_T + tid] = make_float4(px[i], py[i], pz[i], 0.0f);
+        own_pts[i * FPS_T + s.tid] = make_float4(px[i], py[i], pz[i], 0.0f);
     }
-    fps_shared_init<CL>(sh);
+    sh.ring.template start<CL>();
 
     float ox = data[0], oy = data[1], oz = data[2];  // first sample is point 0 (:131-133)
-    if (g == 0) idxs[0] = io.ioff;
+    if (s.g == 0) idxs[0] = io.ioff;
 
     for (int j = 1; j < m; j++) {
-        float best = -1.0f;
-        int bi = 0;
+        FpsScan scan;
 #pragma unroll
         for (int i = 0; i < P; i++) {
-            const float dx = px[i] - ox, dy = py[i] - oy, dz = pz[i] - oz;
-            float d = __fmul_rn(dx, dx);
-            d = __fmaf_rn(dy, dy, d);
-            d = __fmaf_rn(dz, dz, d);
-            const float t = fminf(d, td[i]);
-            td[i] = t;
-            if (t > best) { best = t; bi = i; }
+            td[i] = fminf(fps_d2(px[i] - ox, py[i] - oy, pz[i] - oz), td[i]);
+            scan.see(td[i], i);
         }
-        const float4 c = own_pts[bi * FPS_T + tid];
+        const float4 c = own_pts[scan.at * FPS_T + s.tid];
         uint32_t wkey;
-        fps_exchange<CL, true>(sh, j, rank, best, fps_key(Map::k_of(g, bi)), c.x, c.y, c.z, wkey, ox, oy, oz);
-        if (g == 0) idxs[j] = fps_key_to_k(wkey) + io.ioff;
+        fps_exchange<CL, true>(sh, j, s.rank, scan.best, fps_key(Map::k_of(s.g, scan.at)), c.x, c.y, c.z, wkey, ox, oy, oz);
+        if (s.g == 0) idxs[j] = fps_key_to_k(wkey) + io.ioff;
     }
     if (CL > 1) cluster_sync_all();  // peers may still be storing into this CTA's shared memory
 }
@@ -210,6 +187,7 @@ fps3_cluster_kernel(int n, int m, const float *__restrict__ inp, int *__restrict
 // every CTA keeps a full copy of the scene's coordinates (one bulk TMA copy), so a packet is just (value, key)
 // = 8 bytes and EVERY WARP pushes its candidate straight to all peers -- the intra-CTA reduction stage and its
 // barrier disappear; a round is: register update -> 2 redux -> st.async -> mbarrier wait -> 2 redux -> 3 LDS.
+// Resumable (FpsRounds): the running distances travel through temp[b, n].
 // ---------------------------------------------------------------------------------------------------
 template <int CL, int P>
 __global__ void __launch_bounds__(FPS_T, 1)
@@ -220,27 +198,18 @@ fps3_direct_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
     extern __shared__ float4 dyn_smem[];
     float *sxyz = reinterpret_cast<float *>(dyn_smem);   // [n][3] raw copy of the scene
     __shared__ __align__(16) unsigned long long slots[2][NSLOT];
-    __shared__ __align__(8) unsigned long long mbar[2], load_bar;
+    __shared__ FpsRing ring;
+    __shared__ __align__(8) unsigned long long load_bar;
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t rank = CL > 1 ? cluster_ctarank() : 0u;
-    const int scene = blockIdx.x / CL;
-    const int g = (int)rank * FPS_T + tid;
-    const float *data = inp + (size_t)scene * io.sa;
-    int *idxs = out + (size_t)scene * io.ldo;
-    // Resumable: this launch runs rounds [jbeg, jend) of 1..m-1.  A launch that does not start at round 0 reloads the
-    // running distances from io.temp and the last winner from the index output; one that stops before m saves them.
-    const int jbeg = io.j0 > 1 ? io.j0 : 1, jend = io.j1 < m ? io.j1 : m;
-    const bool resume = io.j0 > 0, save = io.j1 < m;
-    float *tsave = io.temp + (size_t)scene * n;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const FpsScene<CL> s;
+    const FpsRounds rounds(io, m, s.scene, out, n);
 
-    if (tid == 0) {
-        mbar_init(smem_u32(&mbar[0]), 1);
-        mbar_init(smem_u32(&mbar[1]), 1);
+    if (s.tid == 0) {
         mbar_init(smem_u32(&load_bar), 1);
-        fence_mbar_init_cluster();
+        ring.init();
         mbar_arrive_expect_tx(smem_u32(&load_bar), (uint32_t)n * 12u);
-        bulk_g2s(smem_u32(sxyz), data, (uint32_t)n * 12u, smem_u32(&load_bar));
+        bulk_g2s(smem_u32(sxyz), s.in(inp, io.sa), (uint32_t)n * 12u, smem_u32(&load_bar));
     }
     __syncthreads();
     mbar_wait_cta(smem_u32(&load_bar), 0);
@@ -248,73 +217,50 @@ fps3_direct_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
     float px[P], py[P], pz[P], td[P];
 #pragma unroll
     for (int i = 0; i < P; i++) {
-        const int k = Map::k_of(g, i);
-        if (k < n) {
-            px[i] = sxyz[3 * k]; py[i] = sxyz[3 * k + 1]; pz[i] = sxyz[3 * k + 2];
-            td[i] = resume ? tsave[k] : 1e38f;
-        } else { px[i] = py[i] = pz[i] = 0.0f; td[i] = -1.0f; }
+        const int k = Map::k_of(s.g, i);
+        if (k < n) { px[i] = sxyz[3 * k]; py[i] = sxyz[3 * k + 1]; pz[i] = sxyz[3 * k + 2]; }
+        else { px[i] = py[i] = pz[i] = 0.0f; }
+        td[i] = rounds.start(k, k < n);
     }
     if (CL > 1) cluster_sync_all();                      // all peers' barriers are initialised
 
-    int old0 = 0;
-    if (resume) old0 = idxs[jbeg - 1] - io.ioff;         // written by the previous launch of this scene
-    else if (g == 0) idxs[0] = io.ioff;
+    const int old0 = rounds.first(s.g == 0);
     float ox = sxyz[3 * old0], oy = sxyz[3 * old0 + 1], oz = sxyz[3 * old0 + 2];
 
-    for (int j = jbeg; j < jend; j++) {
-        const int r = j - jbeg + 1;                      // 1-based round of THIS launch: slot parity / barrier phase
+    for (int j = rounds.jbeg; j < rounds.jend; j++) {
+        const int r = j - rounds.jbeg + 1;               // round of THIS launch: slot parity / barrier phase
         const int par = r & 1;
-        if (tid == 0) mbar_arrive_expect_tx(smem_u32(&mbar[par]), NSLOT * 8);
+        if (s.tid == 0) ring.expect(r, NSLOT * 8);
         // ---- distance update of the thread's P points, then their arg-max as a TREE (depth log2 P) instead of a serial
-        // "first strictly greater" scan (depth P): the scan's compare + select chain was ~150 of the ~830 cycles of a
-        // round.  Ties keep the lower slot (a higher slot wins only when STRICTLY greater), i.e. the scan's answer.
+        // scan (depth P): the scan's compare + select chain was ~150 of the ~830 cycles of a round.
         float tv[P];
         {
-            // fp32 pairs: same IEEE operations as d = fma(dz,dz, fma(dy,dy, dx*dx))
             const float2 nox = make_float2(-ox, -ox), noy = make_float2(-oy, -oy), noz = make_float2(-oz, -oz);
 #pragma unroll
             for (int i = 0; i + 1 < P; i += 2) {
-                const float2 dx = add2_rn(make_float2(px[i], px[i + 1]), nox);
-                const float2 dy = add2_rn(make_float2(py[i], py[i + 1]), noy);
-                const float2 dz = add2_rn(make_float2(pz[i], pz[i + 1]), noz);
-                float2 d = mul2_rn(dx, dx);
-                d = fma2_rn(dy, dy, d);
-                d = fma2_rn(dz, dz, d);
+                const float2 d = fps_d2(add2_rn(make_float2(px[i], px[i + 1]), nox), add2_rn(make_float2(py[i], py[i + 1]), noy),
+                                        add2_rn(make_float2(pz[i], pz[i + 1]), noz));
                 td[i] = fminf(d.x, td[i]); td[i + 1] = fminf(d.y, td[i + 1]);
                 tv[i] = td[i]; tv[i + 1] = td[i + 1];
             }
             if (P & 1) {
                 constexpr int i = P - 1;
-                const float dx = px[i] - ox, dy = py[i] - oy, dz = pz[i] - oz;
-                float d = __fmul_rn(dx, dx);
-                d = __fmaf_rn(dy, dy, d);
-                d = __fmaf_rn(dz, dz, d);
-                td[i] = fminf(d, td[i]);
+                td[i] = fminf(fps_d2(px[i] - ox, py[i] - oy, pz[i] - oz), td[i]);
                 tv[i] = td[i];
             }
         }
         int tk[P];                                       // k of slot i (compile-time offsets from the thread's base)
 #pragma unroll
-        for (int i = 0; i < P; i++) tk[i] = Map::k_of(g, i);
-#pragma unroll
-        for (int sdist = 1; sdist < P; sdist *= 2) {
-#pragma unroll
-            for (int i = 0; i + sdist < P; i += 2 * sdist) {
-                const bool up = tv[i + sdist] > tv[i];
-                tv[i] = up ? tv[i + sdist] : tv[i];
-                tk[i] = up ? tk[i + sdist] : tk[i];
-            }
-        }
-        const float best = tv[0];
-        const uint32_t u = __float_as_uint(fmaxf(best, 0.0f));
+        for (int i = 0; i < P; i++) tk[i] = Map::k_of(s.g, i);
+        fps_tree_argmax(tv, tk);
+        const uint2 cd = fps_candidate(tv[0], fps_key(tk[0]));
         uint32_t mx, kmin;
-        warp_argmax(u, best >= 0.0f ? fps_key(tk[0]) : KEY_INVALID, mx, kmin);
+        warp_argmax(cd.x, cd.y, mx, kmin);
         if (lane < CL) {
             const unsigned long long pk = ((unsigned long long)mx << 32) | (unsigned long long)kmin;
-            st_async_b64(mapa(smem_u32(&slots[par][rank * FPS_NW + warp]), (uint32_t)lane),
-                         mapa(smem_u32(&mbar[par]), (uint32_t)lane), pk);
+            st_async_b64(mapa(smem_u32(&slots[par][s.rank * FPS_NW + warp]), (uint32_t)lane), mapa(ring.at(r), (uint32_t)lane), pk);
         }
-        mbar_wait_cta(smem_u32(&mbar[par]), ((r - 1) >> 1) & 1);
+        ring.wait(r);
         // reduce the NSLOT packets: value desc, key asc
         unsigned long long a = lane < NSLOT ? slots[par][lane] : 0x00000000ffffffffull;
 #pragma unroll
@@ -327,15 +273,12 @@ fps3_direct_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
         warp_argmax((uint32_t)(a >> 32), (uint32_t)a, m3, k3);
         const int old = fps_key_to_k(k3);
         ox = sxyz[3 * old]; oy = sxyz[3 * old + 1]; oz = sxyz[3 * old + 2];
-        if (g == 0) idxs[j] = old + io.ioff;
+        if (s.g == 0) rounds.put(j, old);
     }
-    if (save) {
-#pragma unroll
-        for (int i = 0; i < P; i++) {
-            const int k = Map::k_of(g, i);
-            if (k < n) tsave[k] = td[i];
-        }
-    }
+    rounds.save_dist(td, [&](int i) {
+        const int k = Map::k_of(s.g, i);
+        return k < n ? k : -1;
+    });
     if (CL > 1) cluster_sync_all();
 }
 
@@ -348,41 +291,37 @@ fpsdist_cluster_kernel(int n, int m, const float *__restrict__ dist, int *__rest
 {
     using Map = FpsMap<CL * FPS_T, P>;
     __shared__ FpsShared<CL> sh;
-    const int tid = threadIdx.x;
-    const uint32_t rank = CL > 1 ? cluster_ctarank() : 0u;
-    const int scene = blockIdx.x / CL;
-    const int g = (int)rank * FPS_T + tid;
-    const float *mat = dist + (size_t)scene * io.sa;
-    int *idxs = out + (size_t)scene * io.ldo;
+    const FpsScene<CL> s;
+    const float *mat = s.in(dist, io.sa);
+    int *idxs = s.row(out, io);
 
     float td[P];
     int kk[P];
 #pragma unroll
     for (int i = 0; i < P; i++) {
-        kk[i] = Map::k_of(g, i);
+        kk[i] = Map::k_of(s.g, i);
         td[i] = kk[i] < n ? 1e38f : -1.0f;
     }
-    fps_shared_init<CL>(sh);
+    sh.ring.template start<CL>();
     int old = 0;
-    if (g == 0) idxs[0] = io.ioff;
+    if (s.g == 0) idxs[0] = io.ioff;
     for (int j = 1; j < m; j++) {
         const float *row = mat + (size_t)old * n;
         float dv[P];
 #pragma unroll
         for (int i = 0; i < P; i++) dv[i] = kk[i] < n ? __ldg(row + kk[i]) : 0.0f;
-        float best = -1.0f;
-        int bi = 0;
+        FpsScan scan;
 #pragma unroll
         for (int i = 0; i < P; i++) {
-            const float t = fminf(dv[i], td[i]);
-            td[i] = t;
-            if (t > best) { best = t; bi = i; }
+            td[i] = fminf(dv[i], td[i]);
+            scan.see(td[i], i);
         }
         uint32_t wkey;
         float ux, uy, uz;
-        fps_exchange<CL, false>(sh, j, rank, best, fps_key(Map::k_of(g, bi)), 0.f, 0.f, 0.f, wkey, ux, uy, uz, mat, n);
+        fps_exchange<CL, false>(sh, j, s.rank, scan.best, fps_key(Map::k_of(s.g, scan.at)), 0.f, 0.f, 0.f, wkey, ux, uy, uz,
+                                mat, n);
         old = fps_key_to_k(wkey);
-        if (g == 0) idxs[j] = old + io.ioff;
+        if (s.g == 0) idxs[j] = old + io.ioff;
     }
     if (CL > 1) cluster_sync_all();
 }
@@ -403,26 +342,22 @@ fpsc_cluster_kernel(int n, int c, int m, const float *__restrict__ inp, int *__r
     float *feat = reinterpret_cast<float *>(dyn_smem);  // [c][NLP]
     float *old_f = feat + (size_t)c * NLP;               // [c]
     __shared__ FpsShared<CL> sh;
-
-    const int tid = threadIdx.x;
-    const uint32_t rank = CL > 1 ? cluster_ctarank() : 0u;
-    const int scene = blockIdx.x / CL;
-    const int g = (int)rank * FPS_T + tid;
-    const float *data = inp + (size_t)scene * io.sa;
-    int *idxs = out + (size_t)scene * io.ldo;
+    const FpsScene<CL> s;
+    const float *data = s.in(inp, io.sa);
+    int *idxs = s.row(out, io);
 
     float td[P];
 #pragma unroll
-    for (int i = 0; i < P; i++) td[i] = Map::k_of(g, i) < n ? 1e38f : -1.0f;
+    for (int i = 0; i < P; i++) td[i] = Map::k_of(s.g, i) < n ? 1e38f : -1.0f;
     // stage features: one warp per point row for coalesced global reads
-    for (int s = tid >> 5; s < NL; s += FPS_NW) {
-        const int st = s % FPS_T, si = s / FPS_T;
-        const int k = Map::k_of((int)rank * FPS_T + st, si);
-        for (int l = tid & 31; l < c; l += 32) feat[(size_t)l * NLP + s] = k < n ? data[(size_t)k * c + l] : 0.0f;
+    for (int q = s.tid >> 5; q < NL; q += FPS_NW) {
+        const int st = q % FPS_T, si = q / FPS_T;
+        const int k = Map::k_of((int)s.rank * FPS_T + st, si);
+        for (int l = s.tid & 31; l < c; l += 32) feat[(size_t)l * NLP + q] = k < n ? data[(size_t)k * c + l] : 0.0f;
     }
-    for (int l = tid; l < c; l += FPS_T) old_f[l] = data[l];  // first sample is point 0
-    fps_shared_init<CL>(sh);  // contains __syncthreads
-    if (g == 0) idxs[0] = io.ioff;
+    for (int l = s.tid; l < c; l += FPS_T) old_f[l] = data[l];  // first sample is point 0
+    sh.ring.template start<CL>();  // contains __syncthreads
+    if (s.g == 0) idxs[0] = io.ioff;
 
     for (int j = 1; j < m; j++) {
         float d[P];
@@ -430,33 +365,31 @@ fpsc_cluster_kernel(int n, int c, int m, const float *__restrict__ inp, int *__r
         for (int i = 0; i < P; i++) d[i] = 0.0f;
         for (int l = 0; l < c; l++) {
             const float o = old_f[l];
-            const float *fl = feat + (size_t)l * NLP + tid;
+            const float *fl = feat + (size_t)l * NLP + s.tid;
 #pragma unroll
             for (int i = 0; i < P; i++) {
                 const float diff = fl[i * FPS_T] - o;
                 d[i] = __fmaf_rn(diff, diff, d[i]);
             }
         }
-        float best = -1.0f;
-        int bi = 0;
+        FpsScan scan;
 #pragma unroll
         for (int i = 0; i < P; i++) {
-            const float t = fminf(d[i], td[i]);
-            td[i] = t;
-            if (t > best) { best = t; bi = i; }
+            td[i] = fminf(d[i], td[i]);
+            scan.see(td[i], i);
         }
         uint32_t wkey;
         float ux, uy, uz;
-        fps_exchange<CL, false>(sh, j, rank, best, fps_key(Map::k_of(g, bi)), 0.f, 0.f, 0.f, wkey, ux, uy, uz);
+        fps_exchange<CL, false>(sh, j, s.rank, scan.best, fps_key(Map::k_of(s.g, scan.at)), 0.f, 0.f, 0.f, wkey, ux, uy, uz);
         const int old = fps_key_to_k(wkey);
-        if (g == 0) idxs[j] = old + io.ioff;
+        if (s.g == 0) idxs[j] = old + io.ioff;
         // fetch the winner's feature vector from its owner CTA (all threads passed the __syncthreads inside
         // fps_exchange, so nobody still reads old_f of this round)
         int og, oi;
         Map::owner_of(old, og, oi);
         const uint32_t orank = (uint32_t)(og / FPS_T);
         const int oslot = oi * FPS_T + (og % FPS_T);
-        for (int l = tid; l < c; l += FPS_T) {
+        for (int l = s.tid; l < c; l += FPS_T) {
             const uint32_t a = smem_u32(feat + (size_t)l * NLP + oslot);
             old_f[l] = CL > 1 ? ld_dsmem_f32(mapa(a, orank)) : feat[(size_t)l * NLP + oslot];
         }
@@ -475,7 +408,8 @@ fpsc_cluster_kernel(int n, int c, int m, const float *__restrict__ inp, int *__r
 // in shared memory so that warp 0 can attach the CTA candidate's whole feature row (+ its squared norm) to the
 // arg-max packet it pushes to the peers with st.async.  After the one mbarrier wait of the round every CTA therefore
 // already holds the winner's features locally: no second hop, no global memory, no [B,N,N] tensor (0.5 GB per step
-// at layer 2) and no kernel to produce it.
+// at layer 2) and no kernel to produce it.  Resumable (FpsRounds): the last winner's feature row is re-read from
+// global memory.
 // ---------------------------------------------------------------------------------------------------
 template <int CP>
 struct __align__(16) FfpsPacket {
@@ -484,6 +418,7 @@ struct __align__(16) FfpsPacket {
     uint32_t pad;
     float feat[CP];
 };
+static_assert(sizeof(FfpsPacket<68>) == 16 + 4 * 68 && sizeof(FfpsPacket<132>) == 16 + 4 * 132, "ffps_smem (fps_plan.h)");
 
 template <int CL, int P, int CP>
 __global__ void __launch_bounds__(FPS_T, 1)
@@ -497,43 +432,32 @@ ffps_cluster_kernel(int n, int ca, int cb, int m, const float *__restrict__ fa, 
     float *sqS = featS + (size_t)NL * CP;                             // [NL]
     Packet *cl_pk = reinterpret_cast<Packet *>(sqS + NL);             // [2][CL]
     __shared__ uint32_t warp_val[2][FPS_NW], warp_key[2][FPS_NW];
-    __shared__ unsigned long long mbar[2];
+    __shared__ FpsRing ring;
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t rank = CL > 1 ? cluster_ctarank() : 0u;
-    const int scene = blockIdx.x / CL;
-    const int g = (int)rank * FPS_T + tid;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const FpsScene<CL> s;
     const int c = ca + cb;
-    const float *A = fa + (size_t)scene * io.sa;
-    const float *B = fb + (size_t)scene * io.sb;
-    int *idxs = out + (size_t)scene * io.ldo;
+    const float *A = s.in(fa, io.sa);
+    const float *B = s.in(fb, io.sb);
+    const FpsRounds rounds(io, m, s.scene, out, n);
 
-    // ---- stage this CTA's rows: local point s = i*256 + t  <->  k = rank*256 + t + i*TT (zero rows beyond n)
-    for (int s = warp; s < NL; s += FPS_NW) {
-        const int k = (int)rank * FPS_T + (s % FPS_T) + (s / FPS_T) * TT;
+    // ---- stage this CTA's rows: local point q = i*256 + t  <->  k = rank*256 + t + i*TT (zero rows beyond n)
+    for (int q = warp; q < NL; q += FPS_NW) {
+        const int k = (int)s.rank * FPS_T + (q % FPS_T) + (q / FPS_T) * TT;
         for (int l = lane; l < CP; l += 32) {
             float v = 0.0f;
             if (k < n && l < c) v = l < ca ? __ldg(A + (size_t)k * ca + l) : __ldg(B + (size_t)k * cb + (l - ca));
-            featS[(size_t)s * CP + l] = v;
+            featS[(size_t)q * CP + l] = v;
         }
     }
-    if (tid == 0) {
-        mbar_init(smem_u32(&mbar[0]), 1);
-        mbar_init(smem_u32(&mbar[1]), 1);
-        fence_mbar_init_cluster();
-    }
+    if (s.tid == 0) ring.init();
     __syncthreads();
-    // Resumable like fps3_direct_kernel: rounds [jbeg, jend); the running distances travel through io.temp, the last
-    // winner is re-read from the index output and its feature row from global memory.
-    const int jbeg = io.j0 > 1 ? io.j0 : 1, jend = io.j1 < m ? io.j1 : m;
-    const bool resume = io.j0 > 0, save = io.j1 < m;
-    float *tsave = io.temp + (size_t)scene * n;
     float f[P][CP], td[P], sq[P];
     uint32_t key[P];
 #pragma unroll
     for (int i = 0; i < P; i++) {
-        const int k = g + i * TT;
-        const float4 *row = reinterpret_cast<const float4 *>(featS + (size_t)(i * FPS_T + tid) * CP);
+        const int k = s.g + i * TT;
+        const float4 *row = reinterpret_cast<const float4 *>(featS + (size_t)(i * FPS_T + s.tid) * CP);
         float s2 = 0.0f;
 #pragma unroll
         for (int l4 = 0; l4 < CP / 4; l4++) {
@@ -543,21 +467,21 @@ ffps_cluster_kernel(int n, int ca, int cb, int m, const float *__restrict__ fa, 
 #pragma unroll
         for (int l = 0; l < CP; l++) s2 = __fmaf_rn(f[i][l], f[i][l], s2);     // sqdist's squared-norm chain
         sq[i] = s2;
-        sqS[i * FPS_T + tid] = s2;
-        td[i] = k < n ? (resume ? tsave[k] : 1e38f) : -1.0f;
+        sqS[i * FPS_T + s.tid] = s2;
+        td[i] = rounds.start(k, k < n);
         key[i] = fps_key(k);
     }
     // the point picked last (point 0 at the start of the sampling): its row is read from global memory by every CTA
     {
-        const int old0 = resume ? idxs[jbeg - 1] - io.ioff : 0;
+        const int old0 = rounds.first(s.g == 0);
         Packet &p0 = cl_pk[0];
-        for (int l = tid; l < CP; l += FPS_T) {
+        for (int l = s.tid; l < CP; l += FPS_T) {
             float v = 0.0f;
             if (l < c) v = l < ca ? __ldg(A + (size_t)old0 * ca + l) : __ldg(B + (size_t)old0 * cb + (l - ca));
             p0.feat[l] = v;
         }
         __syncthreads();
-        if (tid == 0) {
+        if (s.tid == 0) {
             float s2 = 0.0f;
             for (int l = 0; l < CP; l++) s2 = __fmaf_rn(p0.feat[l], p0.feat[l], s2);
             p0.sq = s2;
@@ -565,11 +489,10 @@ ffps_cluster_kernel(int n, int ca, int cb, int m, const float *__restrict__ fa, 
     }
     __syncthreads();
     if (CL > 1) cluster_sync_all();       // every CTA's barriers exist before any peer st.async targets them
-    if (g == 0 && !resume) idxs[0] = io.ioff;
 
     const Packet *oldp = &cl_pk[0];
-    for (int j = jbeg; j < jend; j++) {
-        const int r = j - jbeg + 1;       // 1-based round of THIS launch: buffer parity / barrier phase
+    for (int j = rounds.jbeg; j < rounds.jend; j++) {
+        const int r = j - rounds.jbeg + 1; // round of THIS launch: buffer parity / barrier phase
         const int par = r & 1;
         // ---- row `old` of the distance matrix for this thread's points
         float dot[P];
@@ -598,9 +521,9 @@ ffps_cluster_kernel(int n, int ca, int cb, int m, const float *__restrict__ fa, 
             if (t > best || (t == best && key[i] < bkey)) { best = t; bkey = key[i]; }
         }
         // ---- CTA candidate
-        const uint32_t u = __float_as_uint(fmaxf(best, 0.0f));
+        const uint2 cd = fps_candidate(best, bkey);
         uint32_t mx, kmin;
-        warp_argmax(u, best >= 0.0f ? bkey : KEY_INVALID, mx, kmin);
+        warp_argmax(cd.x, cd.y, mx, kmin);
         if (lane == 0) { warp_val[par][warp] = mx; warp_key[par][warp] = kmin; }
         __syncthreads();
         uint32_t win_key;
@@ -612,8 +535,8 @@ ffps_cluster_kernel(int n, int ca, int cb, int m, const float *__restrict__ fa, 
             uint32_t m2, k2;
             warp_argmax(v, kk, m2, k2);
             // the candidate's row in this CTA's shared memory (k2 == KEY_INVALID: nothing valid left, send row 0)
-            const int kc = k2 != KEY_INVALID ? fps_key_to_k(k2) : (int)rank * FPS_T;
-            const int ls = ((kc - (int)rank * FPS_T) / TT) * FPS_T + ((kc - (int)rank * FPS_T) % TT);
+            const int kc = k2 != KEY_INVALID ? fps_key_to_k(k2) : (int)s.rank * FPS_T;
+            const int ls = ((kc - (int)s.rank * FPS_T) / TT) * FPS_T + ((kc - (int)s.rank * FPS_T) % TT);
             const float4 *crow = reinterpret_cast<const float4 *>(featS + (size_t)ls * CP);
             if (CL == 1) {
                 if (warp == 0) {
@@ -624,10 +547,10 @@ ffps_cluster_kernel(int n, int ca, int cb, int m, const float *__restrict__ fa, 
                     }
                 }
             } else {
-                if (tid == 0) mbar_arrive_expect_tx(smem_u32(&mbar[par]), CL * NP * 16);
+                if (s.tid == 0) ring.expect(r, CL * NP * 16);
                 for (int peer = warp; peer < CL; peer += FPS_NW) {
-                    const uint32_t dst = mapa(smem_u32(&cl_pk[par * CL + rank]), (uint32_t)peer);
-                    const uint32_t dbar = mapa(smem_u32(&mbar[par]), (uint32_t)peer);
+                    const uint32_t dst = mapa(smem_u32(&cl_pk[par * CL + s.rank]), (uint32_t)peer);
+                    const uint32_t dbar = mapa(ring.at(r), (uint32_t)peer);
                     for (int piece = lane; piece < NP; piece += 32) {
                         const float4 v4 = piece == 0 ? make_float4(__uint_as_float(m2), __uint_as_float(k2), sqS[ls], 0.0f) : crow[piece - 1];
                         st_async_v4(dst + piece * 16, dbar,
@@ -642,7 +565,7 @@ ffps_cluster_kernel(int n, int ca, int cb, int m, const float *__restrict__ fa, 
             oldp = &cl_pk[par];
             win_key = oldp->key;
         } else {
-            mbar_wait_cta(smem_u32(&mbar[par]), ((r - 1) >> 1) & 1);
+            ring.wait(r);
             const uint32_t v = lane < CL ? cl_pk[par * CL + lane].val : 0u;
             const uint32_t kk = lane < CL ? cl_pk[par * CL + lane].key : KEY_INVALID;
             uint32_t m3, k3;
@@ -651,15 +574,12 @@ ffps_cluster_kernel(int n, int ca, int cb, int m, const float *__restrict__ fa, 
             oldp = &cl_pk[par * CL + (__ffs(bal) - 1)];
             win_key = k3;
         }
-        if (g == 0) idxs[j] = (win_key != KEY_INVALID ? fps_key_to_k(win_key) : 0) + io.ioff;
+        if (s.g == 0) rounds.put(j, win_key != KEY_INVALID ? fps_key_to_k(win_key) : 0);
     }
-    if (save) {
-#pragma unroll
-        for (int i = 0; i < P; i++) {
-            const int k = g + i * TT;
-            if (k < n) tsave[k] = td[i];
-        }
-    }
+    rounds.save_dist(td, [&](int i) {
+        const int k = s.g + i * TT;
+        return k < n ? k : -1;
+    });
     if (CL > 1) cluster_sync_all();
 }
 
@@ -684,8 +604,7 @@ fps_fallback_kernel(int n, int c, int m, const float *__restrict__ inp, const fl
     int old = 0;
     __syncthreads();
     for (int j = 1; j < m; j++) {
-        float best = -1.0f;
-        int bk = 0;
+        FpsScan scan;
         for (int k = tid; k < n; k += 1024) {
             float d;
             if (mat) d = mat[(size_t)old * n + k];
@@ -698,12 +617,11 @@ fps_fallback_kernel(int n, int c, int m, const float *__restrict__ inp, const fl
             }
             const float t = fminf(d, td[k]);
             td[k] = t;
-            if (t > best) { best = t; bk = k; }
+            scan.see(t, k);
         }
-        const uint32_t u = __float_as_uint(fmaxf(best, 0.0f));
-        const uint32_t key = best >= 0.0f ? fps_key(bk) : KEY_INVALID;
+        const uint2 cd = fps_candidate(scan.best, fps_key(scan.at));
         uint32_t mx, kmin;
-        warp_argmax(u, key, mx, kmin);
+        warp_argmax(cd.x, cd.y, mx, kmin);
         if (lane == 0) { s_val[warp] = mx; s_key[warp] = kmin; }
         __syncthreads();
         if (warp == 0) {
@@ -717,7 +635,7 @@ fps_fallback_kernel(int n, int c, int m, const float *__restrict__ inp, const fl
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Launch logic
+// Launch logic: the entry points validate, ask fps_plan.h for the route and launch what it says.
 // ---------------------------------------------------------------------------------------------------
 template <typename K>
 static cudaError_t launch_cluster(K kernel, int cl, int b, size_t dyn_smem, cudaStream_t stream, void **args)
@@ -743,156 +661,63 @@ static cudaError_t launch_cluster(K kernel, int cl, int b, size_t dyn_smem, cuda
     return cudaLaunchKernelExC(&cfg, (const void *)kernel, args);
 }
 
-// smallest power of two P >= need with P >= residue classes per thread
-static int pick_p(int n, int cl)
-{
-    const int tt = cl * FPS_T;
-    const int r = tt >= 1024 ? 1 : 1024 / tt;
-    int need = (n + tt - 1) / tt;
-    // a residue class holds ceil(n/1024) points; slots per class J = P/R must cover them
-    const int per_class = (n + 1023) / 1024;
-    const int s = tt >= 1024 ? tt / 1024 : 1;
-    const int j = (per_class + s - 1) / s;
-    need = r * j;
-    int p = r;
-    while (p < need) p *= 2;
-    return p;
-}
+// Kernel families of the (CL, P) dispatch: fn<CL, P> is the instantiation, has(CL, P) whether it is built.  The
+// cluster kernels take P a multiple of the residue classes per thread, max(1, 1024 / (CL * 256)).
+struct ClusterFamily {
+    static constexpr bool has(int cl, int p) { return cl * p >= 4; }
+};
+struct Fps3Packet : ClusterFamily {
+    template <int CL, int P> static constexpr auto fn = fps3_cluster_kernel<CL, P>;
+};
+struct Fps3Direct : ClusterFamily {
+    template <int CL, int P> static constexpr auto fn = fps3_direct_kernel<CL, P>;
+};
+struct FpsDist : ClusterFamily {
+    template <int CL, int P> static constexpr auto fn = fpsdist_cluster_kernel<CL, P>;
+};
+struct FpsGeneric : ClusterFamily {
+    template <int CL, int P> static constexpr auto fn = fpsc_cluster_kernel<CL, P>;
+};
+// matrix-free F-FPS: P = 2 points of CP = 68 channels per thread, or P = 1 of 132, on up to 8 CTAs
+struct FfpsFamily {
+    static constexpr bool has(int cl, int p) { return cl <= 8 && p <= 2; }
+    template <int CL, int P> static constexpr auto fn = ffps_cluster_kernel<CL, P, P == 2 ? 68 : 132>;
+};
 
-// Cluster-size request of one call (the `cluster` argument of the *_ex entry points): 0 = heuristic, > 0 = exactly
-// that many CTAs per scene, < 0 = heuristic capped at -cluster (throughput mode: FPS is latency-bound, so fewer SMs
-// per scene cost little time and free SMs for work running concurrently).
-static int cap_cl(int cl, int n, int hint)
+// launch K::fn<plan.cl, plan.p> over CL, P in {1, 2, 4, 8, 16}
+template <class K, int CL = 1, int P = 1>
+static cudaError_t launch_planned(const FpsPlan &pl, int b, cudaStream_t st, void **args)
 {
-    if (hint < 0)
-        while (cl > -hint && cl > 1 && (n + (cl / 2) * FPS_T - 1) / ((cl / 2) * FPS_T) <= 16) cl /= 2;
-    return cl;
-}
-
-static int pick_cl_xyz(int n, int hint)
-{
-    if (hint > 0) return hint;
-    int cl;
-    if (n <= 1024) cl = 1;
-    else if (n <= 2048) cl = 2;
-    else if (n <= 4096) cl = 4;
-    else if (n <= 32768) cl = 8;
-    else cl = 16;
-    return cap_cl(cl, n, hint);
+    if constexpr (CL > 16) {
+        return cudaErrorInvalidValue;
+    } else if constexpr (P > 16) {
+        return launch_planned<K, CL * 2>(pl, b, st, args);
+    } else {
+        if constexpr (K::has(CL, P))
+            if (pl.cl == CL && pl.p == P) return launch_cluster(K::template fn<CL, P>, CL, b, pl.smem, st, args);
+        return launch_planned<K, CL, P * 2>(pl, b, st, args);
+    }
 }
 
 }  // namespace ssd3d
 
 using namespace ssd3d;
 
-// The P values legal for a cluster size are the multiples of R = max(1, 1024/(CL*256)):
-//   CL=1 -> P in {4,8,16}; CL=2 -> {2,4,8,16}; CL>=4 -> {1,2,4,8,16}.
-#define SSD3D_FPS_SWITCH(KERNEL, SMEM_OF_P)                                                               \
-    do {                                                                                                  \
-        cudaError_t e = cudaErrorInvalidValue;                                                            \
-        const int p = pick_p(n, cl);                                                                      \
-        const size_t smem = (SMEM_OF_P);                                                                  \
-        if (cl == 1) {                                                                                    \
-            if (p == 4) e = launch_cluster(KERNEL<1, 4>, 1, b, smem, st, args);                           \
-            else if (p == 8) e = launch_cluster(KERNEL<1, 8>, 1, b, smem, st, args);                      \
-            else if (p == 16) e = launch_cluster(KERNEL<1, 16>, 1, b, smem, st, args);                    \
-            else return -100;                                                                             \
-        } else if (cl == 2) {                                                                             \
-            if (p == 2) e = launch_cluster(KERNEL<2, 2>, 2, b, smem, st, args);                           \
-            else if (p == 4) e = launch_cluster(KERNEL<2, 4>, 2, b, smem, st, args);                      \
-            else if (p == 8) e = launch_cluster(KERNEL<2, 8>, 2, b, smem, st, args);                      \
-            else if (p == 16) e = launch_cluster(KERNEL<2, 16>, 2, b, smem, st, args);                    \
-            else return -100;                                                                             \
-        } else if (cl == 4) {                                                                             \
-            if (p == 1) e = launch_cluster(KERNEL<4, 1>, 4, b, smem, st, args);                           \
-            else if (p == 2) e = launch_cluster(KERNEL<4, 2>, 4, b, smem, st, args);                      \
-            else if (p == 4) e = launch_cluster(KERNEL<4, 4>, 4, b, smem, st, args);                      \
-            else if (p == 8) e = launch_cluster(KERNEL<4, 8>, 4, b, smem, st, args);                      \
-            else if (p == 16) e = launch_cluster(KERNEL<4, 16>, 4, b, smem, st, args);                    \
-            else return -100;                                                                             \
-        } else if (cl == 8) {                                                                             \
-            if (p == 1) e = launch_cluster(KERNEL<8, 1>, 8, b, smem, st, args);                           \
-            else if (p == 2) e = launch_cluster(KERNEL<8, 2>, 8, b, smem, st, args);                      \
-            else if (p == 4) e = launch_cluster(KERNEL<8, 4>, 8, b, smem, st, args);                      \
-            else if (p == 8) e = launch_cluster(KERNEL<8, 8>, 8, b, smem, st, args);                      \
-            else if (p == 16) e = launch_cluster(KERNEL<8, 16>, 8, b, smem, st, args);                    \
-            else return -100;                                                                             \
-        } else if (cl == 16) {                                                                            \
-            if (p == 1) e = launch_cluster(KERNEL<16, 1>, 16, b, smem, st, args);                         \
-            else if (p == 2) e = launch_cluster(KERNEL<16, 2>, 16, b, smem, st, args);                    \
-            else if (p == 4) e = launch_cluster(KERNEL<16, 4>, 16, b, smem, st, args);                    \
-            else if (p == 8) e = launch_cluster(KERNEL<16, 8>, 16, b, smem, st, args);                    \
-            else if (p == 16) e = launch_cluster(KERNEL<16, 16>, 16, b, smem, st, args);                  \
-            else return -100;                                                                             \
-        } else return -100;                                                                               \
-        return (int)e;                                                                                    \
-    } while (0)
-
-static int launch_fps3(int b, int n, int m, int cl, const float *inp, int *out, const FpsIO &io, cudaStream_t st)
-{
-    void *args[] = {&n, &m, (void *)&inp, (void *)&out, (void *)&io};
-    SSD3D_FPS_SWITCH(fps3_cluster_kernel, (size_t)p * FPS_T * sizeof(float4));
-}
-static int launch_fps3_direct(int b, int n, int m, int cl, const float *inp, int *out, const FpsIO &io, cudaStream_t st)
-{
-    void *args[] = {&n, &m, (void *)&inp, (void *)&out, (void *)&io};
-    SSD3D_FPS_SWITCH(fps3_direct_kernel, (size_t)n * 12 + 16);
-}
-static int launch_fpsdist(int b, int n, int m, int cl, const float *dist, int *out, const FpsIO &io, cudaStream_t st)
-{
-    void *args[] = {&n, &m, (void *)&dist, (void *)&out, (void *)&io};
-    SSD3D_FPS_SWITCH(fpsdist_cluster_kernel, (size_t)0);
-}
-static int launch_fpsc(int b, int n, int c, int m, int cl, const float *inp, int *out, const FpsIO &io, cudaStream_t st)
-{
-    void *args[] = {&n, &c, &m, (void *)&inp, (void *)&out, (void *)&io};
-    SSD3D_FPS_SWITCH(fpsc_cluster_kernel, ((size_t)c * (p * FPS_T + 1) + c) * sizeof(float) + 16);
-}
-
-// cluster size for the generic-c kernel: smallest CL whose per-CTA feature slab fits in shared memory
-static int pick_cl_generic(int n, int c, int hint)
-{
-    if (hint > 0) return hint;
-    const size_t budget = 200 * 1024;
-    for (int cl = 1; cl <= 16; cl *= 2) {
-        const int p = pick_p(n, cl);
-        if (p > 16) continue;
-        if (((size_t)c * (p * FPS_T + 1) + c) * sizeof(float) + 16 <= budget && (cl >= 8 || n <= cl * 1024)) return cl;
-    }
-    for (int cl = 1; cl <= 16; cl *= 2) {
-        const int p = pick_p(n, cl);
-        if (p <= 16 && ((size_t)c * (p * FPS_T + 1) + c) * sizeof(float) + 16 <= budget) return cl;
-    }
-    return 0;
-}
-
+// The queries read the plan at the defaults of ssd3d_farthest_point_sample: dense 16-byte aligned input, heuristic
+// cluster size.  Whether a route needs temp does not depend on m.
 extern "C" int ssd3d_fps_needs_temp(int n, int c)
 {
-    if (c == 3) return pick_p(n, 16) > 16;
-    return pick_cl_generic(n, c, 0) == 0;
+    return plan_fps(n, c, 2, 0, 0, true, (long long)n * c, false).kind == FpsKind::Fallback;
 }
 
-// (c == 3) does the resumable direct kernel cover n?  It needs the scene resident in one CTA's shared memory.
-static bool fps3_direct_fits(int n, int cl, const float *inp, long long sa)
-{
-    return cl >= 2 && (size_t)n * 12 + 16 <= 200 * 1024 && (n % 4) == 0 &&
-           (reinterpret_cast<uintptr_t>(inp) & 15u) == 0 && (sa % 4) == 0 && pick_p(n, cl) <= 16;
-}
+// whether the resident-scene kernel runs partial ranges of n points (flags bit 1: the pruned kernel, which also
+// does, is chosen by its own flags)
+extern "C" int ssd3d_fps_supports_rounds(int n, int c) { return plan_fps(n, c, 2, 0, 2, true, (long long)n * c, true).rounds; }
 
 // floats of `temp` per scene a partial range of rounds needs: the running distances, plus (bucket kernel) the permutation
 extern "C" long ssd3d_fps_temp_elems(int n, int c, int m, int flags)
 {
-    if (n <= 0) return 0;
-    if (c == 3 && fps3_bucket_applies(n, m, nullptr, 0, flags)) return 2L * n;
-    return n;
-}
-
-extern "C" int ssd3d_fps_supports_rounds(int n, int c)
-{
-    if (c != 3) return 0;
-    int cl = pick_cl_xyz(n, 0);
-    while (cl < 16 && pick_p(n, cl) > 16) cl *= 2;
-    return cl >= 2 && (size_t)n * 12 + 16 <= 200 * 1024 && (n % 4) == 0 && pick_p(n, cl) <= 16;
+    return n <= 0 ? 0 : plan_fps(n, c, m, 0, flags, true, (long long)n * c, true).temp;
 }
 
 extern "C" int ssd3d_farthest_point_sample_ex(int b, int n, int c, int m, const float *inp, long long in_stride,
@@ -907,38 +732,33 @@ extern "C" int ssd3d_farthest_point_sample_ex(int b, int n, int c, int m, const 
                   "farthest_point_sample: cluster must be 0, +-1, +-2, +-4, +-8 or +-16, got %d", cluster);
     if (b == 0 || m == 0 || j0 == j1) return 0;  // tf_sampling_g.cu:126-127
     SSD3D_REQUIRE(inp && out, "farthest_point_sample: null pointer");
-    cudaStream_t st = (cudaStream_t)stream;
     const bool partial = j0 > 0 || j1 < m;
-    FpsIO io = {in_stride, 0, ldo, idx_offset, j0, j1, temp};
-    int rc = -100;
-    if (c == 3 && fps3_bucket_applies(n, m, inp, in_stride, flags)) {
-        // large scenes: one CTA per scene with spatial pruning (fps_bucket.cu); `cluster` does not apply
-        SSD3D_REQUIRE(!partial || temp != nullptr, "farthest_point_sample: a partial range of rounds carries its state in temp[b, 2n] "
-                      "(ssd3d_fps_temp_elems)");
-        rc = launch_fps3_bucket(b, n, m, inp, out, io, st);
-    } else if (c == 3) {
-        int cl = pick_cl_xyz(n, cluster);
-        while (cl < 16 && pick_p(n, cl) > 16) cl *= 2;
-        // direct variant: whole scene resident in every CTA (bulk copy needs 16-byte aligned source and size)
-        const bool direct_ok = (flags & 1) == 0 && fps3_direct_fits(n, cl, inp, in_stride);
-        if (partial) {
-            SSD3D_REQUIRE(direct_ok, "farthest_point_sample: a partial range of rounds needs the resident-scene kernel "
-                          "(c == 3, n %% 4 == 0, n <= 17000, 16-byte aligned input); see ssd3d_fps_supports_rounds");
-            SSD3D_REQUIRE(temp != nullptr, "farthest_point_sample: a partial range of rounds carries its state in temp[b,n]");
-        }
-        if (direct_ok) rc = launch_fps3_direct(b, n, m, cl, inp, out, io, st);
-        else if (pick_p(n, cl) <= 16) rc = launch_fps3(b, n, m, cl, inp, out, io, st);
-    } else {
-        SSD3D_REQUIRE(!partial, "farthest_point_sample: a partial range of rounds is only built for c == 3");
-        const int cl = pick_cl_generic(n, c, cluster);
-        if (cl > 0) rc = launch_fpsc(b, n, c, m, cl, inp, out, io, st);
+    const FpsPlan pl = plan_fps(n, c, m, cluster, flags, (reinterpret_cast<uintptr_t>(inp) & 15u) == 0, in_stride, partial);
+    if (partial) {
+        SSD3D_REQUIRE(c == 3, "farthest_point_sample: a partial range of rounds is only built for c == 3");
+        SSD3D_REQUIRE(pl.rounds, "farthest_point_sample: a partial range of rounds needs the resident-scene kernel "
+                      "(c == 3, n %% 4 == 0, n <= 17000, 16-byte aligned input); see ssd3d_fps_supports_rounds");
+        if (pl.kind == FpsKind::Bucket)
+            SSD3D_REQUIRE(temp != nullptr, "farthest_point_sample: a partial range of rounds carries its state in temp[b, 2n] "
+                          "(ssd3d_fps_temp_elems)");
+        SSD3D_REQUIRE(temp != nullptr, "farthest_point_sample: a partial range of rounds carries its state in temp[b,n]");
     }
-    if (rc == -100) {
-        SSD3D_REQUIRE(temp != nullptr, "farthest_point_sample: n=%d c=%d needs the temp[b,n] workspace", n, c);
+    SSD3D_REQUIRE(pl.kind != FpsKind::Fallback || temp != nullptr, "farthest_point_sample: n=%d c=%d needs the temp[b,n] workspace", n, c);
+    cudaStream_t st = (cudaStream_t)stream;
+    FpsIO io = {in_stride, 0, ldo, idx_offset, j0, j1, temp};
+    void *args[] = {&n, &m, (void *)&inp, (void *)&out, (void *)&io};
+    void *args_c[] = {&n, &c, &m, (void *)&inp, (void *)&out, (void *)&io};
+    cudaError_t e;
+    switch (pl.kind) {
+    case FpsKind::Bucket: e = (cudaError_t)launch_fps3_bucket(b, n, m, inp, out, io, st); break;
+    case FpsKind::Direct: e = launch_planned<Fps3Direct>(pl, b, st, args); break;
+    case FpsKind::Packet: e = launch_planned<Fps3Packet>(pl, b, st, args); break;
+    case FpsKind::Generic: e = launch_planned<FpsGeneric>(pl, b, st, args_c); break;
+    default:
         fps_fallback_kernel<<<b, 1024, 0, st>>>(n, c, m, inp, nullptr, temp, out, io);
         SSD3D_LAUNCH_CHECK("fps_fallback_kernel");
     }
-    return cuda_status((cudaError_t)rc, "farthest_point_sample launch");
+    return cuda_status(e, "farthest_point_sample launch");
 }
 
 extern "C" int ssd3d_farthest_point_sample(int b, int n, int c, int m, const float *inp, float *temp, int *out,
@@ -957,10 +777,11 @@ extern "C" int ssd3d_farthest_point_sample_with_distance_ex(int b, int n, int m,
     SSD3D_REQUIRE(dist && out, "farthest_point_sample_with_distance: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
     FpsIO io = {(long long)n * n, 0, ldo, idx_offset, 0, m, nullptr};
-    // the per-round row read is a DRAM-latency-bound gather: more CTAs per scene = more loads in flight
-    int cl = cluster > 0 ? cluster : cap_cl(n <= 1024 ? 1 : (n <= 2048 ? 4 : 8), n, cluster);
-    while (cl < 16 && pick_p(n, cl) > 16) cl *= 2;
-    if (pick_p(n, cl) <= 16) return cuda_status((cudaError_t)launch_fpsdist(b, n, m, cl, dist, out, io, st), "fpsdist launch");
+    const FpsPlan pl = plan_fps_dist(n, cluster);
+    if (pl.kind == FpsKind::Dist) {
+        void *args[] = {&n, &m, (void *)&dist, (void *)&out, (void *)&io};
+        return cuda_status(launch_planned<FpsDist>(pl, b, st, args), "fpsdist launch");
+    }
     SSD3D_REQUIRE(temp != nullptr, "farthest_point_sample_with_distance: n=%d needs the temp[b,n] workspace", n);
     fps_fallback_kernel<<<b, 1024, 0, st>>>(n, 0, m, nullptr, dist, temp, out, io);
     SSD3D_LAUNCH_CHECK("fps_fallback_kernel");
@@ -972,26 +793,8 @@ extern "C" int ssd3d_farthest_point_sample_with_distance(int b, int n, int m, co
     return ssd3d_farthest_point_sample_with_distance_ex(b, n, m, dist, temp, out, m, 0, 0, stream);
 }
 
-// ---- matrix-free F-FPS dispatch: CP = 68 (P = 2 points per thread) or 132 (P = 1); smallest cluster that holds n
-template <int CL, int P, int CP>
-static int launch_ffps_t(int b, int n, int ca, int cb, int m, const float *fa, const float *fb, int *out, const FpsIO &io,
-                         cudaStream_t st)
-{
-    const size_t smem = (size_t)P * FPS_T * CP * 4 + (size_t)P * FPS_T * 4 + (size_t)2 * CL * sizeof(FfpsPacket<CP>);
-    void *args[] = { &n, &ca, &cb, &m, &fa, &fb, &out, (void *)&io };
-    return (int)launch_cluster(ffps_cluster_kernel<CL, P, CP>, CL, b, smem, st, args);
-}
-static int ffps_cluster_for(int n, int c)
-{
-    const int per_cta = c <= 68 ? 2 * FPS_T : (c <= 132 ? FPS_T : 0);
-    if (per_cta == 0) return 0;
-    for (int cl = 1; cl <= 8; cl *= 2)
-        if (n <= cl * per_cta) return cl;
-    return 0;
-}
-
 // 1 when the matrix-free F-FPS kernel covers (n points, c = channels of the concatenated feature), else 0.
-extern "C" int ssd3d_ffps_supported(int n, int c) { return n > 0 && c > 0 && ffps_cluster_for(n, c) > 0 ? 1 : 0; }
+extern "C" int ssd3d_ffps_supported(int n, int c) { return plan_ffps(n, c, false).kind == FpsKind::Features; }
 
 // farthest_point_sample_with_distance(m, calc_square_dist(concat[fa, fb])) without the [b,n,n] matrix; same indices.
 extern "C" int ssd3d_farthest_point_sample_features_ex(int b, int n, int ca, int cb, int m, const float *fa,
@@ -1008,26 +811,14 @@ extern "C" int ssd3d_farthest_point_sample_features_ex(int b, int n, int ca, int
     if (b == 0 || m == 0) return 0;
     SSD3D_REQUIRE(fa && out && (fb || cb == 0), "farthest_point_sample_features: null pointer");
     const int c = ca + cb;
-    const int cl = ffps_cluster_for(n, c);
-    if (cl == 0) {
+    const FpsPlan pl = plan_ffps(n, c, j0 > 0 || j1 < m);
+    if (pl.kind != FpsKind::Features) {
         set_error("farthest_point_sample_features: n=%d c=%d not covered (use calc_square_dist + farthest_point_sample_with_distance)", n, c);
         return SSD3D_ERR_UNSUPPORTED;
     }
-    cudaStream_t st = (cudaStream_t)stream;
     const FpsIO io = {fa_stride, fb_stride, ldo, idx_offset, j0, j1, temp};
-    int rc;
-    if (c <= 68) {
-        rc = cl == 1 ? launch_ffps_t<1, 2, 68>(b, n, ca, cb, m, fa, fb, out, io, st)
-           : cl == 2 ? launch_ffps_t<2, 2, 68>(b, n, ca, cb, m, fa, fb, out, io, st)
-           : cl == 4 ? launch_ffps_t<4, 2, 68>(b, n, ca, cb, m, fa, fb, out, io, st)
-                     : launch_ffps_t<8, 2, 68>(b, n, ca, cb, m, fa, fb, out, io, st);
-    } else {
-        rc = cl == 1 ? launch_ffps_t<1, 1, 132>(b, n, ca, cb, m, fa, fb, out, io, st)
-           : cl == 2 ? launch_ffps_t<2, 1, 132>(b, n, ca, cb, m, fa, fb, out, io, st)
-           : cl == 4 ? launch_ffps_t<4, 1, 132>(b, n, ca, cb, m, fa, fb, out, io, st)
-                     : launch_ffps_t<8, 1, 132>(b, n, ca, cb, m, fa, fb, out, io, st);
-    }
-    return cuda_status((cudaError_t)rc, "ffps launch");
+    void *args[] = {&n, &ca, &cb, &m, &fa, &fb, &out, (void *)&io};
+    return cuda_status(launch_planned<FfpsFamily>(pl, b, (cudaStream_t)stream, args), "ffps launch");
 }
 
 extern "C" int ssd3d_farthest_point_sample_features(int b, int n, int ca, int cb, int m, const float *fa, const float *fb,

@@ -38,7 +38,7 @@ constexpr int FB_T = 512;                    // threads per CTA (one CTA per sce
 constexpr int FB_NW = FB_T / 32;             // 16 warps
 constexpr int FB_SLOTS = 32;                 // buckets per warp: lane l OWNS the meta data of the warp's slot l
 constexpr int FB_NBUCKET = FB_NW * FB_SLOTS; // 512
-constexpr int FB_MAXN = FB_NBUCKET * 32;     // 16384 points
+static_assert(FB_NBUCKET * 32 == FB_MAXN, "one point per lane of every bucket slot (fps_plan.h)");
 constexpr uint32_t FB_PAD_KEY = 0xFFFFFFFFu;
 
 // order-preserving float <-> uint map for min/max reductions of signed floats
@@ -90,15 +90,12 @@ fps3_bucket_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     const int scene = blockIdx.x;
     const float *data = inp + (size_t)scene * io.sa;
-    int *idxs = out + (size_t)scene * io.ldo;
-    const int jbeg = io.j0 > 1 ? io.j0 : 1, jend = io.j1 < m ? io.j1 : m;
-    const bool resume = io.j0 > 0, save = io.j1 < m;
-    float *tsave = io.temp ? io.temp + (size_t)scene * 2 * n : nullptr;
-    uint32_t *perm = tsave ? reinterpret_cast<uint32_t *>(tsave + n) : nullptr;
+    const FpsRounds rounds(io, m, scene, out, 2LL * n);
+    uint32_t *perm = io.temp ? reinterpret_cast<uint32_t *>(rounds.dist + n) : nullptr;
 
     float dist[FB_SLOTS];
 
-    if (!resume) {
+    if (!rounds.resume) {
         // ---- scene box -> 2-D Morton keys of the two widest axes -> bitonic sort (key = morton18 : index14)
         float lo[3] = {3.0e38f, 3.0e38f, 3.0e38f}, hi[3] = {-3.0e38f, -3.0e38f, -3.0e38f};
         for (int k = tid; k < n; k += FB_T) {
@@ -160,7 +157,7 @@ fps3_bucket_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
             uint32_t o = 0xffffu;                                  // 0xffff marks "no point" (n <= 16384 < 0xffff)
             if (p < n) o = skey[p] & 0x3fffu;
             orig_of[p] = (uint16_t)o;
-            if (tsave != nullptr && p < n) perm[p] = o;
+            if (perm != nullptr && p < n) perm[p] = o;
         }
         __syncthreads();                                           // sort buffer consumed: xs may be overwritten
     } else {
@@ -182,7 +179,7 @@ fps3_bucket_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
         float x = 0.0f, y = 0.0f, z = 0.0f;
         if (valid) { x = __ldg(data + 3 * o); y = __ldg(data + 3 * o + 1); z = __ldg(data + 3 * o + 2); }
         xs[p] = x; ys[p] = y; zs[p] = z;
-        dist[i] = valid ? (resume ? tsave[o] : 1e38f) : -1.0f;    // tf_sampling_g.cu:136
+        dist[i] = rounds.start(o, valid);                          // tf_sampling_g.cu:136
         const uint32_t mnx = __reduce_min_sync(0xffffffffu, valid ? fb_ord(x) : 0xffffffffu);
         const uint32_t mny = __reduce_min_sync(0xffffffffu, valid ? fb_ord(y) : 0xffffffffu);
         const uint32_t mnz = __reduce_min_sync(0xffffffffu, valid ? fb_ord(z) : 0xffffffffu);
@@ -201,16 +198,14 @@ fps3_bucket_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
         }
     }
 
-    int old0 = 0;
-    if (resume) old0 = idxs[jbeg - 1] - io.ioff;                  // written by the previous launch of this scene
-    else if (tid == 0) idxs[0] = io.ioff;
+    const int old0 = rounds.first(tid == 0);
     float sx = __ldg(data + 3 * old0), sy = __ldg(data + 3 * old0 + 1), sz = __ldg(data + 3 * old0 + 2);
     // the warp's best over its 32 slots, cached between rounds (valid while none of its buckets changes)
     uint32_t wm = 0u, wk = KEY_INVALID;
     bool wdirty = true;
     __syncthreads();                                               // xs / ys / zs complete
 
-    for (int j = jbeg; j < jend; j++) {
+    for (int j = rounds.jbeg; j < rounds.jend; j++) {
         const int par = j & 1;
         // ---- which of this warp's buckets can the new sample change?  (lane l tests slot l)
         const float gx = fmaxf(fmaxf(bminx - sx, sx - bmaxx), 0.0f);
@@ -226,9 +221,7 @@ fps3_bucket_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
             const int p = fb_pos(w, i, lane);
             const uint32_t kk = orig_of[p];
             const float dx = xs[p] - sx, dy = ys[p] - sy, dz = zs[p] - sz;
-            float d = __fmul_rn(dx, dx);
-            d = __fmaf_rn(dy, dy, d);
-            d = __fmaf_rn(dz, dz, d);
+            const float d = fps_d2(dx, dy, dz);
             float nd;
             switch (i) {
                 FB_CASE(0) FB_CASE(1) FB_CASE(2) FB_CASE(3) FB_CASE(4) FB_CASE(5) FB_CASE(6) FB_CASE(7)
@@ -257,33 +250,20 @@ fps3_bucket_kernel(int n, int m, const float *__restrict__ inp, int *__restrict_
         warp_argmax(c.x, c.y, m3, k3);
         const int p = (int)(k3 & 0x3fffu);
         sx = xs[p]; sy = ys[p]; sz = zs[p];
-        if (tid == 0) idxs[j] = fb_key_to_k(k3) + io.ioff;
+        if (tid == 0) rounds.put(j, fb_key_to_k(k3));
     }
 
-    if (save) {
-#pragma unroll
-        for (int i = 0; i < FB_SLOTS; i++) {
-            const uint32_t o = orig_of[fb_pos(w, i, lane)];
-            if (o != 0xffffu) tsave[o] = dist[i];
-        }
-    }
-}
-
-bool fps3_bucket_applies(int n, int m, const float *inp, long long sa, int flags)
-{
-    (void)inp; (void)sa;
-    if (flags & 2) return false;                                   // caller forbids it (tests, experiments)
-    if (n > FB_MAXN || n < 64 || m < 2) return false;
-    if (flags & 4) return true;                                    // caller forces it (tests: any n in range)
-    return n > 8192 && m >= 256;
+    rounds.save_dist(dist, [&](int i) {
+        const uint32_t o = orig_of[fb_pos(w, i, lane)];
+        return o != 0xffffu ? (int)o : -1;
+    });
 }
 
 int launch_fps3_bucket(int b, int n, int m, const float *inp, int *out, const FpsIO &io, cudaStream_t st)
 {
-    const size_t smem = (size_t)3 * FB_MAXN * sizeof(float);
-    cudaError_t e = cudaFuncSetAttribute((const void *)fps3_bucket_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute((const void *)fps3_bucket_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FB_SMEM);
     if (e != cudaSuccess) return (int)e;
-    fps3_bucket_kernel<<<b, FB_T, smem, st>>>(n, m, inp, out, io);
+    fps3_bucket_kernel<<<b, FB_T, FB_SMEM, st>>>(n, m, inp, out, io);
     return (int)cudaGetLastError();
 }
 
