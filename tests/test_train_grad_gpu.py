@@ -22,6 +22,15 @@ def _time_train():
     return mod
 
 
+def rowgroup_max_grad_f32(y, g, cnt=None):
+    """float32 numpy restatement of rowgroup_max_grad: y (groups, pool, c), g (groups, c), cnt (groups,) or None ->
+    (ind / num) * (g * mask), TF's _MinOrMaxGrad after the Mul gradient of the mask, in the kernel's operation order."""
+    ind = (y == y.max(axis=1, keepdims=True)).astype(np.float32)
+    num = ind.sum(axis=1, keepdims=True).astype(np.float32)
+    gm = g * (cnt > 0).astype(np.float32)[:, None] if cnt is not None else g
+    return ((ind / num) * gm[:, None, :]).astype(np.float32)
+
+
 def test_rowgroup_max_grad_bit_exact_with_ties_and_empty_groups(pkg, cuda):
     rng = np.random.default_rng(0)
     groups, pool, c = 300, 16, 40
@@ -32,11 +41,7 @@ def test_rowgroup_max_grad_bit_exact_with_ties_and_empty_groups(pkg, cuda):
     g = rng.standard_normal((groups, c)).astype(np.float32)
     got = pkg.tf_ops.rowgroup_max_grad(torch.from_numpy(y).to(cuda), torch.from_numpy(g).to(cuda), pool,
                                        torch.from_numpy(cnt).to(cuda)).cpu().numpy()
-    ind = (y == y.max(axis=1, keepdims=True)).astype(np.float32)
-    num = ind.sum(axis=1, keepdims=True).astype(np.float32)
-    gm = g * (cnt > 0).astype(np.float32)[:, None]
-    exp = (ind / num) * gm[:, None, :]
-    assert np.array_equal(got.view(np.uint32), exp.astype(np.float32).view(np.uint32))
+    assert np.array_equal(got.view(np.uint32), rowgroup_max_grad_f32(y, g, cnt).view(np.uint32))
 
 
 def test_vote_translate_grad_bit_exact_at_bounds(pkg, cuda):
