@@ -12,14 +12,19 @@
 // split (two bf16 matrices, row-major == K-major), so every operand tile is a plain TMA box in the 128B-swizzled
 // K-major layout the wgmma descriptors read, and no conversion happens on the load path.
 //
-// Kernel shape: 640 threads = 5 warpgroups; warp 0 = TMA producer (warps 1-3 idle), warps 4-11 = operand producers of
-// the gather modes, warps 12-19 = two consumer warpgroups.  Consumer warpgroup g owns rows 64g..64g+63 of the tile: it
-// issues the wgmma chain into its registers and runs the epilogue on the accumulator fragments where they are
-// (scale/shift/ReLU in place -> fp32 / split-bf16 through per-warp TMA tensor stores, or max-pool as a shuffle
-// reduce-and-transpose butterfly over the fragment rows; only pools of 32-128 rows meet other warps, in a 2 KiB exchange).
-// Tile 128 rows x BN<=64 columns (BN = 32 or 64, a template parameter: the wgmma width is part of the
-// instruction), K streamed in 64-element blocks through a multi-stage mbarrier ring; a stage is released as soon as
-// the wgmma group that read it has retired, so the TMA loads of the next k-blocks overlap the MMAs.
+// Two kernels, one per route of the A operand; both stream K in 64-element blocks through a multi-stage mbarrier ring
+// (a stage is released as soon as the wgmma group that read it has retired, so the loads of the next k-blocks overlap the
+// MMAs), and both run the same epilogue, tc_epilogue, on the accumulator fragments where they are (scale/shift/ReLU in
+// place -> fp32 / split-bf16 through per-warp TMA tensor stores, or max-pool as a shuffle reduce-and-transpose butterfly
+// over the fragment rows; only pools of 32-128 rows meet other warps, through a small exchange in shared memory).  Two
+// consumer warpgroups; warpgroup g owns rows 64g..64g+63 of a 128-row tile and issues the wgmma chain into its registers.
+// linear_tc_tma_kernel<BN> (A read from memory): 384 threads = 3 warpgroups; one thread of warp 0 issues the TMA boxes of
+// A_hi/A_lo/B_hi/B_lo, warps 4-11 are the consumers.  Tiles of 128 x BN, BN = 32, 64 or 128: a wider tile reads each A
+// row from L2 and from shared memory fewer times (see linear_tc_launch).  384 threads leave 168 registers per thread, so
+// the 64 accumulators of a BN = 128 consumer fit next to the epilogue.
+// linear_tc_kernel<BN> (gather modes): 640 threads = 5 warpgroups; warp 0 = TMA producer of the weights (warps 1-3 idle),
+// warps 4-11 = operand producers, warps 12-19 = the consumers.  640 threads leave 96 registers per thread, so tiles stop
+// at BN = 64.
 // Gather modes (TcParams::gather): the operand tile is not read from memory but built in shared memory by the
 // producer warps from neighbour indices (1: concat(features, xyz - centre); 2: the hoisted first conv) and kept
 // resident across the n-tiles of its m-tile (TcParams::astat).
@@ -41,30 +46,31 @@ namespace ssd3d {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;                 // bf16 elements per k-block = one 128-byte swizzle row
-constexpr int TC_PROD_WARP0 = 4;          // warps 4..11: A-operand producers of the gather modes: two threads per tile row, each
+constexpr int TC_PROD_WARP0 = 4;          // gather kernel, warps 4..11: A-operand producers: two threads per tile row, each
 constexpr int TC_PROD_WARPS = 8;          // builds 4 of the 8 16-byte chunks of a k-block
-constexpr int TC_EPI_WARP0 = TC_PROD_WARP0 + TC_PROD_WARPS;   // warps 12..19: the two consumer warpgroups (MMA + epilogue)
+constexpr int TC_EPI_WARP0 = TC_PROD_WARP0 + TC_PROD_WARPS;   // gather kernel, warps 12..19: the two consumer warpgroups
 constexpr int TC_EPI_WARPS = 8;
 constexpr int TC_THREADS = (TC_EPI_WARP0 + TC_EPI_WARPS) * 32;
-// 640 threads leave 96 registers per thread: at BN = 64 the consumer's 32 accumulator registers and the fragment epilogue
-// fit without spills, a BN = 128 accumulator would not, so tiles stop at 64 columns.
-constexpr int TC_MAX_BN = 64;
+constexpr int TC_GATHER_MAX_BN = 64;
+constexpr int TC_TMA_EPI_WARP0 = 4;       // TMA kernel, warps 4..11: the two consumer warpgroups
+constexpr int TC_TMA_THREADS = (TC_TMA_EPI_WARP0 + TC_EPI_WARPS) * 32;
+constexpr int TC_MAX_BN = 128;
 constexpr int TC_MAX_STAGES = 4;
 constexpr int TC_MAX_AKB = 4;            // A-stationary mode: k-blocks of an m-tile resident at once (K <= 256)
 constexpr uint32_t TC_A_BYTES = TC_BM * TC_BK * 2;   // one A tile (hi or lo): 16 KiB
+constexpr uint32_t TC_STORE_BLOCK = 4096;            // per-warp TMA-store block: 16 rows x 64 fp32 (or 2 x 64 bf16) columns
 // Shared memory per CTA: the planner hands out at most TC_DYN_SMEM of dynamic shared memory (1 KiB of it is the
-// alignment slack of the carve); the kernel's static __shared__ (mbarriers + pool_xs, allocated in 1 KiB granules) takes
-// the rest of the 227 KiB opt-in limit.  At BN = 64 that is 3 KiB, so the limit is met exactly: anything added to the
-// static footprint must come out of TC_DYN_SMEM.
+// alignment slack of the carve); the kernels' static __shared__ (the mbarriers, allocated in 1 KiB granules) takes the
+// rest of the 227 KiB opt-in limit.
 constexpr size_t TC_DYN_SMEM = 224 * 1024;
-constexpr size_t TC_STATIC_SMEM = (2 * TC_MAX_STAGES + 2 * TC_MAX_AKB) * 8 + TC_EPI_WARPS * TC_MAX_BN * sizeof(float);
+constexpr size_t TC_STATIC_SMEM = (2 * TC_MAX_STAGES + 2 * TC_MAX_AKB) * 8;
 static_assert(TC_DYN_SMEM + (TC_STATIC_SMEM + 1023) / 1024 * 1024 <= 227 * 1024, "linear_tc: shared memory over the opt-in limit");
 
 struct TcParams {
     long rows;
     int kp;          // K padded to a multiple of 16
     int n;           // output channels
-    int bn;          // tile width (multiple of 16, <= 256)
+    int bn;          // tile width (32, 64 or 128)
     int n_tiles, m_tiles, stages;
     const float *scale, *shift;
     int relu, pool;
@@ -140,8 +146,8 @@ __device__ __forceinline__ void store_pooled(const TcParams &p, long gg, int col
 }
 
 // Developer instrumentation (nvcc -DTC_PROFILE): CTA 0 accumulates, per role, the cycles spent waiting on each barrier
-// and the cycles spent working; printed by the launcher.  Slots: 0 total | 1 tma wait-empty | 2 mma wait-afull |
-// 3 mma wait-full(B) | 4 - | 5 mma issue | 6 prod wait-slot | 7 prod load+math | 8 mma drain | 9 epi work
+// and the cycles spent working; printed by the launcher.  Slots: 1 tma wait-empty | 6 prod wait-slot |
+// 7 prod load+math | 8 consumer waits + MMAs of a tile | 9 epi work
 #ifdef TC_PROFILE
 __device__ long long tc_prof[16];
 #define TCP_DECL long long tcp_t = clock64(); const bool tcp_on = blockIdx.x == 0 && lane == 0
@@ -152,34 +158,309 @@ __device__ long long tc_prof[16];
 #endif
 
 // ---------------------------------------------------------------------------------------------------------
+// The epilogue of one 128 x BN tile, run by consumer warp `we` (0..7: rows 16we..16we+15 of the tile, warpgroup we / 4) on
+// its accumulator fragment: folded bias/BN scale/shift, ReLU, then store or pool.  out_stage: the per-warp TMA-store
+// blocks (tma_store launches); pool_xs: [8 warps][BN] floats (pools of 32-128 rows).
+template <int BN>
+__device__ __forceinline__ void tc_epilogue(const TcParams &p, float (&d)[BN / 2], int mt, int nt, long rows, int nunits,
+                                            const float *s_scale, const float *s_shift, uint8_t *out_stage,
+                                            float *pool_xs, int we, int lane, const CUtensorMap *map_ohi,
+                                            const CUtensorMap *map_olo, const CUtensorMap *map_of32)
+{
+    const int g = we >> 2;
+    const int cq = 2 * (lane & 3);                                   // this thread's column pair inside each 8 columns
+    const int col_t = nt * BN;
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+        const float2 sc = *reinterpret_cast<const float2 *>(s_scale + col_t + 8 * j + cq);
+        const float2 sh = *reinterpret_cast<const float2 *>(s_shift + col_t + 8 * j + cq);
+        d[4 * j] = fmaf(d[4 * j], sc.x, sh.x);
+        d[4 * j + 1] = fmaf(d[4 * j + 1], sc.y, sh.y);
+        d[4 * j + 2] = fmaf(d[4 * j + 2], sc.x, sh.x);
+        d[4 * j + 3] = fmaf(d[4 * j + 3], sc.y, sh.y);
+    }
+    if (p.relu) {
+#pragma unroll
+        for (int j = 0; j < BN / 2; j++) d[j] = fmaxf(d[j], 0.0f);
+    }
+    const int row0 = mt * TC_BM + 16 * we;                           // first row of this warp's fragment
+    const int rq = lane >> 2;                                        // fragment row of d[4j], d[4j+1]; +8 for the others
+    if (p.pool <= 1 && p.tma_store) {
+        // Each warp owns a 4 KiB block: its [16 rows x 32 columns] pieces are laid out in the TMA swizzle and one bulk
+        // tensor store per piece writes whole 64/128-byte row segments (rows / columns beyond the tensor are clipped by
+        // the hardware).  Up to 64 columns pass through the block at a time; it is reused once the previous stores
+        // have read it.
+        uint8_t *blk = out_stage + we * TC_STORE_BLOCK;
+        constexpr int PIECES = BN < 64 ? BN / 32 : 2;
+#pragma unroll
+        for (int c64 = 0; c64 < BN / (32 * PIECES); c64++) {
+            if (lane == 0) tma_store_wait_read();
+            __syncwarp();
+#pragma unroll
+            for (int q = 0; q < PIECES; q++) {
+                uint8_t *piece = blk + q * 2048;
+                const int c32 = PIECES * c64 + q;
+                if (p.out_f32) {                                     // 128-byte rows, SWIZZLE_128B: 2 KiB
+#pragma unroll
+                    for (int jj = 0; jj < 4; jj++) {
+                        const int j = 4 * c32 + jj;
+                        const uint32_t off = (uint32_t)rq * 128u + (uint32_t)(((2 * jj + (cq >> 2)) ^ rq) << 4) + (uint32_t)(cq & 2) * 4u;
+                        *reinterpret_cast<float2 *>(piece + off) = make_float2(d[4 * j], d[4 * j + 1]);
+                        *reinterpret_cast<float2 *>(piece + 1024 + off) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+                    }
+                } else {                                             // 64-byte rows (hi | lo), SWIZZLE_64B: 1 KiB each
+#pragma unroll
+                    for (int jj = 0; jj < 4; jj++) {
+                        const int j = 4 * c32 + jj;
+                        const uint32_t off = (uint32_t)rq * 64u + (uint32_t)((jj ^ ((rq >> 1) & 3)) << 4) + (uint32_t)cq * 2u;
+                        uint32_t hw, lw;
+                        split_pair(d[4 * j], d[4 * j + 1], hw, lw);
+                        *reinterpret_cast<uint32_t *>(piece + off) = hw;
+                        *reinterpret_cast<uint32_t *>(piece + 1024 + off) = lw;
+                        split_pair(d[4 * j + 2], d[4 * j + 3], hw, lw);
+                        *reinterpret_cast<uint32_t *>(piece + 512 + off) = hw;
+                        *reinterpret_cast<uint32_t *>(piece + 1536 + off) = lw;
+                    }
+                }
+            }
+            fence_async_smem();
+            __syncwarp();
+            if (lane == 0) {
+#pragma unroll
+                for (int q = 0; q < PIECES; q++) {
+                    const uint32_t piece = smem_u32(blk + q * 2048);
+                    const int col = col_t + 32 * (PIECES * c64 + q);
+                    if (p.out_f32) {
+                        tma_store_2d(map_of32, piece, col, row0);
+                    } else {
+                        tma_store_2d(map_ohi, piece, col, row0);
+                        tma_store_2d(map_olo, piece + 1024, col, row0);
+                    }
+                }
+                tma_store_commit();
+            }
+        }
+    } else if (p.pool <= 1) {
+#pragma unroll
+        for (int hf = 0; hf < 2; hf++) {
+            const long row = (long)row0 + rq + 8 * hf;
+            if (row >= rows) continue;
+#pragma unroll
+            for (int j = 0; j < BN / 8; j++) {
+                const int col = col_t + 8 * j + cq;
+                const float x0 = d[4 * j + 2 * hf], x1 = d[4 * j + 2 * hf + 1];
+                if (p.out_f32) {
+                    float *dst = p.out_f32 + (size_t)row * p.ld_f32 + col;
+                    if (col < p.n) dst[0] = x0;
+                    if (col + 1 < p.n) dst[1] = x1;
+                }
+                // x = hi + lo (bf16 each); columns n..ld_split-1 come out as exact zeros (next layer's K padding)
+                if (p.out_hi && col < p.ld_split) {
+                    uint32_t hw, lw;
+                    split_pair(x0, x1, hw, lw);
+                    *reinterpret_cast<uint32_t *>(p.out_hi + (size_t)row * p.ld_split + col) = hw;
+                    *reinterpret_cast<uint32_t *>(p.out_lo + (size_t)row * p.ld_split + col) = lw;
+                }
+            }
+        }
+    } else if (p.unit_pool) {
+        // each 8-row fragment half is one listed unit; its column maxima go to the unit's GROUP row by atomicMax
+        frag_pool8<BN>(d, lane);
+#pragma unroll
+        for (int i = 0; i < BN / 16; i++) {
+            const int s = i + (BN / 16) * rq;
+            const int ui = mt * (TC_BM / 8) + 2 * we + ((s >> 1) & 1);
+            const int col = col_t + 8 * (s >> 2) + cq + (s & 1);
+            if (ui >= nunits || col >= p.n) continue;
+            atomic_max_nonneg(p.out_f32 + (size_t)unit_group((uint32_t)__ldg(p.units + 1 + ui)) * p.ld_f32 + col, d[i]);
+        }
+    } else if (p.pool == 8) {
+        frag_pool8<BN>(d, lane);
+#pragma unroll
+        for (int i = 0; i < BN / 16; i++) {
+            const int s = i + (BN / 16) * rq;
+            const long gg = (long)mt * (TC_BM / 8) + 2 * we + ((s >> 1) & 1);
+            if (gg * 8 < p.rows) store_pooled(p, gg, col_t + 8 * (s >> 2) + cq + (s & 1), d[i]);
+        }
+    } else {
+        // pools of 16-128 rows: 16-row maxima per warp, then (32-128) the warps of a group combine through pool_xs
+        float u[BN / 4];
+        frag_pool16<BN>(d, u, lane);
+        const int wpg = p.pool / 16;                                 // warps per pooling group
+        if (wpg > 1) {
+#pragma unroll
+            for (int i = 0; i < BN / 32; i++) {
+                const int s = i + (BN / 32) * rq;
+                pool_xs[we * BN + 8 * (s >> 1) + cq + (s & 1)] = u[i];
+            }
+            if (wpg == 8) named_bar_sync(2, 256);
+            else named_bar_sync(4 + g, 128);
+            if (we % wpg == 0) {
+                for (int k = 1; k < wpg; k++) {
+#pragma unroll
+                    for (int i = 0; i < BN / 32; i++) {
+                        const int s = i + (BN / 32) * rq;
+                        u[i] = fmaxf(u[i], pool_xs[(we + k) * BN + 8 * (s >> 1) + cq + (s & 1)]);
+                    }
+                }
+            }
+            if (wpg == 8) named_bar_sync(2, 256);                     // pool_xs reusable by the next tile
+            else named_bar_sync(4 + g, 128);
+        }
+        if (we % wpg == 0) {
+            const long gg = ((long)mt * TC_BM + 16 * we) / p.pool;
+#pragma unroll
+            for (int i = 0; i < BN / 32; i++) {
+                const int s = i + (BN / 32) * rq;
+                if (gg * p.pool < p.rows) store_pooled(p, gg, col_t + 8 * (s >> 1) + cq + (s & 1), u[i]);
+            }
+        }
+    }
+}
+
+// The consumer side shared by both kernels: the wgmma chain of one tile over the k-blocks of the ring, each stage
+// released (release(s, kb)) once the wgmma group that read it has retired.  a_at(s, kb): shared address of this
+// warpgroup's 64-row slab of A_hi for k-block kb in ring stage s (A_lo follows TC_A_BYTES later); b_off: B_hi inside a stage.
+template <int BN, typename AAt, typename Release>
+__device__ __forceinline__ void tc_mma_tile(float (&d)[BN / 2], int &it, int nkb, int kp, int stages, uint32_t ring,
+                                            uint32_t stage_bytes, uint32_t b_off, AAt a_at, Release release,
+                                            const uint64_t *full_bar)
+{
+    constexpr uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;
+    int prev_s = -1, prev_kb = 0;
+    for (int kb = 0; kb < nkb; kb++, it++) {
+        const int s = it % stages;
+        const uint32_t base = ring + (uint32_t)s * stage_bytes;
+        const uint32_t abase = a_at(s, kb, base);
+        mbar_wait_cta(smem_u32(&full_bar[s]), (uint32_t)(it / stages) & 1u);
+        const int ksteps = min(TC_BK, kp - kb * TC_BK) / 16;
+        const uint64_t a_hi = wg_desc(abase, 128), a_lo = wg_desc(abase + TC_A_BYTES, 128);
+        const uint64_t b_hi = wg_desc(base + b_off, 128), b_lo = wg_desc(base + b_off + b_bytes, 128);
+        wg_fence();
+        for (int ks = 0; ks < ksteps; ks++)                          // +2 per k-step: 32 bytes in the address field
+            wg_mma3<BN>(d, a_hi + 2 * ks, a_lo + 2 * ks, b_hi + 2 * ks, b_lo + 2 * ks, (kb | ks) ? 1u : 0u);
+        wg_commit();
+        wg_wait<1>();                                                // the previous k-block's group has retired
+        if (prev_s >= 0) release(prev_s, prev_kb);
+        prev_s = s; prev_kb = kb;
+    }
+    wg_wait<0>();
+    release(prev_s, prev_kb);
+}
+
+// ---- linear_tc_tma_kernel: A from memory ---------------------------------------------------------------------
+template <int BN>
+__global__ void __launch_bounds__(TC_TMA_THREADS, 1)
+linear_tc_tma_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
+                     const __grid_constant__ CUtensorMap map_bhi, const __grid_constant__ CUtensorMap map_blo,
+                     const __grid_constant__ CUtensorMap map_ohi, const __grid_constant__ CUtensorMap map_olo,
+                     const __grid_constant__ CUtensorMap map_of32, const TcParams p)
+{
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    // carve: [stages] x { A_hi | A_lo | B_hi | B_lo }, per-warp output blocks (tma_store), scale/shift, pool exchange
+    constexpr uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;
+    constexpr uint32_t stage_bytes = 2 * TC_A_BYTES + 2 * b_bytes;
+    const int nkb = (p.kp + TC_BK - 1) / TC_BK;
+    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    const int ncov = p.n_tiles * BN + 32;
+    uint8_t *out_stage = smem + (size_t)p.stages * stage_bytes;
+    float *s_scale = reinterpret_cast<float *>(out_stage + (p.tma_store ? TC_EPI_WARPS * TC_STORE_BLOCK : 0));
+    float *s_shift = s_scale + ncov;
+    float *pool_xs = s_shift + ncov;                                     // [8 warps][BN] (pools of 16-128 rows)
+
+    __shared__ uint64_t full_bar[TC_MAX_STAGES], empty_bar[TC_MAX_STAGES];
+
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+    // unit-list mode: the row count comes from the list (written earlier on this stream), p.rows is the buffers' capacity
+    const int nunits = p.units ? __ldg(p.units) : 0;
+    const long rows = p.units ? (long)nunits * 8 : p.rows;
+    const int m_tiles = p.units ? (nunits + TC_BM / 8 - 1) / (TC_BM / 8) : p.m_tiles;
+    const int n_all = m_tiles * p.n_tiles;                               // tiles, n-major round robin over the CTAs
+
+    if (threadIdx.x == 0) {
+        // full barrier: the TMA thread's expect_tx arrival; empty: one arrival per consumer warp
+        for (int s = 0; s < p.stages; s++) { mbar_init(smem_u32(&full_bar[s]), 1); mbar_init(smem_u32(&empty_bar[s]), TC_EPI_WARPS); }
+        fence_mbar_init_cluster();
+    }
+    for (int i = threadIdx.x; i < ncov; i += TC_TMA_THREADS) {  // columns >= n: scale = shift = 0 -> exact zeros
+        s_scale[i] = i < p.n ? __ldg(p.scale + i) : 0.0f;
+        s_shift[i] = i < p.n ? __ldg(p.shift + i) : 0.0f;
+    }
+    __syncthreads();
+    if (warp < TC_TMA_EPI_WARP0) {
+        // ===== TMA producer: one thread issues every box into the ring
+        if (warp == 0 && lane == 0) {
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&map_ahi) : "memory");
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&map_alo) : "memory");
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&map_bhi) : "memory");
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&map_blo) : "memory");
+            int it = 0;
+            TCP_DECL;
+            for (int tile = blockIdx.x; tile < n_all; tile += gridDim.x) {
+                const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
+                for (int kb = 0; kb < nkb; kb++, it++) {
+                    const int s = it % p.stages;
+                    mbar_wait_cta(smem_u32(&empty_bar[s]), ((uint32_t)(it / p.stages) & 1u) ^ 1u);
+                    TCP(1);
+                    const uint32_t base = smem_u32(smem + (size_t)s * stage_bytes);
+                    const uint32_t fb = smem_u32(&full_bar[s]);
+                    mbar_arrive_expect_tx(fb, stage_bytes);
+                    tma_load_2d(base, &map_ahi, kb * TC_BK, mt * TC_BM, fb);
+                    tma_load_2d(base + TC_A_BYTES, &map_alo, kb * TC_BK, mt * TC_BM, fb);
+                    tma_load_2d(base + 2 * TC_A_BYTES, &map_bhi, kb * TC_BK, nt * BN, fb);
+                    tma_load_2d(base + 2 * TC_A_BYTES + b_bytes, &map_blo, kb * TC_BK, nt * BN, fb);
+                }
+            }
+        }
+    } else {
+        // ===== consumers: warpgroup g = rows 64g..64g+63 of the tile
+        const int we = warp - TC_TMA_EPI_WARP0;
+        const uint32_t g_off = (uint32_t)(we >> 2) * (64u * 128u);       // this warpgroup's 64 rows (8 swizzle atoms)
+        int it = 0;
+        TCP_DECL;
+        for (int tile = blockIdx.x; tile < n_all; tile += gridDim.x) {
+            const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
+            float d[BN / 2];
+            tc_mma_tile<BN>(d, it, nkb, p.kp, p.stages, smem_u32(smem), stage_bytes, 2 * TC_A_BYTES,
+                            [&](int, int, uint32_t base) { return base + g_off; },
+                            [&](int s, int) { if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s])); }, full_bar);
+            if (we == 0) TCP(8);
+            tc_epilogue<BN>(p, d, mt, nt, rows, nunits, s_scale, s_shift, out_stage, pool_xs, we, lane, &map_ohi, &map_olo,
+                            &map_of32);
+            if (we == 0) TCP(9);
+        }
+        if (p.tma_store && lane == 0) tma_store_wait_all();           // global writes complete before the CTA retires
+    }
+}
+
+// ---- linear_tc_kernel: the gather modes (A built in shared memory by the producer warps) ---------------------------
 template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
-                 const __grid_constant__ CUtensorMap map_bhi, const __grid_constant__ CUtensorMap map_blo,
+linear_tc_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_constant__ CUtensorMap map_blo,
                  const __grid_constant__ CUtensorMap map_ohi, const __grid_constant__ CUtensorMap map_olo,
                  const __grid_constant__ CUtensorMap map_of32, const TcParams p)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [resident A tiles] [stages] x { A_hi | A_lo | B_hi | B_lo }, per-warp output blocks (4 KiB each), then
-    // scale/shift
-    const uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;
+    // carve: [resident A tiles] [stages] x { A_hi | A_lo (ring A, without astat) | B_hi | B_lo }, per-warp output blocks,
+    // scale/shift, hoisted Wx, pool exchange
+    constexpr uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;
     const int nkb = (p.kp + TC_BK - 1) / TC_BK;
     const uint32_t a_region = p.astat ? (uint32_t)nkb * 2u * TC_A_BYTES : 0u;       // resident A tile: [nkb] x { A_hi | A_lo }
-    const uint32_t stage_bytes = (p.astat ? 0u : 2 * TC_A_BYTES) + 2 * b_bytes;     // ring stage
     const uint32_t b_off = p.astat ? 0u : 2 * TC_A_BYTES;                           // B_hi inside a stage
+    const uint32_t stage_bytes = b_off + 2 * b_bytes;                               // ring stage
     // 1 KiB alignment by pointer arithmetic on the __shared__ array (an integer round-trip would demote every access
     // through these pointers to generic LD/ST with 64-bit address math)
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int ncov = p.n_tiles * p.bn + 32;
+    const int ncov = p.n_tiles * BN + 32;
     uint8_t *ring = smem + a_region;
     uint8_t *out_stage = ring + (size_t)p.stages * stage_bytes;          // [8 warps][4 KiB], 4 KiB aligned
-    float *s_scale = reinterpret_cast<float *>(out_stage + (p.tma_store ? TC_EPI_WARPS * 4096 : 0));
+    float *s_scale = reinterpret_cast<float *>(out_stage + (p.tma_store ? TC_EPI_WARPS * TC_STORE_BLOCK : 0));
     float *s_shift = s_scale + ncov;
     float *s_wx = s_shift + ncov;                                        // [3][kp] (hoisted mode only)
+    float *pool_xs = s_wx + (p.gather == 2 ? 3 * p.kp : 0);              // [8 warps][BN] (pools of 16-128 rows)
 
-    __shared__ unsigned long long full_bar[TC_MAX_STAGES], empty_bar[TC_MAX_STAGES];
-    __shared__ unsigned long long afull_bar[TC_MAX_AKB], aempty_bar[TC_MAX_AKB];   // per k-block of the resident A tile
-    __shared__ __align__(16) float pool_xs[TC_EPI_WARPS * BN];          // 32-128-row pools: per-warp 16-row maxima (TC_STATIC_SMEM)
+    __shared__ uint64_t full_bar[TC_MAX_STAGES], empty_bar[TC_MAX_STAGES];
+    __shared__ uint64_t afull_bar[TC_MAX_AKB], aempty_bar[TC_MAX_AKB];   // per k-block of the resident A tile
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // provably warp-uniform
     // unit-list mode: the row count comes from the list (written earlier on this stream), p.rows is the buffers' capacity
@@ -200,9 +481,9 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
     };
 
     if (threadIdx.x == 0) {
-        // full barrier: the TMA thread's expect_tx arrival (+ one arrival per producer warp in gather mode);
-        // empty barriers: one arrival per consumer warp once its wgmma group reading the slot has retired
-        for (int s = 0; s < p.stages; s++) { mbar_init(smem_u32(&full_bar[s]), (p.gather && !p.astat) ? 1 + TC_PROD_WARPS : 1); mbar_init(smem_u32(&empty_bar[s]), TC_EPI_WARPS); }
+        // full barrier: the TMA thread's expect_tx arrival (+ one arrival per producer warp when A passes through the
+        // ring); empty barriers: one arrival per consumer warp once its wgmma group reading the slot has retired
+        for (int s = 0; s < p.stages; s++) { mbar_init(smem_u32(&full_bar[s]), p.astat ? 1 : 1 + TC_PROD_WARPS); mbar_init(smem_u32(&empty_bar[s]), TC_EPI_WARPS); }
         for (int k = 0; k < TC_MAX_AKB; k++) { mbar_init(smem_u32(&afull_bar[k]), TC_PROD_WARPS); mbar_init(smem_u32(&aempty_bar[k]), TC_EPI_WARPS); }
         fence_mbar_init_cluster();
     }
@@ -217,10 +498,8 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
         }
     __syncthreads();
     if (warp == 0) {
-        // ===== TMA producer =====
+        // ===== TMA producer of the weights =====
         if (lane == 0) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&map_ahi) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&map_alo) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&map_bhi) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&map_blo) : "memory");
             int it = 0, mt, nt;
@@ -234,87 +513,82 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                     TCP(1);
                     const uint32_t base = smem_u32(ring + (size_t)s * stage_bytes);
                     const uint32_t fb = smem_u32(&full_bar[s]);
-                    mbar_arrive_expect_tx(fb, p.gather ? 2 * b_bytes : stage_bytes);
-                    if (!p.gather) {
-                        tma_load_2d(base, &map_ahi, kb * TC_BK, mt * TC_BM, fb);
-                        tma_load_2d(base + TC_A_BYTES, &map_alo, kb * TC_BK, mt * TC_BM, fb);
-                    }
-                    tma_load_2d(base + b_off, &map_bhi, kb * TC_BK, nt * p.bn, fb);
-                    tma_load_2d(base + b_off + b_bytes, &map_blo, kb * TC_BK, nt * p.bn, fb);
+                    mbar_arrive_expect_tx(fb, 2 * b_bytes);
+                    tma_load_2d(base + b_off, &map_bhi, kb * TC_BK, nt * BN, fb);
+                    tma_load_2d(base + b_off + b_bytes, &map_blo, kb * TC_BK, nt * BN, fb);
                 }
             }
         }
     } else if (warp >= TC_PROD_WARP0 && warp < TC_EPI_WARP0) {
-        // ===== A-operand producers (gather mode): 128 threads, one row of the tile each.  A row's source features are
-        // one contiguous run (16-byte loads when c % 4 == 0); all loads of a 64-wide k-block are issued before the
-        // values are split into bf16 hi/lo and stored as 16-byte chunks in the K-major SWIZZLE_128B layout the wgmma
-        // descriptor expects.
-        if (p.gather) {
-            const int pt = threadIdx.x - TC_PROD_WARP0 * 32;
-            const int r = pt & (TC_BM - 1);                      // tile row
-            const int c16_0 = (pt >> 7) * 4;                     // this thread's 4 chunks of every k-block
-            const uint32_t rps = (uint32_t)p.g_m * (uint32_t)p.g_ns;
-            const bool hoisted = p.gather == 2;
-            const int src_pitch = hoisted ? p.g_ldz : p.g_c;
-            const bool vec4 = (p.g_c % 4 == 0) && (src_pitch % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.g_points) & 15u) == 0);
-            const int kend = hoisted ? p.g_c : p.g_c + 3;        // operand columns read from the sources
-            int it = 0, mi = 0, mt, nt;
-            TCP_DECL;
-            for (int i = 0; tile_at(i, mt, nt); i++) {
-                if (p.astat && nt != 0) continue;                 // A-stationary: the tile built for nt == 0 serves every n-tile
-                const uint32_t row = (uint32_t)mt * TC_BM + (uint32_t)r;
-                const bool ok = (long)row < rows;
-                uint32_t rr = ok ? row : 0u;                      // position of this row's neighbour in idx[]
-                if (p.units && ok) rr = unit_slot((uint32_t)__ldg(p.units + 1 + (row >> 3)), (uint32_t)p.g_ns, row & 7u);
-                const uint32_t scene = rr / rps, q = rr / (uint32_t)p.g_ns;
-                const int a = __ldg(p.g_idx + rr);
-                const float *src_f = p.g_points + ((size_t)scene * p.g_n + a) * src_pitch;
-                const float *src_x = p.g_xyz + ((size_t)scene * p.g_n + a) * 3;
-                const float *ctr = p.g_new_xyz + (size_t)q * 3;
-                float dx = 0.0f, dy = 0.0f, dz = 0.0f;
-                if (hoisted && ok) {
-                    dx = __ldg(src_x) - __ldg(ctr); dy = __ldg(src_x + 1) - __ldg(ctr + 1); dz = __ldg(src_x + 2) - __ldg(ctr + 2);
-                }
-                for (int kb = 0; kb < nkb; kb++, it++) {
-                    const int s = it % p.stages;
-                    float f[4][8];
-#pragma unroll
-                    for (int cc = 0; cc < 4; cc++) load_concat8(f[cc], src_f, src_x, ctr, p.g_c, kend, kb * TC_BK + (c16_0 + cc) * 8, vec4, ok);
-                    // (loads already in flight) wait for the slot: ring stage, or this k-block of the resident A tile
-                    if (warp == TC_PROD_WARP0) TCP(7);
-                    if (p.astat) mbar_wait_cta(smem_u32(&aempty_bar[kb]), ((uint32_t)mi & 1u) ^ 1u);
-                    else mbar_wait_cta(smem_u32(&empty_bar[s]), ((uint32_t)(it / p.stages) & 1u) ^ 1u);
-                    if (warp == TC_PROD_WARP0) TCP(6);
-                    uint8_t *blk = p.astat ? smem + (size_t)kb * 2 * TC_A_BYTES : ring + (size_t)s * stage_bytes;
-#pragma unroll
-                    for (int cc = 0; cc < 4; cc++) {
-                        const int c16 = c16_0 + cc;
-                        const int k0 = kb * TC_BK + c16 * 8;
-                        if (k0 >= p.kp) break;
-                        if (hoisted) hoisted_row8(f[cc], s_wx + k0, p.kp, dx, dy, dz);   // rows beyond the tensor stay 0
-                        const uint32_t off = sw128_chunk((uint32_t)r, (uint32_t)c16);
-                        split_store8(blk + off, blk + TC_A_BYTES + off, f[cc]);
-                    }
-                    fence_async_smem();                                   // generic-proxy stores -> visible to the tensor core
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(smem_u32(p.astat ? &afull_bar[kb] : &full_bar[s]));
-                }
-                mi++;
+        // ===== A-operand producers: 128 threads, one row of the tile each.  A row's source features are one contiguous
+        // run (16-byte loads when c % 4 == 0); all loads of a 64-wide k-block are issued before the values are split into
+        // bf16 hi/lo and stored as 16-byte chunks in the K-major SWIZZLE_128B layout the wgmma descriptor expects.
+        const int pt = threadIdx.x - TC_PROD_WARP0 * 32;
+        const int r = pt & (TC_BM - 1);                          // tile row
+        const int c16_0 = (pt >> 7) * 4;                         // this thread's 4 chunks of every k-block
+        const uint32_t rps = (uint32_t)p.g_m * (uint32_t)p.g_ns;
+        const bool hoisted = p.gather == 2;
+        const int src_pitch = hoisted ? p.g_ldz : p.g_c;
+        const bool vec4 = (p.g_c % 4 == 0) && (src_pitch % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.g_points) & 15u) == 0);
+        const int kend = hoisted ? p.g_c : p.g_c + 3;            // operand columns read from the sources
+        int it = 0, mi = 0, mt, nt;
+        TCP_DECL;
+        for (int i = 0; tile_at(i, mt, nt); i++) {
+            if (p.astat && nt != 0) continue;                     // A-stationary: the tile built for nt == 0 serves every n-tile
+            const uint32_t row = (uint32_t)mt * TC_BM + (uint32_t)r;
+            const bool ok = (long)row < rows;
+            uint32_t rr = ok ? row : 0u;                          // position of this row's neighbour in idx[]
+            if (p.units && ok) rr = unit_slot((uint32_t)__ldg(p.units + 1 + (row >> 3)), (uint32_t)p.g_ns, row & 7u);
+            const uint32_t scene = rr / rps, q = rr / (uint32_t)p.g_ns;
+            const int a = __ldg(p.g_idx + rr);
+            const float *src_f = p.g_points + ((size_t)scene * p.g_n + a) * src_pitch;
+            const float *src_x = p.g_xyz + ((size_t)scene * p.g_n + a) * 3;
+            const float *ctr = p.g_new_xyz + (size_t)q * 3;
+            float dx = 0.0f, dy = 0.0f, dz = 0.0f;
+            if (hoisted && ok) {
+                dx = __ldg(src_x) - __ldg(ctr); dy = __ldg(src_x + 1) - __ldg(ctr + 1); dz = __ldg(src_x + 2) - __ldg(ctr + 2);
             }
+            for (int kb = 0; kb < nkb; kb++, it++) {
+                const int s = it % p.stages;
+                float f[4][8];
+#pragma unroll
+                for (int cc = 0; cc < 4; cc++) load_concat8(f[cc], src_f, src_x, ctr, p.g_c, kend, kb * TC_BK + (c16_0 + cc) * 8, vec4, ok);
+                // (loads already in flight) wait for the slot: ring stage, or this k-block of the resident A tile
+                if (warp == TC_PROD_WARP0) TCP(7);
+                if (p.astat) mbar_wait_cta(smem_u32(&aempty_bar[kb]), ((uint32_t)mi & 1u) ^ 1u);
+                else mbar_wait_cta(smem_u32(&empty_bar[s]), ((uint32_t)(it / p.stages) & 1u) ^ 1u);
+                if (warp == TC_PROD_WARP0) TCP(6);
+                uint8_t *blk = p.astat ? smem + (size_t)kb * 2 * TC_A_BYTES : ring + (size_t)s * stage_bytes;
+#pragma unroll
+                for (int cc = 0; cc < 4; cc++) {
+                    const int c16 = c16_0 + cc;
+                    const int k0 = kb * TC_BK + c16 * 8;
+                    if (k0 >= p.kp) break;
+                    if (hoisted) hoisted_row8(f[cc], s_wx + k0, p.kp, dx, dy, dz);   // rows beyond the tensor stay 0
+                    const uint32_t off = sw128_chunk((uint32_t)r, (uint32_t)c16);
+                    split_store8(blk + off, blk + TC_A_BYTES + off, f[cc]);
+                }
+                fence_async_smem();                                   // generic-proxy stores -> visible to the tensor core
+                __syncwarp();
+                if (lane == 0) mbar_arrive(smem_u32(p.astat ? &afull_bar[kb] : &full_bar[s]));
+            }
+            mi++;
         }
     } else if (warp >= TC_EPI_WARP0) {
-        // ===== consumers: warpgroup g = rows 64g..64g+63 of the tile.  MMAs: the whole warpgroup issues the wgmma chain
-        // of every k-block into its registers.  Epilogue: each warp works on its own fragment (16 rows x BN columns, see
-        // quad_rowmax_transpose) in registers; only the 32-128-row pools meet other warps, through pool_xs.
-        const int g = (warp - TC_EPI_WARP0) >> 2;
-        const int we = warp - TC_EPI_WARP0;                              // consumer warp 0..7 = 16-row slab of the tile
-        const int cq = 2 * (lane & 3);                                   // this thread's column pair inside each 8 columns
+        // ===== consumers: warpgroup g = rows 64g..64g+63 of the tile; A from the resident tile (astat) or the ring
+        const int we = warp - TC_EPI_WARP0;
+        const uint32_t g_off = (uint32_t)(we >> 2) * (64u * 128u);       // this warpgroup's 64 rows (8 swizzle atoms)
         int it = 0, mi = 0, mt, nt;
         TCP_DECL;
         for (int i = 0; tile_at(i, mt, nt); i++) {
             const bool last_nt = nt == p.n_tiles - 1;
             float d[BN / 2];
-            int prev_s = -1, prev_kb = 0;
+            // the A slab of k-block kb: a resident k-block is waited for on the m-tile's first n-tile
+            auto a_slab = [&](int, int kb, uint32_t base) -> uint32_t {
+                if (!p.astat) return base + g_off;
+                if (nt == 0) mbar_wait_cta(smem_u32(&afull_bar[kb]), (uint32_t)mi & 1u);
+                return smem_u32(smem) + (uint32_t)kb * 2u * TC_A_BYTES + g_off;
+            };
             // a ring stage (and, after the last n-tile, a resident A k-block) is free once the wgmma group reading it retired
             auto release = [&](int s, int kb) {
                 if (lane == 0) {
@@ -322,173 +596,12 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_const
                     if (p.astat && last_nt) mbar_arrive(smem_u32(&aempty_bar[kb]));
                 }
             };
-            for (int kb = 0; kb < nkb; kb++, it++) {
-                const int s = it % p.stages;
-                if (warp == TC_EPI_WARP0) TCP(5);
-                if (p.astat && nt == 0) mbar_wait_cta(smem_u32(&afull_bar[kb]), (uint32_t)mi & 1u);   // this m-tile's A k-block
-                if (warp == TC_EPI_WARP0) TCP(2);
-                mbar_wait_cta(smem_u32(&full_bar[s]), (uint32_t)(it / p.stages) & 1u);
-                if (warp == TC_EPI_WARP0) TCP(3);
-                const uint32_t base = smem_u32(ring + (size_t)s * stage_bytes);
-                const uint32_t abase = (p.astat ? smem_u32(smem) + (uint32_t)kb * 2u * TC_A_BYTES : base) +
-                                       (uint32_t)g * (64u * 128u);        // this warpgroup's 64 rows (8 swizzle atoms)
-                const int ksteps = min(TC_BK, p.kp - kb * TC_BK) / 16;
-                const uint64_t a_hi = wg_desc(abase, 128), a_lo = wg_desc(abase + TC_A_BYTES, 128);
-                const uint64_t b_hi = wg_desc(base + b_off, 128), b_lo = wg_desc(base + b_off + b_bytes, 128);
-                wg_fence();
-                for (int ks = 0; ks < ksteps; ks++)                      // +2 per k-step: 32 bytes in the address field
-                    wg_mma3<BN>(d, a_hi + 2 * ks, a_lo + 2 * ks, b_hi + 2 * ks, b_lo + 2 * ks, (kb | ks) ? 1u : 0u);
-                wg_commit();
-                wg_wait<1>();                                            // the previous k-block's group has retired
-                if (prev_s >= 0) release(prev_s, prev_kb);
-                prev_s = s; prev_kb = kb;
-            }
-            wg_wait<0>();
-            release(prev_s, prev_kb);
+            tc_mma_tile<BN>(d, it, nkb, p.kp, p.stages, smem_u32(ring), stage_bytes, b_off, a_slab, release, full_bar);
             if (last_nt) mi++;
-            if (warp == TC_EPI_WARP0) TCP(8);
-            // epilogue on the fragment: folded bias/BN scale/shift, ReLU, then store or pool
-            const int col_t = nt * p.bn;
-#pragma unroll
-            for (int j = 0; j < BN / 8; j++) {
-                const float2 sc = *reinterpret_cast<const float2 *>(s_scale + col_t + 8 * j + cq);
-                const float2 sh = *reinterpret_cast<const float2 *>(s_shift + col_t + 8 * j + cq);
-                d[4 * j] = fmaf(d[4 * j], sc.x, sh.x);
-                d[4 * j + 1] = fmaf(d[4 * j + 1], sc.y, sh.y);
-                d[4 * j + 2] = fmaf(d[4 * j + 2], sc.x, sh.x);
-                d[4 * j + 3] = fmaf(d[4 * j + 3], sc.y, sh.y);
-            }
-            if (p.relu) {
-#pragma unroll
-                for (int j = 0; j < BN / 2; j++) d[j] = fmaxf(d[j], 0.0f);
-            }
-            const int row0 = mt * TC_BM + 16 * we;                       // first row of this warp's fragment
-            const int rq = lane >> 2;                                    // fragment row of d[4j], d[4j+1]; +8 for the others
-            if (p.pool <= 1 && p.tma_store) {
-                // Each warp owns a 4 KiB block: its [16 rows x 32 columns] pieces are laid out in the TMA swizzle and one
-                // bulk tensor store per piece writes whole 64/128-byte row segments (rows / columns beyond the tensor are
-                // clipped by the hardware); the block is reused once the previous stores have read it.
-                uint8_t *blk = out_stage + we * 4096;
-                if (lane == 0) tma_store_wait_read();
-                __syncwarp();
-#pragma unroll
-                for (int c32 = 0; c32 < BN / 32; c32++) {
-                    uint8_t *piece = blk + c32 * 2048;
-                    if (p.out_f32) {                                     // 128-byte rows, SWIZZLE_128B: 2 KiB
-#pragma unroll
-                        for (int jj = 0; jj < 4; jj++) {
-                            const int j = 4 * c32 + jj;
-                            const uint32_t off = (uint32_t)rq * 128u + (uint32_t)(((2 * jj + (cq >> 2)) ^ rq) << 4) + (uint32_t)(cq & 2) * 4u;
-                            *reinterpret_cast<float2 *>(piece + off) = make_float2(d[4 * j], d[4 * j + 1]);
-                            *reinterpret_cast<float2 *>(piece + 1024 + off) = make_float2(d[4 * j + 2], d[4 * j + 3]);
-                        }
-                    } else {                                             // 64-byte rows (hi | lo), SWIZZLE_64B: 1 KiB each
-#pragma unroll
-                        for (int jj = 0; jj < 4; jj++) {
-                            const int j = 4 * c32 + jj;
-                            const uint32_t off = (uint32_t)rq * 64u + (uint32_t)((jj ^ ((rq >> 1) & 3)) << 4) + (uint32_t)cq * 2u;
-                            uint32_t hw, lw;
-                            split_pair(d[4 * j], d[4 * j + 1], hw, lw);
-                            *reinterpret_cast<uint32_t *>(piece + off) = hw;
-                            *reinterpret_cast<uint32_t *>(piece + 1024 + off) = lw;
-                            split_pair(d[4 * j + 2], d[4 * j + 3], hw, lw);
-                            *reinterpret_cast<uint32_t *>(piece + 512 + off) = hw;
-                            *reinterpret_cast<uint32_t *>(piece + 1536 + off) = lw;
-                        }
-                    }
-                }
-                fence_async_smem();
-                __syncwarp();
-                if (lane == 0) {
-#pragma unroll
-                    for (int c32 = 0; c32 < BN / 32; c32++) {
-                        const uint32_t piece = smem_u32(blk + c32 * 2048);
-                        if (p.out_f32) {
-                            tma_store_2d(&map_of32, piece, col_t + 32 * c32, row0);
-                        } else {
-                            tma_store_2d(&map_ohi, piece, col_t + 32 * c32, row0);
-                            tma_store_2d(&map_olo, piece + 1024, col_t + 32 * c32, row0);
-                        }
-                    }
-                    tma_store_commit();
-                }
-            } else if (p.pool <= 1) {
-#pragma unroll
-                for (int hf = 0; hf < 2; hf++) {
-                    const long row = (long)row0 + rq + 8 * hf;
-                    if (row >= rows) continue;
-#pragma unroll
-                    for (int j = 0; j < BN / 8; j++) {
-                        const int col = col_t + 8 * j + cq;
-                        const float x0 = d[4 * j + 2 * hf], x1 = d[4 * j + 2 * hf + 1];
-                        if (p.out_f32) {
-                            float *dst = p.out_f32 + (size_t)row * p.ld_f32 + col;
-                            if (col < p.n) dst[0] = x0;
-                            if (col + 1 < p.n) dst[1] = x1;
-                        }
-                        // x = hi + lo (bf16 each); columns n..ld_split-1 come out as exact zeros (next layer's K padding)
-                        if (p.out_hi && col < p.ld_split) {
-                            uint32_t hw, lw;
-                            split_pair(x0, x1, hw, lw);
-                            *reinterpret_cast<uint32_t *>(p.out_hi + (size_t)row * p.ld_split + col) = hw;
-                            *reinterpret_cast<uint32_t *>(p.out_lo + (size_t)row * p.ld_split + col) = lw;
-                        }
-                    }
-                }
-            } else if (p.unit_pool) {
-                // each 8-row fragment half is one listed unit; its column maxima go to the unit's GROUP row by atomicMax
-                frag_pool8<BN>(d, lane);
-#pragma unroll
-                for (int i = 0; i < BN / 16; i++) {
-                    const int s = i + (BN / 16) * rq;
-                    const int ui = mt * (TC_BM / 8) + 2 * we + ((s >> 1) & 1);
-                    const int col = col_t + 8 * (s >> 2) + cq + (s & 1);
-                    if (ui >= nunits || col >= p.n) continue;
-                    atomic_max_nonneg(p.out_f32 + (size_t)unit_group((uint32_t)__ldg(p.units + 1 + ui)) * p.ld_f32 + col, d[i]);
-                }
-            } else if (p.pool == 8) {
-                frag_pool8<BN>(d, lane);
-#pragma unroll
-                for (int i = 0; i < BN / 16; i++) {
-                    const int s = i + (BN / 16) * rq;
-                    const long gg = (long)mt * (TC_BM / 8) + 2 * we + ((s >> 1) & 1);
-                    if (gg * 8 < p.rows) store_pooled(p, gg, col_t + 8 * (s >> 2) + cq + (s & 1), d[i]);
-                }
-            } else {
-                // pools of 16-128 rows: 16-row maxima per warp, then (32-128) the warps of a group combine through pool_xs
-                float u[BN / 4];
-                frag_pool16<BN>(d, u, lane);
-                const int wpg = p.pool / 16;                             // warps per pooling group
-                if (wpg > 1) {
-#pragma unroll
-                    for (int i = 0; i < BN / 32; i++) {
-                        const int s = i + (BN / 32) * rq;
-                        pool_xs[we * BN + 8 * (s >> 1) + cq + (s & 1)] = u[i];
-                    }
-                    if (wpg == 8) named_bar_sync(2, 256);
-                    else named_bar_sync(4 + g, 128);
-                    if (we % wpg == 0) {
-                        for (int k = 1; k < wpg; k++) {
-#pragma unroll
-                            for (int i = 0; i < BN / 32; i++) {
-                                const int s = i + (BN / 32) * rq;
-                                u[i] = fmaxf(u[i], pool_xs[(we + k) * BN + 8 * (s >> 1) + cq + (s & 1)]);
-                            }
-                        }
-                    }
-                    if (wpg == 8) named_bar_sync(2, 256);                 // pool_xs reusable by the next tile
-                    else named_bar_sync(4 + g, 128);
-                }
-                if (we % wpg == 0) {
-                    const long gg = ((long)mt * TC_BM + 16 * we) / p.pool;
-#pragma unroll
-                    for (int i = 0; i < BN / 32; i++) {
-                        const int s = i + (BN / 32) * rq;
-                        if (gg * p.pool < p.rows) store_pooled(p, gg, col_t + 8 * (s >> 1) + cq + (s & 1), u[i]);
-                    }
-                }
-            }
-            if (warp == TC_EPI_WARP0) TCP(9);
+            if (we == 0) TCP(8);
+            tc_epilogue<BN>(p, d, mt, nt, rows, nunits, s_scale, s_shift, out_stage, pool_xs, we, lane, &map_ohi, &map_olo,
+                            &map_of32);
+            if (we == 0) TCP(9);
         }
         if (p.tma_store && lane == 0) tma_store_wait_all();           // global writes complete before the CTA retires
     }
@@ -761,42 +874,48 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     p.tma_store = tma_store ? 1 : 0;
     const size_t budget = TC_DYN_SMEM - 1024;  // the 1 KiB alignment slack is added back at the launch
     const int nkb = (kp + TC_BK - 1) / TC_BK;
-    auto misc_bytes = [&](int bn) {            // scale/shift (+ hoisted Wx) + per-warp store blocks
+    const bool pool_xs = pool >= 32 && !unit_pool;
+    auto misc_bytes = [&](int bn) {            // scale/shift (+ hoisted Wx) + per-warp store blocks + pool exchange
         const int nt = (ncover + bn - 1) / bn;
-        return 2 * ((size_t)nt * bn + 32) * sizeof(float) + (tma_store ? TC_EPI_WARPS * 4096 : 0) +
-               (g && g->wx ? (size_t)3 * kp * sizeof(float) : 0);
+        return 2 * ((size_t)nt * bn + 32) * sizeof(float) + (tma_store ? TC_EPI_WARPS * TC_STORE_BLOCK : 0) +
+               (g && g->wx ? (size_t)3 * kp * sizeof(float) : 0) + (pool_xs ? (size_t)TC_EPI_WARPS * bn * sizeof(float) : 0);
     };
-    // Tile widths are multiples of 32 (columns beyond the weight rows come in as TMA zero fill and are never stored),
-    // widest first: every wgmma re-reads its 64-row A slab from shared memory, so a wide tile reads A fewer times.
+    auto ring_stage = [&](int bn, bool a_in_ring) { return (a_in_ring ? 2 * (size_t)TC_A_BYTES : 0) + 2 * (size_t)bn * TC_BK * 2; };
+    // Tile widths are powers of two from 32 (columns beyond the weight rows come in as TMA zero fill and are never
+    // stored), widest first but no wider than the columns need: a tile of 128 x BN reads 4 (128 + BN) operand bytes per
+    // 6 * 128 * BN FLOP and K element, so a wide tile needs less L2 bandwidth per MMA, and every wgmma re-reads its
+    // 64-row A slab from shared memory, so a wide tile also reads A fewer times.
     const int ncover32 = (ncover + 31) / 32 * 32;
-    const int cands[2] = {TC_MAX_BN, 32};
+    const int widest = g ? TC_GATHER_MAX_BN : TC_MAX_BN;
     int bn = 0, stages = 0;
     p.astat = 0;
     // gather modes keep the produced A tile resident (A-stationary) when all its k-blocks fit next to a >= 2-stage
     // weight ring: the producers then build it once per m-tile, not once per (m, n) tile.
-    if (g && nkb <= TC_MAX_AKB) {
-        const size_t a_tile = (size_t)nkb * 2 * TC_A_BYTES;
-        for (int ci = 0; ci < 2 && !bn; ci++) {
-            const int b = ncover32 < cands[ci] ? ncover32 : cands[ci];
-            const size_t need = a_tile + misc_bytes(b);
-            if (need + 2 * (size_t)(2 * b * TC_BK * 2) <= budget) {
-                bn = b;
-                stages = (int)((budget - need) / (size_t)(2 * b * TC_BK * 2));
-                p.astat = 1;
-            }
+    for (int b = widest; b >= 32 && !bn && g && nkb <= TC_MAX_AKB; b /= 2) {
+        if (b > 32 && b / 2 >= ncover32) continue;
+        const size_t need = (size_t)nkb * 2 * TC_A_BYTES + misc_bytes(b);
+        if (need + 2 * ring_stage(b, false) <= budget) {
+            bn = b;
+            stages = (int)((budget - need) / ring_stage(b, false));
+            p.astat = 1;
         }
     }
-    for (int ci = 0; ci < 2 && !bn; ci++) {
-        const int b = ncover32 < cands[ci] ? ncover32 : cands[ci];
+    // Tiles wider than 64 columns are taken only where they keep a ring of at least 3 stages (with 2, the stage the
+    // producer refills is the one the previous wgmma group still reads, and the loads stop overlapping the MMAs) and
+    // still give every SM a tile.
+    const long m_tiles = (rows + TC_BM - 1) / TC_BM;
+    for (int b = widest; b >= 32 && !bn; b /= 2) {
+        if (b > 32 && b / 2 >= ncover32) continue;
         const size_t misc = misc_bytes(b);
-        const int st = misc < budget ? (int)((budget - misc) / (2 * (size_t)TC_A_BYTES + 2 * (size_t)b * TC_BK * 2)) : 0;
-        if (st >= 2) { bn = b; stages = st; }
+        const int st = misc < budget ? (int)((budget - misc) / ring_stage(b, true)) : 0;
+        const bool wide_ok = b <= 64 || (st >= 3 && m_tiles * ((ncover + b - 1) / b) >= kNumSMs);
+        if (st >= 2 && wide_ok) { bn = b; stages = st; }
     }
     p.bn = bn;
     SSD3D_REQUIRE(bn > 0, "linear_tc: tile does not fit shared memory");
     p.n_tiles = (ncover + p.bn - 1) / p.bn;
     p.m_tiles = (int)((rows + TC_BM - 1) / TC_BM);
-    const size_t stage_bytes = (p.astat ? 0 : 2 * (size_t)TC_A_BYTES) + 2 * (size_t)p.bn * TC_BK * 2;
+    const size_t stage_bytes = ring_stage(p.bn, !p.astat);
     const size_t pool_bytes = misc_bytes(p.bn) + (size_t)p.astat * nkb * 2 * TC_A_BYTES;
     SSD3D_REQUIRE((size_t)p.n_tiles * p.bn <= 4096, "linear_tc: n=%d too wide for the staged scale/shift", n);
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
@@ -811,7 +930,6 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     int rc;
     if ((rc = make_map(&mbh, b_hi, n, kp, p.bn)) != 0) return rc;
     if ((rc = make_map(&mbl, b_lo, n, kp, p.bn)) != 0) return rc;
-    mah = mbh; mal = mbh;                          // placeholders in gather mode (never dereferenced)
     if (!g) {
         if ((rc = make_map(&mah, a_hi, rows, kp, TC_BM)) != 0) return rc;
         if ((rc = make_map(&mal, a_lo, rows, kp, TC_BM)) != 0) return rc;
@@ -824,21 +942,27 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     if (tma_store && want_f32 && (rc = make_out_map(&mof, out_f32, rows, n, ld_f32, true)) != 0) return rc;
 
     const size_t smem = stages * stage_bytes + pool_bytes + 1024;
-    const void *kern = p.bn == 32 ? (const void *)linear_tc_kernel<32> : (const void *)linear_tc_kernel<TC_MAX_BN>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_status(e, "linear_tc attr");
     const int total = p.astat ? p.m_tiles : p.m_tiles * p.n_tiles;    // A-stationary CTAs own whole m-tiles
     const int grid = total < kNumSMs ? total : kNumSMs;
+    const void *kern = g ? (p.bn == 32 ? (const void *)linear_tc_kernel<32> : (const void *)linear_tc_kernel<64>)
+                         : (p.bn == 32 ? (const void *)linear_tc_tma_kernel<32>
+                                       : p.bn == 64 ? (const void *)linear_tc_tma_kernel<64> : (const void *)linear_tc_tma_kernel<128>);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return cuda_status(e, "linear_tc attr");
 #ifdef TC_PROFILE
-    const long long t_host0 = 0;
-    (void)t_host0;
     cudaEvent_t pe0, pe1;
     cudaEventCreate(&pe0); cudaEventCreate(&pe1);
     cudaEventRecord(pe0, stream);
 #endif
-    switch (p.bn) {
-        case 32: linear_tc_kernel<32><<<grid, TC_THREADS, smem, stream>>>(mah, mal, mbh, mbl, moh, mol, mof, p); break;
-        default: linear_tc_kernel<TC_MAX_BN><<<grid, TC_THREADS, smem, stream>>>(mah, mal, mbh, mbl, moh, mol, mof, p); break;
+    if (g) {
+        if (p.bn == 32) linear_tc_kernel<32><<<grid, TC_THREADS, smem, stream>>>(mbh, mbl, moh, mol, mof, p);
+        else linear_tc_kernel<64><<<grid, TC_THREADS, smem, stream>>>(mbh, mbl, moh, mol, mof, p);
+    } else {
+        switch (p.bn) {
+            case 32: linear_tc_tma_kernel<32><<<grid, TC_TMA_THREADS, smem, stream>>>(mah, mal, mbh, mbl, moh, mol, mof, p); break;
+            case 64: linear_tc_tma_kernel<64><<<grid, TC_TMA_THREADS, smem, stream>>>(mah, mal, mbh, mbl, moh, mol, mof, p); break;
+            default: linear_tc_tma_kernel<128><<<grid, TC_TMA_THREADS, smem, stream>>>(mah, mal, mbh, mbl, moh, mol, mof, p); break;
+        }
     }
 #ifdef TC_PROFILE
     {
@@ -849,9 +973,8 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
         long long h[16];
         cudaMemcpyFromSymbol(h, tc_prof, sizeof(h));
         fprintf(stderr, "tc_prof rows=%ld kp=%d n=%d bn=%d astat=%d stages=%d gather=%d pool=%d tiles/cta=%.1f  %.1f us |"
-                " tma_wait %lld | mma: afull %lld bfull %lld tempty %lld issue %lld | prod: wait %lld work %lld | epi: wait %lld work %lld\n",
-                rows, kp, n, p.bn, p.astat, p.stages, p.gather, pool, (double)total / grid, ms * 1e3, h[1], h[2], h[3], h[4], h[5], h[6], h[7],
-                h[8], h[9]);
+                " tma_wait %lld | prod: wait %lld work %lld | mma %lld | epi %lld\n",
+                rows, kp, n, p.bn, p.astat, p.stages, p.gather, pool, (double)total / grid, ms * 1e3, h[1], h[6], h[7], h[8], h[9]);
         memset(h, 0, sizeof(h));
         cudaMemcpyToSymbol(tc_prof, h, sizeof(h));
         cudaEventDestroy(pe0); cudaEventDestroy(pe1);
