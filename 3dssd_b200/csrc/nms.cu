@@ -10,6 +10,11 @@
 //
 // One CTA per scene: bitonic sort of (score, index) keys in shared memory, one thread per candidate builds its
 // row of the "suppresses" bit matrix, one warp walks the rows greedily.
+//
+// The rectangles and the IoU follow the recipe of DESIGN.md section 3.5, which the numpy and C restatements of the test
+// suite share, so that all three make the same decision at an IoU an ulp from the threshold:
+// |cos ry|, |sin ry| in double rounded once to float; every product, sum and quotient through an _rn intrinsic, which
+// nvcc and ptxas never contract into an FMA (the library is built with -fmad=true).
 #include "common.cuh"
 
 namespace ssd3d {
@@ -17,9 +22,11 @@ namespace ssd3d {
 constexpr int NMS_THREADS = 256;
 constexpr int NMS_MAX_N = 512;
 
+// Order-preserving key of a score; -0 is mapped to +0 first, so equal scores of either sign tie (lower index first).
+// NaN scores are outside the contract.
 __device__ __forceinline__ uint32_t nms_f2ord(float x)
 {
-    const uint32_t b = __float_as_uint(x);
+    const uint32_t b = x == 0.0f ? 0u : __float_as_uint(x);
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
@@ -58,29 +65,33 @@ bev_nms_kernel(int n, int npow2, const float *__restrict__ boxes, const float *_
         const int src = (int)(0xffffffffu - (uint32_t)(keys[i] & 0xffffffffull));
         const float *b7 = bx + (size_t)src * 7;
         const float x = b7[0], z = b7[2], l = b7[3], w = b7[5], ry = b7[6];
-        const float c = fabsf(cosf(ry)), s = fabsf(sinf(ry));
-        const float dimx = l * c + w * s, dimz = w * c + l * s;         // box_3d_to_anchor
-        bev[i] = make_float4(x - dimx * 0.5f, z - dimz * 0.5f, x + dimx * 0.5f, z + dimz * 0.5f);   // project_to_bev
+        double sd, cd;
+        sincos((double)ry, &sd, &cd);
+        const float c = fabsf((float)cd), s = fabsf((float)sd);
+        const float dimx = __fadd_rn(__fmul_rn(l, c), __fmul_rn(w, s));               // box_3d_to_anchor
+        const float dimz = __fadd_rn(__fmul_rn(w, c), __fmul_rn(l, s));
+        const float hx = __fmul_rn(dimx, 0.5f), hz = __fmul_rn(dimz, 0.5f);
+        bev[i] = make_float4(__fsub_rn(x, hx), __fsub_rn(z, hz), __fadd_rn(x, hx), __fadd_rn(z, hz));   // project_to_bev
     }
     __syncthreads();
     // ---- suppression rows
     const int nwords = (n + 31) / 32;
     for (int i = tid; i < n; i += NMS_THREADS) {
         const float4 a = bev[i];
-        const float area_a = (a.z - a.x) * (a.w - a.y);
+        const float area_a = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y));
         for (int wd = 0; wd < nwords; wd++) {
             uint32_t bits = 0u;
             for (int t = 0; t < 32; t++) {
                 const int j = wd * 32 + t;
                 if (j <= i || j >= n) continue;
                 const float4 b = bev[j];
-                const float area_b = (b.z - b.x) * (b.w - b.y);
+                const float area_b = __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y));
                 if (area_a <= 0.0f || area_b <= 0.0f) continue;
-                const float iw = fminf(a.z, b.z) - fmaxf(a.x, b.x), ih = fminf(a.w, b.w) - fmaxf(a.y, b.y);
+                const float iw = __fsub_rn(fminf(a.z, b.z), fmaxf(a.x, b.x)), ih = __fsub_rn(fminf(a.w, b.w), fmaxf(a.y, b.y));
                 // disjoint rectangles (the common case): inter == 0, IoU == 0 (or NaN), never > threshold -- skip the divide
                 if (iou_thr >= 0.0f && (!(iw > 0.0f) || !(ih > 0.0f))) continue;
-                const float inter = fmaxf(iw, 0.0f) * fmaxf(ih, 0.0f);
-                if (inter / (area_a + area_b - inter) > iou_thr) bits |= 1u << t;
+                const float inter = __fmul_rn(fmaxf(iw, 0.0f), fmaxf(ih, 0.0f));
+                if (__fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter)) > iou_thr) bits |= 1u << t;
             }
             sup[i][wd] = bits;
         }
@@ -124,8 +135,8 @@ extern "C" int ssd3d_bev_nms(int b, int n, const float *boxes, const float *scor
 {
     SSD3D_REQUIRE(b >= 0 && n > 0 && max_output > 0, "bev_nms: bad shape b=%d n=%d max_output=%d", b, n, max_output);
     SSD3D_REQUIRE(n <= NMS_MAX_N, "bev_nms: at most %d candidates per scene (got %d)", NMS_MAX_N, n);
+    if (b == 0) return 0;                    // nothing read or written: an empty tensor may have a null data pointer
     SSD3D_REQUIRE(boxes && scores && out_block && out_cnt, "bev_nms: null pointer");
-    if (b == 0) return 0;
     int npow2 = 1;
     while (npow2 < n) npow2 <<= 1;
     bev_nms_kernel<<<b, NMS_THREADS, 0, (cudaStream_t)stream>>>(n, npow2, boxes, scores, iou_threshold, max_output, cls_id,

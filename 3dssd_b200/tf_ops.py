@@ -747,7 +747,9 @@ def sa_mlp_fused_hoisted(xyz, z, zoff, wx, new_xyz, idx, cnt, stack, out_f32=Non
 def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
     """Greedy BEV NMS per scene (postprocessor.py:76-88): boxes (b,n,7) = (x,y,z,l,h,w,ry), scores (b,n) ->
     block (b,max_output,9) = (box7, score, class) zero padded, count (b,) int32.  out=(block, count) writes into
-    preallocated contiguous tensors (the send buffer of the multi-GPU gather)."""
+    preallocated contiguous tensors (the send buffer of the multi-GPU gather).  Descending score, ties (-0 and +0
+    included) to the lower index; rectangles and IoU by the float32 recipe of DESIGN.md §3.5, which the CPU
+    restatements of the test suite share decision for decision.  NaN scores are outside the contract."""
     boxes = _req(boxes, "boxes", torch.float32, 3, 7)
     scores = _req(scores, "scores", torch.float32, 2)
     b, n, _ = boxes.shape

@@ -289,7 +289,8 @@ int ssd3d_three_interpolate_grad(int b, int n, int c, int m, const float *grad_o
  * of lib/builder/postprocessor.py:76-88 (one class per call).  boxes [b,n,7] = (x,y,z,l,h,w,ry), scores [b,n];
  * candidates in descending score order (ties: lower index), dropped when axis-aligned BEV IoU with a kept box is
  * > iou_threshold, at most max_output kept.  out_block [b,max_output,9] = (box7, score, class) zero padded,
- * out_cnt [b] = number kept.  n <= 512. */
+ * out_cnt [b] = number kept.  n <= 512.  Rectangles and IoU by the float32 recipe of DESIGN.md section 3.5 (cos / sin
+ * in double, every operation rounded on its own); -0 and +0 scores are equal.  NaN scores are outside the contract. */
 int ssd3d_bev_nms(int b, int n, const float *boxes, const float *scores, float iou_threshold, int max_output,
                   int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream);
 

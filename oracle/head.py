@@ -7,6 +7,8 @@ lib/utils/box_3d_utils.py:25-58 (box_3d_to_anchor), lib/utils/anchors_util.py:11
 lib/builder/postprocessor.py:52-120 with TensorFlow's greedy non_max_suppression (descending score, a candidate is
 dropped when IoU with a kept box is > threshold; ties broken by lower index, which TF 1.4 leaves unspecified).
 """
+import math
+
 import numpy as np
 
 from . import ops
@@ -38,19 +40,38 @@ def head_forward(xyz, feat, params, mlp=(128,), bn=True, scope=""):
     return boxes, score[..., 0], {"feat": y, "cls": cls, "reg": reg}
 
 
+def bev_rects(boxes):
+    """BEV rectangles (x1, z1, x2, z2) of boxes [..., 7] in float32, by the recipe of DESIGN.md §3.5 that the kernel
+    (csrc/nms.cu) and the C twin share: |cos ry| and |sin ry| in double, rounded once to float32 (libm through `math`,
+    as the C twin calls it: numpy's own float32 and SIMD float64 cos are other functions); every product and sum
+    rounded to float32 on its own, no fused multiply-add."""
+    bx = np.asarray(boxes, np.float32)
+    ry = bx[..., 6].ravel().tolist()
+    c = np.abs(np.array([math.cos(a) for a in ry], np.float64).astype(np.float32)).reshape(bx.shape[:-1])
+    s = np.abs(np.array([math.sin(a) for a in ry], np.float64).astype(np.float32)).reshape(bx.shape[:-1])
+    l, w = bx[..., 3], bx[..., 5]
+    dimx = (l * c) + (w * s)                              # float32 arrays: each operation rounded on its own
+    dimz = (w * c) + (l * s)
+    half = np.float32(0.5)
+    return np.stack([bx[..., 0] - dimx * half, bx[..., 2] - dimz * half,
+                     bx[..., 0] + dimx * half, bx[..., 2] + dimz * half], -1)
+
+
 def bev_nms(boxes, scores, iou_threshold=0.1, max_output=100, cls_id=0):
+    """Greedy BEV NMS per scene, the oracle of csrc/nms.cu and oracle/ssd3d_oracle.c:oracle_bev_nms (DESIGN.md §3.5):
+    descending score, ties (+0 and -0 among them) to the lower index; a candidate is dropped when its float32 IoU with
+    a kept box is > float32(iou_threshold); a box of area <= 0 neither suppresses nor is suppressed.  NaN scores are
+    outside the contract."""
     b, n, _ = boxes.shape
+    thr = np.float32(iou_threshold)
+    zero = np.float32(0)
     block = np.zeros((b, max_output, 9), np.float32)
     cnt = np.zeros((b,), np.int32)
     for s in range(b):
         bx, sc = boxes[s], scores[s]
-        c, sn = np.abs(np.cos(bx[:, 6])), np.abs(np.sin(bx[:, 6]))
-        dimx = bx[:, 3] * c + bx[:, 5] * sn
-        dimz = bx[:, 5] * c + bx[:, 3] * sn
-        x1, z1 = bx[:, 0] - dimx * np.float32(0.5), bx[:, 2] - dimz * np.float32(0.5)
-        x2, z2 = bx[:, 0] + dimx * np.float32(0.5), bx[:, 2] + dimz * np.float32(0.5)
+        x1, z1, x2, z2 = bev_rects(bx).T
         area = (x2 - x1) * (z2 - z1)
-        order = sorted(range(n), key=lambda i: (-sc[i], i))
+        order = sorted(range(n), key=lambda i: (-float(sc[i]), i))       # -0.0 == 0.0: the lower index first
         kept = []
         for i in order:
             ok = True
@@ -59,8 +80,8 @@ def bev_nms(boxes, scores, iou_threshold=0.1, max_output=100, cls_id=0):
                     continue
                 iw = min(x2[i], x2[j]) - max(x1[i], x1[j])
                 ih = min(z2[i], z2[j]) - max(z1[i], z1[j])
-                inter = max(iw, np.float32(0)) * max(ih, np.float32(0))
-                if inter / (area[i] + area[j] - inter) > iou_threshold:
+                inter = max(iw, zero) * max(ih, zero)
+                if inter / ((area[i] + area[j]) - inter) > thr:
                     ok = False
                     break
             if ok:

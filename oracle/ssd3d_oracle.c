@@ -431,7 +431,10 @@ void oracle_three_interpolate_grad(int b, int n, int c, int m, const float *grad
  * Follows /root/reference/lib/builder/postprocessor.py:76-88 with lib/utils/box_3d_utils.py:25-58 (box_3d_to_anchor)
  * and lib/utils/anchors_util.py:11-48 (project_to_bev): candidates in descending score order (ties: lower index), a
  * candidate is dropped when its axis-aligned BEV IoU with a kept box is > thr, at most max_out kept.  Used by the
- * `--impl reference` arm of bench.py (the reference runs this stage on the CPU) and by the CPU baseline. */
+ * `--impl reference` arm of bench.py (the reference runs this stage on the CPU) and by the CPU baseline.
+ * Arithmetic: the recipe of DESIGN.md §3.5, shared with csrc/nms.cu and oracle/head.py -- cos / sin in double rounded
+ * once to float, every product and sum rounded (the library is built with -ffp-contract=off).  The comparator treats
+ * -0 and +0 as equal; NaN scores are outside the contract (it is not a consistent order on them). */
 typedef struct { float s; int i; } nms_key;
 static int nms_cmp(const void *a, const void *b)
 {
@@ -451,7 +454,8 @@ void oracle_bev_nms(int b, int n, const float *boxes, const float *scores, float
         float *blk = out_block + (size_t)s * max_out * 9;
         memset(blk, 0, sizeof(float) * (size_t)max_out * 9);
         for (int i = 0; i < n; i++) {
-            const float c = fabsf(cosf(bx[i * 7 + 6])), sn = fabsf(sinf(bx[i * 7 + 6]));
+            const double ry = (double)bx[i * 7 + 6];
+            const float c = fabsf((float)cos(ry)), sn = fabsf((float)sin(ry));
             const float dimx = bx[i * 7 + 3] * c + bx[i * 7 + 5] * sn, dimz = bx[i * 7 + 5] * c + bx[i * 7 + 3] * sn;
             rect[i * 5 + 0] = bx[i * 7 + 0] - dimx * 0.5f; rect[i * 5 + 1] = bx[i * 7 + 2] - dimz * 0.5f;
             rect[i * 5 + 2] = bx[i * 7 + 0] + dimx * 0.5f; rect[i * 5 + 3] = bx[i * 7 + 2] + dimz * 0.5f;
@@ -470,7 +474,7 @@ void oracle_bev_nms(int b, int n, const float *boxes, const float *scores, float
                 float ih = fminf(rect[i * 5 + 3], rect[j * 5 + 3]) - fmaxf(rect[i * 5 + 1], rect[j * 5 + 1]);
                 iw = iw > 0 ? iw : 0; ih = ih > 0 ? ih : 0;
                 const float inter = iw * ih;
-                if (inter / (rect[i * 5 + 4] + rect[j * 5 + 4] - inter) > thr) ok = 0;
+                if (inter / ((rect[i * 5 + 4] + rect[j * 5 + 4]) - inter) > thr) ok = 0;
             }
             if (ok) kept[nk++] = i;
         }
