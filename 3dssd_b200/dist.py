@@ -11,7 +11,9 @@ straight into a preallocated send buffer, ncclAllGather on that buffer is captur
 gathered result is read through views of the receive buffer -- no pack / unpack kernels and no host work per step
 beyond graph.replay().
 """
+import contextlib
 import os
+from typing import NamedTuple
 
 import torch
 import torch.distributed as dist
@@ -186,3 +188,186 @@ def gather_detections(block, count, total_scenes, group=None):
     b.copy_(block); c.copy_(count)
     g.gather()
     return g.result()
+
+
+# ---- data-parallel training (DESIGN.md section 3.9) -----------------------------------------------------------------
+
+ALLREDUCE_CTAS = 64           # CTAs per rank of one allreduce launch; all must be co-resident on the device
+CLIP_NORM = 5.0               # trainer.py:143-145, tf.clip_by_global_norm(grads, 5.0)
+_HEAD_FLOATS = 8              # gathered slice: 7 losses, the rank's gradient norm, then the BN record
+
+
+class AllreduceLayout(NamedTuple):
+    """Where csrc/grad_exchange.cu's allreduce keeps its buffers: n floats cut into `world` chunks of `chunk` floats
+    (rank p owns [p*chunk, (p+1)*chunk), zero past n), each cut into `ctas` sub-slices of `sub` floats (both multiples
+    of 4).  r1 / r2 / f1 / f2: byte offsets per parity inside every rank's symmetric buffer; nbytes: the share's size."""
+    n: int
+    world: int
+    ctas: int
+    chunk: int
+    sub: int
+    r1: tuple
+    r2: tuple
+    f1: tuple
+    f2: tuple
+    nbytes: int
+
+
+def allreduce_layout(n, world, ctas=ALLREDUCE_CTAS, base=0):
+    """AllreduceLayout of an n-float gradient over `world` ranks, placed at byte offset `base` (a 16-byte multiple)."""
+    n, world, ctas, base = int(n), int(world), int(ctas), int(base)
+    if n <= 0 or world < 1 or ctas < 1 or base % 16:
+        raise ValueError("allreduce_layout: n=%d world=%d ctas=%d base=%d" % (n, world, ctas, base))
+    chunk = ((n + world - 1) // world + 3) // 4 * 4
+    sub = ((chunk + ctas - 1) // ctas + 3) // 4 * 4
+    data = world * chunk * 4
+    flags = (world * ctas * 4 + 15) // 16 * 16
+    r1 = (base, base + data)
+    r2 = (base + 2 * data, base + 3 * data)
+    f1 = (base + 4 * data, base + 4 * data + flags)
+    f2 = (base + 4 * data + 2 * flags, base + 4 * data + 3 * flags)
+    return AllreduceLayout(n, world, ctas, chunk, sub, r1, r2, f1, f2, 4 * data + 4 * flags)
+
+
+def simulated_ctas(world, sms, ctas=ALLREDUCE_CTAS):
+    """CTAs per rank when `world` ranks are simulated on ONE device of `sms` SMs.  A rank's kernels before its allreduce
+    (clip scale, loss copy) must still find an SM while the other ranks' allreduce CTAs already spin.  Spinning CTAs are
+    spread one per SM first, and once they cover every SM those kernels were seen not to be placed until the spinners
+    gave up.  So (world - 1) * ctas must stay below the SM count.  Between GPUs this does not arise."""
+    return max(1, min(int(ctas), (int(sms) - 1) // max(1, int(world) - 1)))
+
+
+def _round(x, m):
+    return (int(x) + m - 1) // m * m
+
+
+class DataParallel:
+    """Data-parallel training with the semantics of the reference's towers (trainer.py:143-154, trainer_utils.py:23-46,
+    tf_util.py:438-443): each rank clips its own gradient to global norm 5, the clipped gradients are averaged in rank
+    order, and every rank's batch statistics update the moving averages, in rank order.  Every rank ends a step with the
+    same gradient bits and the same statistics; with the same elementwise optimizer the replicas stay identical.
+
+        dp = DataParallel(tp, arena)                # arena: PeerArena of >= DataParallel.symmetric_bytes(tp, world)
+        for step ...:
+            dp.zero_grad()
+            with dp.recording():
+                losses = <forward on shard_batch(batch, rank, world)>
+            losses["total"].backward()
+            mean_losses = dp.exchange(losses)       # clip -> allreduce mean -> gather -> BN update
+            optimizer.step()                        # e.g. torch.optim.Adam(tp.parameters())
+
+    DataParallel(tp, arena) serves torchrun ranks (world and rank from arena.group) and broadcasts rank 0's parameters
+    and moving statistics at construction.  DataParallel(tp, peers=[base of every rank's symmetric buffer], world=G,
+    rank=r) runs ranks simulated on one device (tests); nothing is broadcast.  Every rank must call exchange() the same
+    number of times; nothing in a step synchronises the host."""
+
+    def __init__(self, tp, arena=None, *, peers=None, world=None, rank=None, ctas=ALLREDUCE_CTAS, clip_norm=CLIP_NORM):
+        from . import tf_ops
+        self._tf_ops = tf_ops
+        self.tp, self.clip_norm = tp, float(clip_norm)
+        dev = tp.device
+        if arena is not None:
+            self.world, self.rank = _world(arena.group)
+            bases = arena.peer_bases
+        else:
+            if peers is None or world is None or rank is None:
+                raise ValueError("DataParallel: pass a PeerArena, or peers, world and rank for simulated ranks")
+            self.world, self.rank, bases = int(world), int(rank), [int(b) for b in peers]
+            sms = torch.cuda.get_device_properties(dev).multi_processor_count
+            if (self.world - 1) * int(ctas) >= sms:
+                raise ValueError("DataParallel: %d simulated ranks x %d CTAs need (world - 1) * ctas < %d SMs (simulated_ctas)"
+                                 % (self.world, ctas, sms))
+        if len(bases) != self.world or not 0 <= self.rank < self.world:
+            raise ValueError("DataParallel: %d peer bases for world=%d rank=%d" % (len(bases), self.world, self.rank))
+        self.grad, stats = tp.flat_grads(), tp.flat_stats()
+        if arena is not None and self.world > 1:
+            self._broadcast(arena.group)
+        self.nstats = stats.numel()
+        self.slice_floats = _round(_HEAD_FLOATS + self.nstats, 4)
+        self.slice_bytes = 4 * self.slice_floats
+        ar_bytes, ga_bytes = self._share_bytes(self.grad.numel(), self.slice_bytes, self.world, ctas)
+        if arena is not None:
+            ar_base, ga_base = arena.take(ar_bytes), arena.take(ga_bytes)
+        else:
+            ar_base, ga_base = 0, _round(ar_bytes, 256)
+        self.layout = allreduce_layout(self.grad.numel(), self.world, ctas, base=ar_base)
+        recv, flag, _ = peer_layout(self.world, self.slice_bytes)
+        self.recv_off = (ga_base + recv[0], ga_base + recv[1])
+        self.flag_off = (ga_base + flag[0], ga_base + flag[1])
+        self.peers = torch.tensor(bases, dtype=torch.int64, device=dev)
+        self.send = torch.zeros((self.slice_floats,), dtype=torch.float32, device=dev)
+        self.gathered = torch.zeros((self.world, self.slice_floats), dtype=torch.float32, device=dev)
+        self.record = self.send[_HEAD_FLOATS:_HEAD_FLOATS + self.nstats]   # the forward writes straight into the slice
+        self.scale = torch.zeros((1,), dtype=torch.float32, device=dev)
+        self.workspace = torch.empty((int(tf_ops.lib().ssd3d_grad_clip_scale_workspace(self.grad.numel())),), dtype=torch.uint8,
+                                     device=dev)
+        self.state_allreduce = torch.zeros((4,), dtype=torch.int32, device=dev)
+        self.state_gather = torch.zeros((4,), dtype=torch.int32, device=dev)
+        self.decay = None
+
+    @staticmethod
+    def _share_bytes(n, slice_bytes, world, ctas):
+        return allreduce_layout(n, world, ctas).nbytes, peer_layout(world, slice_bytes)[2]
+
+    @staticmethod
+    def symmetric_bytes(tp, world, ctas=ALLREDUCE_CTAS):
+        """Bytes of symmetric memory one DataParallel over `world` ranks takes (size a PeerArena with at least this)."""
+        n = sum(t.numel() for t in tp.parameters())
+        nstats = sum(tp.tensors[s + suffix].numel() for s in tp.bn_scopes() for suffix in tp._STATS)
+        ar, ga = DataParallel._share_bytes(n, 4 * _round(_HEAD_FLOATS + nstats, 4), world, ctas)
+        return _round(ar, 256) + _round(ga, 256)
+
+    def _broadcast(self, group):
+        src = dist.get_global_rank(group, 0)
+        with torch.no_grad():
+            for _, t in self.tp.named_parameters():
+                dist.broadcast(t.data, src=src, group=group)
+            dist.broadcast(self.tp.stats_flat, src=src, group=group)
+
+    def zero_grad(self):
+        self.tp.zero_flat_grads()
+
+    @contextlib.contextmanager
+    def recording(self):
+        """The forward of a step: every training BatchNorm records its batch statistics (exactly once per scope, one decay)
+        into this rank's slice of the per-step gather instead of updating the moving statistics in place."""
+        self.tp.start_bn_record(self.record)
+        ok = False
+        try:
+            yield self
+            ok = True
+        finally:
+            decay = self.tp.finish_bn_record(check=ok)
+        self.decay = decay
+
+    def exchange(self, losses):
+        """After backward(): clip scale -> allreduce mean of the clipped gradients (in place in every .grad) -> gather of
+        losses, norms and batch statistics -> BN moving-statistics update of every rank.  losses: dict with
+        loss.LOSS_NAMES and "total" (0-d tensors).  Returns the rank-averaged losses (summed in double in rank order)."""
+        from .loss import LOSS_NAMES
+        keys = LOSS_NAMES + ("total",)
+        if self.decay is None:
+            raise ValueError("exchange: no recorded forward since the last exchange (use recording())")
+        T, W = self._tf_ops, self.world
+        with torch.no_grad():
+            self.send[:len(keys)].copy_(torch.stack([losses[k].detach().reshape(()).float() for k in keys]))
+        T.grad_clip_scale(self.grad, self.send[len(keys):len(keys) + 1], self.scale, self.clip_norm, self.workspace)
+        T.peer_allreduce_mean(self.grad, self.scale, self.peers, W, self.rank, self.layout, self.state_allreduce)
+        T.peer_allgather(self.send.view(torch.uint8), self.peers, W, self.rank, self.slice_bytes, self.recv_off, self.flag_off,
+                         self.state_gather, self.gathered.view(-1).view(torch.uint8))
+        T.bn_moving_update_ranks(self.tp.stats_flat, self.gathered[:, _HEAD_FLOATS:_HEAD_FLOATS + self.nstats], W, self.decay)
+        self.decay = None
+        g = self.gathered[:, :len(keys)].double()
+        acc = g[0].clone()
+        for r in range(1, W):
+            acc += g[r]
+        mean = (acc / W).float()
+        return {k: mean[i] for i, k in enumerate(keys)}
+
+    def norms(self):
+        """Every rank's gradient norm of the last exchange, [world] (a view of the gathered buffer)."""
+        return self.gathered[:, _HEAD_FLOATS - 1]
+
+    def timeouts(self):
+        """Waits that gave up (a peer that never arrived): 0 in a healthy run.  Synchronises."""
+        return int(self.state_allreduce[2].item()) + int(self.state_gather[2].item())

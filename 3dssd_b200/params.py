@@ -294,6 +294,9 @@ class TrainableParams:
         for k, v in params.items():
             t = torch.from_numpy(np.array(v, dtype=np.float32, copy=True)).to(self.device)
             self.tensors[k] = t if k.endswith(self._STATS) else t.requires_grad_(True)
+        self.grad_flat = self.grad_offsets = None          # flat_grads()
+        self.stats_flat = self.bn_offsets = None           # flat_stats()
+        self._bn_record = None                             # start_bn_record() .. finish_bn_record()
 
     def named_parameters(self):
         return [(k, t) for k, t in self.tensors.items() if t.requires_grad]
@@ -309,16 +312,103 @@ class TrainableParams:
         return {k: t.detach().cpu().numpy().copy() for k, t in self.tensors.items()}
 
     def conv_train(self, scope, x, bn=True, bn_decay=None, relu=True, debug=None):
-        """One conv (+ training BatchNorm when bn) (+ ReLU) of `scope`, differentiable (tf_ops.conv_train)."""
+        """One conv (+ training BatchNorm when bn) (+ ReLU) of `scope`, differentiable (tf_ops.conv_train).  While a BN
+        record is open (start_bn_record) the batch statistics go to the record instead of the moving statistics."""
         from . import tf_ops
         t = self.tensors
         g = lambda k: t.get(scope + k)
         b = g("/biases")
         if b is None:
             b = torch.zeros((t[scope + "/weights"].shape[1],), dtype=torch.float32, device=self.device)
-        return tf_ops.conv_train(x, t[scope + "/weights"], b, g("/bn/gamma"), g("/bn/beta"), g("/bn/moving_mean"),
-                                 g("/bn/moving_variance"), bn=bn, relu=relu, decay=0.9 if bn_decay is None else float(bn_decay),
-                                 debug=debug)
+        decay = 0.9 if bn_decay is None else float(bn_decay)
+        moving, stats_out = (g("/bn/moving_mean"), g("/bn/moving_variance")), None
+        if bn and self._bn_record is not None:
+            stats_out, moving = self._record_slot(scope, decay), (None, None)
+        return tf_ops.conv_train(x, t[scope + "/weights"], b, g("/bn/gamma"), g("/bn/beta"), moving[0], moving[1], bn=bn, relu=relu,
+                                 decay=decay, debug=debug, stats_out=stats_out)
+
+    # ---- data-parallel training (dist.DataParallel): both capabilities are opt-in; unused, nothing above changes -----
+    def flat_grads(self):
+        """Make every trainable tensor's .grad a view of ONE flat float32 buffer (grad_flat; grad_offsets[name] = the
+        view's first element, in named_parameters order), so autograd accumulates in place and zeroing is one fill.
+        Returns grad_flat."""
+        if self.grad_flat is None:
+            named = self.named_parameters()
+            self.grad_flat = torch.zeros((sum(t.numel() for _, t in named),), dtype=torch.float32, device=self.device)
+            self.grad_offsets, off = {}, 0
+            for k, t in named:
+                self.grad_offsets[k] = off
+                off += t.numel()
+        self._attach_grads()
+        return self.grad_flat
+
+    def _attach_grads(self):
+        for k, t in self.named_parameters():
+            o = self.grad_offsets[k]
+            t.grad = self.grad_flat[o:o + t.numel()].view(t.shape)
+
+    def zero_flat_grads(self):
+        """grad_flat[:] = 0 (one kernel) and every .grad back on its view (an optimizer may have set it to None)."""
+        from . import tf_ops
+        tf_ops.fill_zero(self.grad_flat)
+        self._attach_grads()
+
+    def bn_scopes(self):
+        return [k[: -len(self._STATS[0])] for k in self.tensors if k.endswith(self._STATS[0])]
+
+    def flat_stats(self):
+        """Move the moving statistics into ONE flat float32 buffer (stats_flat): scope s holds [moving_mean | moving_variance]
+        at bn_offsets[s] = (offset, channels), in bn_scopes() order; the tensors become views of it.  Returns stats_flat."""
+        if self.stats_flat is None:
+            scopes = self.bn_scopes()
+            sizes = [self.tensors[s + self._STATS[0]].numel() for s in scopes]
+            flat = torch.empty((2 * sum(sizes),), dtype=torch.float32, device=self.device)
+            self.bn_offsets, off = {}, 0
+            for s, c in zip(scopes, sizes):
+                self.bn_offsets[s] = (off, c)
+                for i, suffix in enumerate(self._STATS):
+                    v = flat[off + i * c: off + (i + 1) * c]
+                    v.copy_(self.tensors[s + suffix])
+                    self.tensors[s + suffix] = v
+                off += 2 * c
+            self.stats_flat = flat
+        return self.stats_flat
+
+    def start_bn_record(self, record):
+        """Open a BN record: until finish_bn_record(), every training BatchNorm leaves the moving statistics alone and
+        writes its batch mean and variance into `record` (float32 CUDA [>= stats_flat.numel()]) at its scope's
+        bn_offsets, i.e. record mirrors stats_flat.  The record's views are kept for the backward of that forward."""
+        self.flat_stats()
+        if not isinstance(record, torch.Tensor) or record.dtype != torch.float32 or record.dim() != 1 or \
+                record.numel() < self.stats_flat.numel() or record.device != self.stats_flat.device:
+            raise ValueError("start_bn_record: record must be a float32 vector of >= %d elements on %s"
+                             % (self.stats_flat.numel(), self.stats_flat.device))
+        if self._bn_record is not None:
+            raise ValueError("start_bn_record: a BN record is already open")
+        self._bn_record = {"buf": record, "seen": set(), "decay": None}
+
+    def _record_slot(self, scope, decay):
+        rec = self._bn_record
+        if scope not in self.bn_offsets:
+            raise ValueError("BN record: %s has no moving statistics" % scope)
+        if scope in rec["seen"]:
+            raise ValueError("BN record: %s recorded twice in one step" % scope)
+        if rec["decay"] is not None and decay != rec["decay"]:
+            raise ValueError("BN record: %s uses decay %g, the step uses %g" % (scope, decay, rec["decay"]))
+        rec["seen"].add(scope)
+        rec["decay"] = decay
+        off, c = self.bn_offsets[scope]
+        return rec["buf"][off:off + c], rec["buf"][off + c:off + 2 * c]
+
+    def finish_bn_record(self, check=True):
+        """Close the BN record and return its decay.  check: every BN scope must have recorded exactly once."""
+        rec, self._bn_record = self._bn_record, None
+        if rec is None:
+            raise ValueError("finish_bn_record: no BN record is open")
+        missing = [s for s in self.bn_offsets if s not in rec["seen"]]
+        if check and missing:
+            raise ValueError("BN record: %d scope(s) did not record, e.g. %s" % (len(missing), missing[0]))
+        return rec["decay"]
 
 
 def prepare(params, device="cuda"):

@@ -790,6 +790,75 @@ def peer_allgather(send, peers, world, rank, slice_bytes, recv_off, flag_off, st
     return out
 
 
+# ---- data-parallel training: the gradient exchange (csrc/grad_exchange.cu, DESIGN.md section 3.9) -------------------
+
+def grad_clip_scale(grad, norm, scale, clip_norm=5.0, workspace=None):
+    """Global norm and tf.clip_by_global_norm scale of one rank's flat float32 gradient, written to the device floats
+    norm[0] and scale[0] (include/ssd3d.h, ssd3d_grad_clip_scale).  workspace: optional uint8 buffer of
+    ssd3d_grad_clip_scale_workspace bytes (allocated here when None)."""
+    grad = _req(grad, "grad", torch.float32, copy=False)
+    norm, scale = _req(norm, "norm", torch.float32, copy=False), _req(scale, "scale", torch.float32, copy=False)
+    if grad.numel() == 0 or norm.numel() < 1 or scale.numel() < 1:
+        raise ValueError("grad_clip_scale: grad must be non-empty and norm / scale hold one float each")
+    if workspace is not None:
+        workspace = _req(workspace, "workspace", torch.uint8, copy=False)
+    ws_bytes = int(lib().ssd3d_grad_clip_scale_workspace(grad.numel()))
+    if workspace is None:
+        workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=grad.device)
+    if workspace.numel() < ws_bytes:
+        raise ValueError("grad_clip_scale: workspace must hold %d bytes" % ws_bytes)
+    check(lib().ssd3d_grad_clip_scale(_p(grad), grad.numel(), float(clip_norm), _p(workspace), _p(norm), _p(scale), _stream()),
+          "grad_clip_scale")
+    return norm, scale
+
+
+def peer_allreduce_resident_ctas():
+    """CTAs of the allreduce kernel that fit co-resident on the current device (occupancy API)."""
+    n = int(lib().ssd3d_peer_allreduce_resident_ctas())
+    if n < 0:
+        check(n, "peer_allreduce_resident_ctas")
+    return n
+
+
+def peer_allreduce_mean(grad, scale, peers, world, rank, layout, state):
+    """Rank-ordered mean of the ranks' clipped gradients over NVLink peer memory, written back into grad (include/ssd3d.h,
+    ssd3d_peer_allreduce_mean).  grad: float32 [n] 16-byte aligned; scale: this rank's device clip scale; peers: int64
+    CUDA tensor [world] of the ranks' symmetric-buffer bases as mapped here; layout: dist.allreduce_layout(n, world,
+    ctas) shifted to this exchange's share; state: int32 [>= 3] zero-initialised, owned by this exchange."""
+    grad = _req(grad, "grad", torch.float32, copy=False)
+    scale = _req(scale, "scale", torch.float32, copy=False)
+    for name, t, dt in (("peers", peers, torch.int64), ("state", state, torch.int32)):
+        _req(t, name, dt, copy=False)
+    if grad.numel() == 0 or scale.numel() < 1 or peers.numel() < world or state.numel() < 3:
+        raise ValueError("peer_allreduce_mean: grad must be non-empty, scale one float, peers >= world=%d, state >= 3" % world)
+    if grad.numel() != layout.n or world != layout.world:
+        raise ValueError("peer_allreduce_mean: layout is for n=%d world=%d, got n=%d world=%d"
+                         % (layout.n, layout.world, grad.numel(), world))
+    if grad.data_ptr() % 16:
+        raise ValueError("peer_allreduce_mean: grad must be 16-byte aligned")
+    check(lib().ssd3d_peer_allreduce_mean(_p(grad), grad.numel(), _p(scale), _p(peers), int(world), int(rank), int(layout.ctas),
+                                          int(layout.chunk), int(layout.sub), int(layout.r1[0]), int(layout.r1[1]),
+                                          int(layout.r2[0]), int(layout.r2[1]), int(layout.f1[0]), int(layout.f1[1]),
+                                          int(layout.f2[0]), int(layout.f2[1]), _p(state), _stream()), "peer_allreduce_mean")
+    return grad
+
+
+def bn_moving_update_ranks(stats, batch, world, decay):
+    """stats (float32 [n], in place) <- the BatchNorm moving-average update of `world` ranks in rank order from batch,
+    float32 [world, ld >= n] (row r = rank r's batch means / variances at stats' offsets): ssd3d_bn_moving_update_ranks."""
+    stats = _req(stats, "stats", torch.float32, copy=False)
+    batch = _req(batch, "batch", torch.float32, 2, copy=None)
+    n = stats.numel()
+    if n == 0 or batch.shape[0] != world or batch.shape[1] < n or batch.stride(1) != 1 or batch.stride(0) < n:
+        raise ValueError("bn_moving_update_ranks: batch %s (strides %s) must be [world=%d, >= %d] with unit column stride"
+                         % (tuple(batch.shape), tuple(batch.stride()), world, n))
+    if not 0.0 <= float(decay) <= 1.0:
+        raise ValueError("bn_moving_update_ranks: decay=%g must be in [0, 1]" % decay)
+    check(lib().ssd3d_bn_moving_update_ranks(_p(stats), n, _p(batch), batch.stride(0), int(world), float(decay), _stream()),
+          "bn_moving_update_ranks")
+    return stats
+
+
 def split_points(points):
     """(b, n, 3 + c) -> xyz (b, n, 3), features (b, n, c): single_stage_detector.py:116-117."""
     points = _req(points, "points", torch.float32, 3)
@@ -873,10 +942,12 @@ def concat_rows(parts):
 
 # ---- training-mode BatchNorm (SURVEY.md 8f row f3) -----------------------------------------------------------------
 
-def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=True, eps=BN_EPS):
+def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=True, eps=BN_EPS, stats_out=None):
     """Batch-statistics BatchNorm + activation over the last axis of x (tf_util.py:424-444, is_training=True);
     moving_mean / moving_var (float32 CUDA tensors [c]) are updated IN PLACE like updates_collections=None does.
-    Returns (y, scale, shift, batch_mean, batch_var); (scale, shift) is the folded per-channel form."""
+    Returns (y, scale, shift, batch_mean, batch_var); (scale, shift) is the folded per-channel form.
+    stats_out: optional (mean, var) float32 CUDA tensors [c] that receive the batch statistics and are returned as
+    batch_mean / batch_var (the BN record of data-parallel training writes them straight into its exchange buffer)."""
     x = _req(x, "x", torch.float32)
     c = x.shape[-1]
     rows = x.numel() // c
@@ -887,7 +958,11 @@ def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=
         raise ValueError("moving_mean and moving_var go together")
     dev = x.device
     y = torch.empty_like(x)
-    scale, shift, bmean, bvar = (torch.empty((c,), dtype=torch.float32, device=dev) for _ in range(4))
+    scale, shift = (torch.empty((c,), dtype=torch.float32, device=dev) for _ in range(2))
+    if stats_out is None:
+        bmean, bvar = (torch.empty((c,), dtype=torch.float32, device=dev) for _ in range(2))
+    else:
+        bmean, bvar = _vec(stats_out[0], "stats_out mean", c), _vec(stats_out[1], "stats_out var", c)
     ws = torch.empty((int(lib().ssd3d_bn_train_workspace(c)),), dtype=torch.uint8, device=dev)
     check(lib().ssd3d_bn_train(rows, c, _p(x), c, _p(gamma), _p(beta), _p(moving_mean), _p(moving_var), float(decay), float(eps),
                                _p(ws), _p(scale), _p(shift), _p(bmean), _p(bvar), 1 if relu else 0, _p(y), c, _stream()),
@@ -991,16 +1066,18 @@ def vote_translate_grad(offsets, grad_out, min_range):
     return g
 
 
-def linear_bn_train(x, f, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9):
+def linear_bn_train(x, f, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9,
+                    stats_out=None):
     """Forward of one training-mode layer: split_rows -> linear_tc with the BN-less fold f (params.FoldedConv with
     scale = 1, shift = bias) -> bn_train (bn=True: batch statistics, moving statistics updated in place) -> ReLU.
     Returns (y, r): y the conv output before BatchNorm, r bn_train's (out, scale, shift, batch_mean, batch_var), or (y,)
-    when bn=False."""
+    when bn=False.  stats_out: see bn_train."""
     hi, lo = split_rows(x)
     y, _ = linear_tc(hi, lo, f, relu=bool(relu and not bn), want_f32=True, want_split=False)
     if not bn:
         return y, (y,)
-    return y, bn_train(y, gamma, beta, moving_mean, moving_var, decay=decay, relu=relu)
+    extra = {} if stats_out is None else {"stats_out": stats_out}
+    return y, bn_train(y, gamma, beta, moving_mean, moving_var, decay=decay, relu=relu, **extra)
 
 
 class _ConvTrain(torch.autograd.Function):
@@ -1010,11 +1087,11 @@ class _ConvTrain(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, w, b, gamma, beta, opts):
-        bn, relu, decay, moving, debug = opts
+        bn, relu, decay, moving, debug, stats_out = opts
         x = x if x.is_contiguous() else x.contiguous()
         ones = torch.ones((w.shape[1],), dtype=torch.float32, device=x.device)
         y, r = linear_bn_train(x, FoldedConv(w.detach(), ones, b.detach()), gamma.detach(), beta.detach(), moving[0], moving[1],
-                               bn=bn, relu=relu, decay=decay)
+                               bn=bn, relu=relu, decay=decay, stats_out=stats_out)
         out = r[0]
         ctx.bn, ctx.relu = bn, relu
         if bn:
@@ -1048,10 +1125,12 @@ class _ConvTrain(torch.autograd.Function):
         return gx, gw, gb, ggamma, gbeta, None
 
 
-def conv_train(x, w, b, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9, debug=None):
+def conv_train(x, w, b, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9, debug=None,
+               stats_out=None):
     """Differentiable conv (+bias) -> training BatchNorm (bn=True; updates moving_mean / moving_var in place) -> ReLU of
     one layer over the last axis of x, with the forward bits of the non-trainable training path.  x (..., cin),
-    w (cin, cout), b / gamma / beta (cout,).  debug: a list that receives (pre-BN conv output, layer output)."""
+    w (cin, cout), b / gamma / beta (cout,).  debug: a list that receives (pre-BN conv output, layer output).
+    stats_out: optional (mean, var) [cout] that receive the batch statistics (bn=True; kept for the backward)."""
     if not isinstance(x, torch.Tensor) or x.dtype != torch.float32:     # the device is checked by the kernels' wrappers
         raise ValueError("x must be a float32 tensor")
     if w.dim() != 2 or x.shape[-1] != w.shape[0] or tuple(b.shape) != (w.shape[1],):
@@ -1060,7 +1139,7 @@ def conv_train(x, w, b, gamma=None, beta=None, moving_mean=None, moving_var=None
         raise ValueError("conv_train: bn=True needs gamma and beta")
     z = torch.zeros((0,), dtype=torch.float32, device=x.device)
     return _ConvTrain.apply(x, w, b, gamma if bn else z, beta if bn else z,
-                            (bool(bn), bool(relu), float(decay), (moving_mean, moving_var), debug))
+                            (bool(bn), bool(relu), float(decay), (moving_mean, moving_var), debug, stats_out))
 
 
 class _GroupMax(torch.autograd.Function):

@@ -454,6 +454,40 @@ int ssd3d_peer_allgather(const void *src, size_t slice_bytes, void *const *peer_
                          size_t recv_off0, size_t recv_off1, size_t flag_off0, size_t flag_off1, int *state, void *out,
                          ssd3d_stream_t stream);
 
+/* ---- data-parallel training: the per-step gradient exchange (csrc/grad_exchange.cu, DESIGN.md section 3.9) ---------
+ * The reference's towers (lib/core/trainer.py:143-154, lib/utils/trainer_utils.py:23-46) with pinned arithmetic:
+ * clip each rank's gradient, average the clipped gradients in rank order, apply every rank's BatchNorm statistics.
+ * None allocates, uses float atomics or synchronises the host; all are CUDA-graph capturable. */
+
+/* Global norm and clip scale of one rank's flat gradient grad[n]: *norm = float32(sqrt(sum grad^2)), the sum in double
+ * over a fixed tree (256 blocks of 256 threads, each thread in index order, then a halving tree in the block and over
+ * the block partials), so the same bits every run; *scale = rn(clip_norm * minimum(rn(1 / use_norm), rn(1 / clip_norm)))
+ * with use_norm = *norm when finite, else NaN (tf.clip_by_global_norm in float32; the NaN propagates).  norm and scale
+ * are device floats.  workspace: ssd3d_grad_clip_scale_workspace(n) bytes, 8-byte aligned. */
+size_t ssd3d_grad_clip_scale_workspace(long n);
+int ssd3d_grad_clip_scale(const float *grad, long n, float clip_norm, void *workspace, float *norm, float *scale,
+                          ssd3d_stream_t stream);
+/* Mean of the ranks' clipped gradients, written back into every rank's grad[n] (16-byte aligned):
+ * grad[i] = float32((sum over r = 0..world-1 of (double) rn(grad_r[i] * scale_r)) / world), scale = this rank's device
+ * scalar of ssd3d_grad_clip_scale.  ONE launch of `ctas` CTAs: reduce-scatter plus all-gather over the symmetric
+ * buffers (peer_base as in ssd3d_peer_allgather).  Rank p owns floats [p*chunk, (p+1)*chunk), cut into sub-slices of
+ * `sub` floats, one per CTA (chunk and sub multiples of 4, chunk*world >= n, sub*ctas >= chunk).  Inside every rank's
+ * symmetric buffer, per parity q in {0,1}: r1_off<q> and r2_off<q> = world*chunk floats, f1_off<q> and f2_off<q> =
+ * world*ctas int32 flags, all zero before the first call.  state = 3 zero-initialised ints owned by this exchange
+ * ([0] replays done, [2] waits that gave up after ~4 s; a CTA whose wait gave up writes NaN into its part of grad).
+ * All `ctas` CTAs must be co-resident on the device: at most
+ * ssd3d_peer_allreduce_resident_ctas() less whatever else runs there.  Every rank makes the same sequence of calls. */
+int ssd3d_peer_allreduce_resident_ctas(void);
+int ssd3d_peer_allreduce_mean(float *grad, size_t n, const float *scale, void *const *peer_base, int world, int rank, int ctas,
+                              size_t chunk, size_t sub, size_t r1_off0, size_t r1_off1, size_t r2_off0, size_t r2_off1,
+                              size_t f1_off0, size_t f1_off1, size_t f2_off0, size_t f2_off1, int *state,
+                              ssd3d_stream_t stream);
+/* The BatchNorm moving-average update of `world` ranks, in rank order: for r = 0..world-1,
+ * stats[i] = rn(stats[i] - rn(rn(stats[i] - batch[r*ld_batch + i]) * rn(1 - decay))), the update of ssd3d_bn_train.
+ * stats[n] and each rank's batch[.., n] hold means and variances at the same offsets. */
+int ssd3d_bn_moving_update_ranks(float *stats, long n, const float *batch, long ld_batch, int world, float decay,
+                                 ssd3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
