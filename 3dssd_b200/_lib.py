@@ -76,6 +76,8 @@ _SIGNATURES = {
                                                      c_void_p],
     "ssd3d_farthest_point_sample_features_ex": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_longlong, c_void_p,
                                                 c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
+    "ssd3d_farthest_point_sample_features_cl": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_longlong, c_void_p,
+                                                c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "ssd3d_gather_point_ex": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
     "ssd3d_concat_rows": [c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
     "ssd3d_bn_train_workspace": [c_int],

@@ -167,4 +167,22 @@ static inline FpsPlan plan_ffps(int n, int c, bool partial)
     return pl;
 }
 
+// ffps_bucket_kernel (fps.cu): 4 CTAs per scene, 4 points of 68 channels per thread, bucket pruning
+constexpr int FFB_CL = 4;
+constexpr int FFB_MAXN = FFB_CL * FPS_T * 4;
+// rows of slots 2-3, sort keys, bucket centres, per-warp staged rows of both parities, packets
+constexpr size_t ffps_bucket_smem() { return (size_t)2 * FPS_T * 68 * 4 + (size_t)FFB_MAXN * 8 + 8 * 4 * 72 * 4 + 2 * 8 * 72 * 4 + 2 * FFB_CL * 288; }
+
+// ssd3d_farthest_point_sample_features_cl: plan_ffps, except that a full-range call whose cluster request caps the
+// CTAs per scene below the 8 plan_ffps needs for 2048 < n <= 4096 at 3 <= c <= 68 runs ffps_bucket_kernel on 4 CTAs
+// (p = 4 slots per thread) -- the fewest that hold such a scene on chip
+static inline FpsPlan plan_ffps_cl(int n, int c, int cluster, bool partial)
+{
+    FpsPlan pl = plan_ffps(n, c, partial);
+    if (cluster < 0 && -cluster < pl.cl && pl.cl > FFB_CL && !partial && pl.kind == FpsKind::Features && pl.cp == 68 && c >= 3 &&
+        n <= FFB_MAXN)
+        pl.cl = FFB_CL, pl.p = 4, pl.smem = ffps_bucket_smem(), pl.rounds = false;
+    return pl;
+}
+
 }  // namespace ssd3d

@@ -90,7 +90,7 @@ def _side_stream(device, i=0):
     return _SIDE_STREAMS[key]
 
 
-def ffps_indices(npoint, xyz, points, mode, out=None, idx_offset=0):
+def ffps_indices(npoint, xyz, points, mode, out=None, idx_offset=0, cluster=None):
     """F-FPS on concat[xyz, points] (layers_util.py:94-96, :102-104).
     mode 'direct': one kernel, no [B,N,N] tensor, the SAME indices as 'matrix' (each round evaluates the picked point's
                    matrix row on chip with calc_square_dist's arithmetic); falls back to 'matrix' for uncovered shapes;
@@ -98,13 +98,14 @@ def ffps_indices(npoint, xyz, points, mode, out=None, idx_offset=0):
     mode 'fused' : matrix-free -- the generic-c FPS kernel evaluates the feature distance on the fly (no
                    [B,N,N] tensor); identical to the reference's own farthest_point_sample on the features.
     xyz / points may be [:, a:b] slices of dense tensors (read in place); out=(buffer, col) / idx_offset as in
-    tf_ops.farthest_point_sample."""
+    tf_ops.farthest_point_sample; cluster: the 'direct' kernel's CTA cap (tf_ops.farthest_point_sample_features)."""
     if mode == "direct":
         c = xyz.shape[2] + points.shape[2]
         # the 132-channel variant walks a 131-long dependent fma chain per round: at layer-3 sizes (512 points) the
         # small matrix is faster, so 'direct' is used where the matrix is the expensive part (c <= 68, layer 2)
         if c <= 68 and tf_ops.ffps_supported(xyz.shape[1], c):
-            return tf_ops.farthest_point_sample_features(npoint, xyz, points, out=out, idx_offset=idx_offset)
+            kw = {} if cluster is None else {"cluster": cluster}
+            return tf_ops.farthest_point_sample_features(npoint, xyz, points, out=out, idx_offset=idx_offset, **kw)
         mode = "matrix"
     feats = tf_ops.concat_cols(xyz, points) if points.shape[2] else xyz
     if mode == "matrix":
@@ -367,7 +368,8 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
                                                       rounds=(j0, j1), temp=temp)
                 parts.append((col + j0, col + j1, ev_main()))
             return
-        ffps_indices(npoint, tmp_xyz, tmp_points, ffps_mode, out=(fps_idx, col), idx_offset=lo)
+        ffps_indices(npoint, tmp_xyz, tmp_points, ffps_mode, out=(fps_idx, col), idx_offset=lo,
+                     cluster=fps_cluster if fps_cluster < 0 else None)
         parts.append((col, col + npoint, ev_main() if in_parts else None))
 
     lone = len(segs) == 1

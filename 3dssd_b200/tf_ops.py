@@ -161,10 +161,13 @@ def ffps_supported(n, c):
     return bool(lib().ssd3d_ffps_supported(int(n), int(c)))
 
 
-def farthest_point_sample_features(npoint, xyz, points=None, *, out=None, idx_offset=0, rounds=None, temp=None):
+def farthest_point_sample_features(npoint, xyz, points=None, *, out=None, idx_offset=0, rounds=None, temp=None,
+                                   cluster=None):
     """F-FPS on concat[xyz, points] without the distance matrix: the same indices as
     farthest_point_sample_with_distance(npoint, calc_square_dist(concat[xyz, points])) (layers_util.py:94-96).
-    Keyword extensions as farthest_point_sample (out, idx_offset, rounds + temp)."""
+    Keyword extensions as farthest_point_sample (out, idx_offset, rounds + temp); cluster < 0 caps the CTAs per scene
+    at -cluster where a kernel allows it (a full range of 2048 < n <= 4096 points of <= 68 channels then runs on 4 CTAs
+    with bucket pruning), cluster=None or 0 leaves the choice to the library."""
     xyz, sa = _scene_strided(xyz, "xyz")
     b, n, ca = xyz.shape
     cb, sb = 0, 0
@@ -182,9 +185,12 @@ def farthest_point_sample_features(npoint, xyz, points=None, *, out=None, idx_of
         if temp is None:
             raise ValueError("a partial range of rounds needs a contiguous float32 temp buffer of batch * n elements")
         temp = _temp(temp, b * n)
-    check(lib().ssd3d_farthest_point_sample_features_ex(b, n, ca, cb, npoint, _p(xyz), sa, _p(points), sb, _p(temp),
-                                                        ctypes.c_void_p(optr), ldo, int(idx_offset), j0, j1, _stream()),
-          "farthest_point_sample_features")
+    args = (b, n, ca, cb, npoint, _p(xyz), sa, _p(points), sb, _p(temp), ctypes.c_void_p(optr), ldo, int(idx_offset), j0, j1)
+    if cluster is None:
+        rc = lib().ssd3d_farthest_point_sample_features_ex(*args, _stream())
+    else:
+        rc = lib().ssd3d_farthest_point_sample_features_cl(*args, int(cluster), _stream())
+    check(rc, "farthest_point_sample_features")
     return o
 
 

@@ -92,6 +92,12 @@ int ssd3d_farthest_point_sample_features(int b, int n, int ca, int cb, int m, co
 int ssd3d_farthest_point_sample_features_ex(int b, int n, int ca, int cb, int m, const float *fa, long long fa_stride,
                                             const float *fb, long long fb_stride, float *temp, int *out, int ldo,
                                             int idx_offset, int j0, int j1, ssd3d_stream_t stream);
+/* ... with a cluster request: 0 = as _ex, < 0 = CTAs per scene capped at -cluster (-1, -2, -4, -8 or -16).  A cap below
+ * what _ex uses runs a full-range call with 2048 < n <= 4096, 3 <= ca+cb <= 68 on 4 CTAs per scene with bucket
+ * pruning (same indices; fewer SMs per scene for throughput); partial ranges and other shapes run as _ex. */
+int ssd3d_farthest_point_sample_features_cl(int b, int n, int ca, int cb, int m, const float *fa, long long fa_stride,
+                                            const float *fb, long long fb_stride, float *temp, int *out, int ldo,
+                                            int idx_offset, int j0, int j1, int cluster, ssd3d_stream_t stream);
 int ssd3d_ffps_supported(int n, int c);
 
 /* replaces gatherpointLauncher(b,n,m,c,inp,idx,out)
