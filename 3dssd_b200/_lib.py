@@ -112,6 +112,12 @@ _SIGNATURES = {
     "ssd3d_peer_allreduce_mean": [c_void_p, ctypes.c_size_t, c_void_p, c_void_p, c_int, c_int, c_int] + [ctypes.c_size_t] * 10 +
                                  [c_void_p, c_void_p],
     "ssd3d_bn_moving_update_ranks": [c_void_p, c_long, c_void_p, c_long, c_int, c_float, c_void_p],
+    "ssd3d_box_iou": [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "ssd3d_box_iou_matched": [c_long, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "ssd3d_eval_workspace": [c_long],
+    "ssd3d_eval_overlaps": [c_int, c_int, c_int] + [c_void_p] * 7,
+    "ssd3d_eval_first_pass": [c_int, c_int, c_int] + [c_void_p] * 6 + [c_long] + [c_void_p] * 4,
+    "ssd3d_eval_count": [c_int, c_int, c_int] + [c_void_p] * 10,
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["ssd3d_last_error"])
@@ -130,7 +136,8 @@ def lib():
             fn.argtypes = argtypes
             fn.restype = ctypes.c_size_t if name in ("ssd3d_sa_fused_smem", "ssd3d_query_ball_point_workspace", "ssd3d_bn_train_workspace",
                                                    "ssd3d_linear_wgrad_workspace", "ssd3d_bn_train_grad_workspace",
-                                                   "ssd3d_det_loss_workspace", "ssd3d_grad_clip_scale_workspace") else c_int
+                                                   "ssd3d_det_loss_workspace", "ssd3d_grad_clip_scale_workspace",
+                                                   "ssd3d_eval_workspace") else c_int
             if name == "ssd3d_fps_temp_elems":
                 fn.restype = c_long
         l.ssd3d_last_error.restype = ctypes.c_char_p

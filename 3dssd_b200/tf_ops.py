@@ -773,6 +773,125 @@ def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
     return block, cnt
 
 
+# ---- KITTI evaluation (csrc/box_eval.cu, DESIGN.md section 3.10; evaluation/tf_evaluate.py) --------------------------
+
+EVAL_MAX_DETS = 1024          # detections per frame
+EVAL_MAX_LABELS = 256         # label rows per frame
+EVAL_NSAMPLE = 41
+
+
+def calc_iou(detections, groundtruths):
+    """tf_evaluate.py:26-33: detections (bs, n, 7), groundtruths (bs, m, 7) as (x, y, z, l, h, w, ry) ->
+    (iou_bev, iou_3d), each (bs, n, m) float32: rotated BEV and 3-D IoU computed in double."""
+    d = _req(detections, "detections", torch.float32, 3, 7)
+    g = _req(groundtruths, "groundtruths", torch.float32, 3, 7)
+    if g.shape[0] != d.shape[0]:
+        raise ValueError("groundtruths must be (bs, -1, 7) with bs = %d, got %s" % (d.shape[0], tuple(g.shape)))
+    b, n, m = d.shape[0], d.shape[1], g.shape[1]
+    bev = torch.empty((b, n, m), dtype=torch.float32, device=d.device)
+    v3 = torch.empty((b, n, m), dtype=torch.float32, device=d.device)
+    check(lib().ssd3d_box_iou(b, n, m, _p(d), _p(g), _p(bev), _p(v3), _stream()), "calc_iou")
+    return bev, v3
+
+
+def calc_iou_match(detections, groundtruths):
+    """tf_evaluate.py:35-42: row i of detections (-1, 7) against row i of groundtruths (-1, 7) -> (iou_bev, iou_3d),
+    each (-1,) float32."""
+    d = _req(detections, "detections", torch.float32, 2, 7)
+    g = _req(groundtruths, "groundtruths", torch.float32, 2, 7)
+    if g.shape[0] != d.shape[0]:
+        raise ValueError("groundtruths must be (%d, 7), got %s" % (d.shape[0], tuple(g.shape)))
+    n = d.shape[0]
+    bev = torch.empty((n,), dtype=torch.float32, device=d.device)
+    v3 = torch.empty((n,), dtype=torch.float32, device=d.device)
+    check(lib().ssd3d_box_iou_matched(n, _p(d), _p(g), _p(bev), _p(v3), _stream()), "calc_iou_match")
+    return bev, v3
+
+
+def evaluate(detections, names, numlist):
+    """tf_evaluate.py:9-23: detections (n, 14) float32 rows as evaluate_map builds them, names (m,) KITTI label_2 file
+    paths, numlist (m,) int32 detections per frame -> (precision_image, aos_image, precision_ground, aos_ground,
+    precision_3d, aos_3d), each (3, 3, 41) float32 = [Car / Pedestrian / Cyclist, easy / moderate / hard, sample].
+    A class is evaluated in a metric only when one of its detections has the fields the metric needs; its other entries,
+    and every AOS entry (the reference never computes AOS), are -1."""
+    from .evaluation import read_label_file
+    names = [n.decode() if isinstance(n, bytes) else str(n) for n in names]
+    nl = _req(numlist, "numlist", torch.int32, 1)
+    if nl.shape[0] != len(names):
+        raise ValueError("numlist must be (%d,) like names, got %s" % (len(names), tuple(nl.shape)))
+    return evaluate_labels(detections, [read_label_file(n) for n in names], nl)
+
+
+def _eval_frames(detections, labels, numlist):
+    """Operand checks and CSR offsets of evaluate_labels, all before anything reaches the library."""
+    import numpy as np
+    det = _req(detections, "detections", torch.float32, 2, 14)
+    nl = _req(numlist, "numlist", torch.int32, 1)
+    labels = [np.asarray(x, np.float64) for x in labels]
+    if any(x.ndim != 2 or x.shape[1] != 15 for x in labels):
+        raise ValueError("labels must be one (rows, 15) float64 array per frame (evaluation.read_label_file)")
+    if nl.shape[0] != len(labels):
+        raise ValueError("numlist must be (%d,) like labels, got %s" % (len(labels), tuple(nl.shape)))
+    counts = nl.cpu().numpy().astype(np.int64)
+    lc = np.array([x.shape[0] for x in labels], np.int64)
+    if (counts < 0).any() or counts.sum() != det.shape[0]:
+        raise ValueError("numlist must be non-negative and sum to the %d detection rows" % det.shape[0])
+    if len(counts) and counts.max() > EVAL_MAX_DETS:
+        raise ValueError("evaluate: at most %d detections per frame (frame %d has %d)" %
+                         (EVAL_MAX_DETS, int(counts.argmax()), int(counts.max())))
+    if len(lc) and lc.max() > EVAL_MAX_LABELS:
+        raise ValueError("evaluate: at most %d label rows per frame (frame %d has %d)" %
+                         (EVAL_MAX_LABELS, int(lc.argmax()), int(lc.max())))
+    return det, labels, counts, lc
+
+
+def evaluate_labels(detections, labels, numlist):
+    """evaluate() on label rows already read (one (rows, 15) float64 array per frame, evaluation.read_label_file)."""
+    import numpy as np
+    from .evaluation import eval_flags, get_thresholds, precision_curve
+    det, labels, counts, lc = _eval_frames(detections, labels, numlist)
+    dev = det.device
+    frames = len(labels)
+    out = np.full((6, 3, 3, EVAL_NSAMPLE), -1.0, np.float32)
+    flags = eval_flags(det.cpu().numpy())
+    if frames and any(any(f) for f in flags):
+        rows = int(lc.sum())
+        det_off = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+        label_off = np.concatenate([[0], np.cumsum(lc)]).astype(np.int32)
+        pairs = counts * lc
+        pair_off = np.concatenate([[0], np.cumsum(pairs)[:-1]]).astype(np.int64)
+        up = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(dev, dt)
+        d_det_off, d_label_off, d_pair_off = up(det_off, torch.int32), up(label_off, torch.int32), up(pair_off, torch.int64)
+        d_lab = up(np.concatenate(labels, 0) if rows else np.zeros((0, 15)), torch.float64)
+        ws = torch.empty((max(1, int(lib().ssd3d_eval_workspace(int(pairs.sum()))) // 8),), dtype=torch.float64, device=dev)
+        md, ml = int(counts.max()), int(lc.max())
+        args = (frames, md, ml, _p(det), _p(d_det_off), _p(d_lab), _p(d_label_off), _p(d_pair_off), _p(ws))
+        check(lib().ssd3d_eval_overlaps(*args, _stream()), "evaluate")
+        tp_scores = torch.empty((27, max(rows, 1)), dtype=torch.float64, device=dev)
+        tp_count = torch.empty((27, frames), dtype=torch.int32, device=dev)
+        n_gt = torch.empty((27, frames), dtype=torch.int32, device=dev)
+        check(lib().ssd3d_eval_first_pass(*args, rows, _p(tp_scores), _p(tp_count), _p(n_gt), _stream()), "evaluate")
+        # getThresholds on the host (float64, evaluate.cpp:539-572)
+        scores, tpc, ngt = tp_scores.cpu().numpy(), tp_count.cpu().numpy(), n_gt.cpu().numpy()
+        frame_of_row = np.repeat(np.arange(frames), lc)
+        k_of_row = np.arange(rows) - label_off[:-1][frame_of_row]
+        thr = np.zeros((27, EVAL_NSAMPLE), np.float64)
+        nthr = np.zeros((27,), np.int32)
+        for cs in range(27):
+            if flags[cs // 9][(cs // 3) % 3]:
+                t = get_thresholds(scores[cs, :rows][k_of_row < tpc[cs][frame_of_row]], int(ngt[cs].sum()))
+                thr[cs, :len(t)], nthr[cs] = t, len(t)
+        d_thr, d_nthr = up(thr, torch.float64), up(nthr, torch.int32)
+        cnt = torch.empty((27, EVAL_NSAMPLE, 3), dtype=torch.int32, device=dev)
+        check(lib().ssd3d_eval_count(*args, _p(d_thr), _p(d_nthr), _p(cnt), _stream()), "evaluate")
+        cnt = cnt.cpu().numpy()
+        for cs in range(27):
+            m, c, d = cs // 9, (cs // 3) % 3, cs % 3
+            if flags[m][c]:
+                out[2 * m, c, d] = precision_curve(cnt[cs, :, 0], cnt[cs, :, 1], int(nthr[cs]))
+    return tuple(torch.from_numpy(a.copy()).to(dev) for a in out)
+
+
 # ---- the small elementwise stages (csrc/misc.cu): one kernel each, so a captured step holds no framework kernels ----
 
 def fill_zero(t):

@@ -494,6 +494,36 @@ int ssd3d_peer_allreduce_mean(float *grad, size_t n, const float *scale, void *c
 int ssd3d_bn_moving_update_ranks(float *stats, long n, const float *batch, long ld_batch, int world, float decay,
                                  ssd3d_stream_t stream);
 
+/* ---- KITTI evaluation (csrc/box_eval.cu, DESIGN.md section 3.10; evaluation/evaluate.cpp, tf_evaluate.cpp) ----------
+ * Boxes are (x, y, z, l, h, w, ry), camera frame, origin at the bottom-face centre.  Overlaps are computed in double by
+ * the recipe of DESIGN.md section 3.10; a pair whose union area or volume is <= 0 has overlap 0.
+ * calc_iou (tf_evaluate.cpp:35-48): iou_bev, iou_3d [b, n, m] = rotated BEV / 3-D IoU of dets [b, n, 7] x gts [b, m, 7]. */
+int ssd3d_box_iou(int b, int n, int m, const float *dets, const float *gts, float *iou_bev, float *iou_3d,
+                  ssd3d_stream_t stream);
+/* calc_iou_match (tf_evaluate.cpp:50-63): iou_bev[i], iou_3d[i] of dets[i] [n, 7] against gts[i] [n, 7]. */
+int ssd3d_box_iou_matched(long n, const float *dets, const float *gts, float *iou_bev, float *iou_3d, ssd3d_stream_t stream);
+/* The Evaluate op (tf_evaluate.cpp:14-33) in three launches.  Frames are CSR-packed: dets [N, 14] float rows (class, x1,
+ * y1, x2, y2, alpha, t1, t2, t3, h, w, l, ry, score) with frame f at rows det_off[f] .. det_off[f+1]-1; labels [R, 15]
+ * DOUBLE rows (the 15 fields of a KITTI label line, the type replaced by 0 Car, 1 Pedestrian, 2 Cyclist, 3 Van,
+ * 4 Person_sitting, 5 DontCare, 6 other) indexed by label_off; pair_off [frames] int64 = sum over earlier frames of
+ * (detections * label rows).  Every frame holds at most max_dets <= 1024 detections and max_labels <= 256 label rows.
+ * Cases are numbered metric * 9 + class * 3 + difficulty (metric: image, ground, 3-D).
+ * Workspace of ssd3d_eval_overlaps: ssd3d_eval_workspace(total pairs) bytes, 8-byte aligned. */
+size_t ssd3d_eval_workspace(long pairs);
+int ssd3d_eval_overlaps(int frames, int max_dets, int max_labels, const float *dets, const int *det_off,
+                        const double *labels, const int *label_off, const long *pair_off, void *workspace,
+                        ssd3d_stream_t stream);
+/* First pass of computeStatistics (evaluate.cpp:649-830, no false positives counted), all 27 cases in one launch:
+ * tp_scores[case * label_rows + label_off[f] + k] for k < tp_count[case * frames + f]; n_gt[case * frames + f]. */
+int ssd3d_eval_first_pass(int frames, int max_dets, int max_labels, const float *dets, const int *det_off,
+                          const double *labels, const int *label_off, const long *pair_off, const void *workspace,
+                          long label_rows, double *tp_scores, int *tp_count, int *n_gt, ssd3d_stream_t stream);
+/* Counting pass at each case's score thresholds (thresholds [27, 41] double, n_thresholds [27] <= 41, from getThresholds,
+ * evaluate.cpp:539-572): counts [27, 41, 3] int = tp, fp, fn summed over the frames (cleared here first). */
+int ssd3d_eval_count(int frames, int max_dets, int max_labels, const float *dets, const int *det_off,
+                     const double *labels, const int *label_off, const long *pair_off, const void *workspace,
+                     const double *thresholds, const int *n_thresholds, int *counts, ssd3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
