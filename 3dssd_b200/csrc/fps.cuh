@@ -1,4 +1,5 @@
-// fps.cuh -- the round protocol shared by the FPS kernels (fps.cu, fps_bucket.cu).
+// fps.cuh -- the round protocol shared by the FPS kernels (fps.cu, fps_bucket.cu) and the set-up shared by the pruned
+// kernels (fps_bucket.cu).
 #pragma once
 #include "common.cuh"
 #include "fps_plan.h"
@@ -145,7 +146,114 @@ struct FpsRing {
     __device__ __forceinline__ void wait(int r) { mbar_wait_cta(at(r), ((r - 1) >> 1) & 1); }
 };
 
-// fps_bucket.cu: single-CTA D-FPS with spatial pruning for large xyz scenes
+// The arg-max packet of the matrix-free F-FPS kernels (ffps_cluster_kernel, ffps_bucket_kernel): header + feature row.
+template <int CP>
+struct __align__(16) FfpsPacket {
+    uint32_t val, key;
+    float sq;
+    uint32_t pad;
+    float feat[CP];
+};
+static_assert(sizeof(FfpsPacket<68>) == 16 + 4 * 68 && sizeof(FfpsPacket<132>) == 16 + 4 * 132, "ffps_smem (fps_plan.h)");
+
+// ---- set-up pieces of the pruned kernels (fps_bucket.cu) -------------------------------------------------------------
+
+// order-preserving float <-> uint map: min/max reductions of signed floats (and of NaNs) as unsigned words
+__device__ __forceinline__ uint32_t fps_ord(float x)
+{
+    const uint32_t b = __float_as_uint(x);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float fps_unord(uint32_t u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
+
+// Scene box: per-axis min / max of channels 0-2 (at(k, a) = channel a of point k) over points 0..n-1, on the CTA's NT
+// threads.  Each thread folds its points with fminf / fmaxf (8 loads in flight), warps and the CTA fold the
+// order-preserving words, through red[6][NT / 32] in shared memory.  Every thread returns the box.
+template <int NT, class At>
+__device__ __forceinline__ void fps_scene_box(int n, At at, uint32_t (&red)[6][NT / 32], float (&lo)[3], float (&hi)[3])
+{
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int a = 0; a < 3; a++) lo[a] = 3.0e38f, hi[a] = -3.0e38f;
+#pragma unroll 8
+    for (int k = tid; k < n; k += NT)
+#pragma unroll
+        for (int a = 0; a < 3; a++) { const float v = at(k, a); lo[a] = fminf(lo[a], v); hi[a] = fmaxf(hi[a], v); }
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+        const uint32_t mn = __reduce_min_sync(0xffffffffu, fps_ord(lo[a])), mx = __reduce_max_sync(0xffffffffu, fps_ord(hi[a]));
+        if ((tid & 31) == 0) { red[a][tid >> 5] = mn; red[3 + a][tid >> 5] = mx; }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+        uint32_t mn = 0xffffffffu, mx = 0u;
+        for (int q = 0; q < NT / 32; q++) { mn = min(mn, red[a][q]); mx = max(mx, red[3 + a][q]); }
+        lo[a] = fps_unord(mn); hi[a] = fps_unord(mx);
+    }
+}
+
+// Ascending bitonic sort of np unique keys in shared memory (np a power of two, 2 NT <= np <= MAXN) on the CTA's NT
+// threads.  A stage's compare-exchanges are disjoint, so a thread loads all of its pairs before storing any.
+template <class Key, int NT, int MAXN>
+__device__ __forceinline__ void fps_bitonic_sort(Key *key, int np)
+{
+    constexpr int PAIRS = MAXN / 2 / NT;
+    for (int k = 2; k <= np; k <<= 1)
+        for (int jj = k >> 1; jj > 0; jj >>= 1) {
+            Key a[PAIRS], b[PAIRS];
+#pragma unroll
+            for (int u = 0; u < PAIRS; u++) {
+                const int t = threadIdx.x + u * NT, l = ((t & ~(jj - 1)) << 1) | (t & (jj - 1));
+                if (t < np / 2) { a[u] = key[l]; b[u] = key[l | jj]; }
+            }
+#pragma unroll
+            for (int u = 0; u < PAIRS; u++) {
+                const int t = threadIdx.x + u * NT, l = ((t & ~(jj - 1)) << 1) | (t & (jj - 1));
+                if (t < np / 2 && (a[u] > b[u]) == ((l & k) == 0)) { key[l] = b[u]; key[l | jj] = a[u]; }
+            }
+            __syncthreads();
+        }
+}
+
+// Tie-break key of point o WITH its place p (where the kernel keeps it) in the low 21 - W bits, W = bits of o div 1024:
+// ordered like fps_key(o) -- (o mod 1024, o div 1024) -- because those two fields are unique per point and sit above the
+// place.  A min-reduction over these words returns the reference's winner AND where it is; no lane or position has to
+// be tracked through the stages (a ballot + find-first per stage costs as much as the stage's reductions).
+template <int W>
+__device__ __forceinline__ uint32_t fps_place_key(uint32_t o, uint32_t p) { return ((o & 1023u) << 21) | ((o >> 10) << (21 - W)) | p; }
+template <int W>
+__device__ __forceinline__ int fps_place_key_to_k(uint32_t key) { return (int)((((key >> (21 - W)) & ((1u << W) - 1u)) << 10) | (key >> 21)); }
+
+// Launch `kernel` on b scenes of cl CTAs (a cluster each) of FPS_T threads.
+template <typename K>
+static cudaError_t launch_cluster(K kernel, int cl, int b, size_t dyn_smem, cudaStream_t stream, void **args)
+{
+    cudaError_t e = cudaFuncSetAttribute((const void *)kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem);
+    if (e != cudaSuccess) return e;
+    if (cl > 8) {
+        e = cudaFuncSetAttribute((const void *)kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+        if (e != cudaSuccess) return e;
+    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(b * cl));
+    cfg.blockDim = dim3(FPS_T);
+    cfg.dynamicSmemBytes = dyn_smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cl;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelExC(&cfg, (const void *)kernel, args);
+}
+
+// fps_bucket.cu, the pruned kernels: single-CTA D-FPS for large xyz scenes (FpsKind::Bucket) and 4-CTA F-FPS
+// (FpsKind::FeaturesBucket)
 int launch_fps3_bucket(int b, int n, int m, const float *inp, int *out, const FpsIO &io, cudaStream_t st);
+int launch_ffps_bucket(int b, int n, int ca, int cb, int m, const float *fa, const float *fb, int *out, const FpsIO &io,
+                       cudaStream_t st);
 
 }  // namespace ssd3d

@@ -7,22 +7,24 @@
 namespace ssd3d {
 
 constexpr int FPS_T = 256;                      // threads per CTA of the cluster kernels
+constexpr int FPS_NW = FPS_T / 32;
 constexpr size_t FPS_SMEM_BUDGET = 200 * 1024;  // dynamic shared memory a cluster kernel may plan for
 constexpr int FB_MAXN = 16384;                  // points the single-CTA pruned kernel holds (fps_bucket.cu)
 
 enum class FpsKind {
-    Bucket,    // fps3_bucket_kernel: one CTA per scene with spatial pruning (c == 3)
-    Direct,    // fps3_direct_kernel<CL,P>: scene resident in every CTA (c == 3)
-    Packet,    // fps3_cluster_kernel<CL,P>: coordinates travel in the packets (c == 3)
-    Generic,   // fpsc_cluster_kernel<CL,P>: any c, features in the cluster's shared memory
-    Dist,      // fpsdist_cluster_kernel<CL,P>: given distance matrix
-    Features,  // ffps_cluster_kernel<CL,P,CP>: matrix-free F-FPS
-    Fallback,  // no on-chip kernel: fps_fallback_kernel with temp[b,n]; for features, SSD3D_ERR_UNSUPPORTED
+    Bucket,          // fps3_bucket_kernel: one CTA per scene with spatial pruning (c == 3)
+    Direct,          // fps3_direct_kernel<CL,P>: scene resident in every CTA (c == 3)
+    Packet,          // fps3_cluster_kernel<CL,P>: coordinates travel in the packets (c == 3)
+    Generic,         // fpsc_cluster_kernel<CL,P>: any c, features in the cluster's shared memory
+    Dist,            // fpsdist_cluster_kernel<CL,P>: given distance matrix
+    Features,        // ffps_cluster_kernel<CL,P,CP>: matrix-free F-FPS
+    FeaturesBucket,  // ffps_bucket_kernel: matrix-free F-FPS on 4 CTAs with bucket pruning
+    Fallback,        // no on-chip kernel: fps_fallback_kernel with temp[b,n]; for features, SSD3D_ERR_UNSUPPORTED
 };
 
 struct FpsPlan {
     FpsKind kind = FpsKind::Fallback;
-    int cl = 0, p = 0, cp = 0;  // CTAs per scene, points per thread, padded channels (Features)
+    int cl = 0, p = 0, cp = 0;  // CTAs per scene, points per thread, padded channels (Features, FeaturesBucket)
     size_t smem = 0;            // dynamic shared memory per CTA, bytes
     long temp = 0;              // floats of temp per scene the call uses (0: temp may be NULL)
     bool rounds = false;        // the route runs a partial range of rounds
@@ -154,34 +156,26 @@ static inline FpsPlan plan_fps_dist(int n, int cluster)
     return pl;
 }
 
-// ssd3d_farthest_point_sample_features_ex: c = channels of the concatenated feature
-static inline FpsPlan plan_ffps(int n, int c, bool partial)
-{
-    FpsPlan pl;
-    const int cl = n > 0 && c > 0 ? ffps_cluster_for(n, c) : 0;
-    if (cl > 0) {
-        pl.kind = FpsKind::Features, pl.cl = cl, pl.p = c <= 68 ? 2 : 1, pl.cp = c <= 68 ? 68 : 132;
-        pl.smem = ffps_smem(cl, pl.p, pl.cp), pl.rounds = true;
-    }
-    if (partial) pl.temp = n;
-    return pl;
-}
-
-// ffps_bucket_kernel (fps.cu): 4 CTAs per scene, 4 points of 68 channels per thread, bucket pruning
+// ffps_bucket_kernel (fps_bucket.cu): 4 CTAs per scene, 4 points of 68 channels per thread, bucket pruning
 constexpr int FFB_CL = 4;
 constexpr int FFB_MAXN = FFB_CL * FPS_T * 4;
 // rows of slots 2-3, sort keys, bucket centres, per-warp staged rows of both parities, packets
 constexpr size_t ffps_bucket_smem() { return (size_t)2 * FPS_T * 68 * 4 + (size_t)FFB_MAXN * 8 + 8 * 4 * 72 * 4 + 2 * 8 * 72 * 4 + 2 * FFB_CL * 288; }
 
-// ssd3d_farthest_point_sample_features_cl: plan_ffps, except that a full-range call whose cluster request caps the
-// CTAs per scene below the 8 plan_ffps needs for 2048 < n <= 4096 at 3 <= c <= 68 runs ffps_bucket_kernel on 4 CTAs
-// (p = 4 slots per thread) -- the fewest that hold such a scene on chip
-static inline FpsPlan plan_ffps_cl(int n, int c, int cluster, bool partial)
+// ssd3d_farthest_point_sample_features_cl: c = channels of the concatenated feature, `cluster` = 0 or a cap (< 0).  A
+// full-range call whose cap is below the 8 CTAs that 2048 < n <= 4096 at 3 <= c <= 68 needs runs ffps_bucket_kernel
+// on 4 CTAs -- the fewest that hold such a scene on chip; its partial ranges stay on ffps_cluster_kernel.
+static inline FpsPlan plan_ffps(int n, int c, int cluster, bool partial)
 {
-    FpsPlan pl = plan_ffps(n, c, partial);
-    if (cluster < 0 && -cluster < pl.cl && pl.cl > FFB_CL && !partial && pl.kind == FpsKind::Features && pl.cp == 68 && c >= 3 &&
-        n <= FFB_MAXN)
-        pl.cl = FFB_CL, pl.p = 4, pl.smem = ffps_bucket_smem(), pl.rounds = false;
+    FpsPlan pl;
+    const int cl = n > 0 && c > 0 ? ffps_cluster_for(n, c) : 0;
+    if (cl > FFB_CL && cluster < 0 && -cluster < cl && !partial && c >= 3 && c <= 68 && n <= FFB_MAXN) {
+        pl.kind = FpsKind::FeaturesBucket, pl.cl = FFB_CL, pl.p = 4, pl.cp = 68, pl.smem = ffps_bucket_smem();
+    } else if (cl > 0) {
+        pl.kind = FpsKind::Features, pl.cl = cl, pl.p = c <= 68 ? 2 : 1, pl.cp = c <= 68 ? 68 : 132;
+        pl.smem = ffps_smem(cl, pl.p, pl.cp), pl.rounds = true;
+    }
+    if (partial) pl.temp = n;
     return pl;
 }
 

@@ -21,7 +21,8 @@ _i32p = ctypes.POINTER(ctypes.c_int)
 
 def build(force=False):
     """Compile liboracle.so with gcc (seconds)."""
-    newest = max(os.path.getmtime(os.path.join(_HERE, f)) for f in ("ssd3d_oracle.c", "fps_pruned_model.c", "bq_grid_model.c", "Makefile"))
+    srcs = ("ssd3d_oracle.c", "fps_pruned_model.c", "ffps_prune_model.c", "bq_grid_model.c", "Makefile")
+    newest = max(os.path.getmtime(os.path.join(_HERE, f)) for f in srcs)
     if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < newest:
         subprocess.check_call(["make", "-C", _HERE, "liboracle.so"], stdout=subprocess.DEVNULL)
     return _LIB_PATH
@@ -86,6 +87,24 @@ def fps_pruned_model(npoint, inp, rounds=None, temp=None, out=None, idx_offset=0
     if rc != 0:
         raise ValueError("fps_pruned_model: unsupported arguments (n <= 16384, temp needed for partial rounds)")
     return out, tuple(int(v) for v in stats)
+
+
+def ffps_prune_model(npoint, x, with_margin=True):
+    """CPU model of the skip rule of the PRODUCT's pruned F-FPS (ffps_bucket_kernel in 3dssd_b200/csrc/fps_bucket.cu, see
+    oracle/ffps_prune_model.c) on one scene x [n, c] (n <= 4096, 3 <= c <= 68): used by the CPU tests to check that
+    kernel's exactness claim.  with_margin=False drops the rounding margin of the skip test.  Returns (indices, stats)
+    with stats = (points of skipped buckets whose value was below their running distance, bucket updates summed over
+    rounds)."""
+    x, p = _f(x)
+    n, c = x.shape
+    out = np.zeros(int(npoint), np.int32)
+    touched = ctypes.c_longlong(0)
+    fn = lib().oracle_ffps_prune_model
+    fn.restype = ctypes.c_longlong
+    bad = fn(n, c, int(npoint), p, int(bool(with_margin)), out.ctypes.data_as(_i32p), ctypes.byref(touched))
+    if bad < 0:
+        raise ValueError("ffps_prune_model: unsupported arguments (n <= 4096, 3 <= c <= 68)")
+    return out, (int(bad), int(touched.value))
 
 
 def farthest_point_sample_with_distance(npoint, dist):

@@ -1,6 +1,6 @@
 """Every FPS kernel instantiation the launch plan can pick, run on the GPU against the CPU oracle.
 
-Each `fn<CL,P>` of csrc/fps.cu (and the F-FPS `<CL,P,CP>` variants, the bucket and the fallback kernel) hands its threads
+Each `fn<CL,P>` of csrc/fps.cu (and the F-FPS `<CL,P,CP>` variants, the pruned kernels and the fallback kernel) hands its threads
 a different mix of residue classes and slots and leaves a different number of threads and CTAs without points, so an
 index or tie-break mistake in one instantiation is invisible to the others.  FPS indices are bit-exact: a wrong
 tie-break shows up as a different sample set, not as a tolerance.
@@ -50,7 +50,7 @@ def _outcome(o):
 
 def _reach(table):
     """(outcome, family, n, c, key m, cluster request, flags, aligned) for every route entry, in table order; for the
-    features family the per-entry argument is the channel count."""
+    features family the key holds the cluster request and the per-entry argument is the channel count."""
     out = []
     for key, ids in table["routes"].items():
         fam, *kv = key.split()
@@ -58,7 +58,7 @@ def _reach(table):
         n = int(kv["n"])
         if fam == "features":
             for c, i in zip((int(v) for v in kv["c"].split(",")), ids):
-                out.append((_outcome(table["outcomes"][i]), fam, n, c, 0, 0, 0, 1))
+                out.append((_outcome(table["outcomes"][i]), fam, n, c, 0, int(kv["cluster"]), 0, 1))
         else:
             for cl, i in zip(table["clusters"], ids):
                 o = table["outcomes"][i]
@@ -112,7 +112,7 @@ def _picks(table):
         for r, smallest in ((lo, True), (hi, False)):
             if r is None:
                 continue
-            for c in sorted({q[3] for q in rs if q[2] == r[2]}) if r[1] == "features" else [r[3]]:
+            for c in sorted({q[3] for q in rs if q[2] == r[2] and q[5] == r[5]}) if r[1] == "features" else [r[3]]:
                 out.append(r[:3] + (c,) + r[4:] + (smallest,))
     return out
 
@@ -156,7 +156,7 @@ def _plan_query(case, launch):
         return "fps %d %d %d %d %d %d" % (case.n, case.c, launch.m, case.cluster, case.flags, case.aligned)
     if case.family == "dist":
         return "dist %d %d" % (case.n, case.cluster)
-    return "features %d %d" % (case.n, case.c)
+    return "features %d %d %d" % (case.n, case.c, case.cluster)
 
 
 def _coverage_gaps(table, cases):
@@ -179,7 +179,7 @@ def test_cases_cover_every_outcome(tmp_path):
                            check=True).stdout.split("\n")[:-1]
     assert len(lines) == len(queries)
     for (case, launch, q), line in zip(queries, lines):
-        kind, cl, p, cp, _, _, _, rounds = line.split()
+        kind, cl, p, cp, _, _, _, rounds = line.split()[:8]
         assert (kind, int(cl), int(p), int(cp)) == case.outcome, (case.id, launch, q, line)
         assert launch.cuts is None or rounds == "1", (case.id, launch, q, line)
 
@@ -309,7 +309,7 @@ class _Runner:
             xyz, pts = (self.torch.from_numpy(np.ascontiguousarray(v)).to(self.cuda) for v in (x[..., :3], x[..., 3:]))
             if placed:                  # [:, a:a+n] slices of two wider tensors: xyz and features with their own strides
                 b, n = x.shape[:2]
-                w = self.torch.zeros((b, n + 5, 3), dtype=self.torch.float32, device=self.cuda)
+                w = self.torch.zeros((b, n + 5, xyz.shape[2]), dtype=self.torch.float32, device=self.cuda)
                 v = self.torch.zeros((b, n + 4, pts.shape[2]), dtype=self.torch.float32, device=self.cuda)
                 w[:, 2:2 + n], v[:, 1:1 + n] = xyz, pts
                 xyz, pts = w[:, 2:2 + n], v[:, 1:1 + n]
@@ -322,7 +322,8 @@ class _Runner:
             return pkg.farthest_point_sample(m, inp, out=out, idx_offset=ioff, rounds=rounds, temp=temp, **self.kw)
         if case.family == "features":
             xyz, pts = inp
-            return pkg.farthest_point_sample_features(m, xyz, pts, out=out, idx_offset=ioff, rounds=rounds, temp=temp)
+            return pkg.farthest_point_sample_features(m, xyz, pts, out=out, idx_offset=ioff, rounds=rounds, temp=temp,
+                                                      cluster=case.cluster)
         return pkg.farthest_point_sample_with_distance(m, inp, out=out, idx_offset=ioff, cluster=case.cluster)
 
     def temp(self, b, m):

@@ -5,7 +5,8 @@ This test records which kernel, cluster size, points per thread and shared memor
 query entry points answer, and the return code and message of every call the library rejects before any CUDA call.
 The table must equal tests/golden/fps_routes.json; SSD3D_RECORD_FPS_ROUTES=<file> re-records it (the library it reads
 is the one SSD3D_LIB names, if set).  The file lists every distinct outcome once, numbered, then one line per swept
-shape with the outcome of each cluster request (fps, dist) or of each channel count (features)."""
+shape with the outcome of each cluster request (fps, dist) or, per cluster request, of each channel count (features).
+Queries are swept in the order they joined the table, so a new one never renumbers the recorded outcomes."""
 import json
 import os
 import subprocess
@@ -17,6 +18,9 @@ NS = (1, 64, 300, 512, 1000, 1024, 1025, 2048, 2049, 4095, 4096, 8192, 8193, 120
 CLUSTERS = (0, 1, 2, 4, 8, 16, -1, -2, -4, -8, -16)
 ALIGNED, UNALIGNED = 16, 20                                  # never dereferenced: every call below returns before CUDA
 OUT = 16
+FEATURE_NS = tuple(sorted(NS + (3000, 4097)))
+FEATURE_CS = (2, 3, 67, 68, 69, 131, 132, 133)
+FEATURE_CLUSTERS = (0, -1, -2, -4, -8, -16)             # the requests ssd3d_farthest_point_sample_features_cl accepts
 
 
 def _queries():
@@ -33,7 +37,9 @@ def _queries():
         for cluster in CLUSTERS:
             q.append(("dist", n, cluster))
         for c in (67, 68, 69, 131, 132, 133):
-            q.append(("features", n, c))
+            q.append(("features", n, c, 0))
+    seen = set(q)
+    q += [f for n in FEATURE_NS for cl in FEATURE_CLUSTERS for c in FEATURE_CS if (f := ("features", n, c, cl)) not in seen]
     return q
 
 
@@ -67,10 +73,11 @@ def _abi(L, q, plan, messages):
         _, n, cluster = q
         return [None, call(L.ssd3d_farthest_point_sample_with_distance_ex, 1, n, 256, ALIGNED, None, OUT, 256, 0, cluster, None)
                 if kind == "fallback" else None]
-    _, n, c = q
-    args = (1, n, 3, c - 3, 256, ALIGNED, n * 3, ALIGNED, n * (c - 3), None, OUT, 256, 0)
-    part = call(L.ssd3d_farthest_point_sample_features_ex, *args, 0, 1, None)
-    full = call(L.ssd3d_farthest_point_sample_features_ex, *args, 0, 256, None) if kind == "fallback" else None
+    _, n, c, cluster = q
+    ca = min(c, 3)
+    args = (1, n, ca, c - ca, 256, ALIGNED, n * ca, ALIGNED, n * (c - ca), None, OUT, 256, 0)
+    part = call(L.ssd3d_farthest_point_sample_features_cl, *args, 0, 1, cluster, None)
+    full = call(L.ssd3d_farthest_point_sample_features_cl, *args, 0, 256, cluster, None) if kind == "fallback" else None
     return [part, full]
 
 
@@ -79,10 +86,11 @@ def test_fps_routes_match_recording(pkg, tmp_path):
     queries = _queries()
     plans = _plans(tmp_path, queries)
     messages = {}
-    rows = [list(q) + p + _abi(L, q, p, messages) for q, p in zip(queries, plans)]
+    abis = [_abi(L, q, p, messages) for q, p in zip(queries, plans)]
+    rows = [list(q) + p + a for q, p, a in zip(queries, plans, abis)]
     text = sorted(messages, key=messages.get)
     by_key = {tuple(r[:7]): r[7:] for r in rows if r[0] == "fps"}
-    feat = {(r[1], r[2]): r[3:] for r in rows if r[0] == "features"}
+    feat = {q[1:]: p + a for q, p, a in zip(queries, plans, abis) if q[0] == "features"}
     answers = []
     for n in NS:
         for c in (3, 5, 67, 131, 200):
@@ -100,18 +108,18 @@ def test_fps_routes_match_recording(pkg, tmp_path):
             answers.append(ans)
         for c in (67, 68, 69, 131, 132, 133):
             s = L.ssd3d_ffps_supported(n, c)
-            assert s == (feat[(n, c)][0] != "fallback")
+            assert s == (feat[(n, c, 0)][0] == "features")
             answers.append([n, c, s])
-    for r in rows:
-        part, full = r[-2:]
-        kind, rounds = r[-10], r[-3]
+    for q, p, (part, full) in zip(queries, plans, abis):
+        kind, rounds = p[0], p[7]
         if part is not None:
-            assert part[0] == -1 and text[part[1]], r                 # no temp: never launched
-        if r[0] == "fps":
-            assert ("resident-scene" in text[part[1]] or "c == 3" in text[part[1]]) == (not rounds), r
-        assert (full is not None) == (kind == "fallback"), r
+            assert part[0] == -1 and text[part[1]], q                 # no temp: never launched
+        if q[0] == "fps":
+            assert ("resident-scene" in text[part[1]] or "c == 3" in text[part[1]]) == (not rounds), q
+        assert (full is not None) == (kind == "fallback"), q
         if full is not None:
-            assert full[0] in (-1, -2) and text[full[1]], r
+            assert full[0] in (-1, -2) and text[full[1]], q
+    _check_features_caps(feat)
     outcomes, routes = _table(rows)
     record = os.environ.get("SSD3D_RECORD_FPS_ROUTES")
     if record:
@@ -133,6 +141,23 @@ def test_fps_routes_match_recording(pkg, tmp_path):
     assert [a for n in NS for a in exp["queries"][str(n)]] == json.loads(json.dumps(answers))
 
 
+def _check_features_caps(feat):
+    """A cap below the 8 CTAs that 2048 < n <= 4096 points of 3 <= c <= 68 channels need runs a full range on the 4-CTA
+    bucket kernel (4 slots per thread) and sends partial ranges where cluster 0 sends them; every other request plans
+    as cluster 0 does."""
+    smem = 2 * 256 * 68 * 4 + 4096 * 8 + 8 * 4 * 72 * 4 + 2 * 8 * 72 * 4 + 2 * 4 * 288
+    picked = 0
+    for (n, c, cl), got in feat.items():
+        base = feat[(n, c, 0)]
+        if cl in (-1, -2, -4) and 2048 < n <= 4096 and 3 <= c <= 68:
+            picked += 1
+            assert got[:8] == ["features_bucket", 4, 4, 68, smem, 0, base[6], 0], (n, c, cl, got)
+            assert got[8:13] == base[:5] and got[13:] == base[8:], (n, c, cl, got, base)
+        else:
+            assert got == base, (n, c, cl, got, base)
+    assert picked == 3 * 4 * 3            # cap -1 / -2 / -4, n in (2049, 3000, 4095, 4096), c in (3, 67, 68)
+
+
 def _line(v):
     return json.dumps(v, separators=(",", ":"))
 
@@ -143,16 +168,16 @@ def _table(rows):
     outcomes, index, routes = [], {}, {}
     for r in rows:
         if r[0] == "fps":
-            key, res = "fps n=%d c=%d m=%d flags=%d aligned=%d" % (r[1], r[2], r[3], r[5], r[6]), r[7:]
+            key, arg, res = "fps n=%d c=%d m=%d flags=%d aligned=%d" % (r[1], r[2], r[3], r[5], r[6]), r[4], r[7:]
         elif r[0] == "dist":
-            key, res = "dist n=%d" % r[1], r[3:]
+            key, arg, res = "dist n=%d" % r[1], r[2], r[3:]
         else:
-            key, res = "features n=%d c=67,68,69,131,132,133" % r[1], r[3:]
+            key, arg, res = "features n=%d cluster=%d c=%s" % (r[1], r[3], ",".join(map(str, FEATURE_CS))), r[2], r[4:]
         i = index.setdefault(_line(res), len(outcomes))
         if i == len(outcomes):
             outcomes.append(res)
-        routes.setdefault(key, []).append(i)
-    return outcomes, routes
+        routes.setdefault(key, {})[arg] = i
+    return outcomes, {k: [ids[a] for a in (FEATURE_CS if k.startswith("features") else CLUSTERS)] for k, ids in routes.items()}
 
 
 def _decode(outcome, messages):
