@@ -112,6 +112,9 @@ _SIGNATURES = {
     "ssd3d_peer_allreduce_mean": [c_void_p, ctypes.c_size_t, c_void_p, c_void_p, c_int, c_int, c_int] + [ctypes.c_size_t] * 10 +
                                  [c_void_p, c_void_p],
     "ssd3d_bn_moving_update_ranks": [c_void_p, c_long, c_void_p, c_long, c_int, c_float, c_void_p],
+    "ssd3d_adam_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_long, c_void_p, c_float, c_float, c_float, c_int, c_void_p,
+                        c_void_p, c_void_p],
+    "ssd3d_weight_operands": [c_void_p, c_void_p, c_int, c_long, c_void_p, c_void_p],
     "ssd3d_box_iou": [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_box_iou_matched": [c_long, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_eval_workspace": [c_long],

@@ -178,24 +178,26 @@ class TrainOutputs(NamedTuple):
     vote_base: torch.Tensor
 
 
-def train_forward(arch, tp, xyz, feat):
+def train_forward(arch, tp, xyz, feat, *, bn_decay=None):
     """The backbone loop of SABackbone.forward in training mode (SA and vote layers, batch-statistics BatchNorm) with
     params.TrainableParams, then conv1d_0 and the box-regression head of the 3DSSD head on the last layer's features
-    (single_stage_detector.py:115-125, head_builder.py:81-114).  Everything is differentiable w.r.t. tp's parameters."""
+    (single_stage_detector.py:115-125, head_builder.py:81-114).  Everything is differentiable w.r.t. tp's parameters.
+    bn_decay: the decay of every BatchNorm's moving statistics in this forward (model_forward(bn_decay),
+    trainer.py:130; solver.Solver.bn_decay gives the scheduled value); None keeps the layers' default of 0.9."""
     from . import head as _head
     xyz_l, feat_l, fps_l, offs, vote_base = [xyz], [feat], [None], [], None
     for spec in arch:
         (xyz_i, feat_i, radius, nsample, mlps, bn, rng, method, npoint, former, attn, ltype, scope, dilated, vote_idx, agg) = spec
         if ltype == "SA_Layer":
-            r = L.pointnet_sa_module_msg(xyz_l[xyz_i[0]], feat_l[feat_i[0]], radius, nsample, mlps, True, None, bn, rng, method,
+            r = L.pointnet_sa_module_msg(xyz_l[xyz_i[0]], feat_l[feat_i[0]], radius, nsample, mlps, True, bn_decay, bn, rng, method,
                                          npoint, fps_l[former] if former != -1 else None, attn, scope, dilated,
                                          xyz_l[vote_idx] if vote_idx != -1 else None, agg, params=tp)
             xyz_l.append(r[0]); feat_l.append(r[1]); fps_l.append(r[2])
         elif ltype == "Vote_Layer":
             vote_base = xyz_l[xyz_i[0]]                                 # PRED_VOTE_BASE (layer_builder.py:96)
-            nx, nf, off = L.vote_layer(vote_base, feat_l[feat_i[0]], mlps, True, None, bn, scope, params=tp)
+            nx, nf, off = L.vote_layer(vote_base, feat_l[feat_i[0]], mlps, True, bn_decay, bn, scope, params=tp)
             xyz_l.append(nx); feat_l.append(nf); fps_l.append(None); offs.append(off)
         else:
             raise ValueError("layer type %r has no training driver here" % (ltype,))
-    f = tp.conv_train("conv1d_0", feat_l[-1], True)
-    return TrainOutputs(_head.box_regression_head(f, 1, 1, 6, True, True, params=tp), offs, xyz_l[-1], vote_base)
+    f = tp.conv_train("conv1d_0", feat_l[-1], True, bn_decay)
+    return TrainOutputs(_head.box_regression_head(f, 1, 1, 6, True, True, params=tp, bn_decay=bn_decay), offs, xyz_l[-1], vote_base)

@@ -40,17 +40,17 @@ def _conv_chain(pp, hi, lo, scopes_bn_relu):
 
 
 def box_regression_head(feature_input, pred_cls_channel, pred_reg_base_num, pred_reg_channel_num, bn, is_training, *,
-                        params, scope=''):
+                        params, scope='', bn_decay=None):
     """head_util.py:26-59 without the nuScenes attribute / velocity branches.  feature_input (bs, n, c) fp32.
     Returns (pred_cls (bs,n,cls), pred_offset (bs,n,base,6), pred_angle_cls (bs,n,base,12), pred_angle_res (...)).
     is_training=True needs params as a params.TrainableParams: both conv chains then run with batch-statistics BatchNorm
-    through the differentiable tf_ops.conv_train."""
+    through the differentiable tf_ops.conv_train, their BatchNorms with moving-statistics decay bn_decay (None: 0.9)."""
     bs, n, _ = feature_input.shape
     if is_training:
         if not isinstance(params, TrainableParams):
             raise NotImplementedError("is_training=True needs params.TrainableParams (the inference forms are folded)")
-        chain = lambda base, pred: params.conv_train(_scope(scope, pred), params.conv_train(_scope(scope, base), feature_input, bn),
-                                                     False, relu=False)
+        chain = lambda base, pred: params.conv_train(_scope(scope, pred), params.conv_train(_scope(scope, base), feature_input, bn, bn_decay),
+                                                     False, bn_decay, relu=False)
         pred_cls, pred_reg = chain("pred_cls_base", "pred_cls"), chain("pred_reg_base", "pred_reg")
     else:
         pp = prepare(params, feature_input.device)

@@ -108,6 +108,36 @@ class FoldedConv:
         self.b_hi = wt.to(torch.bfloat16)                       # round-to-nearest-even, like the device split
         self.b_lo = (wt - self.b_hi.to(torch.float32)).to(torch.bfloat16)
 
+    @classmethod
+    def from_operands(cls, w, scale, shift, b_hi, b_lo):
+        """A fold whose split operand already exists (b_hi, b_lo [cout, round16(cin)], built from w elsewhere)."""
+        f = cls.__new__(cls)
+        f.w, f.scale, f.shift, f.b_hi, f.b_lo = w, scale, shift, b_hi, b_lo
+        f.cin, f.cout = w.shape
+        f.kp = round16(f.cin)
+        if tuple(b_hi.shape) != (f.cout, f.kp) or tuple(b_lo.shape) != (f.cout, f.kp):
+            raise ValueError("from_operands: operands %s / %s of a [%d, %d] weight" % (tuple(b_hi.shape), tuple(b_lo.shape), f.cin, f.cout))
+        return f
+
+
+OPERAND_TILE = 32             # csrc/solver.cu works on 32 x 32 tiles of a weight
+
+
+def operand_layout(weights):
+    """Where ssd3d_weight_operands finds and puts every conv weight.  weights: [(offset in the flat parameter buffer, cin,
+    cout)].  Returns (table, arena_elems, tiles): table int64 [nw, 8] with rows (param offset, cin, cout, fwd_hi, fwd_lo,
+    bwd_hi, bwd_lo, tile_start) -- offsets in bf16 elements of one arena, each weight's four blocks back to back: the
+    forward operand [cout, round16(cin)] hi then lo, the grad-x operand [cin, round16(cout)] hi then lo.  Every block is a
+    multiple of 16 elements, so all start on 16-byte boundaries."""
+    table = np.zeros((len(weights), 8), np.int64)
+    off = tiles = 0
+    for r, (poff, cin, cout) in enumerate(weights):
+        fwd, bwd = cout * round16(cin), cin * round16(cout)
+        table[r] = (poff, cin, cout, off, off + fwd, off + 2 * fwd, off + 2 * fwd + bwd, tiles)
+        off += 2 * fwd + 2 * bwd
+        tiles += -(-round16(cin) // OPERAND_TILE) * -(-round16(cout) // OPERAND_TILE)
+    return table, off, tiles
+
 
 def fold(params, scope, bn, device):
     """inv = gamma * rsqrt(var + eps);  y = (xW + b) * inv + (beta - mean * inv)   (tf_util.py:439-444)."""
@@ -297,6 +327,8 @@ class TrainableParams:
         self.grad_flat = self.grad_offsets = None          # flat_grads()
         self.stats_flat = self.bn_offsets = None           # flat_stats()
         self._bn_record = None                             # start_bn_record() .. finish_bn_record()
+        self.param_flat = self.param_offsets = None        # flat_params()
+        self.operand_cache = None                          # enable_operand_cache(): {scope: (forward fold, grad-x fold)}
 
     def named_parameters(self):
         return [(k, t) for k, t in self.tensors.items() if t.requires_grad]
@@ -324,8 +356,65 @@ class TrainableParams:
         moving, stats_out = (g("/bn/moving_mean"), g("/bn/moving_variance")), None
         if bn and self._bn_record is not None:
             stats_out, moving = self._record_slot(scope, decay), (None, None)
+        extra = {} if self.operand_cache is None else {"operands": self.operand_cache[scope]}
         return tf_ops.conv_train(x, t[scope + "/weights"], b, g("/bn/gamma"), g("/bn/beta"), moving[0], moving[1], bn=bn, relu=relu,
-                                 decay=decay, debug=debug, stats_out=stats_out)
+                                 decay=decay, debug=debug, stats_out=stats_out, **extra)
+
+    # ---- the solver (solver.Adam): both capabilities are opt-in; unused, nothing above changes ------------------------
+    def flat_params(self):
+        """Move every trainable tensor into ONE flat float32 buffer (param_flat; param_offsets[name] = its first element,
+        the offsets of flat_grads): the tensors stay autograd leaves and become views of it, so one kernel can update all
+        of them.  Returns param_flat."""
+        if self.param_flat is None:
+            named = self.named_parameters()
+            flat = torch.empty((sum(t.numel() for _, t in named),), dtype=torch.float32, device=self.device)
+            self.param_offsets, off = {}, 0
+            for k, t in named:
+                view = flat[off:off + t.numel()].view(t.shape)
+                view.copy_(t.detach())
+                t.data = view
+                self.param_offsets[k] = off
+                off += t.numel()
+            self.param_flat = flat
+        return self.param_flat
+
+    def weight_scopes(self):
+        return [k[: -len("/weights")] for k, _ in self.named_parameters() if k.endswith("/weights")]
+
+    def enable_operand_cache(self):
+        """Keep the split tensor-core operands of every conv weight in one bf16 arena (operand_layout) and hand them to
+        conv_train instead of rebuilding them in every forward and backward.  The cache holds what refresh_operands() last
+        built: it is valid from then until the next write to a weight, so whatever writes weights calls refresh_operands()
+        (solver.Adam.step does).  The biases are read live (shift is a view of them)."""
+        if self.operand_cache is not None:
+            return
+        self.flat_params()
+        scopes = self.weight_scopes()
+        shapes = [tuple(self.tensors[s + "/weights"].shape) for s in scopes]
+        table, elems, self._operand_tiles = operand_layout([(self.param_offsets[s + "/weights"], ci, co)
+                                                            for s, (ci, co) in zip(scopes, shapes)])
+        self._operand_table = torch.from_numpy(table).to(self.device)
+        self.operand_arena = torch.zeros((elems,), dtype=torch.bfloat16, device=self.device)
+        width = max(max(sh) for sh in shapes)
+        ones = torch.ones((width,), dtype=torch.float32, device=self.device)
+        zeros = torch.zeros((width,), dtype=torch.float32, device=self.device)
+        cache = {}
+        for s, (ci, co), row in zip(scopes, shapes, table.tolist()):
+            w = self.tensors[s + "/weights"].detach()
+            b = self.tensors.get(s + "/biases")
+            blk = lambda o, r, c: self.operand_arena[o:o + r * c].view(r, c)
+            fwd = FoldedConv.from_operands(w, ones[:co], zeros[:co] if b is None else b.detach(),
+                                           blk(row[3], co, round16(ci)), blk(row[4], co, round16(ci)))
+            bwd = FoldedConv.from_operands(w.t(), ones[:ci], zeros[:ci], blk(row[5], ci, round16(co)), blk(row[6], ci, round16(co)))
+            cache[s] = (fwd, bwd)
+        self.operand_cache = cache
+        self.refresh_operands()
+
+    def refresh_operands(self):
+        """Rebuild the operand cache from the current weights (one launch); nothing to do when the cache is not enabled."""
+        if self.operand_cache is not None:
+            from . import tf_ops
+            tf_ops.weight_operands(self.param_flat, self._operand_table, self._operand_tiles, self.operand_arena)
 
     # ---- data-parallel training (dist.DataParallel): both capabilities are opt-in; unused, nothing above changes -----
     def flat_grads(self):

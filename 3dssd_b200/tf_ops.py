@@ -984,6 +984,45 @@ def bn_moving_update_ranks(stats, batch, world, decay):
     return stats
 
 
+# ---- the solver: Adam and the weight operands (csrc/solver.cu, DESIGN.md section 3.11) -------------------------------
+
+ADAM_STATE_INTS = 8           # the 32-byte state block as int32: [0:2] global_step, [2:5] float bits, [5] block counter
+
+
+def adam_step(param, grad, m, v, state, boundaries, values, beta1=0.9, beta2=0.999, epsilon=1e-8):
+    """One Adam step of the flat float32 buffers param / m / v (in place) from grad, in one launch (include/ssd3d.h,
+    ssd3d_adam_step).  state: int32 CUDA [8], the device state block { global_step, beta1_power, beta2_power, lr_used };
+    boundaries (<= 8 increasing ints) and values (one more float) are the piecewise-constant learning-rate schedule, read
+    with the step before the increment."""
+    bufs = [_req(t, name, torch.float32, 1, copy=False) for name, t in (("param", param), ("grad", grad), ("m", m), ("v", v))]
+    state = _req(state, "state", torch.int32, 1, copy=False)
+    n = bufs[0].numel()
+    if n == 0 or any(t.numel() != n for t in bufs) or state.numel() < ADAM_STATE_INTS:
+        raise ValueError("adam_step: param, grad, m, v must hold the same n > 0 floats and state %d int32" % ADAM_STATE_INTS)
+    if any(t.data_ptr() % 16 for t in bufs) or state.data_ptr() % 8:
+        raise ValueError("adam_step: param, grad, m, v must be 16-byte and state 8-byte aligned")
+    nb = len(boundaries)
+    if nb > 8 or len(values) != nb + 1:
+        raise ValueError("adam_step: %d boundaries (at most 8) need %d values, got %d" % (nb, nb + 1, len(values)))
+    bd = (ctypes.c_longlong * max(nb, 1))(*[int(b) for b in boundaries])
+    vals = (ctypes.c_float * (nb + 1))(*[float(x) for x in values])
+    check(lib().ssd3d_adam_step(*[_p(t) for t in bufs], n, _p(state), float(beta1), float(beta2), float(epsilon), nb,
+                                ctypes.cast(bd, ctypes.c_void_p), ctypes.cast(vals, ctypes.c_void_p), _stream()), "adam_step")
+    return param
+
+
+def weight_operands(param, table, tiles, arena):
+    """Rebuild the split-bf16 operands of every conv weight from the flat parameter buffer in one launch (include/ssd3d.h,
+    ssd3d_weight_operands).  table: int64 CUDA [nw, 8] and tiles as laid out by params.operand_layout; arena: bfloat16."""
+    param = _req(param, "param", torch.float32, 1, copy=False)
+    table = _req(table, "table", torch.int64, 2, last=8, copy=False)
+    arena = _req(arena, "arena", torch.bfloat16, 1, copy=False)
+    if table.shape[0] == 0 or arena.data_ptr() % 16:
+        raise ValueError("weight_operands: the table must have rows and the arena be 16-byte aligned")
+    check(lib().ssd3d_weight_operands(_p(param), _p(table), table.shape[0], int(tiles), _p(arena), _stream()), "weight_operands")
+    return arena
+
+
 def split_points(points):
     """(b, n, 3 + c) -> xyz (b, n, 3), features (b, n, c): single_stage_detector.py:116-117."""
     points = _req(points, "points", torch.float32, 3)
@@ -1208,17 +1247,24 @@ def linear_bn_train(x, f, gamma=None, beta=None, moving_mean=None, moving_var=No
 class _ConvTrain(torch.autograd.Function):
     """conv (+bias) -> [training BatchNorm] -> [ReLU] of one layer (tf_util.conv2d / conv1d with is_training=True).
     Forward: linear_bn_train with a fold of the live weights, the sequence of the non-trainable training path.
-    Backward: bn_train_grad -> split -> linear_tc with W^T (grad_x) and linear_wgrad (grad_w, grad_b)."""
+    Backward: bn_train_grad -> split -> linear_tc with W^T (grad_x) and linear_wgrad (grad_w, grad_b).
+    opts may end with operands = (forward fold, grad-x fold) prebuilt from the same weights (params.TrainableParams'
+    operand cache): they are then used instead of building both folds here."""
 
     @staticmethod
     def forward(ctx, x, w, b, gamma, beta, opts):
-        bn, relu, decay, moving, debug, stats_out = opts
+        bn, relu, decay, moving, debug, stats_out = opts[:6]
+        operands = opts[6] if len(opts) > 6 else None
         x = x if x.is_contiguous() else x.contiguous()
-        ones = torch.ones((w.shape[1],), dtype=torch.float32, device=x.device)
-        y, r = linear_bn_train(x, FoldedConv(w.detach(), ones, b.detach()), gamma.detach(), beta.detach(), moving[0], moving[1],
+        if operands is None:
+            f = FoldedConv(w.detach(), torch.ones((w.shape[1],), dtype=torch.float32, device=x.device), b.detach())
+        else:
+            f = operands[0]
+        y, r = linear_bn_train(x, f, gamma.detach(), beta.detach(), moving[0], moving[1],
                                bn=bn, relu=relu, decay=decay, stats_out=stats_out)
         out = r[0]
         ctx.bn, ctx.relu = bn, relu
+        ctx.wt = None if operands is None else operands[1]
         if bn:
             ctx.save_for_backward(x, w, y, *r[1:], gamma)       # scale, shift, batch_mean, batch_var
         else:
@@ -1243,19 +1289,23 @@ class _ConvTrain(torch.autograd.Function):
         gx = None
         if ctx.needs_input_grad[0]:
             d_hi, d_lo = split_rows(dz)
-            wt = FoldedConv(w.detach().t().contiguous(), torch.ones((cin,), dtype=torch.float32, device=dz.device),
-                         torch.zeros((cin,), dtype=torch.float32, device=dz.device))
+            wt = ctx.wt
+            if wt is None:
+                wt = FoldedConv(w.detach().t().contiguous(), torch.ones((cin,), dtype=torch.float32, device=dz.device),
+                                torch.zeros((cin,), dtype=torch.float32, device=dz.device))
             gx, _ = linear_tc(d_hi, d_lo, wt, relu=False, want_f32=True, want_split=False)
         gw, gb = linear_wgrad(x, dz, want_bias=True)
         return gx, gw, gb, ggamma, gbeta, None
 
 
 def conv_train(x, w, b, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9, debug=None,
-               stats_out=None):
+               stats_out=None, operands=None):
     """Differentiable conv (+bias) -> training BatchNorm (bn=True; updates moving_mean / moving_var in place) -> ReLU of
     one layer over the last axis of x, with the forward bits of the non-trainable training path.  x (..., cin),
     w (cin, cout), b / gamma / beta (cout,).  debug: a list that receives (pre-BN conv output, layer output).
-    stats_out: optional (mean, var) [cout] that receive the batch statistics (bn=True; kept for the backward)."""
+    stats_out: optional (mean, var) [cout] that receive the batch statistics (bn=True; kept for the backward).
+    operands: optional (forward fold of w with scale 1 and shift b, grad-x fold of w^T with scale 1 and shift 0), current
+    for w -- the caller's promise; both are otherwise built here on every call."""
     if not isinstance(x, torch.Tensor) or x.dtype != torch.float32:     # the device is checked by the kernels' wrappers
         raise ValueError("x must be a float32 tensor")
     if w.dim() != 2 or x.shape[-1] != w.shape[0] or tuple(b.shape) != (w.shape[1],):
@@ -1264,7 +1314,7 @@ def conv_train(x, w, b, gamma=None, beta=None, moving_mean=None, moving_var=None
         raise ValueError("conv_train: bn=True needs gamma and beta")
     z = torch.zeros((0,), dtype=torch.float32, device=x.device)
     return _ConvTrain.apply(x, w, b, gamma if bn else z, beta if bn else z,
-                            (bool(bn), bool(relu), float(decay), (moving_mean, moving_var), debug, stats_out))
+                            (bool(bn), bool(relu), float(decay), (moving_mean, moving_var), debug, stats_out, operands))
 
 
 class _GroupMax(torch.autograd.Function):

@@ -494,6 +494,33 @@ int ssd3d_peer_allreduce_mean(float *grad, size_t n, const float *scale, void *c
 int ssd3d_bn_moving_update_ranks(float *stats, long n, const float *batch, long ld_batch, int world, float decay,
                                  ssd3d_stream_t stream);
 
+/* ---- the solver: Adam and the weight operands (csrc/solver.cu, DESIGN.md section 3.11) ------------------------------
+ * The update of tf.train.AdamOptimizer (lib/core/trainer.py:74-75) under the learning-rate schedule of
+ * tf.train.piecewise_constant (lib/core/trainer_utils.py:7-13), with every float32 operation rounded once.  Neither
+ * entry allocates, uses float atomics or synchronises the host; both are CUDA-graph capturable. */
+
+/* One Adam step over flat buffers param, m, v (updated in place) and grad [n], all 16-byte aligned, in ONE launch.
+ * state: the caller's 32-byte, 8-byte aligned device block { int64 global_step; float beta1_power; float beta2_power;
+ * float lr_used; uint32 done; uint32 reserved[2] }, initialised to { 0, beta1, beta2, 0, 0, 0, 0 }; `done` is the
+ * launch's own block counter and is 0 between launches.  boundaries [nb] (increasing, nb <= 8) and values [nb + 1] are
+ * HOST arrays copied into the launch.  With the state as it was BEFORE the launch:
+ *   lr    = values[k], k = number of boundaries < global_step   (values[0] while global_step <= boundaries[0])
+ *   alpha = rn(rn(lr * rn(sqrt(rn(1 - beta2_power)))) / rn(1 - beta1_power))
+ *   m = rn(m + rn(rn(g - m) * rn(1 - beta1)));  v = rn(v + rn(rn(rn(g * g) - v) * rn(1 - beta2)))
+ *   param = rn(param - rn(rn(m * alpha) / rn(rn(sqrt(v)) + epsilon)))
+ * and, once every element is done: beta1_power = rn(beta1_power * beta1), beta2_power likewise, global_step += 1,
+ * lr_used = lr.  Non-finite gradients propagate. */
+int ssd3d_adam_step(float *param, const float *grad, float *m, float *v, long n, void *state, float beta1, float beta2,
+                    float epsilon, int nb, const long long *boundaries, const float *values, ssd3d_stream_t stream);
+/* The split-bf16 tensor-core operands of nw conv weights, rebuilt from the flat parameter buffer in ONE launch.
+ * table: DEVICE int64 [nw][8], row = { offset of W [cin, cout] in param (floats), cin, cout, then offsets in arena (bf16
+ * elements, multiples of 8) of fwd_hi, fwd_lo [cout, round16(cin)] = split of W^T and of bwd_hi, bwd_lo
+ * [cin, round16(cout)] = split of W, then tile_start }.  hi = bf16_rne(w), lo = bf16_rne(w - float(hi)); padding
+ * columns are +0.  A weight takes ceil(round16(cin) / 32) * ceil(round16(cout) / 32) tiles; tile_start is the running
+ * sum over the rows before it and `tiles` the total.  arena: 16-byte aligned. */
+int ssd3d_weight_operands(const float *param, const long long *table, int nw, long tiles, void *arena,
+                          ssd3d_stream_t stream);
+
 /* ---- KITTI evaluation (csrc/box_eval.cu, DESIGN.md section 3.10; evaluation/evaluate.cpp, tf_evaluate.cpp) ----------
  * Boxes are (x, y, z, l, h, w, ry), camera frame, origin at the bottom-face centre.  Overlaps are computed in double by
  * the recipe of DESIGN.md section 3.10; a pair whose union area or volume is <= 0 has overlap 0.
