@@ -14,7 +14,7 @@
 // one recipe (Cody-Waite reduction by pi/2, fdlibm's minimax polynomials with explicit fma), because CUDA's sincos and
 // glibc's differ in the last bit on some inputs; corners rn(rn(rn(c*a) + rn(s*b)) + t) from |l|/2 and |w|/2;
 // Sutherland-Hodgman clipping of the detection rectangle by the label rectangle, then a shoelace area in vertex order.
-#include "common.cuh"
+#include "box_geom.cuh"
 
 namespace ssd3d {
 
@@ -26,44 +26,6 @@ constexpr int EVAL_NSAMPLE = 41;         // N_SAMPLE_PTS (evaluate.cpp:55)
 constexpr int CLIP_MAXV = 16;
 
 enum { T_CAR = 0, T_PED = 1, T_CYC = 2, T_VAN = 3, T_SIT = 4, T_DONTCARE = 5 };
-
-// ---- sincos ----------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ double k_sin(double r)
-{
-    const double z = __dmul_rn(r, r);
-    double p = __fma_rn(z, 1.58969099521155010221e-10, -2.50507602534068634195e-08);
-    p = __fma_rn(z, p, 2.75573137070700676789e-06);
-    p = __fma_rn(z, p, -1.98412698298579493134e-04);
-    p = __fma_rn(z, p, 8.33333333332248946124e-03);
-    p = __fma_rn(z, p, -1.66666666666666324348e-01);
-    return __fma_rn(__dmul_rn(r, z), p, r);
-}
-
-__device__ __forceinline__ double k_cos(double r)
-{
-    const double z = __dmul_rn(r, r);
-    double p = __fma_rn(z, -1.13596475577881948265e-11, 2.08757232129817482790e-09);
-    p = __fma_rn(z, p, -2.75573143513906633035e-07);
-    p = __fma_rn(z, p, 2.48015872894767294178e-05);
-    p = __fma_rn(z, p, -1.38888888888741095749e-03);
-    p = __fma_rn(z, p, 4.16666666666666019037e-02);
-    const double hz = __dmul_rn(0.5, z), w = __dsub_rn(1.0, hz);
-    return __dadd_rn(w, __fma_rn(z, __dmul_rn(z, p), __dsub_rn(__dsub_rn(1.0, w), hz)));
-}
-
-__device__ __forceinline__ void eval_sincos(double x, double &s, double &c)
-{
-    const double n = rint(__dmul_rn(x, 0x1.45f306dc9c883p-1));          // x * 2/pi, to the nearest integer
-    double r = __fma_rn(-n, 0x1.921fb54442d18p+0, x);                   // x - n * pi/2, pi/2 in two parts
-    r = __fma_rn(-n, 0x1.1a62633145c07p-54, r);
-    const double sr = k_sin(r), cr = k_cos(r);
-    switch (((long long)n) & 3) {
-        case 0: s = sr; c = cr; break;
-        case 1: s = cr; c = -sr; break;
-        case 2: s = -sr; c = -cr; break;
-        default: s = -cr; c = sr; break;
-    }
-}
 
 // ---- rotated rectangles --------------------------------------------------------------------------------------------
 // Corners as toPolygon builds them (evaluate.cpp:461-485): (l/2, w/2), (l/2, -w/2), (-l/2, -w/2), (-l/2, w/2) turned by

@@ -10,7 +10,7 @@
 // No float atomics anywhere: every run gives the same bits.
 #include <math.h>
 
-#include "common.cuh"
+#include "box_geom.cuh"
 
 namespace ssd3d {
 
@@ -20,58 +20,6 @@ constexpr int kMaxBins = 32;
 constexpr float kExpand = 0.1f;       // TRAIN.AUGMENTATIONS.EXPAND_DIMS_LENGTH (lib/core/config.py:84)
 constexpr float kSampleRange = 10.0f; // CLASSIFICATION_LOSS.SOFTMAX_SAMPLE_RANGE (configs/kitti/3dssd/3dssd.yaml:80)
 constexpr double kCtrEps = 1e-6;      // epsilon of _generate_centerness_label (loss_builder.py:99)
-
-// The six face planes of a box in the frame check_inside_points uses (voxelnet_aug.py:318-342): point (x, z, y),
-// box (x, z, y, l, w, h, ry), corners of center_to_corner_box3d(origin (0.5, 0.5, 1), axis 2), surfaces of
-// corner_to_surfaces_3d_jit, plane (n, d) of surface_equ_3d_jit.  Every operation is one IEEE float32 op (no FMA
-// contraction) in a fixed order, so that a numpy restatement gives the same bits.
-struct Planes {
-    float n[6][3];
-    float d[6];
-};
-
-__device__ __forceinline__ void box_planes(const float *bx, float expand, float sn, float cs, Planes &P)
-{
-    const float c0 = bx[0], c1 = bx[2], c2 = bx[1];                          // centre in (x, z, y)
-    const float dl = __fadd_rn(bx[3], expand), dw = __fadd_rn(bx[5], expand), dh = __fadd_rn(bx[4], expand);
-    // corners_nd after its [0, 1, 3, 2, 4, 5, 7, 6] reordering, minus the origin (0.5, 0.5, 1.0)
-    const float na[8] = {-0.5f, -0.5f, -0.5f, -0.5f, 0.5f, 0.5f, 0.5f, 0.5f};
-    const float nb[8] = {-0.5f, -0.5f, 0.5f, 0.5f, -0.5f, -0.5f, 0.5f, 0.5f};
-    const float nc[8] = {-1.0f, 0.0f, 0.0f, -1.0f, -1.0f, 0.0f, 0.0f, -1.0f};
-    float C[8][3];
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-        const float p0 = __fmul_rn(dl, na[k]), p1 = __fmul_rn(dw, nb[k]), p2 = __fmul_rn(dh, nc[k]);
-        // rotation_3d_in_axis(axis=2): [p0, p1] @ [[cos, -sin], [sin, cos]]
-        C[k][0] = __fadd_rn(__fadd_rn(__fmul_rn(p0, cs), __fmul_rn(p1, sn)), c0);
-        C[k][1] = __fadd_rn(__fsub_rn(__fmul_rn(p1, cs), __fmul_rn(p0, sn)), c1);
-        C[k][2] = __fadd_rn(p2, c2);
-    }
-    const int F[6][3] = {{0, 1, 2}, {7, 6, 5}, {0, 3, 7}, {1, 5, 6}, {0, 4, 5}, {3, 2, 6}};   // first 3 corners per face
-#pragma unroll
-    for (int f = 0; f < 6; f++) {
-        const float *a = C[F[f][0]], *b = C[F[f][1]], *c = C[F[f][2]];
-        const float u0 = __fsub_rn(a[0], b[0]), u1 = __fsub_rn(a[1], b[1]), u2 = __fsub_rn(a[2], b[2]);
-        const float v0 = __fsub_rn(b[0], c[0]), v1 = __fsub_rn(b[1], c[1]), v2 = __fsub_rn(b[2], c[2]);
-        const float n0 = __fsub_rn(__fmul_rn(u1, v2), __fmul_rn(u2, v1));
-        const float n1 = __fsub_rn(__fmul_rn(u2, v0), __fmul_rn(u0, v2));
-        const float n2 = __fsub_rn(__fmul_rn(u0, v1), __fmul_rn(u1, v0));
-        P.n[f][0] = n0; P.n[f][1] = n1; P.n[f][2] = n2;
-        P.d[f] = -__fadd_rn(__fadd_rn(__fmul_rn(n0, a[0]), __fmul_rn(n1, a[1])), __fmul_rn(n2, a[2]));
-    }
-}
-
-// points_in_convex_polygon_3d_jit (voxelnet_aug.py:532-567): outside as soon as one face gives sign >= 0
-__device__ __forceinline__ bool inside(const Planes &P, float q0, float q1, float q2)
-{
-#pragma unroll
-    for (int f = 0; f < 6; f++) {
-        const float s = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q0, P.n[f][0]), __fmul_rn(q1, P.n[f][1])), __fmul_rn(q2, P.n[f][2])),
-                                  P.d[f]);
-        if (s >= 0.0f) return false;
-    }
-    return true;
-}
 
 // encode_angle2class_tf (anchor_encoder.py:21-33) in float32, tf.mod / np.mod being a floor-mod
 __device__ __forceinline__ float floor_mod(float a, float b)

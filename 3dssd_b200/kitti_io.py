@@ -198,3 +198,27 @@ def make_label_batch(samples):
         out_b[i, :len(b)] = b
         out_c[i, :len(c)] = c
     return out_b, out_c
+
+
+KEY_LABEL_SEM_SEG = "label_sem_seg"
+
+
+def make_ragged_batch(samples, pin=True):
+    """The full clouds of a batch of frames for the augmentor (augment.Augmentor), in host buffers (pinned when a GPU is
+    present): (points [T, 4] fp32 packed frame after frame, offsets [B + 1] int32, semantic labels [T] int32 or None when
+    a frame has none, gt_boxes [B, G, 7] fp32, gt_labels [B, G] int32 padded as make_label_batch pads them)."""
+    import torch
+    clouds = [np.asarray(s[KEY_POINT_CLOUD], np.float32).reshape(-1, 4) for s in samples]
+    offsets = np.zeros(len(clouds) + 1, np.int32)
+    offsets[1:] = np.cumsum([len(c) for c in clouds])
+    sem = None
+    if samples and all(KEY_LABEL_SEM_SEG in s for s in samples):
+        sem = np.concatenate([np.asarray(s[KEY_LABEL_SEM_SEG]).reshape(-1).astype(np.int32) for s in samples])
+        if len(sem) != offsets[-1]:
+            raise ValueError("label_sem_seg holds %d labels for %d points" % (len(sem), offsets[-1]))
+    boxes, labels = make_label_batch(samples)
+    out = [torch.from_numpy(np.concatenate(clouds, 0) if clouds else np.zeros((0, 4), np.float32)), torch.from_numpy(offsets),
+           None if sem is None else torch.from_numpy(sem), torch.from_numpy(boxes), torch.from_numpy(labels)]
+    if pin and torch.cuda.is_available():
+        out = [t if t is None else t.pin_memory() for t in out]
+    return tuple(out)

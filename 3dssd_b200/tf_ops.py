@@ -1490,3 +1490,107 @@ class _DetLoss(torch.autograd.Function):
 def det_loss_train(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins=12):
     """Differentiable det_loss -> loss (6,); gradients reach base_xyz, the four head outputs and vote_offset."""
     return _DetLoss.apply(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, int(angle_bins))
+
+
+# ---- training-scene augmentation (csrc/augment.cu, DESIGN.md section 3.12) -------------------------------------------
+AUG_TRIES = 100               # noise tries per box
+AUG_MAX_BOXES = 256           # GT rows per scene
+AUG_MAX_POINTS = 131072       # points per scene
+AUG_MAX_CHOOSE = 16384        # points chosen per scene (sorted in shared memory)
+
+
+def _aug_ragged(points, offsets, max_n):
+    """points [T, 4] float32 and device offsets [b + 1] int32 of ragged scenes whose largest holds max_n points."""
+    points = _req(points, "points", torch.float32, 2, 4)
+    offsets = _req(offsets, "offsets", torch.int32, 1)
+    if offsets.shape[0] < 2:
+        raise ValueError("offsets must hold b + 1 >= 2 entries, got %d" % offsets.shape[0])
+    if not 1 <= int(max_n) <= AUG_MAX_POINTS:
+        raise ValueError("a scene must hold 1 .. %d points, got max_n=%d" % (AUG_MAX_POINTS, max_n))
+    return points, offsets, offsets.shape[0] - 1
+
+
+def _aug_boxes_in(gt_boxes, b=None):
+    gt_boxes = _req(gt_boxes, "gt_boxes", torch.float32, 3, 7)
+    if b is not None and gt_boxes.shape[0] != b:
+        raise ValueError("gt_boxes %s does not hold %d scenes" % (tuple(gt_boxes.shape), b))
+    if gt_boxes.shape[1] > AUG_MAX_BOXES:
+        raise ValueError("at most %d GT rows per scene, got %d" % (AUG_MAX_BOXES, gt_boxes.shape[1]))
+    return gt_boxes
+
+
+def augment_sem_labels(points, offsets, gt_boxes, gt_labels, max_n):
+    """Semantic labels of ragged scenes (ssd3d_augment_sem_labels) -> [T] int32: the class of the first valid box grown by
+    0.1 that holds the point, else 0."""
+    points, offsets, b = _aug_ragged(points, offsets, max_n)
+    gt_boxes = _aug_boxes_in(gt_boxes, b)
+    gt_labels = _req(gt_labels, "gt_labels", torch.int32, 2)
+    if tuple(gt_labels.shape) != tuple(gt_boxes.shape[:2]):
+        raise ValueError("gt_labels %s does not match gt_boxes %s" % (tuple(gt_labels.shape), tuple(gt_boxes.shape)))
+    sem = torch.empty((points.shape[0],), dtype=torch.int32, device=points.device)
+    check(lib().ssd3d_augment_sem_labels(b, gt_boxes.shape[1], int(max_n), _p(points), _p(offsets), _p(gt_boxes), _p(gt_labels),
+                                         _p(sem), _stream()), "augment_sem_labels")
+    return sem
+
+
+def augment_boxes(gt_boxes, scene_u, loc_noise, rot_u):
+    """Flip, per-object noise, global rotation and scale of the boxes (ssd3d_augment_boxes) -> (boxes [b, g, 7], chosen
+    try [b, g] int32, -1 for none, workspace uint8 for augment_points)."""
+    gt_boxes = _aug_boxes_in(gt_boxes)
+    b, g = gt_boxes.shape[:2]
+    scene_u = _req(scene_u, "scene_u", torch.float64, 2, 6)
+    loc_noise = _req(loc_noise, "loc_noise", torch.float64, 4, 2)
+    rot_u = _req(rot_u, "rot_u", torch.float64, 3)
+    if scene_u.shape[0] != b or tuple(loc_noise.shape[:3]) != (b, g, AUG_TRIES) or tuple(rot_u.shape) != (b, g, AUG_TRIES):
+        raise ValueError("draws scene_u %s, loc_noise %s, rot_u %s do not match gt_boxes %s" % (
+            tuple(scene_u.shape), tuple(loc_noise.shape), tuple(rot_u.shape), tuple(gt_boxes.shape)))
+    dev = gt_boxes.device
+    out = torch.empty((b, g, 7), dtype=torch.float32, device=dev)
+    chosen = torch.empty((b, g), dtype=torch.int32, device=dev)
+    ws = torch.empty((int(lib().ssd3d_augment_workspace(b, g)),), dtype=torch.uint8, device=dev)
+    check(lib().ssd3d_augment_boxes(b, g, _p(gt_boxes), _p(scene_u), _p(loc_noise), _p(rot_u), _p(out), _p(chosen), _p(ws),
+                                    _stream()), "augment_boxes")
+    return out, chosen, ws
+
+
+def augment_points(points, offsets, max_n, sem_labels, keys, workspace, g, want_moved=False):
+    """Flip, noise move, global transform and context filter of the points (ssd3d_augment_points) with the workspace of
+    augment_boxes for g GT rows -> (points [T, 4], sort keys [T] int64 (-1: dropped), survivors [b] int32, the box
+    that moved each point [T] int32 (-1: none) when want_moved else None)."""
+    points, offsets, b = _aug_ragged(points, offsets, max_n)
+    t = points.shape[0]
+    sem_labels = _req(sem_labels, "sem_labels", torch.int32, 1)
+    keys = _req(keys, "keys", torch.int32, 1)
+    workspace = _req(workspace, "workspace", torch.uint8, 1, copy=False)
+    if sem_labels.shape[0] != t or keys.shape[0] != t:
+        raise ValueError("sem_labels %s and keys %s must hold one entry per point (%d)" % (
+            tuple(sem_labels.shape), tuple(keys.shape), t))
+    if not 0 <= int(g) <= AUG_MAX_BOXES or workspace.numel() < int(lib().ssd3d_augment_workspace(b, int(g))):
+        raise ValueError("workspace does not come from augment_boxes of %d scenes x %d rows" % (b, g))
+    dev = points.device
+    out = torch.empty((t, 4), dtype=torch.float32, device=dev)
+    sort_keys = torch.empty((t,), dtype=torch.int64, device=dev)
+    survivors = torch.empty((b,), dtype=torch.int32, device=dev)
+    moved = torch.empty((t,), dtype=torch.int32, device=dev) if want_moved else None
+    check(lib().ssd3d_augment_points(b, int(g), int(max_n), _p(points), _p(offsets), _p(sem_labels), _p(keys), _p(workspace),
+                                     _p(out), _p(sort_keys), _p(survivors), _p(moved), _stream()), "augment_points")
+    return out, sort_keys, survivors, moved
+
+
+def augment_choose(points, offsets, sort_keys, survivors, refill):
+    """The point choice (ssd3d_augment_choose) -> [b, num_points, 4], num_points = refill.shape[1]."""
+    points = _req(points, "points", torch.float32, 2, 4)
+    offsets = _req(offsets, "offsets", torch.int32, 1)
+    sort_keys = _req(sort_keys, "sort_keys", torch.int64, 1)
+    survivors = _req(survivors, "survivors", torch.int32, 1)
+    refill = _req(refill, "refill", torch.int32, 2)
+    b, m = refill.shape
+    if offsets.shape[0] != b + 1 or survivors.shape[0] != b or sort_keys.shape[0] != points.shape[0]:
+        raise ValueError("augment_choose: offsets %s, survivors %s, sort_keys %s, points %s, refill %s disagree" % (
+            tuple(offsets.shape), tuple(survivors.shape), tuple(sort_keys.shape), tuple(points.shape), tuple(refill.shape)))
+    if not 1 <= m <= AUG_MAX_CHOOSE:
+        raise ValueError("num_points must be 1 .. %d, got %d" % (AUG_MAX_CHOOSE, m))
+    out = torch.empty((b, m, 4), dtype=torch.float32, device=points.device)
+    check(lib().ssd3d_augment_choose(b, m, _p(points), _p(offsets), _p(sort_keys), _p(survivors), _p(refill), _p(out), _stream()),
+          "augment_choose")
+    return out

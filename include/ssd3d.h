@@ -551,6 +551,34 @@ int ssd3d_eval_count(int frames, int max_dets, int max_labels, const float *dets
                      const double *labels, const int *label_off, const long *pair_off, const void *workspace,
                      const double *thresholds, const int *n_thresholds, int *counts, ssd3d_stream_t stream);
 
+/* ---- training-scene augmentation (csrc/augment.cu, DESIGN.md section 3.12) -----------------------------------------
+ * DataAugmentor.kitti_forward of 3dssd.yaml after the mixup paste (flip, per-object noise, global rotation and scale,
+ * the context filter) and the point choice of kitti_dataloader.py:137-147, on ragged scenes: points [T, 4] (x, y, z,
+ * intensity) with scene s at rows offsets[s] .. offsets[s+1]-1 (DEVICE int32 [b+1]), gt_boxes [b, g, 7] (x, y, z, l, h, w,
+ * ry) zero-padded, gt_labels [b, g].  Limits: g <= 256, 1 <= points per scene <= max_n <= 131072, num_points <= 16384.
+ * Every random number comes from the draw block: scene_u [b, 6] (flip, c0, c1, c2, rotation, scale), loc_noise
+ * [b, g, 100, 2] standard normals (x, z), rot_u [b, g, 100] uniforms, keys [T] and refill [b, num_points] uint32.  The
+ * same draws give the same bits; nothing synchronises the host.  Workspace: ssd3d_augment_workspace(b, g) bytes,
+ * 256-byte aligned, written by ssd3d_augment_boxes and read by ssd3d_augment_points. */
+size_t ssd3d_augment_workspace(int b, int g);
+/* sem_labels [T] = class of the first valid box grown by 0.1 that holds the point, else 0 (kitti_dataloader.py:211-219). */
+int ssd3d_augment_sem_labels(int b, int g, int max_n, const float *points, const int *offsets, const float *gt_boxes,
+                             const int *gt_labels, int *sem_labels, ssd3d_stream_t stream);
+/* Flip, noise search, box transforms, global rotation and scale, context-filter dims: out_boxes [b, g, 7];
+ * chosen_try [b, g] = the try a box took, -1 when all 100 collided (the box keeps the identity transform) or padded. */
+int ssd3d_augment_boxes(int b, int g, const float *gt_boxes, const double *scene_u, const double *loc_noise,
+                        const double *rot_u, float *out_boxes, int *chosen_try, void *workspace, ssd3d_stream_t stream);
+/* out_points [T, 4] transformed; sort_keys [T] = keys << 32 | index in the scene for a survivor of the context filter,
+ * all ones for a dropped point; survivors [b] counts (cleared here); moved_by [T] (may be NULL) = the box that moved the
+ * point or -1.  sem_labels are >= 0. */
+int ssd3d_augment_points(int b, int g, int max_n, const float *points, const int *offsets, const int *sem_labels,
+                         const unsigned *keys, const void *workspace, float *out_points, unsigned long long *sort_keys,
+                         int *survivors, int *moved_by, ssd3d_stream_t stream);
+/* out [b, num_points, 4]: with N = survivors[s], the min(N, num_points) survivors of smallest sort key in key order, then
+ * for slot t >= N the survivor at rank (refill[s, t] * N) >> 32.  A scene without survivors gets zeros. */
+int ssd3d_augment_choose(int b, int num_points, const float *points, const int *offsets, const unsigned long long *sort_keys,
+                         const int *survivors, const unsigned *refill, float *out, ssd3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

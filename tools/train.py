@@ -1,14 +1,18 @@
 """Train the 3DSSD backbone + head with the reference's solver (solver.Trainer: scheduled BatchNorm decay, detection
 loss, per-rank clip, rank-ordered gradient mean, TF-style Adam under the step-driven learning rate; DESIGN.md 3.11).
 
-    python tools/train.py --steps N [--batch 4] [--gpus G] [--ckpt DIR] [--resume FILE] [--data DIR]
+    python tools/train.py --steps N [--batch 4] [--gpus G] [--ckpt DIR] [--resume FILE] [--data DIR] [--augment]
     torchrun --nproc_per_node G tools/train.py --gpus G ...
 
 Scenes are synth.kitti_like_with_boxes draws (a fresh seed every step) or, with --data, the reference's per-frame sample
 dicts (*.npy, kitti_io.read_sample) taken in order, --batch per rank.  The losses are logged every --log-interval steps
 (reading them synchronises; the steps in between do not), a checkpoint named model-<global_step>.npz is written to --ckpt
 every Solver.checkpoint_interval steps and after the last one (rank 0), and --resume continues from such a file at its
-step, learning rate and BatchNorm decay."""
+step, learning rate and BatchNorm decay.
+
+With --augment the scenes go through the reference's training augmentation on the GPU (augment.Augmentor: flip,
+per-object noise, global rotation and scale, the context filter, then the choice of --points points), with draws seeded
+from (--seed, step, rank); without it the points are chosen on the host and nothing is augmented."""
 import argparse
 import glob
 import importlib
@@ -40,6 +44,19 @@ def file_batch(files, step, rank, world, batch, points):
     return block, torch.from_numpy(boxes), torch.from_numpy(labels)
 
 
+def synthetic_ragged(step, rank, world, batch, points, max_boxes):
+    p, b, l = synthetic_batch(step, rank, world, batch, points, max_boxes)
+    n = p.shape[0]
+    offsets = torch.arange(0, (n + 1) * points, points, dtype=torch.int32)
+    return p.reshape(-1, 4), offsets, None, b, l
+
+
+def file_ragged(files, step, rank, world, batch):
+    first = (step * world + rank) * batch
+    samples = [pkg.kitti_io.read_sample(files[(first + i) % len(files)]) for i in range(batch)]
+    return pkg.kitti_io.make_ragged_batch(samples)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, required=True, help="training steps to run in this invocation")
@@ -52,6 +69,8 @@ def main():
     ap.add_argument("--warm-start", default=None, help="pre-trained variables to start from (model only, step 0)")
     ap.add_argument("--data", default=None, help="directory of the reference's per-frame sample dicts (*.npy)")
     ap.add_argument("--log-interval", type=int, default=10)
+    ap.add_argument("--augment", action="store_true", help="augment the scenes on the GPU as the reference's training does")
+    ap.add_argument("--seed", type=int, default=0, help="seed of the augmentation draws")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("train.py trains on CUDA devices; none is available (there is no CPU path)")
@@ -79,6 +98,7 @@ def main():
         if not files:
             raise SystemExit("--data %s holds no *.npy sample" % a.data)
     log = (lambda *s: print(*s, flush=True)) if rank == 0 else (lambda *s: None)
+    aug = pkg.augment.Augmentor(a.points, dev) if a.augment else None
     log("start at global_step %d: learning rate %.6g, bn decay %.6g, %d rank(s) x %d scenes"
         % (tr.global_step, solver.learning_rate(tr.global_step), solver.bn_decay(tr.global_step), world, a.batch))
 
@@ -97,7 +117,15 @@ def main():
             break
         if i and step % solver.checkpoint_interval == 0:
             save()
-        if files is None:
+        if aug is not None:
+            if files is None:
+                cloud, offsets, sem, boxes, labels = synthetic_ragged(step, rank, world, a.batch, a.points, a.max_boxes)
+            else:
+                cloud, offsets, sem, boxes, labels = file_ragged(files, step, rank, world, a.batch)
+            gen = torch.Generator(device=dev).manual_seed(pkg.augment.draw_seed(a.seed, step, rank))
+            draws = pkg.augment.draw(boxes.shape[0], boxes.shape[1], cloud.shape[0], a.points, gen, dev)
+            pts, boxes, labels = aug(cloud, offsets, sem, boxes, labels, draws)
+        elif files is None:
             pts, boxes, labels = synthetic_batch(step, rank, world, a.batch, a.points, a.max_boxes)
         else:
             pts, boxes, labels = file_batch(files, step, rank, world, a.batch, a.points)
