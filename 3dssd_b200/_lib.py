@@ -126,6 +126,10 @@ _SIGNATURES = {
     "ssd3d_augment_boxes": [c_int, c_int] + [c_void_p] * 8,
     "ssd3d_augment_points": [c_int, c_int, c_int] + [c_void_p] * 10,
     "ssd3d_augment_choose": [c_int, c_int] + [c_void_p] * 7,
+    "ssd3d_mixup_db_count": [c_int, c_int, c_int] + [c_void_p] * 5,
+    "ssd3d_mixup_db_write": [c_int, c_int] + [c_void_p] * 7,
+    "ssd3d_mixup_paste_boxes": [c_int, c_int, c_int] + [c_void_p] * 10,
+    "ssd3d_mixup_paste_points": [c_int, c_int, c_int] + [c_void_p] * 15,
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["ssd3d_last_error"])

@@ -1,18 +1,18 @@
-"""Training-scene augmentation of 3dssd.yaml on the GPU (DESIGN.md section 3.12).
+"""Training-scene augmentation of 3dssd.yaml on the GPU (DESIGN.md sections 3.12 and 3.13).
 
-DataAugmentor.kitti_forward (lib/builder/data_augmentor.py:62-100) after the mixup paste -- flip, per-object noise,
-global rotation, global scale, the context filter -- followed by the choice of the points the network sees
-(kitti_dataloader.py:137-147), on ragged scenes.  The kernels (csrc/augment.cu) are pure functions of the scenes and a
-draw block, so the same draws give the same bits; draw() fills one from a seeded torch.Generator on the device.
-
-Mixup is not applied here: it needs the object database the sample dicts do not carry.  Its output would be another
-ragged cloud, which is what Augmentor takes.
+DataAugmentor.kitti_forward (lib/builder/data_augmentor.py:62-100) -- the mixup paste when a Mixup is given
+(mixup.py), then flip, per-object noise, global rotation, global scale, the context filter -- followed by the choice
+of the points the network sees (kitti_dataloader.py:137-147), on ragged scenes.  The kernels (csrc/augment.cu,
+csrc/mixup.cu) are pure functions of the scenes, the drawn objects and a draw block, so the same draws give the same
+bits; draw() fills one from a seeded torch.Generator on the device.  With mixup the draw block is sized for the pasted
+layout (mixup.layout: rows and total).
 """
 import collections
 
 import numpy as np
 import torch
 
+from . import mixup as _mixup
 from . import tf_ops
 
 # configs/kitti/3dssd/3dssd.yaml over lib/core/config.py:82-109
@@ -84,7 +84,11 @@ class Augmentor:
 
     offsets and sem_labels are host arrays (they are checked there); the rest may be host or device tensors.  Without
     sem_labels they are computed on the device from the boxes, as the reference's preprocessing does.  Padded GT rows
-    (all zero) stay zero; boxes are never removed, so the shapes are kept."""
+    (all zero) stay zero; boxes are never removed, so the shapes are kept.
+
+    mixup (mixup.Mixup: database on the device, ids and planes on the host) pastes the drawn objects first, on the
+    semantic labels of the original boxes; the stages after it run on the pasted layout, so the boxes and labels come
+    back as [B, G + S, ...] and the draws must be sized for mixup.layout's rows and total slots."""
 
     def __init__(self, num_points=POINTS_NUM_FOR_TRAINING, device="cuda"):
         if not 1 <= int(num_points) <= tf_ops.AUG_MAX_CHOOSE:
@@ -95,7 +99,7 @@ class Augmentor:
     def _dev(self, t, dtype):
         return torch.as_tensor(t).to(self.device, dtype, non_blocking=True).contiguous()
 
-    def __call__(self, points, offsets, sem_labels, gt_boxes, gt_labels, draws, debug=None):
+    def __call__(self, points, offsets, sem_labels, gt_boxes, gt_labels, draws, debug=None, mixup=None):
         max_n = check_scenes(offsets, sem_labels, gt_boxes.shape[1])
         gt_boxes, gt_labels = self._dev(gt_boxes, torch.float32), self._dev(gt_labels, torch.int32)
         if draws.refill.shape[1] != self.num_points:
@@ -105,6 +109,12 @@ class Augmentor:
             sem = tf_ops.augment_sem_labels(pts, off, gt_boxes, gt_labels, max_n)
         else:
             sem = self._dev(sem_labels, torch.int32)
+        if mixup is not None:
+            m = _mixup.paste(mixup, pts, offsets, off, sem, gt_boxes, gt_labels)
+            if debug is not None:
+                debug.update(input_sem_labels=sem, pasted_points=m.points, pasted_boxes=m.boxes, accepted=m.accepted,
+                             layout=m.layout)
+            pts, off, sem, gt_boxes, gt_labels, max_n = m.points, m.offsets, m.sem_labels, m.boxes, m.labels, m.layout.max_slots
         boxes, chosen, ws = tf_ops.augment_boxes(gt_boxes, draws.scene_u, draws.loc_noise, draws.rot_u)
         moved_pts, keys, survivors, moved = tf_ops.augment_points(pts, off, max_n, sem, draws.keys, ws, gt_boxes.shape[1],
                                                                   want_moved=debug is not None)

@@ -43,60 +43,8 @@ struct AugBox {
     double lx, lz;          // the chosen translation
 };
 
-__device__ __forceinline__ bool box_is_valid(const float *b)
-{
-    return b[0] != 0.f || b[1] != 0.f || b[2] != 0.f || b[3] != 0.f || b[4] != 0.f || b[5] != 0.f || b[6] != 0.f;
-}
-
 // np.random.uniform(-pi/3, pi/3) from its uniform draw: low + (high - low) * u
 __device__ __forceinline__ double rot_of(double u) { return __dadd_rn(-kRotPerturb, __dmul_rn(2.0 * kRotPerturb, u)); }
-
-__device__ __forceinline__ void sincos32(double a, float &s, float &c)
-{
-    double sd, cd;
-    eval_sincos(a, sd, cd);
-    s = (float)sd;
-    c = (float)cd;
-}
-
-__device__ __forceinline__ bool ccw_gt(const float *A, const float *B, const float *C)   // (C1-A1)(B0-A0) > (B1-A1)(C0-A0)
-{
-    return __fmul_rn(__fsub_rn(C[1], A[1]), __fsub_rn(B[0], A[0])) > __fmul_rn(__fsub_rn(B[1], A[1]), __fsub_rn(C[0], A[0]));
-}
-
-// every corner of q strictly inside the clockwise rectangle a (box_collision_test's containment, clockwise=True)
-__device__ __forceinline__ bool holds(const float (*a)[2], const float (*q)[2])
-{
-    for (int l = 0; l < 4; l++)
-        for (int k = 0; k < 4; k++) {
-            const int k1 = (k + 1) & 3;
-            const float v0 = __fsub_rn(a[k1][0], a[k][0]), v1 = __fsub_rn(a[k1][1], a[k][1]);
-            const float cr = __fsub_rn(__fmul_rn(v1, __fsub_rn(a[k][0], q[l][0])), __fmul_rn(v0, __fsub_rn(a[k][1], q[l][1])));
-            if (cr >= 0.0f) return false;
-        }
-    return true;
-}
-
-// box_collision_test (voxelnet_aug.py:632-712) of one pair of BEV rectangles, float32 op by op
-__device__ bool collide(const float (*a)[2], const float (*q)[2])
-{
-    float amin0 = a[0][0], amax0 = a[0][0], amin1 = a[0][1], amax1 = a[0][1];
-    float qmin0 = q[0][0], qmax0 = q[0][0], qmin1 = q[0][1], qmax1 = q[0][1];
-    for (int k = 1; k < 4; k++) {
-        amin0 = fminf(amin0, a[k][0]); amax0 = fmaxf(amax0, a[k][0]); amin1 = fminf(amin1, a[k][1]); amax1 = fmaxf(amax1, a[k][1]);
-        qmin0 = fminf(qmin0, q[k][0]); qmax0 = fmaxf(qmax0, q[k][0]); qmin1 = fminf(qmin1, q[k][1]); qmax1 = fmaxf(qmax1, q[k][1]);
-    }
-    if (!(__fsub_rn(fminf(amax0, qmax0), fmaxf(amin0, qmin0)) > 0.0f)) return false;
-    if (!(__fsub_rn(fminf(amax1, qmax1), fmaxf(amin1, qmin1)) > 0.0f)) return false;
-    for (int k = 0; k < 4; k++) {
-        const float *A = a[k], *B = a[(k + 1) & 3];
-        for (int l = 0; l < 4; l++) {
-            const float *C = q[l], *D = q[(l + 1) & 3];
-            if (ccw_gt(A, C, D) != ccw_gt(B, C, D) && ccw_gt(A, B, C) != ccw_gt(A, B, D)) return true;
-        }
-    }
-    return holds(a, q) || holds(q, a);
-}
 
 __global__ void __launch_bounds__(kAugBoxThreads) aug_boxes_kernel(
     int g, const float *__restrict__ boxes, const double *__restrict__ scene_u, const double *__restrict__ loc_noise,
@@ -122,16 +70,10 @@ __global__ void __launch_bounds__(kAugBoxThreads) aug_boxes_kernel(
         }
         sv[j] = v;
         stry[j] = -1;
-        if (noise && v) {                                                       // box2d_to_corner_jit of the grown box
-            const float dl = __fadd_rn(sb[j][3], kAugExpand), dw = __fadd_rn(sb[j][5], kAugExpand);
+        if (noise && v) {                                                       // the corners of the grown box
             float sn, cs;
             sincos32((double)sb[j][6], sn, cs);
-            const float na[4] = {-0.5f, -0.5f, 0.5f, 0.5f}, nb[4] = {-0.5f, 0.5f, 0.5f, -0.5f};
-            for (int k = 0; k < 4; k++) {
-                const float a = __fmul_rn(dl, na[k]), bb = __fmul_rn(dw, nb[k]);
-                sc[j][k][0] = __fadd_rn(__fadd_rn(__fmul_rn(a, cs), __fmul_rn(bb, sn)), sb[j][0]);
-                sc[j][k][1] = __fadd_rn(__fsub_rn(__fmul_rn(bb, cs), __fmul_rn(a, sn)), sb[j][2]);
-            }
+            bev_corners(sb[j][0], sb[j][2], __fadd_rn(sb[j][3], kAugExpand), __fadd_rn(sb[j][5], kAugExpand), sn, cs, sc[j]);
         }
     }
     __syncthreads();
@@ -242,7 +184,13 @@ __global__ void __launch_bounds__(kAugPointThreads) aug_points_kernel(
     float x = pts[gi * 4], y = pts[gi * 4 + 1], z = pts[gi * 4 + 2];
     const float in = pts[gi * 4 + 3];
     const int lab = sem[gi];
-    if (S.flip) x = -x;                                                         // flip_points (kitti_aug.py:14-19)
+    if (lab < 0) {                                                              // an absent slot of the mixup layout
+        out[gi * 4] = 0.0f; out[gi * 4 + 1] = 0.0f; out[gi * 4 + 2] = 0.0f; out[gi * 4 + 3] = 0.0f;
+        if (moved) moved[gi] = -1;
+        sort_keys[gi] = ~0ull;
+        return;
+    }
+    if (S.flip) x = -x;                                                      // flip_points (kitti_aug.py:14-19)
     int mover = -1;
     if (S.noise && lab != 0) {
         // points_transform_ (voxelnet_aug.py:590-618): the first pre-noise box holding the point moves it

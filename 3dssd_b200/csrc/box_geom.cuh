@@ -1,5 +1,6 @@
-// box_geom.cuh -- box geometry shared by the target assignment (det_loss.cu), the evaluator (box_eval.cu) and the
-// augmentor (augment.cu): the face planes of a box with the point-in-box test, and the one pinned double sincos.
+// box_geom.cuh -- box geometry shared by the target assignment (det_loss.cu), the evaluator (box_eval.cu), the
+// augmentor (augment.cu) and the mixup paste (mixup.cu): the face planes of a box with the point-in-box test, the one
+// pinned double sincos, and the float32 BEV corners and collision test of the noise search and the paste.
 #pragma once
 #include "common.cuh"
 
@@ -95,6 +96,72 @@ __device__ __forceinline__ void eval_sincos(double x, double &s, double &c)
         case 2: s = -sr; c = -cr; break;
         default: s = -cr; c = sr; break;
     }
+}
+
+__device__ __forceinline__ void sincos32(double a, float &s, float &c)
+{
+    double sd, cd;
+    eval_sincos(a, sd, cd);
+    s = (float)sd;
+    c = (float)cd;
+}
+
+// ---- BEV rectangles (voxelnet_aug.py) ----------------------------------------------------------------------------------
+// A padded GT row is all zeros.
+__device__ __forceinline__ bool box_is_valid(const float *b)
+{
+    return b[0] != 0.f || b[1] != 0.f || b[2] != 0.f || b[3] != 0.f || b[4] != 0.f || b[5] != 0.f || b[6] != 0.f;
+}
+
+// box2d_to_corner_jit (voxelnet_aug.py:510-529) of one BEV box (x, z, l, w) whose dims the caller has already grown,
+// float32 op by op: corners_norm * (l, w) @ [[cos, -sin], [sin, cos]] + (x, z)
+__device__ __forceinline__ void bev_corners(float x, float z, float dl, float dw, float sn, float cs, float (*c)[2])
+{
+    const float na[4] = {-0.5f, -0.5f, 0.5f, 0.5f}, nb[4] = {-0.5f, 0.5f, 0.5f, -0.5f};
+    for (int k = 0; k < 4; k++) {
+        const float a = __fmul_rn(dl, na[k]), bb = __fmul_rn(dw, nb[k]);
+        c[k][0] = __fadd_rn(__fadd_rn(__fmul_rn(a, cs), __fmul_rn(bb, sn)), x);
+        c[k][1] = __fadd_rn(__fsub_rn(__fmul_rn(bb, cs), __fmul_rn(a, sn)), z);
+    }
+}
+
+__device__ __forceinline__ bool ccw_gt(const float *A, const float *B, const float *C)   // (C1-A1)(B0-A0) > (B1-A1)(C0-A0)
+{
+    return __fmul_rn(__fsub_rn(C[1], A[1]), __fsub_rn(B[0], A[0])) > __fmul_rn(__fsub_rn(B[1], A[1]), __fsub_rn(C[0], A[0]));
+}
+
+// every corner of q strictly inside the clockwise rectangle a (box_collision_test's containment, clockwise=True)
+__device__ __forceinline__ bool holds(const float (*a)[2], const float (*q)[2])
+{
+    for (int l = 0; l < 4; l++)
+        for (int k = 0; k < 4; k++) {
+            const int k1 = (k + 1) & 3;
+            const float v0 = __fsub_rn(a[k1][0], a[k][0]), v1 = __fsub_rn(a[k1][1], a[k][1]);
+            const float cr = __fsub_rn(__fmul_rn(v1, __fsub_rn(a[k][0], q[l][0])), __fmul_rn(v0, __fsub_rn(a[k][1], q[l][1])));
+            if (cr >= 0.0f) return false;
+        }
+    return true;
+}
+
+// box_collision_test (voxelnet_aug.py:632-712) of one pair of BEV rectangles, float32 op by op
+static __device__ bool collide(const float (*a)[2], const float (*q)[2])
+{
+    float amin0 = a[0][0], amax0 = a[0][0], amin1 = a[0][1], amax1 = a[0][1];
+    float qmin0 = q[0][0], qmax0 = q[0][0], qmin1 = q[0][1], qmax1 = q[0][1];
+    for (int k = 1; k < 4; k++) {
+        amin0 = fminf(amin0, a[k][0]); amax0 = fmaxf(amax0, a[k][0]); amin1 = fminf(amin1, a[k][1]); amax1 = fmaxf(amax1, a[k][1]);
+        qmin0 = fminf(qmin0, q[k][0]); qmax0 = fmaxf(qmax0, q[k][0]); qmin1 = fminf(qmin1, q[k][1]); qmax1 = fmaxf(qmax1, q[k][1]);
+    }
+    if (!(__fsub_rn(fminf(amax0, qmax0), fmaxf(amin0, qmin0)) > 0.0f)) return false;
+    if (!(__fsub_rn(fminf(amax1, qmax1), fmaxf(amin1, qmin1)) > 0.0f)) return false;
+    for (int k = 0; k < 4; k++) {
+        const float *A = a[k], *B = a[(k + 1) & 3];
+        for (int l = 0; l < 4; l++) {
+            const float *C = q[l], *D = q[(l + 1) & 3];
+            if (ccw_gt(A, C, D) != ccw_gt(B, C, D) && ccw_gt(A, B, C) != ccw_gt(A, B, D)) return true;
+        }
+    }
+    return holds(a, q) || holds(q, a);
 }
 
 }  // namespace ssd3d

@@ -222,3 +222,28 @@ def make_ragged_batch(samples, pin=True):
     if pin and torch.cuda.is_available():
         out = [t if t is None else t.pin_memory() for t in out]
     return tuple(out)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# ground planes (the mixup paste stands its objects on them, mixup.py)
+# ------------------------------------------------------------------------------------------------------------------
+def plane_path(planes_dir, sample_name):
+    """'<planes_dir>/%06d.txt', the plane file of a frame (kitti_util.py:295)."""
+    return os.path.join(planes_dir, "%06d.txt" % int(sample_name))
+
+
+def read_plane(path):
+    """get_road_plane (kitti_util.py:286-318): the 4th line of a KITTI plane file -> (a, b, c, d) float64 with the normal
+    facing up (negated when b > 0: +y points down) and divided by the norm of (a, b, c).  A missing file raises."""
+    if not os.path.isfile(path):
+        raise FileNotFoundError("ground plane file %s does not exist" % path)
+    with open(path) as fh:
+        lines = fh.readlines()
+    if len(lines) < 4:
+        raise ValueError("%s: a plane file holds the plane on its 4th line" % path)
+    plane = np.asarray([float(v) for v in lines[3].split()], np.float64)
+    if plane.shape != (4,):
+        raise ValueError("%s: the plane line must hold 4 numbers" % path)
+    if plane[1] > 0:
+        plane = -plane
+    return plane / np.linalg.norm(plane[0:3])

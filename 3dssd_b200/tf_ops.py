@@ -1594,3 +1594,107 @@ def augment_choose(points, offsets, sort_keys, survivors, refill):
     check(lib().ssd3d_augment_choose(b, m, _p(points), _p(offsets), _p(sort_keys), _p(survivors), _p(refill), _p(out), _stream()),
           "augment_choose")
     return out
+
+
+# ---- mixup paste and its object database (csrc/mixup.cu, DESIGN.md section 3.13) -------------------------------------
+MIXUP_MAX_ROWS = 256          # GT rows plus drawn objects per scene
+MIXUP_MAX_SLOTS = AUG_MAX_POINTS
+
+
+def mixup_db_count(points, offsets, max_n, gt_boxes):
+    """Points of each frame inside each valid GT row grown by 0.1 (ssd3d_mixup_db_count) -> counts [b, g] int32."""
+    points, offsets, b = _aug_ragged(points, offsets, max_n)
+    gt_boxes = _aug_boxes_in(gt_boxes, b)
+    if gt_boxes.shape[1] < 1:
+        raise ValueError("mixup_db_count needs at least one GT row")
+    counts = torch.empty((b, gt_boxes.shape[1]), dtype=torch.int32, device=points.device)
+    check(lib().ssd3d_mixup_db_count(b, gt_boxes.shape[1], int(max_n), _p(points), _p(offsets), _p(gt_boxes), _p(counts),
+                                     _stream()), "mixup_db_count")
+    return counts
+
+
+def mixup_db_write(points, offsets, gt_boxes, objects, object_offsets, total):
+    """The points of each database object (ssd3d_mixup_db_write): objects [O, 2] int32 (frame, row), object_offsets [O + 1]
+    int64 (device), total = object_offsets[-1] -> points [total, 4], each object's points in frame order."""
+    points = _req(points, "points", torch.float32, 2, 4)
+    offsets = _req(offsets, "offsets", torch.int32, 1)
+    gt_boxes = _aug_boxes_in(gt_boxes, offsets.shape[0] - 1)
+    objects = _req(objects, "objects", torch.int32, 2, 2)
+    object_offsets = _req(object_offsets, "object_offsets", torch.int64, 1)
+    o = objects.shape[0]
+    if object_offsets.shape[0] != o + 1 or o < 1 or gt_boxes.shape[1] < 1:
+        raise ValueError("objects %s and object_offsets %s disagree (or hold no object)" % (
+            tuple(objects.shape), tuple(object_offsets.shape)))
+    out = torch.empty((int(total), 4), dtype=torch.float32, device=points.device)
+    check(lib().ssd3d_mixup_db_write(gt_boxes.shape[1], o, _p(points), _p(offsets), _p(gt_boxes), _p(objects), _p(object_offsets),
+                                     _p(out), _stream()), "mixup_db_write")
+    return out
+
+
+def _mixup_db_in(db_boxes, db_classes):
+    db_boxes = _req(db_boxes, "db_boxes", torch.float32, 2, 7)
+    db_classes = _req(db_classes, "db_classes", torch.int32, 1)
+    if db_classes.shape[0] != db_boxes.shape[0]:
+        raise ValueError("db_classes %s does not match db_boxes %s" % (tuple(db_classes.shape), tuple(db_boxes.shape)))
+    return db_boxes, db_classes
+
+
+def mixup_paste_boxes(gt_boxes, gt_labels, ids, db_boxes, db_classes, planes):
+    """box_3d_collision_test of the drawn objects ids [b, s] int32 (-1: none) against each scene (ssd3d_mixup_paste_boxes)
+    -> (boxes [b, g + s, 7], labels [b, g + s] int32, accepted [b, s] int32).  The ids must be in range (checked on the
+    host by mixup.layout)."""
+    gt_boxes = _aug_boxes_in(gt_boxes)
+    b, g = gt_boxes.shape[:2]
+    gt_labels = _req(gt_labels, "gt_labels", torch.int32, 2)
+    ids = _req(ids, "ids", torch.int32, 2)
+    db_boxes, db_classes = _mixup_db_in(db_boxes, db_classes)
+    planes = _req(planes, "planes", torch.float64, 2, 4)
+    s = ids.shape[1]
+    if tuple(gt_labels.shape) != (b, g) or ids.shape[0] != b or planes.shape[0] != b:
+        raise ValueError("gt_boxes %s, gt_labels %s, ids %s and planes %s disagree" % (
+            tuple(gt_boxes.shape), tuple(gt_labels.shape), tuple(ids.shape), tuple(planes.shape)))
+    if s < 1 or g + s > MIXUP_MAX_ROWS:
+        raise ValueError("GT rows plus drawn objects must be at most %d (and s >= 1), got %d + %d" % (MIXUP_MAX_ROWS, g, s))
+    dev = gt_boxes.device
+    out = torch.empty((b, g + s, 7), dtype=torch.float32, device=dev)
+    labels = torch.empty((b, g + s), dtype=torch.int32, device=dev)
+    accepted = torch.empty((b, s), dtype=torch.int32, device=dev)
+    check(lib().ssd3d_mixup_paste_boxes(b, g, s, _p(gt_boxes), _p(gt_labels), _p(ids), _p(db_boxes), _p(db_classes), _p(planes),
+                                        _p(out), _p(labels), _p(accepted), _stream()), "mixup_paste_boxes")
+    return out, labels, accepted
+
+
+def mixup_paste_points(points, offsets, sem_labels, ids, db_points, db_offsets, db_boxes, db_classes, planes, accepted,
+                       out_offsets, slot_start, max_slots, total):
+    """The pasted clouds (ssd3d_mixup_paste_points) of the layout out_offsets [b + 1], slot_start [b, s + 1] (device int32,
+    from mixup.layout), total = out_offsets[-1] -> (points [total, 4], semantic labels [total] int32, -1 where a dropped
+    object's slot holds no point)."""
+    points = _req(points, "points", torch.float32, 2, 4)
+    offsets = _req(offsets, "offsets", torch.int32, 1)
+    b = offsets.shape[0] - 1
+    sem_labels = _req(sem_labels, "sem_labels", torch.int32, 1)
+    ids = _req(ids, "ids", torch.int32, 2)
+    db_points = _req(db_points, "db_points", torch.float32, 2, 4)
+    db_offsets = _req(db_offsets, "db_offsets", torch.int64, 1)
+    db_boxes, db_classes = _mixup_db_in(db_boxes, db_classes)
+    planes = _req(planes, "planes", torch.float64, 2, 4)
+    accepted = _req(accepted, "accepted", torch.int32, 2)
+    out_offsets = _req(out_offsets, "out_offsets", torch.int32, 1)
+    slot_start = _req(slot_start, "slot_start", torch.int32, 2)
+    s = ids.shape[1]
+    if (b < 1 or sem_labels.shape[0] != points.shape[0] or ids.shape[0] != b or planes.shape[0] != b or
+            tuple(accepted.shape) != (b, s) or out_offsets.shape[0] != b + 1 or tuple(slot_start.shape) != (b, s + 1) or
+            db_offsets.shape[0] != db_boxes.shape[0] + 1):
+        raise ValueError("mixup_paste_points: points %s, offsets %s, sem_labels %s, ids %s, planes %s, accepted %s, out_offsets %s,"
+                         " slot_start %s, db_offsets %s, db_boxes %s disagree" % tuple(tuple(t.shape) for t in (
+                             points, offsets, sem_labels, ids, planes, accepted, out_offsets, slot_start, db_offsets, db_boxes)))
+    if not 1 <= s <= MIXUP_MAX_ROWS or not 1 <= int(max_slots) <= MIXUP_MAX_SLOTS:
+        raise ValueError("1 <= s <= %d and 1 <= max_slots <= %d, got s=%d max_slots=%d" % (MIXUP_MAX_ROWS, MIXUP_MAX_SLOTS, s,
+                                                                                            max_slots))
+    dev = points.device
+    out = torch.empty((int(total), 4), dtype=torch.float32, device=dev)
+    sem = torch.empty((int(total),), dtype=torch.int32, device=dev)
+    check(lib().ssd3d_mixup_paste_points(b, s, int(max_slots), _p(points), _p(offsets), _p(sem_labels), _p(ids), _p(db_points),
+                                         _p(db_offsets), _p(db_boxes), _p(db_classes), _p(planes), _p(accepted), _p(out_offsets),
+                                         _p(slot_start), _p(out), _p(sem), _stream()), "mixup_paste_points")
+    return out, sem

@@ -570,7 +570,8 @@ int ssd3d_augment_boxes(int b, int g, const float *gt_boxes, const double *scene
                         const double *rot_u, float *out_boxes, int *chosen_try, void *workspace, ssd3d_stream_t stream);
 /* out_points [T, 4] transformed; sort_keys [T] = keys << 32 | index in the scene for a survivor of the context filter,
  * all ones for a dropped point; survivors [b] counts (cleared here); moved_by [T] (may be NULL) = the box that moved the
- * point or -1.  sem_labels are >= 0. */
+ * point or -1.  A negative semantic label marks a slot that holds no point (a dropped object of the mixup layout): it
+ * is not moved, its sort key is all ones, it is not a survivor, moved_by is -1 and its output is zeros. */
 int ssd3d_augment_points(int b, int g, int max_n, const float *points, const int *offsets, const int *sem_labels,
                          const unsigned *keys, const void *workspace, float *out_points, unsigned long long *sort_keys,
                          int *survivors, int *moved_by, ssd3d_stream_t stream);
@@ -578,6 +579,34 @@ int ssd3d_augment_points(int b, int g, int max_n, const float *points, const int
  * for slot t >= N the survivor at rank (refill[s, t] * N) >> 32.  A scene without survivors gets zeros. */
 int ssd3d_augment_choose(int b, int num_points, const float *points, const int *offsets, const unsigned long long *sort_keys,
                          const int *survivors, const unsigned *refill, float *out, ssd3d_stream_t stream);
+
+/* ---- mixup paste and its object database (csrc/mixup.cu, DESIGN.md section 3.13) ------------------------------------
+ * Scenes as for the augmentation: points [T, 4], DEVICE offsets [b + 1], gt_boxes [b, g, 7] zero-padded, gt_labels [b, g].
+ * Database: db_points [P, 4] with object o at rows db_offsets[o] .. db_offsets[o+1]-1 (int64), db_boxes [O, 7],
+ * db_classes [O].  Limits: g + s <= 256, points per scene before and after the paste <= 131072.  Nothing synchronises the
+ * host; the same inputs give the same bits. */
+/* counts [b, g] (cleared here) = the points of each frame inside each valid row grown by 0.1 on (l, h, w). */
+int ssd3d_mixup_db_count(int b, int g, int max_n, const float *points, const int *offsets, const float *gt_boxes,
+                         int *counts, ssd3d_stream_t stream);
+/* out_points rows object_offsets[o] .. object_offsets[o+1]-1 = the points of frame objects[o, 0] inside its row
+ * objects[o, 1] grown by 0.1, in frame order (object_offsets from the counts of ssd3d_mixup_db_count). */
+int ssd3d_mixup_db_write(int g, int n_objects, const float *points, const int *offsets, const float *gt_boxes,
+                         const int *objects, const long long *object_offsets, float *out_points, ssd3d_stream_t stream);
+/* box_3d_collision_test of the s drawn objects ids [b, s] (-1: none) against each scene: drawn box i with (l, w) grown by
+ * 0.5 is kept iff it collides with no valid scene row and no kept drawn box k < i; a kept box stands on the scene's plane
+ * planes [b, 4] float64 (a, b, c, d), y -= y - (-d - a x - c z) / b.  out_boxes [b, g + s, 7] / out_labels [b, g + s] = the
+ * valid scene rows in order, the kept boxes in draw order (label db_classes[id]), zero rows; accepted [b, s] 0 / 1. */
+int ssd3d_mixup_paste_boxes(int b, int g, int s, const float *gt_boxes, const int *gt_labels, const int *ids,
+                            const float *db_boxes, const int *db_classes, const double *planes, float *out_boxes,
+                            int *out_labels, int *accepted, ssd3d_stream_t stream);
+/* Scene s's output slots out_offsets[s] .. out_offsets[s+1]-1 (DEVICE int32 [b + 1]): its points with their semantic
+ * labels, then drawn object i at slots slot_start[s, i] .. slot_start[s, i+1]-1 (DEVICE int32 [b, s + 1], slot_start[s, 0]
+ * = the scene's point count): the database points with y moved as the box when accepted (label db_classes[id]), else
+ * zeros with label -1.  max_slots = the largest scene after the paste. */
+int ssd3d_mixup_paste_points(int b, int s, int max_slots, const float *points, const int *offsets, const int *sem_labels,
+                             const int *ids, const float *db_points, const long long *db_offsets, const float *db_boxes,
+                             const int *db_classes, const double *planes, const int *accepted, const int *out_offsets,
+                             const int *slot_start, float *out_points, int *out_sem_labels, ssd3d_stream_t stream);
 
 #ifdef __cplusplus
 }

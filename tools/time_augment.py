@@ -2,9 +2,10 @@
 from device-resident scenes and draws to the [B, 16384, 4] block, timed with CUDA events after a warm-up.  Scenes are
 synth.kitti_like_with_boxes draws of 18k..24k points with up to 40 boxes (a KITTI frame in the camera's field of view
 holds about 20k points), half of them noised, rotated and scaled.  Prints the card name and its power limit, then one
-JSON line.
+JSON line.  With --mixup the same call with the mixup paste in front (15 objects drawn per scene from a database
+built from other synthetic scenes, flat ground planes) is timed in the same run, the two alternating rep by rep.
 
-    python tools/time_augment.py [--scenes 8] [--reps 50]
+    python tools/time_augment.py [--scenes 8] [--reps 50] [--mixup]
 """
 import argparse
 import importlib
@@ -27,6 +28,7 @@ def main():
     ap.add_argument("--scenes", type=int, default=8)
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--seed", type=int, default=3)
+    ap.add_argument("--mixup", action="store_true", help="also time the call with the mixup paste, alternating")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("time_augment.py needs a CUDA device")
@@ -52,18 +54,37 @@ def main():
     gen = torch.Generator(device=dev).manual_seed(a.seed)
     draws = pkg.augment.draw(a.scenes, 40, int(offsets[-1]), 16384, gen, dev)
     draws = draws._replace(scene_u=torch.full((a.scenes, 6), 0.25, dtype=torch.float64, device=dev))   # every stage on
-    for _ in range(3):
-        aug(pts, offsets, None, gb, gl, draws)
+    calls = {"augment_ms": lambda: aug(pts, offsets, None, gb, gl, draws)}
+    extra = {}
+    if a.mixup:
+        MX = pkg.mixup
+        p, b, l = synth.kitti_like_with_boxes(16, 20000, 40, seed=a.seed + 7777)
+        db = MX.ObjectDatabase.build(p.reshape(-1, 4), np.arange(0, 17 * 20000, 20000), b, l, device=dev)
+        ids = MX.Sampler(db, seed=a.seed).ids(0, a.scenes)
+        planes = np.tile(np.asarray(MX.FLAT_PLANE, np.float64), (a.scenes, 1))
+        lay = MX.layout(offsets, ids, db.host_offsets, 40)
+        mdraws = pkg.augment.draw(a.scenes, lay.rows, lay.total, 16384, gen, dev)
+        mdraws = mdraws._replace(scene_u=torch.full((a.scenes, 6), 0.25, dtype=torch.float64, device=dev))
+        mix = MX.Mixup(db, ids, planes)
+        calls["augment_mixup_ms"] = lambda: aug(pts, offsets, None, gb, gl, mdraws, mixup=mix)
+        extra = {"db_objects": len(db), "drawn": int((ids >= 0).sum()), "pasted_points": lay.total - int(offsets[-1])}
+    for f in calls.values():
+        for _ in range(3):
+            f()
     torch.cuda.synchronize()
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
-    for _ in range(a.reps):
-        aug(pts, offsets, None, gb, gl, draws)
-    t1.record()
-    torch.cuda.synchronize()
-    ms = t0.elapsed_time(t1) / a.reps
-    print(json.dumps({"card": card, "power_limit": power, "scenes": a.scenes, "points": int(offsets[-1]), "boxes": 40,
-                      "augment_ms": round(ms, 4)}))
+    total = {k: 0.0 for k in calls}
+    for _ in range(a.reps):                                # alternate the variants rep by rep
+        for k, f in calls.items():
+            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0.record()
+            f()
+            t1.record()
+            torch.cuda.synchronize()
+            total[k] += t0.elapsed_time(t1)
+    res = {"card": card, "power_limit": power, "scenes": a.scenes, "points": int(offsets[-1]), "boxes": 40}
+    res.update({k: round(v / a.reps, 4) for k, v in total.items()})
+    res.update(extra)
+    print(json.dumps(res))
 
 
 if __name__ == "__main__":

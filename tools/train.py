@@ -12,7 +12,11 @@ step, learning rate and BatchNorm decay.
 
 With --augment the scenes go through the reference's training augmentation on the GPU (augment.Augmentor: flip,
 per-object noise, global rotation and scale, the context filter, then the choice of --points points), with draws seeded
-from (--seed, step, rank); without it the points are chosen on the host and nothing is augmented."""
+from (--seed, step, rank); without it the points are chosen on the host and nothing is augmented.  --mixup DB.npz (an
+object database of tools/build_mixup_db.py) adds the mixup paste before those stages: each scene draws 15 Car objects at
+each step (mixup.Sampler, seeded from --seed, rank and the scene's place in the batch) and keeps those that collide with
+nothing, standing on the frame's ground plane -- read from --planes DIR (<DIR>/%06d.txt per sample name) with --data,
+the flat y = 1.65 plane of the synthetic scenes without it."""
 import argparse
 import glob
 import importlib
@@ -54,7 +58,8 @@ def synthetic_ragged(step, rank, world, batch, points, max_boxes):
 def file_ragged(files, step, rank, world, batch):
     first = (step * world + rank) * batch
     samples = [pkg.kitti_io.read_sample(files[(first + i) % len(files)]) for i in range(batch)]
-    return pkg.kitti_io.make_ragged_batch(samples)
+    return pkg.kitti_io.make_ragged_batch(samples), [s.get(pkg.kitti_io.KEY_SAMPLE_NAME, (first + i) % len(files))
+                                                     for i, s in enumerate(samples)]
 
 
 def main():
@@ -71,7 +76,13 @@ def main():
     ap.add_argument("--log-interval", type=int, default=10)
     ap.add_argument("--augment", action="store_true", help="augment the scenes on the GPU as the reference's training does")
     ap.add_argument("--seed", type=int, default=0, help="seed of the augmentation draws")
+    ap.add_argument("--mixup", default=None, help="object database (.npz of tools/build_mixup_db.py): paste objects first")
+    ap.add_argument("--planes", default=None, help="directory of the KITTI ground planes of --data (with --mixup)")
     a = ap.parse_args()
+    if a.mixup and not a.augment:
+        raise SystemExit("--mixup works with --augment")
+    if a.mixup and a.data and not a.planes:
+        raise SystemExit("--mixup with --data needs --planes DIR (the ground plane of every sample)")
     if not torch.cuda.is_available():
         raise SystemExit("train.py trains on CUDA devices; none is available (there is no CPU path)")
     D = pkg.dist
@@ -99,6 +110,9 @@ def main():
             raise SystemExit("--data %s holds no *.npy sample" % a.data)
     log = (lambda *s: print(*s, flush=True)) if rank == 0 else (lambda *s: None)
     aug = pkg.augment.Augmentor(a.points, dev) if a.augment else None
+    MX = pkg.mixup
+    db = MX.ObjectDatabase.load(a.mixup, dev) if a.mixup else None
+    sampler = MX.Sampler(db, seed=a.seed) if db is not None else None
     log("start at global_step %d: learning rate %.6g, bn decay %.6g, %d rank(s) x %d scenes"
         % (tr.global_step, solver.learning_rate(tr.global_step), solver.bn_decay(tr.global_step), world, a.batch))
 
@@ -120,11 +134,20 @@ def main():
         if aug is not None:
             if files is None:
                 cloud, offsets, sem, boxes, labels = synthetic_ragged(step, rank, world, a.batch, a.points, a.max_boxes)
+                names = None
             else:
-                cloud, offsets, sem, boxes, labels = file_ragged(files, step, rank, world, a.batch)
+                (cloud, offsets, sem, boxes, labels), names = file_ragged(files, step, rank, world, a.batch)
+            mix, rows, total = None, boxes.shape[1], cloud.shape[0]
+            if sampler is not None:
+                ids = sampler.ids(step, boxes.shape[0], rank)
+                planes = (np.tile(np.asarray(MX.FLAT_PLANE, np.float64), (boxes.shape[0], 1)) if names is None else
+                          np.stack([pkg.kitti_io.read_plane(pkg.kitti_io.plane_path(a.planes, n)) for n in names]))
+                mix = MX.Mixup(db, ids, planes)
+                lay = MX.layout(offsets, ids, db.host_offsets, boxes.shape[1])
+                rows, total = lay.rows, lay.total
             gen = torch.Generator(device=dev).manual_seed(pkg.augment.draw_seed(a.seed, step, rank))
-            draws = pkg.augment.draw(boxes.shape[0], boxes.shape[1], cloud.shape[0], a.points, gen, dev)
-            pts, boxes, labels = aug(cloud, offsets, sem, boxes, labels, draws)
+            draws = pkg.augment.draw(boxes.shape[0], rows, total, a.points, gen, dev)
+            pts, boxes, labels = aug(cloud, offsets, sem, boxes, labels, draws, mixup=mix)
         elif files is None:
             pts, boxes, labels = synthetic_batch(step, rank, world, a.batch, a.points, a.max_boxes)
         else:
