@@ -1,7 +1,7 @@
 """3dssd_b200 -- H100 (sm_90a) set-abstraction operators behind the tf_ops / layers_util surface of
 dvlab-research/3DSSD.  Import with importlib.import_module("3dssd_b200") or through the `ssd3d_b200` alias.
 """
-from . import augment, config, dist, evaluation, head, kitti_io, layers_util, loss, mixup, params, solver, tf_ops  # noqa: F401
+from . import augment, config, dist, evaluation, head, kitti_io, layers_util, loss, mixup, params, prepare, solver, tf_ops  # noqa: F401
 from ._lib import EXPORTS, LIB_PATH, lib  # noqa: F401
 from .backbone import SABackbone, train_forward  # noqa: F401
 from .head import DetectionHead  # noqa: F401

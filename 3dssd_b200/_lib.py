@@ -130,6 +130,8 @@ _SIGNATURES = {
     "ssd3d_mixup_db_write": [c_int, c_int] + [c_void_p] * 7,
     "ssd3d_mixup_paste_boxes": [c_int, c_int, c_int] + [c_void_p] * 10,
     "ssd3d_mixup_paste_points": [c_int, c_int, c_int] + [c_void_p] * 15,
+    "ssd3d_prepare_workspace": [c_int, c_int],
+    "ssd3d_prepare_points": [c_int, c_int, c_int] + [c_void_p] * 9,
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["ssd3d_last_error"])
@@ -149,7 +151,8 @@ def lib():
             fn.restype = ctypes.c_size_t if name in ("ssd3d_sa_fused_smem", "ssd3d_query_ball_point_workspace", "ssd3d_bn_train_workspace",
                                                    "ssd3d_linear_wgrad_workspace", "ssd3d_bn_train_grad_workspace",
                                                    "ssd3d_det_loss_workspace", "ssd3d_grad_clip_scale_workspace",
-                                                   "ssd3d_eval_workspace", "ssd3d_augment_workspace") else c_int
+                                                   "ssd3d_eval_workspace", "ssd3d_augment_workspace",
+                                                   "ssd3d_prepare_workspace") else c_int
             if name == "ssd3d_fps_temp_elems":
                 fn.restype = c_long
         l.ssd3d_last_error.restype = ctypes.c_char_p

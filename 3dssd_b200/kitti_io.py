@@ -247,3 +247,85 @@ def read_plane(path):
     if plane[1] > 0:
         plane = -plane
     return plane / np.linalg.norm(plane[0:3])
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# raw KITTI frames (the preprocessing pass of prepare.py reads them)
+# ------------------------------------------------------------------------------------------------------------------
+KEY_LABEL_DIST = "label_dist"
+KEY_LABEL_NUM = "label_num"
+CALIB_KEYS = ("Tr_velo_to_cam", "R0_rect", "P2")
+CALIB_SHAPES = {"Tr_velo_to_cam": (3, 4), "R0_rect": (3, 3), "P2": (3, 4)}
+_PNG_MAGIC = b"\x89PNG\r\n\x1a\n"
+
+
+def read_velodyne(path):
+    """load_velo_scan (kitti_util.py:323-326): the float32 words of a velodyne .bin as [N, 4] (x, y, z, reflectance)."""
+    raw = np.fromfile(path, dtype=np.float32)
+    if raw.size % 4:
+        raise ValueError("%s: %d float32 words is not a whole number of (x, y, z, r) points" % (path, raw.size))
+    return raw.reshape(-1, 4)
+
+
+def read_calib(path):
+    """read_calib_file (kitti_util.py:120-138): 'key: v v v ...' lines -> dict of float64 arrays; blank lines are
+    skipped, a line without ':' or a value that is not a float list is skipped as the reference skips dates.  The three
+    matrices the preprocessing needs (Tr_velo_to_cam, R0_rect, P2) must be present with 12, 9 and 12 values."""
+    data = {}
+    with open(path) as fh:
+        for line in fh:
+            line = line.rstrip()
+            if not line:
+                continue
+            if ":" not in line:
+                raise ValueError("%s: calibration line without ':': %r" % (path, line[:40]))
+            key, value = line.split(":", 1)
+            try:
+                data[key] = np.array([float(x) for x in value.split()], np.float64)
+            except ValueError:
+                pass
+    for k in CALIB_KEYS:
+        if k not in data:
+            raise ValueError("%s: no %s in the calibration file" % (path, k))
+        if data[k].size != int(np.prod(CALIB_SHAPES[k])):
+            raise ValueError("%s: %s holds %d values, expected %d" % (path, k, data[k].size, int(np.prod(CALIB_SHAPES[k]))))
+    return data
+
+
+def calib_block(calib):
+    """The [33] float64 calibration block of csrc/prepare.cu: Tr_velo_to_cam (12), R0_rect (9), P2 (12), row-major."""
+    return np.concatenate([np.asarray(calib[k], np.float64).reshape(-1) for k in CALIB_KEYS])
+
+
+def read_label(path, cls_list=("Car",)):
+    """read_label + Object3d (kitti_util.py:13-44, 279-284) and object_label_to_box_3d (box_3d_utils.py:5-22) for the
+    types in cls_list: (boxes [G, 7] float64 (x, y, z, l, h, w, ry) in file order, classes [G] int64, 1-based index in
+    cls_list).  Each line is rstripped and split on single spaces; fields 1.. must be floats (15 or 16 fields)."""
+    boxes, classes = [], []
+    with open(path) as fh:
+        lines = [ln.rstrip() for ln in fh]
+    for k, line in enumerate(lines):
+        data = line.split(" ")
+        if len(data) not in (15, 16):
+            raise ValueError("%s:%d: a label line holds 15 or 16 fields, got %d" % (path, k + 1, len(data)))
+        try:
+            v = [float(x) for x in data[1:]]
+        except ValueError:
+            raise ValueError("%s:%d: label fields 1.. must be numbers: %r" % (path, k + 1, line[:60])) from None
+        if data[0] in cls_list:
+            h, w, l, x, y, z, ry = v[7], v[8], v[9], v[10], v[11], v[12], v[13]
+            boxes.append((x, y, z, l, h, w, ry))
+            classes.append(cls_list.index(data[0]) + 1)
+    return np.asarray(boxes, np.float64).reshape(-1, 7), np.asarray(classes, np.int64)
+
+
+def png_size(path):
+    """(H, W) of a PNG from its IHDR chunk (the preprocessing uses the image shape only, never the pixels)."""
+    with open(path, "rb") as fh:
+        head = fh.read(24)
+    if len(head) < 24 or head[:8] != _PNG_MAGIC or head[12:16] != b"IHDR":
+        raise ValueError("%s: not a PNG file" % path)
+    w, h = int.from_bytes(head[16:20], "big"), int.from_bytes(head[20:24], "big")
+    if w <= 0 or h <= 0:
+        raise ValueError("%s: PNG size %d x %d" % (path, w, h))
+    return h, w

@@ -13,6 +13,7 @@ TF's allocate_output, and the kernels run on torch's current stream (CUDA-graph 
 import ctypes
 import math
 
+import numpy as np
 import torch
 
 from ._lib import check, lib
@@ -1698,3 +1699,57 @@ def mixup_paste_points(points, offsets, sem_labels, ids, db_points, db_offsets, 
                                          _p(db_offsets), _p(db_boxes), _p(db_classes), _p(planes), _p(accepted), _p(out_offsets),
                                          _p(slot_start), _p(out), _p(sem), _stream()), "mixup_paste_points")
     return out, sem
+
+
+# ---- KITTI preprocessing (csrc/prepare.cu, DESIGN.md section 3.14) --------------------------------------------------
+PREP_MAX_FRAMES = 4096              # frames per call
+PREP_MAX_FRAME_POINTS = 262144      # raw points per frame
+PREP_MAX_BATCH_POINTS = 16777216    # raw points per call
+PREP_EXTENTS = (-40.0, 40.0, -5.0, 3.0, 0.0, 70.0)   # POINT_CLOUD_RANGE of 3dssd.yaml: x, y, z of the rect frame
+
+
+def _prep_host(a, name, dtype):
+    if isinstance(a, torch.Tensor):
+        if a.device.type != "cpu":
+            raise ValueError("%s must be a host array (it is checked before the launch)" % name)
+        a = a.numpy()
+    return np.ascontiguousarray(np.asarray(a), dtype)
+
+
+def prepare_points(points, offsets, calib, image_hw, extents=PREP_EXTENTS):
+    """The image-FOV and extents filters of raw velodyne frames in the rect frame (ssd3d_prepare_points): points [T, 4]
+    float32 (device) packed frame after frame, offsets [b + 1] (host), calib [b, 33] float64 (device: V2C 12, R0 9, P2 12,
+    row-major), image_hw [b, 2] (host, H and W > 0), extents 6 floats (host) -> (kept [T, 4] float64, kept_offsets [b + 1]
+    int32) on the device: frame s's kept points (rect x, y, z, intensity) in input order at rows kept_offsets[s] ..
+    kept_offsets[s+1]-1; rows from kept_offsets[b] on are not written.  Nothing synchronises the host, so the kept total
+    is known on the host only after the caller reads kept_offsets."""
+    points = _req(points, "points", torch.float32, 2, 4)
+    calib = _req(calib, "calib", torch.float64, 2, 33)
+    off = _prep_host(offsets, "offsets", np.int64).reshape(-1)
+    hw = _prep_host(image_hw, "image_hw", np.int64)
+    ext = _prep_host(extents, "extents", np.float64).reshape(-1)
+    b = off.size - 1
+    if b < 1 or b > PREP_MAX_FRAMES:
+        raise ValueError("offsets must hold b + 1 entries with 1 <= b <= %d, got %d" % (PREP_MAX_FRAMES, off.size))
+    n = np.diff(off)
+    if off[0] != 0 or off[-1] != points.shape[0] or (n < 0).any():
+        raise ValueError("offsets must rise from 0 to the point count %d, got %s .. %s" % (points.shape[0], off[0], off[-1]))
+    if n.max() > PREP_MAX_FRAME_POINTS or off[-1] > PREP_MAX_BATCH_POINTS:
+        raise ValueError("at most %d points per frame and %d per call, got %d and %d" % (
+            PREP_MAX_FRAME_POINTS, PREP_MAX_BATCH_POINTS, n.max(), off[-1]))
+    if calib.shape[0] != b or hw.shape != (b, 2):
+        raise ValueError("calib %s and image_hw %s must hold %d frames" % (tuple(calib.shape), hw.shape, b))
+    if (hw <= 0).any() or (hw > 2 ** 31 - 1).any():
+        raise ValueError("every image size H, W must be positive, got %s" % hw[(hw <= 0).any(1)][:1].tolist())
+    if ext.shape != (6,) or np.isnan(ext).any():
+        raise ValueError("extents must be 6 numbers (x0, x1, y0, y1, z0, z1), got %s" % (ext.tolist(),))
+    max_n = int(n.max())
+    dev = points.device
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev, non_blocking=True)
+    d_off, d_hw, d_ext = up(off.astype(np.int32)), up(hw.astype(np.int32)), up(ext)
+    ws = torch.empty((int(lib().ssd3d_prepare_workspace(b, max_n)),), dtype=torch.uint8, device=dev)
+    kept = torch.empty((points.shape[0], 4), dtype=torch.float64, device=dev)
+    kept_off = torch.empty((b + 1,), dtype=torch.int32, device=dev)
+    check(lib().ssd3d_prepare_points(b, max_n, int(off[-1]), _p(points), _p(d_off), _p(calib), _p(d_hw), _p(d_ext), _p(ws), _p(kept),
+                                     _p(kept_off), _stream()), "prepare_points")
+    return kept, kept_off

@@ -608,6 +608,28 @@ int ssd3d_mixup_paste_points(int b, int s, int max_slots, const float *points, c
                              const int *db_classes, const double *planes, const int *accepted, const int *out_offsets,
                              const int *slot_start, float *out_points, int *out_sem_labels, ssd3d_stream_t stream);
 
+/* ---- KITTI preprocessing (csrc/prepare.cu, DESIGN.md section 3.14) --------------------------------------------------
+ * A batch of b raw velodyne frames: points [total, 4] float32 (x, y, z, intensity) packed frame after frame, DEVICE
+ * offsets [b + 1] int32, calib [b, 33] float64 per frame (Tr_velo_to_cam V [3, 4], R0_rect R [3, 3], P2 P [3, 4], each
+ * row-major), image_hw [b, 2] int32 (H, W > 0), extents [6] float64 (x0, x1, y0, y1, z0, z1 of the rect frame).  Limits:
+ * b <= 4096 frames, max_n (the largest frame) <= 262144 points, total <= 16777216 points.  In float64, every product,
+ * sum and quotient rounded once and the inputs widened exactly from float32:
+ *   ref_j  = ((x V[j,0] + y V[j,1]) + z V[j,2]) + V[j,3]
+ *   rect_i = (R[i,0] ref_0 + R[i,1] ref_1) + R[i,2] ref_2
+ *   h_k    = ((rect_0 P[k,0] + rect_1 P[k,1]) + rect_2 P[k,2]) + P[k,3],   u = h_0 / h_2,  v = h_1 / h_2
+ * a point is kept iff 0 <= u < W, 0 <= v < H, rect_2 >= 0 and x0 < rect_0 < x1, y0 < rect_1 < y1, z0 < rect_2 < z1 (a NaN
+ * fails every test).  out_points [total, 4] float64: rows out_offsets[s] .. out_offsets[s+1]-1 (DEVICE int32 [b + 1], an
+ * exclusive scan of the kept counts) hold frame s's kept points (rect_0, rect_1, rect_2, intensity) in input order; rows
+ * from out_offsets[b] on are not written.  No atomics, nothing synchronises the host; the same inputs give the same bits.
+ * Workspace: ssd3d_prepare_workspace(b, max_n) bytes (0 when a limit is exceeded). */
+#define SSD3D_PREPARE_MAX_FRAMES 4096
+#define SSD3D_PREPARE_MAX_FRAME_POINTS 262144
+#define SSD3D_PREPARE_MAX_BATCH_POINTS 16777216
+size_t ssd3d_prepare_workspace(int b, int max_n);
+int ssd3d_prepare_points(int b, int max_n, int total, const float *points, const int *offsets, const double *calib,
+                         const int *image_hw, const double *extents, void *workspace, double *out_points, int *out_offsets,
+                         ssd3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
