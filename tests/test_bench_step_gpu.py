@@ -555,8 +555,12 @@ def test_ball_query_vs_float64(bench, step):
 def test_last_scene_vs_oracle_layerwise(oracle_ops, bench, step):
     """Teacher-forced: every oracle layer takes scene 7's own GPU outputs of the layers before it, so the indices
     (D-FPS, F-FPS on features, ball query) must match bit for bit by construction of the arithmetic."""
+    scene_vs_oracle_layerwise(oracle_ops, bench, step, SCENES - 1)
+
+
+def scene_vs_oracle_layerwise(oracle_ops, bench, step, s):
+    """Scene s of a step against the CPU oracle, layer by layer on the step's own inputs to each layer."""
     from oracle import layers as olayers
-    s = SCENES - 1
     xyz_l, feat_l, fps_l, dbg = step[0]
     npy = lambda t: None if t is None else t[s:s + 1].cpu().numpy()
     for li, spec in enumerate(bench.arch, start=1):
