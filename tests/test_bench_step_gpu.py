@@ -342,6 +342,11 @@ def sa_layer64(params, spec, xyz, feats, fps_idx, src_xyz, idx_list, cnt_list):
 
 @pytest.mark.gpu
 def test_every_layer_vs_float64(pkg, bench, step):
+    every_layer_vs_float64(pkg, bench, step)
+
+
+def every_layer_vs_float64(pkg, bench, step):
+    """Every inference layer and the head of a step against float64, teacher-forced on the step's own indices."""
     (xyz_l, feat_l, fps_l, dbg), (_, _, raw) = step
     d = lambda t: t.double()
     checked = []
@@ -413,6 +418,11 @@ def assert_scores_2ulp(got, cls):
 
 @pytest.mark.gpu
 def test_decode_and_nms(pkg, bench, step):
+    decode_and_nms(pkg, step)
+
+
+def decode_and_nms(pkg, step):
+    """A step's decoded boxes and scores, forced ties on scene 0's outputs, and the BEV NMS of every scene."""
     from oracle import head as ohead
     (xyz_l, feat_l, _, _), (blk, cnt, raw) = step
     ctr, reg, cls = xyz_l[6], head_reg(raw), raw["cls"]
@@ -482,6 +492,11 @@ def assert_fps(p, idx, what, feature_space=False):
 
 @pytest.mark.gpu
 def test_fps_farthest_point_property(bench, step):
+    fps_farthest_point_property(step)
+
+
+def fps_farthest_point_property(step):
+    """Every D-FPS and F-FPS of a step maximises the running min-distance (assert_fps)."""
     xyz_l, feat_l, fps_l, _ = step[0]
     d = lambda t: t.double()
     assert_fps(d(xyz_l[0]), fps_l[1], "layer-1 D-FPS")
@@ -540,6 +555,11 @@ def ball_query_check(xyz, new_xyz, radii, nsamples, dilated, idx_list, cnt_list,
 
 @pytest.mark.gpu
 def test_ball_query_vs_float64(bench, step):
+    ball_query_vs_float64(bench, step)
+
+
+def ball_query_vs_float64(bench, step):
+    """Every ball query of a step against float64 squared distances (ball_query_check)."""
     xyz_l, _, _, dbg = step[0]
     for li, spec in enumerate(bench.arch, start=1):
         if spec[11] != "SA_Layer" or not len(spec[2]):

@@ -446,17 +446,22 @@ def test_linear_tc_transposed_at_step_shapes(pkg, cuda):
 # ---- G: full-size gradients against the teacher-forced float64 restatement ------------------------------------------
 
 def test_full_size_gradients_teacher_forced(pkg, cuda):
-    """ARCH_3DSSD + conv1d_0 + head at b = 2 x 16384 through the trainable path, loss = a random linear functional of
-    the head outputs and the vote offsets.  The layer loop of backbone.train_forward is driven here with return_debug, so
+    """Two KITTI-like scenes (full_size_gradients_teacher_forced)."""
+    synth = importlib.import_module("3dssd_b200.synth")
+    full_size_gradients_teacher_forced(pkg, cuda, synth.kitti_like(2, 16384, seed=3))
+
+
+def full_size_gradients_teacher_forced(pkg, cuda, points):
+    """ARCH_3DSSD + conv1d_0 + head on points [b, 16384, 4] through the trainable path, loss = a random linear
+    functional of the head outputs and the vote offsets.  The layer loop of backbone.train_forward is driven here with return_debug, so
     that sampling, neighbour lists, ReLU masks and pooling winners can be handed to the float64 restatement of
     test_train_grad_cpu (run on the GPU); its outputs must first equal train_forward's bit for bit.  Every trainable
     tensor's gradient is then held to 1e-3 (compare_grads)."""
     from test_train_grad_cpu import compare_grads, gather_rows, recording, ref_conv, ref_head, ref_leaves, ref_sa_msg, ref_vote
     cfg, L = pkg.config, pkg.layers_util
-    arch, b, n = cfg.ARCH_3DSSD, 2, 16384
+    arch = cfg.ARCH_3DSSD
     assert cfg.AGGREGATION_SA_FEATURE
-    synth = importlib.import_module("3dssd_b200.synth")
-    xyz, feat = pkg.tf_ops.split_points(torch.from_numpy(synth.kitti_like(b, n, seed=3)).to(cuda))
+    xyz, feat = pkg.tf_ops.split_points(torch.from_numpy(np.ascontiguousarray(points, dtype=np.float32)).to(cuda))
     d = pkg.params.init_params(arch, 1, seed=5, random_bias=True)
     d.update(pkg.params.init_head_params(cfg.layer_channels(arch, 1)[-1], seed=6))
     with torch.no_grad():
