@@ -28,6 +28,7 @@ _SIGNATURES = {
     "ssd3d_group_point": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_three_nn": [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_three_interpolate": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "ssd3d_fp_interp_split": [c_int, c_int, c_int, c_int, c_int] + [c_void_p] * 6 + [c_int, c_void_p],
     "ssd3d_calc_square_dist": [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "ssd3d_group_concat": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                            c_void_p],
@@ -89,6 +90,8 @@ _SIGNATURES = {
     "ssd3d_vote_translate": [c_long, c_void_p, c_void_p, c_int, c_float, c_float, c_float, c_void_p, c_void_p],
     "ssd3d_decode_dist_anchor_free": [c_long, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                       c_void_p],
+    "ssd3d_decode_bin_anchor": [c_long, c_int, c_float, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                c_void_p, c_void_p],
     "ssd3d_linear_wgrad_workspace": [c_long, c_int, c_int],
     "ssd3d_linear_wgrad": [c_long, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, ctypes.c_size_t, c_void_p, c_void_p,
                            c_void_p],

@@ -25,19 +25,22 @@ class SABackbone:
 
     def __init__(self, arch=None, params=None, in_channels=_cfg.INPUT_CHANNELS - 3, device="cuda", ffps_mode="direct",
                  seed=0, mlp_mode="tc", fuse_scale=True, head=None, gather_in_kernel=True, hoist_first=2, fps_cluster=0,
-                 latency_mode=False, fps_parts=(0.34, 0.28, 0.22, 0.16), fps_packet=False, fps_bucket=None):
+                 latency_mode=False, fps_parts=(0.34, 0.28, 0.22, 0.16), fps_packet=False, fps_bucket=None, aggregation=None):
         """fps_cluster: CTAs per scene of the D-FPS kernels (0 heuristic, < 0 cap; see tf_ops.farthest_point_sample).
         latency_mode: minimise the time of ONE step instead of the throughput of many in flight -- every SA layer
         consumes its sampling in parts (pointnet_sa_module_msg `fps_parts`): a lone D-FPS (layer 1) is cut into
         resumable launches with the given round fractions, fusion-sampling layers hand over their halves separately.
         fps_bucket: layer-1 D-FPS kernel (tf_ops.farthest_point_sample `bucket_kernel`): the single-CTA kernel with spatial
         pruning occupies one SM per scene but its round is longer than the 8-CTA cluster kernel's, so the default takes it
-        for throughput (many steps in flight share the SMs) and the cluster kernel in latency mode.  Same indices."""
+        for throughput (many steps in flight share the SMs) and the cluster kernel in latency mode.  Same indices.
+        aggregation: whether SA layers end in their aggregation conv (MODEL.NETWORK.AGGREGATION_SA_FEATURE; None takes
+        config.AGGREGATION_SA_FEATURE, 3DSSD's True; PointRCNN's RPN is built with False)."""
         self.arch = _cfg.ARCH_3DSSD if arch is None else arch
         self.in_channels = in_channels
         self.device = torch.device(device)
+        self.aggregation = _cfg.AGGREGATION_SA_FEATURE if aggregation is None else bool(aggregation)
         if params is None:
-            params = init_params(self.arch, in_channels, seed=seed)
+            params = init_params(self.arch, in_channels, seed=seed, aggregation=self.aggregation)
         self.params = prepare(params, self.device).prepare_all()
         self.ffps_mode = ffps_mode
         self.mlp_mode = mlp_mode
@@ -51,6 +54,7 @@ class SABackbone:
         self.fps_parts = fps_parts if isinstance(fps_parts, int) else list(fps_parts)
         self.head = head                      # optional head.DetectionHead: real detections instead of the stand-in block
         self._graph = None
+        self._split = {}                      # layer index -> (features, split features) of the FP layer the head reads
 
     def forward(self, points, return_debug=False):
         if points.dim() != 3 or points.shape[-1] != 3 + self.in_channels:
@@ -70,7 +74,8 @@ class SABackbone:
                     parts = self.fps_parts if (len(npoint) == 1 and method[0] == "D-FPS") else True
                 r = L.pointnet_sa_module_msg(xyz_list[xyz_i[0]], feat_list[feat_i[0]], radius, nsample, mlps, False,
                                              None, bn, rng, method, npoint, former_idx, attn, scope, dilated, vote_ctr,
-                                             agg, params=self.params, ffps_mode=self.ffps_mode, return_debug=True,
+                                             agg, params=self.params, ffps_mode=self.ffps_mode, aggregation=self.aggregation,
+                                             return_debug=True,
                                              mlp_mode=self.mlp_mode, fuse_scale=self.fuse_scale,
                                              gather_in_kernel=self.gather_in_kernel, hoist_first=self.hoist_first,
                                              fps_cluster=self.fps_cluster, fps_parts=parts, fps_packet=self.fps_packet,
@@ -87,9 +92,15 @@ class SABackbone:
                 fps_list.append(None); dbg.append({})
             elif ltype == "FP_Layer":
                 xyz_list.append(xyz_list[xyz_i[0]])
-                feat_list.append(L.pointnet_fp_module(xyz_list[xyz_i[0]], xyz_list[xyz_i[1]], feat_list[feat_i[0]],
-                                                      feat_list[feat_i[1]], mlps, False, None, scope, bn,
-                                                      params=self.params))
+                # the layer the head reads alone hands it its split features (the operand of the head's first convs)
+                li = len(feat_list)
+                split = self.head is not None and list(self.head.feature_index) == [li] and len(mlps) > 0
+                r = L.pointnet_fp_module(xyz_list[xyz_i[0]], xyz_list[xyz_i[1]], feat_list[feat_i[0]], feat_list[feat_i[1]],
+                                         mlps, False, None, scope, bn, params=self.params, want_split=split)
+                if split:
+                    r, sp = r
+                    self._split[li] = (r, sp)
+                feat_list.append(r)
                 fps_list.append(None); dbg.append({})
             else:
                 raise ValueError("unknown layer type %r" % (ltype,))
@@ -104,7 +115,10 @@ class SABackbone:
         """Per-scene detection block [B,100,9] + count [B]: the detection head + decode + BEV NMS when a head is
         attached, otherwise the stand-in derived from the CG layer.  out=(block, count) preallocated outputs."""
         if self.head is not None:
-            return self.head(xyz_list, feat_list, out=out)
+            fi = list(self.head.feature_index)
+            kept = self._split.get(fi[0]) if len(fi) == 1 else None
+            split = kept[1] if kept is not None and kept[0] is feat_list[fi[0]] else None   # only for these very features
+            return self.head(xyz_list, feat_list, out=out, split=split)
         blk, cnt = self.detection_block(xyz_list, feat_list)
         if out is not None:
             out[0].copy_(blk); out[1].copy_(cnt)

@@ -36,6 +36,49 @@ AGGREGATION_SA_FEATURE = True
 POINTS_NUM = 16384
 INPUT_CHANNELS = 4  # x, y, z, intensity
 
+# PointRCNN's first stage (the RPN): FIRST_STAGE.ARCHITECTURE of
+# /root/reference/configs/kitti/pointrcnn/tiny_pointrcnn_stage1.yaml:48-81.  The model sets AGGREGATION_SA_FEATURE to
+# False (yaml:45), so the aggregation_channel fields below are not used: build it with aggregation=False.
+ARCH_POINTRCNN_RPN = [
+    [[0], [0], [0.1, 0.5], [16, 32], [[16, 16, 32], [32, 32, 64]], True,
+     [-1], ['D-FPS'], [4096],
+     -1, False, 'SA_Layer', 'rpn_layer1', False, -1, 128],
+    [[1], [1], [0.5, 1.0], [16, 32], [[64, 64, 128], [64, 96, 128]], True,
+     [-1], ['D-FPS'], [1024],
+     -1, False, 'SA_Layer', 'rpn_layer2', False, -1, 256],
+    [[2], [2], [1.0, 2.0], [16, 32], [[128, 196, 256], [128, 196, 256]], True,
+     [-1], ['D-FPS'], [256],
+     -1, False, 'SA_Layer', 'rpn_layer3', False, -1, 256],
+    [[3], [3], [2.0, 4.0], [16, 32], [[256, 256, 512], [256, 384, 512]], True,
+     [-1], ['D-FPS'], [64],
+     -1, False, 'SA_Layer', 'rpn_layer4', False, -1, 256],
+    [[3, 4], [3, 4], -1, -1, [512, 512], True,
+     [], [], [],
+     -1, False, 'FP_Layer', 'rpn_fp_layer4', False, -1, 256],
+    [[2, 5], [2, 5], -1, -1, [512, 512], True,
+     [], [], [],
+     -1, False, 'FP_Layer', 'rpn_fp_layer3', False, -1, 256],
+    [[1, 6], [1, 6], -1, -1, [256, 256], True,
+     [], [], [],
+     -1, False, 'FP_Layer', 'rpn_fp_layer2', False, -1, 256],
+    [[0, 7], [0, 7], -1, -1, [128, 128], True,
+     [], [], [],
+     -1, False, 'FP_Layer', 'rpn_fp_layer1', False, -1, 256],
+]
+AGGREGATION_POINTRCNN = False      # MODEL.NETWORK.AGGREGATION_SA_FEATURE (tiny_pointrcnn_stage1.yaml:45)
+
+# Detection heads: (xyz_index, feature_index, op_type, mlp_list, bn, layer_type, scope), with the MODEL.FIRST_STAGE
+# constants that select and parametrise their regression and post-processing.
+HEAD_3DSSD = [[6], [6], 'conv1d', [128], True, 'Det', '']                     # 3dssd.yaml:68
+STAGE_3DSSD = {"REGRESSION": "Dist-Anchor-free", "MAX_OUTPUT_NUM": 100, "NMS_THRESH": 0.1}   # 3dssd.yaml:70-72
+HEAD_POINTRCNN_RPN = [[8], [8], 'conv1d', [], True, 'Det', 'rpn_head']       # tiny_pointrcnn_stage1.yaml:82
+STAGE_POINTRCNN_RPN = {                                                        # tiny_pointrcnn_stage1.yaml:102-116
+    "REGRESSION": "Bin-Anchor", "MAX_OUTPUT_NUM": 100, "NMS_THRESH": 0.85,
+    "HALF_BIN_SEARCH_RANGE": 3.0, "BIN_CLASS_NUM": 12, "CLS_ACTIVATION": "Sigmoid",
+    # the Car mean size (l, h, w), the one anchor of CLS_LIST ('Car',): g_type_mean_size['Kitti_Car'] (lib/utils/model_util.py:19)
+    "ANCHOR_SIZE": (3.88311640418, 1.62856739989, 1.52563191462),
+}
+
 # BASELINE.json configs[0] / SURVEY.md section 8d "config 1": one SA layer N=4096 -> 1024, plain ball query
 ARCH_SINGLE_SA = [
     [[0], [0], [0.4], [32], [[64, 64, 128]], True,
@@ -44,8 +87,10 @@ ARCH_SINGLE_SA = [
 ]
 
 
-def layer_channels(arch, in_channels):
-    """Feature channel count after every layer of `arch` (index 0 = network input)."""
+def layer_channels(arch, in_channels, aggregation=None):
+    """Feature channel count after every layer of `arch` (index 0 = network input).  aggregation: whether SA layers end
+    in their aggregation conv (MODEL.NETWORK.AGGREGATION_SA_FEATURE); None takes AGGREGATION_SA_FEATURE."""
+    aggregation = AGGREGATION_SA_FEATURE if aggregation is None else aggregation
     ch = [in_channels]
     for spec in arch:
         ltype, mlps, agg = spec[11], spec[4], spec[15]
@@ -53,7 +98,7 @@ def layer_channels(arch, in_channels):
         if ltype == 'SA_Layer':
             if len(spec[2]) == 0:
                 ch.append(cin)
-            elif agg is not None and agg != -1 and AGGREGATION_SA_FEATURE:
+            elif agg is not None and agg != -1 and aggregation:
                 ch.append(agg)
             else:
                 ch.append(sum(m[-1] for m in mlps))

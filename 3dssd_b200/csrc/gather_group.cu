@@ -5,7 +5,7 @@
 // (interpolation/tf_interpolate_g.cu:87-113).  The reference launches a fixed <<<512,64>>> grid-stride
 // grid whatever the size; here the grid covers the output with 16-byte vector accesses when the channel
 // count allows it, so a warp moves whole contiguous rows.
-#include "common.cuh"
+#include "three_nn.cuh"
 
 namespace ssd3d {
 
@@ -84,7 +84,7 @@ __global__ void group_concat_kernel(long rows, int n, int c, int m, int ns, cons
     }
 }
 
-// out[b,i,ch] = fma(w3,c3, fma(w1,c1, w2*c2))   -- the reference's contraction (PTX of tf_interpolate_g.cu:110)
+// out[b,i,ch] = fma(w3,c3, fma(w1,c1, w2*c2))   -- three_interp_value, the reference's contraction
 __global__ void three_interpolate_kernel(long total, int m, int c, int n, const float *__restrict__ points,
                                          const int *__restrict__ idx, const float *__restrict__ weight,
                                          float *__restrict__ out)
@@ -98,9 +98,7 @@ __global__ void three_interpolate_kernel(long total, int m, int c, int n, const 
         const float w1 = __ldg(weight + pt * 3), w2 = __ldg(weight + pt * 3 + 1), w3 = __ldg(weight + pt * 3 + 2);
         const float c1 = __ldg(pts + (size_t)i1 * c + ch), c2 = __ldg(pts + (size_t)i2 * c + ch),
                     c3 = __ldg(pts + (size_t)i3 * c + ch);
-        float t = __fmul_rn(w2, c2);
-        t = __fmaf_rn(w1, c1, t);
-        out[e] = __fmaf_rn(w3, c3, t);
+        out[e] = three_interp_value(w1, w2, w3, c1, c2, c3);
     }
 }
 

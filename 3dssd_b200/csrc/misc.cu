@@ -7,6 +7,8 @@
 //   * decode_dist_anchor_free  anchor_decoder.py:86-112 + decode_class2angle :6-14 + the sigmoid of
 //                         single_stage_detector.py:210-211: raw head outputs -> (x,y,z,l,h,w,ry) + score, the
 //                         inputs of bev_nms.
+//   * decode_bin_anchor   the same for PointRCNN's 'Bin-Anchor' regression: anchor_decoder.py:115-164 on the anchors of
+//                         generate_anchors.py:33-65 (one anchor size per point) + the sigmoid.
 // All HBM-bound copies / a few flops per element; sized far below one wave, so launch latency is the cost.
 #include "common.cuh"
 
@@ -98,6 +100,46 @@ __global__ void decode_kernel(long rows, int nbins, const float *__restrict__ ct
     scores[r] = (float)(1.0 / (1.0 + exp(-(double)cls[r * ldcls])));
 }
 
+// argmax over nb logits, ties to the first index (tf.argmax)
+__device__ __forceinline__ int first_argmax(const float *g, int nb)
+{
+    int bin = 0;
+    float bv = g[0];
+    for (int k = 1; k < nb; k++)
+        if (g[k] > bv) { bv = g[k]; bin = k; }
+    return bin;
+}
+
+// one thread per candidate point; reg row = [x_bin nb | x_res nb | z_bin nb | z_res nb | y_res | size_res 3 |
+// angle_cls na | angle_res na].  TF's fp32 order, one rounding per operation:
+//   x = (ax - half_range) + ((bin + res) + 0.5) * interval,  z likewise
+//   y = (ay + h / 2) + y_res,  lhw = max(anchor_lhw + res, 0.1),  ry = 0 + (bin + res) * (2 pi / na)
+__global__ void decode_bin_kernel(long rows, int nb, int na, const float *__restrict__ ctr, const float *__restrict__ reg,
+                                  int ldreg, const float *__restrict__ cls, int ldcls, float half_range, float bin_interval,
+                                  float angle_interval, float al, float ah, float aw, float *__restrict__ boxes,
+                                  float *__restrict__ scores)
+{
+    const long r = blockIdx.x * (long)blockDim.x + threadIdx.x;
+    if (r >= rows) return;
+    const float *g = reg + r * ldreg;
+    const float *c = ctr + r * 3;
+    float *o = boxes + r * 7;
+    const int xb = first_argmax(g, nb), zb = first_argmax(g + 2 * nb, nb);
+    const float dx = __fmul_rn(__fadd_rn(__fadd_rn((float)xb, g[nb + xb]), 0.5f), bin_interval);
+    const float dz = __fmul_rn(__fadd_rn(__fadd_rn((float)zb, g[3 * nb + zb]), 0.5f), bin_interval);
+    const float *off = g + 4 * nb;
+    o[0] = __fadd_rn(__fsub_rn(c[0], half_range), dx);
+    o[1] = __fadd_rn(__fadd_rn(c[1], __fmul_rn(ah, 0.5f)), off[0]);
+    o[2] = __fadd_rn(__fsub_rn(c[2], half_range), dz);
+    o[3] = fmaxf(__fadd_rn(al, off[1]), 0.1f);
+    o[4] = fmaxf(__fadd_rn(ah, off[2]), 0.1f);
+    o[5] = fmaxf(__fadd_rn(aw, off[3]), 0.1f);
+    const float *ang = off + 4;
+    const int ab = first_argmax(ang, na);
+    o[6] = __fadd_rn(0.0f, __fmul_rn(__fadd_rn(__fadd_rn((float)ab, ang[na + ab]), 0.0f), angle_interval));
+    scores[r] = (float)(1.0 / (1.0 + exp(-(double)cls[r * ldcls])));    // as decode_kernel
+}
+
 // out[s, off_i + q, :] = src_i[s, q, :] for the (up to 8) row blocks of a scene: tf.concat(axis=1) of per-part results
 struct ConcatRowsArgs {
     const float *src[8];
@@ -180,6 +222,25 @@ extern "C" int ssd3d_decode_dist_anchor_free(long rows, int angle_bins, const fl
     decode_kernel<<<(int)((rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>(rows, angle_bins, center_xyz, pred_reg, ld_reg,
                                                                               pred_cls, ld_cls, interval, boxes, scores);
     SSD3D_LAUNCH_CHECK("decode_kernel");
+}
+
+extern "C" int ssd3d_decode_bin_anchor(long rows, int bin_num, float half_bin_search_range, int angle_bins,
+                                       const float *center_xyz, const float *pred_reg, int ld_reg, const float *pred_cls,
+                                       int ld_cls, const float *anchor_lhw, float *boxes, float *scores, ssd3d_stream_t stream)
+{
+    SSD3D_REQUIRE(rows >= 0 && bin_num >= 1 && angle_bins >= 1 && ld_reg >= 4 * bin_num + 4 + 2 * angle_bins && ld_cls >= 1,
+                  "decode_bin_anchor: bad shape rows=%ld bins=%d angle_bins=%d ld_reg=%d ld_cls=%d", rows, bin_num, angle_bins,
+                  ld_reg, ld_cls);
+    SSD3D_REQUIRE(anchor_lhw != nullptr, "decode_bin_anchor: null anchor size");
+    if (rows == 0) return 0;
+    SSD3D_REQUIRE(center_xyz && pred_reg && pred_cls && boxes && scores, "decode_bin_anchor: null pointer");
+    // the Python constants of anchor_decoder.py:137-145 / :160, rounded once to the float32 TF computes in
+    const float bin_interval = (float)((double)half_bin_search_range * 2.0 / bin_num);
+    const float angle_interval = (float)(2.0 * 3.14159265358979323846 / angle_bins);
+    decode_bin_kernel<<<(int)((rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+        rows, bin_num, angle_bins, center_xyz, pred_reg, ld_reg, pred_cls, ld_cls, half_bin_search_range, bin_interval,
+        angle_interval, anchor_lhw[0], anchor_lhw[1], anchor_lhw[2], boxes, scores);
+    SSD3D_LAUNCH_CHECK("decode_bin_kernel");
 }
 
 extern "C" int ssd3d_concat_rows(int b, int parts, const float *const *src, const int *m, int c, float *out,

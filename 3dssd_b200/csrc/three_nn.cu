@@ -3,18 +3,13 @@
 // Replaces three_nn_gpu (/root/reference/lib/utils/tf_ops/interpolation/tf_interpolate_g.cu:24-84; CPU twin
 // tf_interpolate.cpp:86-129).  The reference runs one thread per unknown point with a serial loop over the
 // m known points read from global memory; here a block stages the known points once per 1024-point tile in
-// shared memory (read by all lanes as a broadcast) and every thread keeps its running best-3 in registers.
-//
-// Bit-exactness: squared distance with the reference's contraction (dy*dy, fma(dx,dx,.), fma(dz,dz,.)),
-// strict '<' so the earliest index wins ties.  The reference widens to double only to compare against its
-// 1e40 initial value; an fp32 compare against +inf takes exactly the same decisions (inf < inf is false,
-// as inf < 1e40 is), and (float)1e40 == +inf is what the reference stores when fewer than 3 points exist.
-#include "common.cuh"
+// shared memory (read by all lanes as a broadcast) and every thread keeps its running best-3 in registers
+// (three_nn.cuh, which also states why the indices and distances are the reference's bit for bit).
+#include "three_nn.cuh"
 
 namespace ssd3d {
 
 constexpr int TNN_THREADS = 256;
-constexpr int TNN_TILE = 1024;
 
 __global__ void __launch_bounds__(TNN_THREADS)
 three_nn_kernel(int n, int m, const float *__restrict__ xyz1, const float *__restrict__ xyz2,
@@ -25,32 +20,13 @@ three_nn_kernel(int n, int m, const float *__restrict__ xyz1, const float *__res
     const int i = blockIdx.x * TNN_THREADS + threadIdx.x;
     const bool valid = i < n;
     const float *u = xyz1 + ((size_t)scene * n + (valid ? i : 0)) * 3;
-    const float ux = u[0], uy = u[1], uz = u[2];
-    const float *known = xyz2 + (size_t)scene * m * 3;
-
-    float b1 = INFINITY, b2 = INFINITY, b3 = INFINITY;
-    int i1 = 0, i2 = 0, i3 = 0;
-    for (int base = 0; base < m; base += TNN_TILE) {
-        const int npts = min(TNN_TILE, m - base);
-        __syncthreads();
-        for (int e = threadIdx.x; e < npts * 3; e += TNN_THREADS) tile[e] = known[(size_t)base * 3 + e];
-        __syncthreads();
-#pragma unroll 4
-        for (int j = 0; j < npts; j++) {
-            const float dx = tile[j * 3] - ux, dy = tile[j * 3 + 1] - uy, dz = tile[j * 3 + 2] - uz;
-            float d = __fmul_rn(dy, dy);
-            d = __fmaf_rn(dx, dx, d);
-            d = __fmaf_rn(dz, dz, d);
-            const int k = base + j;
-            if (d < b1) { b3 = b2; i3 = i2; b2 = b1; i2 = i1; b1 = d; i1 = k; }
-            else if (d < b2) { b3 = b2; i3 = i2; b2 = d; i2 = k; }
-            else if (d < b3) { b3 = d; i3 = k; }
-        }
-    }
+    float best[3];
+    int bidx[3];
+    three_nn_scan(m, xyz2 + (size_t)scene * m * 3, tile, u[0], u[1], u[2], best, bidx);
     if (valid) {
         const size_t o = ((size_t)scene * n + i) * 3;
-        dist[o] = b1; dist[o + 1] = b2; dist[o + 2] = b3;
-        idx[o] = i1; idx[o + 1] = i2; idx[o + 2] = i3;
+        dist[o] = best[0]; dist[o + 1] = best[1]; dist[o + 2] = best[2];
+        idx[o] = bidx[0]; idx[o + 1] = bidx[1]; idx[o + 2] = bidx[2];
     }
 }
 

@@ -15,6 +15,7 @@ import math
 
 import torch
 
+from . import config as _cfg
 from . import tf_ops
 from .params import TrainableParams, prepare
 
@@ -22,7 +23,16 @@ ANGLE_CLS_NUM = 12          # MODEL.ANGLE_CLS_NUM (3dssd.yaml:38)
 REG_CHANNELS = 6            # 'Dist-Anchor-free': distances to the 6 faces (head_builder.py:49-55)
 MAX_OUTPUT_NUM = 100        # MODEL.FIRST_STAGE.MAX_OUTPUT_NUM (3dssd.yaml:70)
 NMS_THRESH = 0.1            # MODEL.FIRST_STAGE.NMS_THRESH (3dssd.yaml:71)
-HEAD_3DSSD = [[6], [6], 'conv1d', [128], True, 'Det', '']
+HEAD_3DSSD = _cfg.HEAD_3DSSD
+
+
+def reg_channels(stage):
+    """pred_reg_channel_num of a regression method (head_builder.py:51-58), before the 2 * ANGLE_CLS_NUM angle channels."""
+    if stage["REGRESSION"] == "Dist-Anchor-free":
+        return REG_CHANNELS
+    if stage["REGRESSION"] == "Bin-Anchor":
+        return stage["BIN_CLASS_NUM"] * 4 + 4                 # bin_x / res_x / bin_z / res_z, res_y, 3 size residuals
+    raise NotImplementedError("regression method %r" % (stage["REGRESSION"],))
 
 
 def _scope(scope, name):
@@ -90,39 +100,50 @@ def postprocess(pred_anchors_3d, pred_score, max_output=MAX_OUTPUT_NUM, nms_thre
 
 
 class DetectionHead:
-    """HeadBuilder (head_builder.py) + test_forward + PostProcessor for the 3DSSD head spec."""
+    """HeadBuilder (head_builder.py) + test_forward + PostProcessor for a 'conv1d' / 'Det' head spec.  stage: the
+    MODEL.FIRST_STAGE constants (config.STAGE_3DSSD, the default, or config.STAGE_POINTRCNN_RPN): REGRESSION selects the
+    decode ('Dist-Anchor-free': tf_ops.decode_dist_anchor_free, 'Bin-Anchor': tf_ops.decode_bin_anchor on one anchor of
+    ANCHOR_SIZE per point), MAX_OUTPUT_NUM and NMS_THRESH the post-processing."""
 
-    def __init__(self, head_cfg=None, params=None, device="cuda", cls_num=1):
+    def __init__(self, head_cfg=None, params=None, device="cuda", cls_num=1, stage=None):
         self.cfg = HEAD_3DSSD if head_cfg is None else head_cfg
         self.xyz_index, self.feature_index, self.op_type, self.mlp_list, self.bn, self.layer_type, self.scope = self.cfg
         if self.op_type != 'conv1d' or self.layer_type != 'Det':
-            raise NotImplementedError("only the 'conv1d' / 'Det' head of the 3DSSD configuration is built")
+            raise NotImplementedError("only 'conv1d' / 'Det' heads are built")
+        self.stage = _cfg.STAGE_3DSSD if stage is None else stage
+        self.reg_channels = reg_channels(self.stage)
         self.cls_num = cls_num
         self.params = prepare(params, device)
 
-    def forward(self, xyz_list, feature_list, return_raw=False, out=None):
-        """out=(block, count): preallocated outputs of the NMS (the send buffer of the multi-GPU gather)."""
+    def forward(self, xyz_list, feature_list, return_raw=False, out=None, split=None):
+        """out=(block, count): preallocated outputs of the NMS (the send buffer of the multi-GPU gather).  split: the
+        features' split operand (hi, lo) when the layer that produced them already wrote it."""
         xs = [xyz_list[i] for i in self.xyz_index]                                 # head_builder.py:82-85
         fs = [feature_list[i] for i in self.feature_index]
         xyz = xs[0] if len(xs) == 1 else torch.cat(xs, dim=1)
         feat = (fs[0] if len(fs) == 1 else torch.cat(fs, dim=1)).contiguous()
-        hi, lo = tf_ops.split_rows(feat)
+        hi, lo = tf_ops.split_rows(feat) if split is None else split
         y = feat
         for i, ch in enumerate(self.mlp_list):                                    # :93-95
             y, (hi, lo) = tf_ops.linear_tc(hi, lo, self.params.conv(_scope(self.scope, "conv1d_%d" % i), self.bn),
                                            want_f32=True, want_split=True)
-        pp, sc = self.params, self.scope
+        pp, sc, st = self.params, self.scope, self.stage
         cls = _conv_chain(pp, hi, lo, [(_scope(sc, "pred_cls_base"), self.bn, True), (_scope(sc, "pred_cls"), False, False)])
         reg = _conv_chain(pp, hi, lo, [(_scope(sc, "pred_reg_base"), self.bn, True), (_scope(sc, "pred_reg"), False, False)])
-        # decode_dist_anchor_free + sigmoid (anchor_decoder.py:86-112, single_stage_detector.py:210-211): one kernel
-        boxes, score = tf_ops.decode_dist_anchor_free(xyz, reg, cls, ANGLE_CLS_NUM)
-        block, cnt = tf_ops.bev_nms(boxes, score, NMS_THRESH, MAX_OUTPUT_NUM, cls_id=0, out=out)   # postprocessor.py:52-120
+        # decode + sigmoid (anchor_decoder.py:86-164, single_stage_detector.py:210-211): one kernel
+        if st["REGRESSION"] == "Bin-Anchor":
+            boxes, score = tf_ops.decode_bin_anchor(xyz, reg, cls, st["ANCHOR_SIZE"], st["HALF_BIN_SEARCH_RANGE"],
+                                                    st["BIN_CLASS_NUM"], ANGLE_CLS_NUM)
+        else:
+            boxes, score = tf_ops.decode_dist_anchor_free(xyz, reg, cls, ANGLE_CLS_NUM)
+        block, cnt = tf_ops.bev_nms(boxes, score, st["NMS_THRESH"], st["MAX_OUTPUT_NUM"], cls_id=0, out=out)   # postprocessor.py:52-120
         if return_raw:
             bs, n, _ = reg.shape
-            r4 = reg.view(bs, n, 1, REG_CHANNELS + 2 * ANGLE_CLS_NUM)
-            return block, cnt, {"boxes": boxes.unsqueeze(2), "score": score.unsqueeze(-1), "cls": cls,
-                                "offset": r4[..., :REG_CHANNELS], "angle_cls": r4[..., REG_CHANNELS:REG_CHANNELS + ANGLE_CLS_NUM],
-                                "angle_res": r4[..., REG_CHANNELS + ANGLE_CLS_NUM:], "feat": y}
+            r4 = reg.view(bs, n, 1, self.reg_channels + 2 * ANGLE_CLS_NUM)
+            k = self.reg_channels
+            return block, cnt, {"boxes": boxes.unsqueeze(2), "score": score.unsqueeze(-1), "cls": cls, "reg": reg,
+                                "offset": r4[..., :k], "angle_cls": r4[..., k:k + ANGLE_CLS_NUM],
+                                "angle_res": r4[..., k + ANGLE_CLS_NUM:], "feat": y}
         return block, cnt
 
     __call__ = forward

@@ -474,9 +474,22 @@ def pointnet_sa_module(xyz, points, mlp, is_training, bn_decay, bn, scope, *, pa
     return g.max(dim=1).values if n else g
 
 
-def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay, scope, bn=True, *, params):
-    """Feature propagation: inverse-distance interpolation from (xyz2, points2) onto xyz1, then an MLP."""
+def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay, scope, bn=True, *, params,
+                       want_split=False):
+    """Feature propagation: inverse-distance interpolation from (xyz2, points2) onto xyz1, then an MLP.
+    At inference one kernel (tf_ops.fp_interp_split) writes the first conv's split operand [interpolated | points1] and
+    the convs chain on the tensor cores; there want_split=True returns (features, (hi, lo)), the split features being the
+    operand of whatever conv follows (the detection head).  The training route is the reference's op sequence."""
     pp = params if _trainable(params, is_training) else prepare(params, xyz1.device)
+    if not is_training and len(mlp):
+        hi, lo = tf_ops.fp_interp_split(xyz1, xyz2, points2, points1)                        # :206-214
+        for i in range(len(mlp)):
+            last = i == len(mlp) - 1
+            x, sp = tf_ops.linear_tc(hi, lo, pp.conv("%s/conv_%d" % (scope, i), bn), want_f32=last,
+                                     want_split=want_split or not last)
+            if sp is not None:
+                hi, lo = sp
+        return (x, (hi, lo)) if want_split else x
     dist, idx = tf_ops.three_nn(xyz1, xyz2)
     dist = torch.clamp_min(dist, 1e-10)                            # :207
     inv = 1.0 / dist

@@ -28,11 +28,13 @@ def _conv_init(rng, params, scope, cin, cout, bn):
         params[scope + "/bn/moving_variance"] = rng.uniform(0.5, 1.5, size=(cout,)).astype(np.float32)
 
 
-def init_params(arch, in_channels, seed=0, random_bias=False):
-    """Random weights for every conv of `arch` (numpy dict keyed by TF variable name)."""
+def init_params(arch, in_channels, seed=0, random_bias=False, aggregation=None):
+    """Random weights for every conv of `arch` (numpy dict keyed by TF variable name).  aggregation: as
+    config.layer_channels (None: config.AGGREGATION_SA_FEATURE)."""
+    aggregation = _cfg.AGGREGATION_SA_FEATURE if aggregation is None else aggregation
     rng = np.random.default_rng(seed)
     params = {}
-    ch = _cfg.layer_channels(arch, in_channels)
+    ch = _cfg.layer_channels(arch, in_channels, aggregation)
     for li, spec in enumerate(arch):
         (_, feat_i, radius, _, mlps, bn, _, _, _, _, _, ltype, scope, _, _, agg) = spec
         cin = ch[feat_i[0]]
@@ -44,7 +46,7 @@ def init_params(arch, in_channels, seed=0, random_bias=False):
                 for j, cout in enumerate(mlp):
                     _conv_init(rng, params, "%s/conv%d_%d" % (scope, i, j), c, cout, bn)
                     c = cout
-            if agg is not None and agg != -1 and _cfg.AGGREGATION_SA_FEATURE:
+            if agg is not None and agg != -1 and aggregation:
                 _conv_init(rng, params, scope + "/ensemble", sum(m[-1] for m in mlps), agg, bn)
         elif ltype == "Vote_Layer":
             c = cin

@@ -406,6 +406,32 @@ def three_interpolate(points, idx, weight):
     return _three_interpolate_fwd(points, idx, weight)
 
 
+def fp_interp_split(xyz1, xyz2, points2, points1=None, kp=None):
+    """The first conv operand of an FP layer (layers_util.py:206-214) in one kernel: xyz1 (b,n,3) unknown, xyz2 (b,m,3)
+    known (m >= 1), points2 (b,m,c2), points1 (b,n,c1) or None -> (hi, lo) bf16 (b, n, kp), kp = round16(c2 + c1) by
+    default: split_rows(concat(three_interpolate(points2, idx, w), points1)) bit for bit, with (dist, idx) of three_nn and
+    w_k = inv_k / ((inv_0 + inv_1) + inv_2), inv_k = 1 / max(d_k, 1e-10) in fp32 (include/ssd3d.h)."""
+    xyz1 = _req(xyz1, "xyz1", torch.float32, 3, 3)
+    xyz2 = _req(xyz2, "xyz2", torch.float32, 3, 3)
+    points2 = _req(points2, "points2", torch.float32, 3)
+    b, n, _ = xyz1.shape
+    m, c2 = xyz2.shape[1], points2.shape[2]
+    if xyz2.shape[0] != b or tuple(points2.shape[:2]) != (b, m):
+        raise ValueError("fp_interp_split: xyz2 must be (b, m, 3) and points2 (b, m, c2) with the batch of xyz1")
+    c1 = 0
+    if points1 is not None:
+        points1 = _req(points1, "points1", torch.float32, 3)
+        if tuple(points1.shape[:2]) != (b, n):
+            raise ValueError("fp_interp_split: points1 must be (b, n, c1) with the points of xyz1")
+        c1 = points1.shape[2]
+    kp = round16(c2 + c1) if kp is None else int(kp)
+    hi = torch.empty((b, n, kp), dtype=torch.bfloat16, device=xyz1.device)
+    lo = torch.empty_like(hi)
+    check(lib().ssd3d_fp_interp_split(b, n, m, c2, c1, _p(xyz1), _p(xyz2), _p(points2), _p(points1), _p(hi), _p(lo), kp,
+                                      _stream()), "fp_interp_split")
+    return hi, lo
+
+
 def _three_interpolate_fwd(points, idx, weight):
     b, m, c = points.shape
     n = idx.shape[1]
@@ -1083,6 +1109,25 @@ def decode_dist_anchor_free(center_xyz, pred_reg, pred_cls, angle_bins=12):
     check(lib().ssd3d_decode_dist_anchor_free(b * n, int(angle_bins), _p(center_xyz), _p(pred_reg), pred_reg.shape[2],
                                               _p(pred_cls), pred_cls.shape[2], _p(boxes), _p(scores), _stream()),
           "decode_dist_anchor_free")
+    return boxes, scores
+
+
+def decode_bin_anchor(center_xyz, pred_reg, pred_cls, anchor_lhw, half_bin_search_range=3.0, bin_num=12, angle_bins=12):
+    """anchor_decoder.decode_bin_anchor on the anchors of generate_3d_anchors_by_point_tf + sigmoid in one kernel (one
+    anchor size per point, PointRCNN's RPN): center_xyz (b, n, 3), pred_reg (b, n, >= 4*bin_num + 4 + 2*angle_bins),
+    pred_cls (b, n, >= 1), anchor_lhw = (l, h, w) -> boxes (b, n, 7), scores (b, n)."""
+    center_xyz = _req(center_xyz, "center_xyz", torch.float32, 3, 3)
+    pred_reg = _req(pred_reg, "pred_reg", torch.float32, 3)
+    pred_cls = _req(pred_cls, "pred_cls", torch.float32, 3)
+    b, n, _ = center_xyz.shape
+    if pred_reg.shape[:2] != (b, n) or pred_cls.shape[:2] != (b, n) or pred_reg.shape[2] < 4 * bin_num + 4 + 2 * angle_bins:
+        raise ValueError("pred_reg must be (b, n, >= 4*bin_num + 4 + 2*angle_bins) and pred_cls (b, n, >= 1)")
+    lhw = (ctypes.c_float * 3)(*[float(v) for v in anchor_lhw])
+    boxes = torch.empty((b, n, 7), dtype=torch.float32, device=center_xyz.device)
+    scores = torch.empty((b, n), dtype=torch.float32, device=center_xyz.device)
+    check(lib().ssd3d_decode_bin_anchor(b * n, int(bin_num), float(half_bin_search_range), int(angle_bins), _p(center_xyz),
+                                        _p(pred_reg), pred_reg.shape[2], _p(pred_cls), pred_cls.shape[2],
+                                        ctypes.cast(lhw, ctypes.c_void_p), _p(boxes), _p(scores), _stream()), "decode_bin_anchor")
     return boxes, scores
 
 

@@ -167,6 +167,16 @@ int ssd3d_three_nn(int b, int n, int m, const float *xyz1, const float *xyz2, fl
 int ssd3d_three_interpolate(int b, int m, int c, int n, const float *points, const int *idx, const float *weight,
                             float *out, ssd3d_stream_t stream);
 
+/* The operand of an FP layer's first conv in one pass (pointnet_fp_module, lib/utils/layers_util.py:206-214): for every
+ * unknown point of xyz1[b,n,3] the three nearest of xyz2[b,m,3] (as ssd3d_three_nn), the weights w_k = inv_k / norm
+ * with inv_k = 1 / max(d_k, 1e-10) and norm = (inv_0 + inv_1) + inv_2 (fp32, one rounding per operation), and the row
+ * [three_interpolate(points2[b,m,c2]) | points1[b,n,c1]] written split into out_hi / out_lo [b*n, kp] bf16 (hi = bf16(x),
+ * lo = bf16(x - hi), zero beyond c2 + c1; the operand of ssd3d_linear_tc).  m >= 1, kp % 16 == 0, kp >= c2 + c1,
+ * points1 may be null when c1 == 0, outputs 16-byte aligned.  Bit for bit the split of the concatenation of
+ * ssd3d_three_interpolate's output with points1. */
+int ssd3d_fp_interp_split(int b, int n, int m, int c2, int c1, const float *xyz1, const float *xyz2, const float *points2,
+                          const float *points1, void *out_hi, void *out_lo, int kp, ssd3d_stream_t stream);
+
 /* ---- dense parts of the SA layer (TF stock ops in the reference) ---------------------------- */
 
 /* model_util.calc_square_dist(a, a, norm=False)  (lib/utils/model_util.py:144-160) for a[b,n,c]:
@@ -295,7 +305,8 @@ int ssd3d_three_interpolate_grad(int b, int n, int c, int m, const float *grad_o
  * of lib/builder/postprocessor.py:76-88 (one class per call).  boxes [b,n,7] = (x,y,z,l,h,w,ry), scores [b,n];
  * candidates in descending score order (ties: lower index), dropped when axis-aligned BEV IoU with a kept box is
  * > iou_threshold, at most max_output kept.  out_block [b,max_output,9] = (box7, score, class) zero padded,
- * out_cnt [b] = number kept.  n <= 512.  Rectangles and IoU by the float32 recipe of DESIGN.md section 3.5 (cos / sin
+ * out_cnt [b] = number kept.  n <= 16384 (PointRCNN's RPN keeps every point a candidate); max_output is bounded only
+ * by the shared memory of min(n, max_output) kept boxes next to the sort keys.  Rectangles and IoU by the float32 recipe of DESIGN.md section 3.5 (cos / sin
  * in double, every operation rounded on its own); -0 and +0 scores are equal.  NaN scores are outside the contract. */
 int ssd3d_bev_nms(int b, int n, const float *boxes, const float *scores, float iou_threshold, int max_output,
                   int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream);
@@ -382,6 +393,15 @@ int ssd3d_vote_translate(long rows, const float *xyz, const float *offsets, int 
  * -> boxes[rows,7] = (x, y, z, l, h, w, ry), scores[rows]. */
 int ssd3d_decode_dist_anchor_free(long rows, int angle_bins, const float *center_xyz, const float *pred_reg, int ld_reg,
                                   const float *pred_cls, int ld_cls, float *boxes, float *scores, ssd3d_stream_t stream);
+/* decode_bin_anchor on the anchors of generate_3d_anchors_by_point_tf + the score sigmoid (lib/utils/anchor_decoder.py:
+ * 115-164, lib/utils/generate_anchors.py:33-65; PointRCNN's 'Bin-Anchor' regression, one anchor size per point).
+ * pred_reg[rows, ld_reg] = [x_bin | x_res | z_bin | z_res (bin_num each) | y_res | 3 size residuals | angle_bins logits |
+ * angle_bins residuals], pred_cls[rows, ld_cls] (column 0), center_xyz[rows,3], anchor_lhw = host float[3] ->
+ * boxes[rows,7] = (x, y, z, l, h, w, ry), scores[rows].  TF's fp32 operation order, one rounding per operation; argmax
+ * ties to the first index. */
+int ssd3d_decode_bin_anchor(long rows, int bin_num, float half_bin_search_range, int angle_bins, const float *center_xyz,
+                            const float *pred_reg, int ld_reg, const float *pred_cls, int ld_cls, const float *anchor_lhw,
+                            float *boxes, float *scores, ssd3d_stream_t stream);
 
 /* ---- training targets and detection losses (csrc/det_loss.cu, DESIGN.md section 3.8) -------- */
 

@@ -6,6 +6,10 @@ precision_ground / precision_3d R40 tables as logger_and_select_best_map logs th
     python tools/eval_kitti.py --samples <dir of .npy sample dicts> --labels <label_2 dir> --weights weights.npz
 
 weights.npz: the reference checkpoint exported as INTEGRATION.md section D shows (TF variable name -> array).
+
+--model pointrcnn-rpn runs PointRCNN's first stage (tiny_pointrcnn_stage1.yaml, TEST_MODE 'Recall') instead and prints
+the proposal recall of evaluation.recall against each sample's label boxes.  As the reference's evaluator does
+(lib/core/evaluator.py:116 -> kitti_dataloader.py:385), --cls-thresh is the recall's 3D-IoU threshold there.
 """
 import argparse
 import glob
@@ -25,8 +29,9 @@ def main(argv=None):
     ap.add_argument("--weights", required=True, help=".npz of TF variable name -> array")
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--num-points", type=int, default=16384)
-    ap.add_argument("--cls-thresh", type=float, default=0.3, help="score threshold of the detection rows (evaluator.py:26)")
+    ap.add_argument("--cls-thresh", type=float, default=0.3, help="score threshold of the detection rows (evaluator.py:26); the recall's 3D-IoU threshold with --model pointrcnn-rpn")
     ap.add_argument("--classes", default="Car", help="comma-separated class list of the model")
+    ap.add_argument("--model", default="3dssd", choices=("3dssd", "pointrcnn-rpn"))
     args = ap.parse_args(argv)
 
     import numpy as np
@@ -40,6 +45,8 @@ def main(argv=None):
     if not paths:
         raise SystemExit("no *.npy sample dicts under %s" % args.samples)
     weights = io.params_from_tf_variables(dict(np.load(args.weights)))
+    if args.model == "pointrcnn-rpn":
+        return rpn_recall(pkg, args, paths, weights, dev)
     head = pkg.DetectionHead(params=weights, device=dev)
     net = pkg.SABackbone(params=weights, in_channels=1, device=dev, head=head)
     cls_list = tuple(c.strip() for c in args.classes.split(","))
@@ -54,6 +61,29 @@ def main(argv=None):
     print("evaluated %d frames" % len(acc))
     for line in ev.format_ap_tables([r.cpu().numpy() for r in result], cls_list):
         print(line)
+    return 0
+
+
+def rpn_recall(pkg, args, paths, weights, dev):
+    """PointRCNN's RPN proposals (at most MAX_OUTPUT_NUM per frame after the IoU-0.85 NMS) against the label boxes."""
+    import numpy as np
+    import torch
+    io, C = pkg.kitti_io, pkg.config
+    head = pkg.DetectionHead(C.HEAD_POINTRCNN_RPN, weights, device=dev, stage=C.STAGE_POINTRCNN_RPN)
+    net = pkg.SABackbone(C.ARCH_POINTRCNN_RPN, weights, in_channels=1, device=dev, head=head, aggregation=False)
+    preds, gts = [], []
+    for i in range(0, len(paths), args.batch):
+        samples = [io.read_sample(p) for p in paths[i:i + args.batch]]
+        points = io.make_batch(samples, args.num_points, seed=i)[0]
+        xyz, feat = net.forward(points.to(dev, non_blocking=True))[:2]
+        block, count = net.detections(xyz, feat)
+        cnt = count.cpu().tolist()
+        for s, smp in enumerate(samples):
+            preds.append(block[s, :cnt[s], :7])
+            gts.append(torch.from_numpy(np.asarray(smp[io.KEY_LABEL_BOXES_3D], np.float32).reshape(-1, 7)).to(dev))
+    detected, total = pkg.evaluation.recall(preds, gts, args.cls_thresh)
+    print("evaluated %d frames" % len(preds))
+    print("recall: %d / %d = %.4f at 3D IoU %g" % (detected, total, detected / max(total, 1), args.cls_thresh))
     return 0
 
 
