@@ -575,15 +575,17 @@ def ball_query_vs_float64(bench, step):
 def test_last_scene_vs_oracle_layerwise(oracle_ops, bench, step):
     """Teacher-forced: every oracle layer takes scene 7's own GPU outputs of the layers before it, so the indices
     (D-FPS, F-FPS on features, ball query) must match bit for bit by construction of the arithmetic."""
-    scene_vs_oracle_layerwise(oracle_ops, bench, step, SCENES - 1)
+    scene_vs_oracle_layerwise(oracle_ops, bench.arch, bench.params, step, SCENES - 1)
 
 
-def scene_vs_oracle_layerwise(oracle_ops, bench, step, s):
-    """Scene s of a step against the CPU oracle, layer by layer on the step's own inputs to each layer."""
+def scene_vs_oracle_layerwise(oracle_ops, arch, params, step, s):
+    """Scene s of a step against the CPU oracle, layer by layer on the step's own inputs to each layer: SA, vote and FP
+    layers of the table `arch` with the raw parameter dict `params` (an SA layer whose aggregation_channel is -1 has no
+    aggregation conv)."""
     from oracle import layers as olayers
     xyz_l, feat_l, fps_l, dbg = step[0]
     npy = lambda t: None if t is None else t[s:s + 1].cpu().numpy()
-    for li, spec in enumerate(bench.arch, start=1):
+    for li, spec in enumerate(arch, start=1):
         (xyz_i, feat_i, radius, nsample, mlps, bn, rng, method, npoint, former, attn, ltype, scope, dilated,
          vote_idx, agg) = spec
         xin, fin = npy(xyz_l[xyz_i[0]]), npy(feat_l[feat_i[0]])
@@ -592,7 +594,7 @@ def scene_vs_oracle_layerwise(oracle_ops, bench, step, s):
             vote_ctr = npy(xyz_l[vote_idx]) if vote_idx != -1 else None
             ex, ef, ei, ed = olayers.pointnet_sa_module_msg(xin, fin, radius, nsample, mlps, False, None, bn, rng, method,
                                                             npoint, former_idx, attn, scope, dilated, vote_ctr, agg,
-                                                            params=bench.params, ffps_mode="matrix", return_debug=True)
+                                                            params=params, ffps_mode="matrix", return_debug=True)
             np.testing.assert_array_equal(npy(fps_l[li]), ei, err_msg="fps_idx of layer %d" % li)
             for sc, (a, b) in enumerate(zip(dbg[li - 1].get("idx", []), ed["idx"])):
                 np.testing.assert_array_equal(npy(a), b, err_msg="ball-query idx layer %d scale %d" % (li, sc))
@@ -600,10 +602,14 @@ def scene_vs_oracle_layerwise(oracle_ops, bench, step, s):
                 np.testing.assert_array_equal(npy(a), b, err_msg="pts_cnt layer %d scale %d" % (li, sc))
             np.testing.assert_array_equal(npy(xyz_l[li]), ex, err_msg="new_xyz of layer %d" % li)
         elif ltype == "Vote_Layer":
-            ex, ef, _ = olayers.vote_layer(xin, fin, mlps, False, None, bn, scope, params=bench.params)
+            ex, ef, _ = olayers.vote_layer(xin, fin, mlps, False, None, bn, scope, params=params)
             e = rel_err(npy(xyz_l[li]), ex, rtol=FEATURE_TOL)
             assert e < FEATURE_TOL, "vote xyz of layer %d: rel err %g" % (li, e)
+        elif ltype == "FP_Layer":                 # unknown points xyz_i[0], known points and features xyz_i[1] / feat_i[1]
+            ef = olayers.pointnet_fp_module(xin, npy(xyz_l[xyz_i[1]]), fin, npy(feat_l[feat_i[1]]), mlps, False, None, scope,
+                                            bn, params=params)
+            np.testing.assert_array_equal(npy(xyz_l[li]), xin, err_msg="xyz of layer %d" % li)
         else:
-            continue
+            raise AssertionError("unexpected layer type %r" % ltype)
         e = rel_err(npy(feat_l[li]), ef, rtol=FEATURE_TOL)
         assert e < FEATURE_TOL, "features of layer %d: rel err %g" % (li, e)

@@ -96,7 +96,7 @@ def test_decode_and_nms(pkg, step):
 
 @pytest.mark.parametrize("name", ["S0", "S3", "S7"])
 def test_scene_vs_oracle_layerwise(oracle_ops, real, step, name):
-    scene_vs_oracle_layerwise(oracle_ops, real, step, NAMES.index(name))
+    scene_vs_oracle_layerwise(oracle_ops, real.arch, real.params, step, NAMES.index(name))
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -322,4 +322,4 @@ def test_step_with_one_transformed_scene(oracle_ops, bench, step_nets, name):
     a, b = (flatten(bench.arch, *steps[k]) for k in NETS)
     for key in a:
         assert torch.equal(a[key][:1], b[key][:1]), "%s: %s of scene 0 differs between the nets" % (name, key)
-    scene_vs_oracle_layerwise(oracle_ops, bench, steps["throughput"], 0)
+    scene_vs_oracle_layerwise(oracle_ops, bench.arch, bench.params, steps["throughput"], 0)
