@@ -1,10 +1,11 @@
 """3dssd_b200 -- H100 (sm_90a) set-abstraction operators behind the tf_ops / layers_util surface of
 dvlab-research/3DSSD.  Import with importlib.import_module("3dssd_b200") or through the `ssd3d_b200` alias.
 """
-from . import augment, config, dist, evaluation, head, kitti_io, layers_util, loss, mixup, params, prepare, solver, tf_ops  # noqa: F401
+from . import augment, config, dist, evaluation, head, kitti_io, layers_util, loss, mixup, params, prepare, rcnn, solver, tf_ops  # noqa: F401
 from ._lib import EXPORTS, LIB_PATH, lib  # noqa: F401
 from .backbone import SABackbone, train_forward  # noqa: F401
 from .head import DetectionHead  # noqa: F401
+from .rcnn import PointRCNN  # noqa: F401
 from .loss import assign_targets, detection_loss  # noqa: F401
 from .params import TrainableParams  # noqa: F401
 from .layers_util import (pointnet_fp_module, pointnet_sa_module, pointnet_sa_module_msg,  # noqa: F401

@@ -65,6 +65,12 @@ _SIGNATURES = {
     "ssd3d_group_point_grad": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_three_interpolate_grad": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_bev_nms": [c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "ssd3d_bev_nms_counted": [c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "ssd3d_query_boxes_3d_points": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "ssd3d_region_pool_smem": [c_int, c_int, c_int],
+    "ssd3d_region_pool": [c_int] * 6 + [c_void_p] * 4 + [c_int, c_void_p, c_float, c_float] + [c_void_p] * 8,
+    "ssd3d_decode_bin_anchor_rows": [c_long, c_int, c_float, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                     c_void_p, c_void_p, c_void_p],
     "ssd3d_farthest_point_sample_features": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_ffps_supported": [c_int, c_int],
     "ssd3d_farthest_point_sample_ex": [c_int, c_int, c_int, c_int, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_int,
@@ -154,7 +160,7 @@ def lib():
             fn.restype = ctypes.c_size_t if name in ("ssd3d_sa_fused_smem", "ssd3d_query_ball_point_workspace", "ssd3d_bn_train_workspace",
                                                    "ssd3d_linear_wgrad_workspace", "ssd3d_bn_train_grad_workspace",
                                                    "ssd3d_det_loss_workspace", "ssd3d_grad_clip_scale_workspace",
-                                                   "ssd3d_eval_workspace", "ssd3d_augment_workspace",
+                                                   "ssd3d_eval_workspace", "ssd3d_augment_workspace", "ssd3d_region_pool_smem",
                                                    "ssd3d_prepare_workspace") else c_int
             if name == "ssd3d_fps_temp_elems":
                 fn.restype = c_long

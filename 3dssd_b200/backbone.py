@@ -60,8 +60,13 @@ class SABackbone:
         if points.dim() != 3 or points.shape[-1] != 3 + self.in_channels:
             raise ValueError("points must be [B, N, %d], got %s" % (3 + self.in_channels, tuple(points.shape)))
         xyz0, feat0 = tf_ops.split_points(points)                  # single_stage_detector.py:116-117
-        xyz_list, feat_list = [xyz0], [feat0]
-        fps_list = [None]
+        return self.forward_lists([xyz0], [feat0], return_debug)
+
+    def forward_lists(self, xyz_list, feat_list, return_debug=False):
+        """The layer loop on the given starting lists (forward starts from [xyz], [features] of the points; PointRCNN's
+        stage 2 from [proposal centres, pooled xyz], [None, pooled features], double_stage_detector.py:210)."""
+        xyz_list, feat_list = list(xyz_list), list(feat_list)
+        fps_list = [None] * len(xyz_list)
         dbg = []
         for spec in self.arch:
             (xyz_i, feat_i, radius, nsample, mlps, bn, rng, method, npoint, former, attn, ltype, scope, dilated,

@@ -79,6 +79,33 @@ STAGE_POINTRCNN_RPN = {                                                        #
     "ANCHOR_SIZE": (3.88311640418, 1.62856739989, 1.52563191462),
 }
 
+# PointRCNN's two-stage detector at test time: /root/reference/configs/kitti/pointrcnn/tiny_pointrcnn_stage2_test.yaml.
+# The RPN is ARCH_POINTRCNN_RPN / HEAD_POINTRCNN_RPN with the test yaml's FIRST_STAGE post-processing (yaml:104-117: NMS
+# at 0.8 instead of stage1.yaml's 0.85).
+STAGE_POINTRCNN_RPN_TEST = dict(STAGE_POINTRCNN_RPN, NMS_THRESH=0.8)
+# NETWORK.FIRST_STAGE.POINTS_POOLER (yaml:85): type, info keys, info conv channels, points per proposal, context range,
+# (PointsPool-only voxel grid), (PointsPool-only VFE channels), bn, scope
+POINTS_POOLER_POINTRCNN = ['RegionPool', ['mask', 'dist'], [128], 512, 1.0, [6, 6, 6, 10], [128], True, 'roi_pool']
+POOLER_MASK_THRESHOLD = 0.5        # NETWORK.FIRST_STAGE.POOLER_MASK_THRESHOLD (yaml:86)
+# NETWORK.SECOND_STAGE.ARCHITECTURE (yaml:89-102).  Index 0 of its lists is the proposal centres
+# (cast_bottom_to_center(proposals)[..., :3], double_stage_detector.py:192,210), index 1 the pooled points.
+ARCH_POINTRCNN_RCNN = [
+    [[1], [1], [0.2], [64], [[128, 128, 128]], True,
+     [-1], ['D-FPS'], [128],
+     -1, False, 'SA_Layer', 'rcnn_layer1', False, -1, 128],
+    [[2], [2], [0.4], [64], [[128, 128, 256]], True,
+     [-1], ['D-FPS'], [32],
+     -1, False, 'SA_Layer', 'rcnn_layer2', False, -1, 256],
+    [[3], [3], [], [], [256, 256, 512], True,
+     [], [], [],
+     -1, False, 'SA_Layer_SSG_Last', 'rcnn_layer3', False, -1, 256],
+]
+HEAD_POINTRCNN_RCNN = [[0], [4], 'conv1d', [256], True, 'Det', 'rcnn_head']   # yaml:103
+STAGE_POINTRCNN_RCNN = {                                                        # MODEL.SECOND_STAGE, yaml:118-136
+    "REGRESSION": "Bin-Anchor", "MAX_OUTPUT_NUM": 100, "NMS_THRESH": 0.1,
+    "HALF_BIN_SEARCH_RANGE": 1.5, "BIN_CLASS_NUM": 6, "CLS_ACTIVATION": "Softmax",
+}
+
 # BASELINE.json configs[0] / SURVEY.md section 8d "config 1": one SA layer N=4096 -> 1024, plain ball query
 ARCH_SINGLE_SA = [
     [[0], [0], [0.4], [32], [[64, 64, 128]], True,

@@ -9,6 +9,8 @@
 //                         inputs of bev_nms.
 //   * decode_bin_anchor   the same for PointRCNN's 'Bin-Anchor' regression: anchor_decoder.py:115-164 on the anchors of
 //                         generate_anchors.py:33-65 (one anchor size per point) + the sigmoid.
+//   * decode_bin_anchor_rows  the same decode against per-row anchors (PointRCNN's stage 2: the bottom-centred
+//                         proposals, double_stage_detector.py:298-337) + the 2-way softmax score times the pool mask.
 // All HBM-bound copies / a few flops per element; sized far below one wave, so launch latency is the cost.
 #include "common.cuh"
 
@@ -140,6 +142,38 @@ __global__ void decode_bin_kernel(long rows, int nb, int na, const float *__rest
     scores[r] = (float)(1.0 / (1.0 + exp(-(double)cls[r * ldcls])));    // as decode_kernel
 }
 
+// one thread per proposal; anchors[r] = (x, y_bottom, z, l, h, w, ry).  As decode_bin_kernel with the anchor's own
+// centre, size and angle: x = (ax - half_range) + ((bin + res) + 0.5) * interval (camera x / z, not the anchor's axes),
+// y = ay + y_res, lhw = max(anchor_lhw + res, 0.1), ry = ary + ((bin + res) + 0) * (2 pi / na).  score = softmax(cls)[1]
+// in double, rounded once, times (pool_cnt > 0) (double_stage_detector.py:317-328)
+__global__ void decode_bin_rows_kernel(long rows, int nb, int na, const float *__restrict__ anchors, int ldanc,
+                                       const float *__restrict__ reg, int ldreg, const float *__restrict__ cls, int ldcls,
+                                       const int *__restrict__ pool_cnt, float half_range, float bin_interval,
+                                       float angle_interval, float *__restrict__ boxes, float *__restrict__ scores)
+{
+    const long r = blockIdx.x * (long)blockDim.x + threadIdx.x;
+    if (r >= rows) return;
+    const float *g = reg + r * ldreg;
+    const float *an = anchors + r * ldanc;
+    float *o = boxes + r * 7;
+    const int xb = first_argmax(g, nb), zb = first_argmax(g + 2 * nb, nb);
+    const float dx = __fmul_rn(__fadd_rn(__fadd_rn((float)xb, g[nb + xb]), 0.5f), bin_interval);
+    const float dz = __fmul_rn(__fadd_rn(__fadd_rn((float)zb, g[3 * nb + zb]), 0.5f), bin_interval);
+    const float *off = g + 4 * nb;
+    o[0] = __fadd_rn(__fsub_rn(an[0], half_range), dx);
+    o[1] = __fadd_rn(an[1], off[0]);
+    o[2] = __fadd_rn(__fsub_rn(an[2], half_range), dz);
+    o[3] = fmaxf(__fadd_rn(an[3], off[1]), 0.1f);
+    o[4] = fmaxf(__fadd_rn(an[4], off[2]), 0.1f);
+    o[5] = fmaxf(__fadd_rn(an[5], off[3]), 0.1f);
+    const float *ang = off + 4;
+    const int ab = first_argmax(ang, na);
+    o[6] = __fadd_rn(an[6], __fmul_rn(__fadd_rn(__fadd_rn((float)ab, ang[na + ab]), 0.0f), angle_interval));
+    const float *c = cls + r * ldcls;
+    const float p1 = (float)(1.0 / (1.0 + exp((double)c[0] - (double)c[1])));
+    scores[r] = pool_cnt == nullptr ? p1 : __fmul_rn(p1, pool_cnt[r] > 0 ? 1.0f : 0.0f);
+}
+
 // out[s, off_i + q, :] = src_i[s, q, :] for the (up to 8) row blocks of a scene: tf.concat(axis=1) of per-part results
 struct ConcatRowsArgs {
     const float *src[8];
@@ -241,6 +275,25 @@ extern "C" int ssd3d_decode_bin_anchor(long rows, int bin_num, float half_bin_se
         rows, bin_num, angle_bins, center_xyz, pred_reg, ld_reg, pred_cls, ld_cls, half_bin_search_range, bin_interval,
         angle_interval, anchor_lhw[0], anchor_lhw[1], anchor_lhw[2], boxes, scores);
     SSD3D_LAUNCH_CHECK("decode_bin_kernel");
+}
+
+extern "C" int ssd3d_decode_bin_anchor_rows(long rows, int bin_num, float half_bin_search_range, int angle_bins,
+                                            const float *anchors, int ld_anchors, const float *pred_reg, int ld_reg,
+                                            const float *pred_cls, int ld_cls, const int *pool_cnt, float *boxes, float *scores,
+                                            ssd3d_stream_t stream)
+{
+    SSD3D_REQUIRE(rows >= 0 && bin_num >= 1 && angle_bins >= 1 && ld_anchors >= 7 &&
+                  ld_reg >= 4 * bin_num + 4 + 2 * angle_bins && ld_cls >= 2,
+                  "decode_bin_anchor_rows: bad shape rows=%ld bins=%d angle_bins=%d ld_anchors=%d ld_reg=%d ld_cls=%d", rows,
+                  bin_num, angle_bins, ld_anchors, ld_reg, ld_cls);
+    if (rows == 0) return 0;
+    SSD3D_REQUIRE(anchors && pred_reg && pred_cls && boxes && scores, "decode_bin_anchor_rows: null pointer");
+    const float bin_interval = (float)((double)half_bin_search_range * 2.0 / bin_num);     // as ssd3d_decode_bin_anchor
+    const float angle_interval = (float)(2.0 * 3.14159265358979323846 / angle_bins);
+    decode_bin_rows_kernel<<<(int)((rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+        rows, bin_num, angle_bins, anchors, ld_anchors, pred_reg, ld_reg, pred_cls, ld_cls, pool_cnt, half_bin_search_range,
+        bin_interval, angle_interval, boxes, scores);
+    SSD3D_LAUNCH_CHECK("decode_bin_rows_kernel");
 }
 
 extern "C" int ssd3d_concat_rows(int b, int parts, const float *const *src, const int *m, int c, float *out,

@@ -11,7 +11,8 @@
 // One CTA of 1024 threads per scene, up to 16384 candidates: the 64-bit keys are bitonic-sorted in shared memory (128 KiB
 // at n = 16384), then the sorted candidates are walked in chunks of 32: each chunk is tested against the kept set (at
 // most max_output boxes) and against itself in parallel, then resolved greedily in order; the walk stops once
-// max_output boxes are kept.  (An n x n suppression matrix would need 32 MiB per scene at n = 16384; at 3DSSD's
+// max_output boxes are kept; ssd3d_bev_nms_counted takes only the first n_valid[scene] candidates of each scene (PointRCNN's
+// stage 2, whose proposal rows past the RPN's count are padding).  (An n x n suppression matrix would need 32 MiB per scene at n = 16384; at 3DSSD's
 // n = 256 the chunked walk also measured faster than the matrix kernel it replaced, BASELINE.md.)
 //
 // The rectangles and the IoU follow the recipe of DESIGN.md section 3.5, which the numpy and C restatements of the test
@@ -102,7 +103,8 @@ static size_t nms_smem_bytes(int npow2, int kcap) { return nms_keys_bytes(npow2)
 
 __global__ void __launch_bounds__(NMS_THREADS)
 bev_nms_kernel(int n, int npow2, int kcap, const float *__restrict__ boxes, const float *__restrict__ scores,
-                     float iou_thr, int max_out, int cls_id, float *__restrict__ out_block, int *__restrict__ out_cnt)
+                     const int *__restrict__ n_valid, float iou_thr, int max_out, int cls_id, float *__restrict__ out_block,
+                     int *__restrict__ out_cnt)
 {
     extern __shared__ __align__(16) unsigned char nms_smem[];
     unsigned long long *keys = reinterpret_cast<unsigned long long *>(nms_smem);
@@ -118,16 +120,18 @@ bev_nms_kernel(int n, int npow2, int kcap, const float *__restrict__ boxes, cons
     const int scene = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float *bx = boxes + (size_t)scene * n * 7;
     const float *sc = scores + (size_t)scene * n;
+    // candidates n_valid[scene] .. n-1 are padding: key 0 sorts them last and the walk below stops before them
+    const int nv = n_valid == nullptr ? n : max(0, min(n, n_valid[scene]));
 
-    for (int i = tid; i < npow2; i += NMS_THREADS) keys[i] = i < n ? nms_key(sc, i) : 0ull;
+    for (int i = tid; i < npow2; i += NMS_THREADS) keys[i] = i < nv ? nms_key(sc, i) : 0ull;
     if (tid == 0) nkept = 0;
     __syncthreads();
     nms_sort_desc(keys, npow2);
 
-    for (int base = 0; base < n; base += NMS_CHUNK) {
+    for (int base = 0; base < nv; base += NMS_CHUNK) {
         const int nk = nkept;                 // read by all threads after the barrier that ended the last step
         if (nk >= max_out) break;
-        const int cn = min(NMS_CHUNK, n - base);
+        const int cn = min(NMS_CHUNK, nv - base);
         if (tid < cn) {
             const float4 r = nms_rect(bx + (size_t)nms_key_index(keys[base + tid]) * 7);
             crect[tid] = r;
@@ -174,23 +178,39 @@ bev_nms_kernel(int n, int npow2, int kcap, const float *__restrict__ boxes, cons
 
 using namespace ssd3d;
 
-extern "C" int ssd3d_bev_nms(int b, int n, const float *boxes, const float *scores, float iou_threshold, int max_output,
-                             int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream)
+static int bev_nms_launch(const char *op, int b, int n, const float *boxes, const float *scores, const int *n_valid,
+                          float iou_threshold, int max_output, int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream)
 {
-    SSD3D_REQUIRE(b >= 0 && n > 0 && max_output > 0, "bev_nms: bad shape b=%d n=%d max_output=%d", b, n, max_output);
-    SSD3D_REQUIRE(n <= NMS_MAX_N, "bev_nms: at most %d candidates per scene (got %d)", NMS_MAX_N, n);
+    SSD3D_REQUIRE(b >= 0 && n > 0 && max_output > 0, "%s: bad shape b=%d n=%d max_output=%d", op, b, n, max_output);
+    SSD3D_REQUIRE(n <= NMS_MAX_N, "%s: at most %d candidates per scene (got %d)", op, NMS_MAX_N, n);
     if (b == 0) return 0;                    // nothing read or written: an empty tensor may have a null data pointer
-    SSD3D_REQUIRE(boxes && scores && out_block && out_cnt, "bev_nms: null pointer");
+    SSD3D_REQUIRE(boxes && scores && out_block && out_cnt, "%s: null pointer", op);
     int npow2 = 1;
     while (npow2 < n) npow2 <<= 1;
     const int kcap = max_output < n ? max_output : n;
     const size_t smem = nms_smem_bytes(npow2, kcap);
-    SSD3D_REQUIRE(smem <= NMS_SMEM_MAX, "bev_nms: max_output=%d at n=%d needs %zu bytes of shared memory (at most %zu)",
-                  max_output, n, smem, NMS_SMEM_MAX);
+    SSD3D_REQUIRE(smem <= NMS_SMEM_MAX, "%s: max_output=%d at n=%d needs %zu bytes of shared memory (at most %zu)",
+                  op, max_output, n, smem, NMS_SMEM_MAX);
     const int e = cuda_status(cudaFuncSetAttribute(bev_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
                               "bev_nms_kernel shared memory");
     if (e) return e;
-    bev_nms_kernel<<<b, NMS_THREADS, smem, (cudaStream_t)stream>>>(n, npow2, kcap, boxes, scores, iou_threshold,
-                                                                               max_output, cls_id, out_block, out_cnt);
+    bev_nms_kernel<<<b, NMS_THREADS, smem, (cudaStream_t)stream>>>(n, npow2, kcap, boxes, scores, n_valid, iou_threshold,
+                                                                   max_output, cls_id, out_block, out_cnt);
     SSD3D_LAUNCH_CHECK("bev_nms_kernel");
+}
+
+extern "C" int ssd3d_bev_nms(int b, int n, const float *boxes, const float *scores, float iou_threshold, int max_output,
+                             int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream)
+{
+    return bev_nms_launch("bev_nms", b, n, boxes, scores, nullptr, iou_threshold, max_output, cls_id, out_block, out_cnt,
+                          stream);
+}
+
+extern "C" int ssd3d_bev_nms_counted(int b, int n, const float *boxes, const float *scores, const int *n_valid,
+                                     float iou_threshold, int max_output, int cls_id, float *out_block, int *out_cnt,
+                                     ssd3d_stream_t stream)
+{
+    if (b > 0) SSD3D_REQUIRE(n_valid != nullptr, "bev_nms_counted: null n_valid");
+    return bev_nms_launch("bev_nms_counted", b, n, boxes, scores, n_valid, iou_threshold, max_output, cls_id, out_block,
+                          out_cnt, stream);
 }

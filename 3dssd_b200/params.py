@@ -95,6 +95,29 @@ def init_head_params(cin, mlp=(128,), cls_channels=1, reg_channels=6 + 2 * 12, s
     return params
 
 
+def init_rcnn_params(feat_channels=128, pooler=None, arch=None, head=None, reg_channels=6 * 4 + 4 + 2 * 12, seed=2):
+    """Random weights of PointRCNN's second stage keyed by the reference's variable names: <pooler scope>/conv{i} of the
+    region pool's info network (align_channel_network, pool_utils.py:5-16; 5 -> 128 at roi_pool/conv0), the stage-2 SA
+    layers (rcnn_layer1-3) on the pooled [info conv | RPN feature] channels, and the head (rcnn_head: conv1d_0, 2 softmax
+    class channels, Bin-Anchor regression with BIN_CLASS_NUM 6)."""
+    pooler = _cfg.POINTS_POOLER_POINTRCNN if pooler is None else pooler
+    arch = _cfg.ARCH_POINTRCNN_RCNN if arch is None else arch
+    head = _cfg.HEAD_POINTRCNN_RCNN if head is None else head
+    rng = np.random.default_rng(seed)
+    params = {}
+    c = 5                                                   # [canonical xyz | mask | dist]
+    for i, cout in enumerate(pooler[2]):
+        _conv_init(rng, params, "%s/conv%d" % (pooler[8], i), c, cout, pooler[7])
+        c = cout
+    # the stage-2 lists start with [proposal centres, pooled points]: the table's indices are one past init_params's
+    shifted = [[[i - 1 for i in spec[0]], [i - 1 for i in spec[1]]] + list(spec[2:]) for spec in arch]
+    params.update(init_params(shifted, c + feat_channels, seed=seed + 1, aggregation=False))
+    cin = _cfg.layer_channels(shifted, c + feat_channels, aggregation=False)[head[1][0] - 1]
+    params.update(init_head_params(cin, mlp=tuple(head[3]), cls_channels=2, reg_channels=reg_channels, seed=seed + 2,
+                                   scope=head[6]))
+    return params
+
+
 class FoldedConv:
     """One conv+BN layer folded for inference: y = act((x @ w) * scale + shift).
     For the tensor-core path the weight also exists split in two bf16 terms, transposed to K-major:

@@ -777,12 +777,7 @@ def sa_mlp_fused_hoisted(xyz, z, zoff, wx, new_xyz, idx, cnt, stack, out_f32=Non
     return y
 
 
-def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
-    """Greedy BEV NMS per scene (postprocessor.py:76-88): boxes (b,n,7) = (x,y,z,l,h,w,ry), scores (b,n) ->
-    block (b,max_output,9) = (box7, score, class) zero padded, count (b,) int32.  out=(block, count) writes into
-    preallocated contiguous tensors (the send buffer of the multi-GPU gather).  Descending score, ties (-0 and +0
-    included) to the lower index; rectangles and IoU by the float32 recipe of DESIGN.md §3.5, which the CPU
-    restatements of the test suite share decision for decision.  NaN scores are outside the contract."""
+def _nms_io(boxes, scores, max_output, out):
     boxes = _req(boxes, "boxes", torch.float32, 3, 7)
     scores = _req(scores, "scores", torch.float32, 2)
     b, n, _ = boxes.shape
@@ -795,9 +790,91 @@ def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
         block, cnt = _req(out[0], "out block", torch.float32, 3, 9, copy=False), _req(out[1], "out count", torch.int32, 1, copy=False)
         if tuple(block.shape) != (b, int(max_output), 9) or tuple(cnt.shape) != (b,):
             raise ValueError("out must be (float32 (b, max_output, 9), int32 (b,)) contiguous tensors")
+    return boxes, scores, block, cnt
+
+
+def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
+    """Greedy BEV NMS per scene (postprocessor.py:76-88): boxes (b,n,7) = (x,y,z,l,h,w,ry), scores (b,n) ->
+    block (b,max_output,9) = (box7, score, class) zero padded, count (b,) int32.  out=(block, count) writes into
+    preallocated contiguous tensors (the send buffer of the multi-GPU gather).  Descending score, ties (-0 and +0
+    included) to the lower index; rectangles and IoU by the float32 recipe of DESIGN.md §3.5, which the CPU
+    restatements of the test suite share decision for decision.  NaN scores are outside the contract."""
+    boxes, scores, block, cnt = _nms_io(boxes, scores, max_output, out)
+    b, n, _ = boxes.shape
     check(lib().ssd3d_bev_nms(b, n, _p(boxes), _p(scores), float(iou_threshold), int(max_output), int(cls_id),
                               _p(block), _p(cnt), _stream()), "bev_nms")
     return block, cnt
+
+
+def bev_nms_counted(boxes, scores, n_valid, iou_threshold, max_output, cls_id=0, out=None):
+    """bev_nms over the first n_valid[s] candidates of each scene only (int32 CUDA (b,), clamped to [0, n]): rows past
+    it are padding and never kept.  Equals bev_nms when n_valid == n."""
+    boxes, scores, block, cnt = _nms_io(boxes, scores, max_output, out)
+    b, n, _ = boxes.shape
+    n_valid = _req(n_valid, "n_valid", torch.int32, 1)
+    if n_valid.shape[0] != b:
+        raise ValueError("n_valid must be (b,)")
+    check(lib().ssd3d_bev_nms_counted(b, n, _p(boxes), _p(scores), _p(n_valid), float(iou_threshold), int(max_output),
+                                      int(cls_id), _p(block), _p(cnt), _stream()), "bev_nms_counted")
+    return block, cnt
+
+
+# ---- PointRCNN's region pool (csrc/roi_pool.cu, DESIGN.md section 3.16) ---------------------------------------------
+
+def query_boxes_3d_points(nsample, xyz, proposals):
+    """tf_grouping.py:39 query_boxes_3d_points: xyz (b,n,3), bottom-centred proposals (b,m,7) -> idx (b,m,nsample)
+    int32 (the first nsample points inside each box in index order, padded with the first hit, 0 without a hit),
+    pts_cnt (b,m) int32."""
+    xyz = _req(xyz, "xyz", torch.float32, 3, 3)
+    proposals = _req(proposals, "proposals", torch.float32, 3, 7)
+    b, n, _ = xyz.shape
+    m = proposals.shape[1]
+    if proposals.shape[0] != b:
+        raise ValueError("xyz and proposals must have the same batch size")
+    if int(nsample) <= 0:
+        raise ValueError("nsample must be positive")
+    idx = torch.empty((b, m, int(nsample)), dtype=torch.int32, device=xyz.device)
+    cnt = torch.empty((b, m), dtype=torch.int32, device=xyz.device)
+    check(lib().ssd3d_query_boxes_3d_points(b, n, m, int(nsample), _p(xyz), _p(proposals), _p(idx), _p(cnt), _stream()),
+          "query_boxes_3d_points")
+    return idx, cnt
+
+
+def region_pool(xyz, features, point_score, proposals, count, info_conv, nsample=512, context=1.0, mask_thresh=0.5):
+    """PointsPooler.region_pool at inference (points_pooler.py:40-61, :119-170) in one kernel.  xyz (b,n,3), features
+    (b,n,cf), point_score (b,n) (the RPN's per-point sigmoid score, 'mask' = score >= mask_thresh), proposals (b,p,>=7)
+    bottom-centred (e.g. the RPN's NMS block (b,p,9)), count (b,) int32 or None (rows >= count[s] are padding),
+    info_conv: the folded roi_pool/conv0 (params.FoldedConv, 5 -> c_info).  Returns (xyz (b*p,nsample,3) canonical,
+    features (b*p,nsample,c_info+cf), idx (b,p,nsample), pts_cnt (b,p)); pool_mask = pts_cnt > 0."""
+    xyz = _req(xyz, "xyz", torch.float32, 3, 3)
+    b, n, _ = xyz.shape
+    features = _req(features, "features", torch.float32, 3)
+    point_score = _req(point_score, "point_score", torch.float32, 2)
+    proposals = _req(proposals, "proposals", torch.float32, 3)
+    if features.shape[:2] != (b, n) or tuple(point_score.shape) != (b, n):
+        raise ValueError("features must be (b, n, c) and point_score (b, n)")
+    if proposals.shape[0] != b or proposals.shape[2] < 7:
+        raise ValueError("proposals must be (b, p, >= 7)")
+    if count is not None:
+        count = _req(count, "count", torch.int32, 1)
+        if count.shape[0] != b:
+            raise ValueError("count must be (b,)")
+    w = _req(info_conv.w, "info_conv.w", torch.float32, 2)
+    co = w.shape[1]
+    if w.shape[0] != 5:
+        raise ValueError("info_conv must take 5 input channels (canonical xyz, mask, dist)")
+    scale = _vec(info_conv.scale, "info_conv.scale", co)
+    shift = _vec(info_conv.shift, "info_conv.shift", co)
+    p, cf, ns = proposals.shape[1], features.shape[2], int(nsample)
+    dev = xyz.device
+    idx = torch.empty((b, p, ns), dtype=torch.int32, device=dev)
+    cnt = torch.empty((b, p), dtype=torch.int32, device=dev)
+    oxyz = torch.empty((b * p, ns, 3), dtype=torch.float32, device=dev)
+    ofeat = torch.empty((b * p, ns, co + cf), dtype=torch.float32, device=dev)
+    check(lib().ssd3d_region_pool(b, n, p, ns, cf, co, _p(xyz), _p(features), _p(point_score), _p(proposals),
+                                  proposals.shape[2], _p(count), float(context), float(mask_thresh), _p(w), _p(scale),
+                                  _p(shift), _p(idx), _p(cnt), _p(oxyz), _p(ofeat), _stream()), "region_pool")
+    return oxyz, ofeat, idx, cnt
 
 
 # ---- KITTI evaluation (csrc/box_eval.cu, DESIGN.md section 3.10; evaluation/tf_evaluate.py) --------------------------
@@ -1128,6 +1205,29 @@ def decode_bin_anchor(center_xyz, pred_reg, pred_cls, anchor_lhw, half_bin_searc
     check(lib().ssd3d_decode_bin_anchor(b * n, int(bin_num), float(half_bin_search_range), int(angle_bins), _p(center_xyz),
                                         _p(pred_reg), pred_reg.shape[2], _p(pred_cls), pred_cls.shape[2],
                                         ctypes.cast(lhw, ctypes.c_void_p), _p(boxes), _p(scores), _stream()), "decode_bin_anchor")
+    return boxes, scores
+
+
+def decode_bin_anchor_rows(anchors, pred_reg, pred_cls, pool_cnt=None, half_bin_search_range=1.5, bin_num=6, angle_bins=12):
+    """PointRCNN's stage-2 decode (double_stage_detector.py:298-337, anchor_decoder.py:115-164): anchors (b,n,>=7) the
+    bottom-centred proposals, pred_reg (b,n,>= 4*bin_num + 4 + 2*angle_bins), pred_cls (b,n,>=2) softmax logits,
+    pool_cnt (b,n) int32 or None -> boxes (b,n,7), scores (b,n) = softmax(pred_cls)[...,1] * (pool_cnt > 0)."""
+    anchors = _req(anchors, "anchors", torch.float32, 3)
+    pred_reg = _req(pred_reg, "pred_reg", torch.float32, 3)
+    pred_cls = _req(pred_cls, "pred_cls", torch.float32, 3)
+    b, n, la = anchors.shape
+    if la < 7 or pred_reg.shape[:2] != (b, n) or pred_cls.shape[:2] != (b, n) or pred_cls.shape[2] < 2 or \
+            pred_reg.shape[2] < 4 * bin_num + 4 + 2 * angle_bins:
+        raise ValueError("anchors must be (b, n, >= 7), pred_reg (b, n, >= 4*bin_num + 4 + 2*angle_bins), pred_cls (b, n, >= 2)")
+    if pool_cnt is not None:
+        pool_cnt = _req(pool_cnt, "pool_cnt", torch.int32, 2)
+        if tuple(pool_cnt.shape) != (b, n):
+            raise ValueError("pool_cnt must be (b, n)")
+    boxes = torch.empty((b, n, 7), dtype=torch.float32, device=anchors.device)
+    scores = torch.empty((b, n), dtype=torch.float32, device=anchors.device)
+    check(lib().ssd3d_decode_bin_anchor_rows(b * n, int(bin_num), float(half_bin_search_range), int(angle_bins), _p(anchors), la,
+                                             _p(pred_reg), pred_reg.shape[2], _p(pred_cls), pred_cls.shape[2], _p(pool_cnt),
+                                             _p(boxes), _p(scores), _stream()), "decode_bin_anchor_rows")
     return boxes, scores
 
 

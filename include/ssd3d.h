@@ -310,6 +310,37 @@ int ssd3d_three_interpolate_grad(int b, int n, int c, int m, const float *grad_o
  * in double, every operation rounded on its own); -0 and +0 scores are equal.  NaN scores are outside the contract. */
 int ssd3d_bev_nms(int b, int n, const float *boxes, const float *scores, float iou_threshold, int max_output,
                   int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream);
+/* ssd3d_bev_nms over the first n_valid[s] candidates of each scene s only (DEVICE int32 [b], clamped to [0, n]); the
+ * rest are padding and never kept.  With n_valid[s] == n it is ssd3d_bev_nms bit for bit (the same kernel body).
+ * PointRCNN's stage 2, whose proposal rows at or past the RPN's count are padding (DESIGN.md section 3.16). */
+int ssd3d_bev_nms_counted(int b, int n, const float *boxes, const float *scores, const int *n_valid, float iou_threshold,
+                          int max_output, int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream);
+
+/* ---- PointRCNN's region pool (DESIGN.md section 3.16) -------------------------------------------- */
+
+/* query_boxes_3d_points (lib/utils/tf_ops/grouping/tf_grouping_g.cu:27-94, queryBoxes3dPointsLauncher :447-449):
+ * for every bottom-centred box proposals[b,m,7] = (x, y_bottom, z, l, h, w, ry) the first nsample points of xyz[b,n,3]
+ * inside it, in index order, by point_inside_box_3d's arithmetic; idx[b,m,nsample] is padded with the first hit and
+ * pts_cnt[b,m] = hits (<= nsample).  Rows without a hit get idx 0 (the reference leaves them unwritten; its pooler
+ * zeroes them, points_pooler.py:125-126).  Indices and counts equal the reference kernel's bit for bit. */
+int ssd3d_query_boxes_3d_points(int b, int n, int m, int nsample, const float *xyz, const float *proposals, int *idx,
+                                int *pts_cnt, ssd3d_stream_t stream);
+/* Dynamic shared memory of ssd3d_region_pool: the scene's xyz plus the conv and the index lists (<= 227 KiB). */
+size_t ssd3d_region_pool_smem(int n, int nsample, int c_info);
+/* PointsPooler.region_pool (lib/builder/points_pooler.py:40-61, :119-170) at inference in one launch.  Proposal r of
+ * scene s is row proposals[s, r, 0:7] (row stride ld_proposals floats, e.g. 9 for the NMS block); rows r >= count[s]
+ * (DEVICE int32 [b]; null: none) are padding and pool nothing.  Each real proposal grows by `context` in l, h and w
+ * (expand_proposals_context, the bottom centre kept) and collects its points as ssd3d_query_boxes_3d_points
+ * (idx [b,p,nsample], pts_cnt [b,p]; pool_mask = pts_cnt > 0, rows without a hit use point 0).  Per pooled point k:
+ * canonical = rotate_points(xyz[k] - box[0:3], -ry), mask = point_score[s,k] >= mask_thresh, dist = |xyz[k]|, and
+ * out_xyz [b*p, nsample, 3] = canonical, out_features [b*p, nsample, c_info + c_feat] =
+ * [relu((canonical | mask | dist) @ info_w[5, c_info] * info_scale + info_shift) | features[s,k,0:c_feat]]
+ * (roi_pool/conv0 folded as params.FoldedConv).  c_feat, c_info multiples of 4, features / out_features 16-byte
+ * aligned, ssd3d_region_pool_smem(n, nsample, c_info) <= 227 KiB (n <= 16384 at nsample 512, c_info 128). */
+int ssd3d_region_pool(int b, int n, int p, int nsample, int c_feat, int c_info, const float *xyz, const float *features,
+                      const float *point_score, const float *proposals, int ld_proposals, const int *count, float context,
+                      float mask_thresh, const float *info_w, const float *info_scale, const float *info_shift, int *idx,
+                      int *pts_cnt, float *out_xyz, float *out_features, ssd3d_stream_t stream);
 
 /* ymax[g, 0:c] = max over rows g*pool .. g*pool+pool-1 of y[., 0:c] (times rowmask[g] != 0): the
  * tf.reduce_max(axis=2) * mask of layers_util.py:178-180 for nsample values the fused epilogue of
@@ -402,6 +433,14 @@ int ssd3d_decode_dist_anchor_free(long rows, int angle_bins, const float *center
 int ssd3d_decode_bin_anchor(long rows, int bin_num, float half_bin_search_range, int angle_bins, const float *center_xyz,
                             const float *pred_reg, int ld_reg, const float *pred_cls, int ld_cls, const float *anchor_lhw,
                             float *boxes, float *scores, ssd3d_stream_t stream);
+/* decode_bin_anchor against per-row anchors (lib/utils/anchor_decoder.py:115-164 as PointRCNN's stage 2 calls it,
+ * double_stage_detector.py:298-337): anchors[rows, ld_anchors] = the bottom-centred proposals (x, y, z, l, h, w, ry),
+ * pred_reg as ssd3d_decode_bin_anchor, y = anchor y + y_res, sizes = anchor size + residual (>= 0.1), ry = anchor ry +
+ * the decoded angle; scores[rows] = softmax(pred_cls[r, 0:2])[1] (in double, rounded once) times (pool_cnt[r] > 0)
+ * (pool_cnt may be null: no mask).  TF's fp32 operation order; argmax ties to the first index. */
+int ssd3d_decode_bin_anchor_rows(long rows, int bin_num, float half_bin_search_range, int angle_bins, const float *anchors,
+                                 int ld_anchors, const float *pred_reg, int ld_reg, const float *pred_cls, int ld_cls,
+                                 const int *pool_cnt, float *boxes, float *scores, ssd3d_stream_t stream);
 
 /* ---- training targets and detection losses (csrc/det_loss.cu, DESIGN.md section 3.8) -------- */
 

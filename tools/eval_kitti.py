@@ -7,6 +7,9 @@ precision_ground / precision_3d R40 tables as logger_and_select_best_map logs th
 
 weights.npz: the reference checkpoint exported as INTEGRATION.md section D shows (TF variable name -> array).
 
+--model pointrcnn runs PointRCNN's two-stage detector (tiny_pointrcnn_stage2_test.yaml, 3dssd_b200.PointRCNN) through the
+same evaluator and AP tables; its weights are a full stage-2 checkpoint (rpn_*, roi_pool, rcnn_* variables).
+
 --model pointrcnn-rpn runs PointRCNN's first stage (tiny_pointrcnn_stage1.yaml, TEST_MODE 'Recall') instead and prints
 the proposal recall of evaluation.recall against each sample's label boxes.  As the reference's evaluator does
 (lib/core/evaluator.py:116 -> kitti_dataloader.py:385), --cls-thresh is the recall's 3D-IoU threshold there.
@@ -31,7 +34,7 @@ def main(argv=None):
     ap.add_argument("--num-points", type=int, default=16384)
     ap.add_argument("--cls-thresh", type=float, default=0.3, help="score threshold of the detection rows (evaluator.py:26); the recall's 3D-IoU threshold with --model pointrcnn-rpn")
     ap.add_argument("--classes", default="Car", help="comma-separated class list of the model")
-    ap.add_argument("--model", default="3dssd", choices=("3dssd", "pointrcnn-rpn"))
+    ap.add_argument("--model", default="3dssd", choices=("3dssd", "pointrcnn", "pointrcnn-rpn"))
     args = ap.parse_args(argv)
 
     import numpy as np
@@ -47,15 +50,19 @@ def main(argv=None):
     weights = io.params_from_tf_variables(dict(np.load(args.weights)))
     if args.model == "pointrcnn-rpn":
         return rpn_recall(pkg, args, paths, weights, dev)
-    head = pkg.DetectionHead(params=weights, device=dev)
-    net = pkg.SABackbone(params=weights, in_channels=1, device=dev, head=head)
+    if args.model == "pointrcnn":
+        rcnn = pkg.PointRCNN(params=weights, device=dev)
+        detect = lambda pts: rcnn.forward(pts)
+    else:
+        head = pkg.DetectionHead(params=weights, device=dev)
+        net = pkg.SABackbone(params=weights, in_channels=1, device=dev, head=head)
+        detect = lambda pts: net.detections(*net.forward(pts)[:2])
     cls_list = tuple(c.strip() for c in args.classes.split(","))
     acc = ev.EvalAccumulator(cls_list=cls_list, cls_thresh=args.cls_thresh)
     for i in range(0, len(paths), args.batch):
         samples = [io.read_sample(p) for p in paths[i:i + args.batch]]
         points, calibs, names = io.make_batch(samples, args.num_points, seed=i)
-        xyz, feat = net.forward(points.to(dev, non_blocking=True))[:2]
-        block, count = net.detections(xyz, feat)
+        block, count = detect(points.to(dev, non_blocking=True))
         acc.add(block, count, calibs, [os.path.join(args.labels, "%06d.txt" % int(n)) for n in names])
     result = acc.evaluate(dev)
     print("evaluated %d frames" % len(acc))
