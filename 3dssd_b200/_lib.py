@@ -142,6 +142,11 @@ _SIGNATURES = {
     "ssd3d_prepare_workspace": [c_int, c_int],
     "ssd3d_prepare_points": [c_int, c_int, c_int] + [c_void_p] * 9,
 }
+# the *_ex forms: the prototype of the named call followed by one more argument
+for _base, _extra in (("ssd3d_query_ball_point_multi_ws", c_void_p), ("ssd3d_hoist_expand_split_units", c_int),
+                      ("ssd3d_linear_tc_units", c_int), ("ssd3d_linear_tc_hoisted_units", c_int),
+                      ("ssd3d_sa_mlp_fused", c_int), ("ssd3d_sa_mlp_fused_hoisted", c_int)):
+    _SIGNATURES[_base + "_ex"] = _SIGNATURES[_base] + [_extra]
 
 EXPORTS = sorted(list(_SIGNATURES) + ["ssd3d_last_error"])
 

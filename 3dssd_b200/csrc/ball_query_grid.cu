@@ -184,10 +184,12 @@ struct BqgParams {
     float t_max;
     int *idx[BQG_MAX_SHELLS];
     int *cnt[BQG_MAX_SHELLS];
-    // optional per-shell UNIT LISTS for the grouped MLP (include/ssd3d.h, ssd3d_query_ball_point_multi_ws): units[s][0] counts
-    // the units, units[s][1 + u] = (group << 4) | j names rows 8j .. 8j+7 of that group's neighbour list.  A group with cnt
-    // hits gets ceil(cnt / 8) units: the slots beyond cnt repeat the first hit and cannot change a max-pool.
+    // optional per-shell UNIT LISTS for the grouped MLP (include/ssd3d.h, ssd3d_query_ball_point_multi_ws_ex): units[s][0]
+    // counts the units, units[s][1 + u] = (group << 4) | j names rows Wj .. Wj+W-1 of that group's neighbour list, W =
+    // 1 << lgu[s] (8 or 4).  A group with cnt hits gets ceil(cnt / W) units: the slots beyond cnt repeat the first hit and
+    // cannot change a max-pool.
     int *units[BQG_MAX_SHELLS];
+    int lgu[BQG_MAX_SHELLS];
 };
 
 // Bitmap word wi of a shell lives at wi + (wi >> lg): one pad word per lane chunk of 2^lg words, so that the chunks of
@@ -195,10 +197,10 @@ struct BqgParams {
 // bank conflicts (unpadded, 16-word chunks collide 16 ways: that alone was ~90% of the first version's run time).
 constexpr int BQG_WORDS_P = BQG_WORDS + 32;
 
-__device__ __forceinline__ void bqg_emit_units(int *units, int group, int cnt)
+__device__ __forceinline__ void bqg_emit_units(int *units, int group, int cnt, int lgu)
 {
     if (units == nullptr || cnt <= 0) return;
-    const int nu = (cnt + 7) >> 3;
+    const int nu = (cnt + (1 << lgu) - 1) >> lgu;
     const int base = atomicAdd(units, nu);                 // order of the list is irrelevant: the consumer max-pools
     for (int j = 0; j < nu; j++) units[1 + base + j] = (group << 4) | j;
 }
@@ -285,7 +287,7 @@ ball_query_grid_kernel(const float *__restrict__ xyz1, const float *__restrict__
                 for (int l = c + lane; l < ns; l += 32) dst[l] = first[s];   // back-fill (zeros for an empty ball)
                 if (lane == 0) {
                     p.cnt[s][(size_t)scene * m + qi] = c;
-                    bqg_emit_units(p.units[s], scene * m + qi, c);
+                    bqg_emit_units(p.units[s], scene * m + qi, c, p.lgu[s]);
                 }
             }
             continue;
@@ -360,7 +362,7 @@ ball_query_grid_kernel(const float *__restrict__ xyz1, const float *__restrict__
             else for (int l = lane; l < ns; l += 32) dst[l] = 0;                     // empty ball: the caller's idx * (cnt > 0)
             if (lane == 0) {
                 p.cnt[s][(size_t)scene * m + qi] = c;
-                bqg_emit_units(p.units[s], scene * m + qi, c);
+                bqg_emit_units(p.units[s], scene * m + qi, c, p.lgu[s]);
             }
         }
         __syncwarp();
@@ -370,9 +372,9 @@ ball_query_grid_kernel(const float *__restrict__ xyz1, const float *__restrict__
 float bq_sq_threshold(float r);   // ball_query.cu
 
 // Unit lists from finished neighbour counts (the exhaustive kernel's route: small candidate sets): one CTA per shell scans
-// the groups in order -- a group with cnt hits owns ceil(cnt / 8) units -- so this list is in group order.
+// the groups in order -- a group with cnt hits owns ceil(cnt / W) units of W = 1 << lgu rows -- so this list is in group order.
 constexpr int GU_THREADS = 1024;
-struct GuParams { const int *cnt[BQG_MAX_SHELLS]; int *units[BQG_MAX_SHELLS]; int nsample[BQG_MAX_SHELLS]; };
+struct GuParams { const int *cnt[BQG_MAX_SHELLS]; int *units[BQG_MAX_SHELLS]; int nsample[BQG_MAX_SHELLS]; int lgu[BQG_MAX_SHELLS]; };
 
 __global__ void __launch_bounds__(GU_THREADS)
 group_units_kernel(int groups, const GuParams p)
@@ -381,13 +383,13 @@ group_units_kernel(int groups, const GuParams p)
     int *units = p.units[s];
     if (units == nullptr) return;
     const int *cnt = p.cnt[s];
-    const int ns = p.nsample[s];
+    const int ns = p.nsample[s], lgu = p.lgu[s], w1 = (1 << lgu) - 1;
     __shared__ int warp_tot[GU_THREADS / 32];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int per = (groups + GU_THREADS - 1) / GU_THREADS;
     const int g0 = min(groups, tid * per), g1 = min(groups, g0 + per);
     int mine = 0;
-    for (int g = g0; g < g1; g++) mine += (min(__ldg(cnt + g), ns) + 7) >> 3;
+    for (int g = g0; g < g1; g++) mine += (min(__ldg(cnt + g), ns) + w1) >> lgu;
     int incl = mine;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
@@ -409,7 +411,7 @@ group_units_kernel(int groups, const GuParams p)
     int pos = incl - mine + (warp > 0 ? warp_tot[warp - 1] : 0);
     if (tid == GU_THREADS - 1) units[0] = pos + mine;
     for (int g = g0; g < g1; g++) {
-        const int nu = (min(__ldg(cnt + g), ns) + 7) >> 3;
+        const int nu = (min(__ldg(cnt + g), ns) + w1) >> lgu;
         for (int j = 0; j < nu; j++) units[1 + pos + j] = (g << 4) | j;
         pos += nu;
     }
@@ -445,15 +447,40 @@ extern "C" int ssd3d_query_ball_point_multi_ws(int b, int n, int m, int nqueries
                                                const float *xyz2, int *const *idx, int *const *pts_cnt, int *const *units,
                                                void *workspace, size_t workspace_bytes, ssd3d_stream_t stream)
 {
+    return ssd3d_query_ball_point_multi_ws_ex(b, n, m, nqueries, dilated, min_radius, max_radius, nsample, xyz1, xyz2, idx, pts_cnt,
+                                              units, workspace, workspace_bytes, stream, nullptr);
+}
+
+// rows per unit of shell s's list: 8 (no unit_rows array) or unit_rows[s], 8 or 4; a list names at most 16 units per group
+static int bq_unit_lg(const int *unit_rows, int s) { return unit_rows == nullptr || unit_rows[s] == 8 ? 3 : 2; }
+static int bq_check_units(int *const *units, const int *unit_rows, const int *nsample, int nqueries, int b, int m)
+{
+    if (!units) return 0;
+    SSD3D_REQUIRE(nqueries >= 1 && nqueries <= BQG_MAX_SHELLS, "query_ball_point: unit lists for 1..%d radius shells per call, got %d", BQG_MAX_SHELLS, nqueries);
+    for (int s = 0; s < nqueries; s++) {
+        if (!units[s]) continue;
+        const int w = unit_rows ? unit_rows[s] : 8;
+        SSD3D_REQUIRE(w == 8 || w == 4, "query_ball_point: unit_rows[%d]=%d must be 8 or 4", s, w);
+        SSD3D_REQUIRE(nsample[s] <= 16 * w, "query_ball_point: unit lists of %d-row units cover nsample <= %d, got %d", w, 16 * w, nsample[s]);
+        SSD3D_REQUIRE((long)b * m < (1L << 27), "query_ball_point: too many groups for a unit list");
+    }
+    return 0;
+}
+
+extern "C" int ssd3d_query_ball_point_multi_ws_ex(int b, int n, int m, int nqueries, int dilated, const float *min_radius,
+                                                  const float *max_radius, const int *nsample, const float *xyz1,
+                                                  const float *xyz2, int *const *idx, int *const *pts_cnt, int *const *units,
+                                                  void *workspace, size_t workspace_bytes, ssd3d_stream_t stream,
+                                                  const int *unit_rows)
+{
+    if (int rc = bq_check_units(units, unit_rows, nsample, nqueries, b, m)) return rc;
     if (workspace == nullptr || workspace_bytes == 0) {
         const int rc = ssd3d_query_ball_point_multi(b, n, m, nqueries, dilated, min_radius, max_radius, nsample, xyz1, xyz2, idx,
                                                     pts_cnt, stream);
         if (rc || units == nullptr || b == 0 || m == 0) return rc;
         GuParams gp = {};
         for (int s = 0; s < nqueries; s++) {
-            gp.cnt[s] = pts_cnt[s]; gp.units[s] = units[s]; gp.nsample[s] = nsample[s];
-            SSD3D_REQUIRE(!units[s] || nsample[s] <= 128, "query_ball_point: unit lists cover nsample <= 128");
-            SSD3D_REQUIRE(!units[s] || (long)b * m < (1L << 27), "query_ball_point: too many groups for a unit list");
+            gp.cnt[s] = pts_cnt[s]; gp.units[s] = units[s]; gp.nsample[s] = nsample[s]; gp.lgu[s] = bq_unit_lg(unit_rows, s);
         }
         group_units_kernel<<<nqueries, GU_THREADS, 0, (cudaStream_t)stream>>>(b * m, gp);
         SSD3D_LAUNCH_CHECK("group_units_kernel");
@@ -481,8 +508,7 @@ extern "C" int ssd3d_query_ball_point_multi_ws(int b, int n, int m, int nqueries
         p.idx[s] = idx[s];
         p.cnt[s] = pts_cnt[s];
         p.units[s] = units ? units[s] : nullptr;
-        SSD3D_REQUIRE(!p.units[s] || nsample[s] <= 128, "query_ball_point: unit lists cover nsample <= 128");
-        SSD3D_REQUIRE(!p.units[s] || (long)b * m < (1L << 27), "query_ball_point: too many groups for a unit list");
+        p.lgu[s] = bq_unit_lg(unit_rows, s);
     }
     p.t_max = tmax;
     if (b == 0 || m == 0) return 0;

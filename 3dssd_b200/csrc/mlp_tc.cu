@@ -91,13 +91,14 @@ struct TcParams {
     int gather, g_n, g_c, g_m, g_ns, g_ldz;
     const float *g_xyz, *g_points, *g_new_xyz, *g_wx;
     const int *g_idx;
-    // UNIT-LIST mode (include/ssd3d.h, ssd3d_query_ball_point_multi_ws): units[0] = U, units[1 + u] = (group << 4) | j names
-    // rows 8j .. 8j+7 of a group's neighbour list.  The matrix this launch works on then has U * 8 rows -- compact row
-    // 8u + e is neighbour slot 8j + e of that group -- instead of `rows` (which stays the capacity of the buffers): the
-    // gather producers look their source up through the list, and unit_pool max-pools each 8-row unit and combines the
-    // units of a group with atomicMax on out_f32[group] (zero-filled by the caller; values are post-ReLU, >= 0).
+    // UNIT-LIST mode (include/ssd3d.h, ssd3d_query_ball_point_multi_ws_ex): units[0] = number of units, units[1 + u] =
+    // (group << 4) | j names rows Wj .. Wj+W-1 of a group's neighbour list, W = 1 << unit_lg (8 or 4).  The matrix this
+    // launch works on then has units[0] * W rows -- compact row Wu + e is neighbour slot Wj + e of that group -- instead of
+    // `rows` (which stays the capacity of the buffers): the gather producers look their source up through the list, and
+    // unit_pool max-pools each W-row unit and combines the units of a group with atomicMax on out_f32[group] (zero-filled
+    // by the caller; values are post-ReLU, >= 0).
     const int *units;
-    int unit_pool;
+    int unit_pool, unit_lg;
 };
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------------
@@ -263,6 +264,18 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &p, float (&d)[BN / 2
                 }
             }
         }
+    } else if (p.unit_pool && p.unit_lg == 2) {
+        // each 4-row quarter of the warp's 16 rows is one listed unit: two butterfly steps, then lane t owns slots
+        // s = i + (BN/8)((t/4) % 4) of rows 4(t/16) .. 4(t/16)+3 of row half (s/2)%2
+        quad_rowmax4_transpose<BN / 2>(d, lane);
+#pragma unroll
+        for (int i = 0; i < BN / 8; i++) {
+            const int s = i + (BN / 8) * (rq & 3);
+            const int ui = mt * (TC_BM / 4) + 4 * we + 2 * ((s >> 1) & 1) + (rq >> 2);
+            const int col = col_t + 8 * (s >> 2) + cq + (s & 1);
+            if (ui >= nunits || col >= p.n) continue;
+            atomic_max_nonneg(p.out_f32 + (size_t)unit_group((uint32_t)__ldg(p.units + 1 + ui)) * p.ld_f32 + col, d[i]);
+        }
     } else if (p.unit_pool) {
         // each 8-row fragment half is one listed unit; its column maxima go to the unit's GROUP row by atomicMax
         frag_pool8<BN>(d, lane);
@@ -373,8 +386,8 @@ linear_tc_tma_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_c
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     // unit-list mode: the row count comes from the list (written earlier on this stream), p.rows is the buffers' capacity
     const int nunits = p.units ? __ldg(p.units) : 0;
-    const long rows = p.units ? (long)nunits * 8 : p.rows;
-    const int m_tiles = p.units ? (nunits + TC_BM / 8 - 1) / (TC_BM / 8) : p.m_tiles;
+    const long rows = p.units ? (long)nunits << p.unit_lg : p.rows;
+    const int m_tiles = p.units ? (nunits + (TC_BM >> p.unit_lg) - 1) / (TC_BM >> p.unit_lg) : p.m_tiles;
     const int n_all = m_tiles * p.n_tiles;                               // tiles, n-major round robin over the CTAs
 
     if (threadIdx.x == 0) {
@@ -465,8 +478,8 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_const
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // provably warp-uniform
     // unit-list mode: the row count comes from the list (written earlier on this stream), p.rows is the buffers' capacity
     const int nunits = p.units ? __ldg(p.units) : 0;
-    const long rows = p.units ? (long)nunits * 8 : p.rows;
-    const int m_tiles = p.units ? (nunits + TC_BM / 8 - 1) / (TC_BM / 8) : p.m_tiles;
+    const long rows = p.units ? (long)nunits << p.unit_lg : p.rows;
+    const int m_tiles = p.units ? (nunits + (TC_BM >> p.unit_lg) - 1) / (TC_BM >> p.unit_lg) : p.m_tiles;
     // local tile i of this CTA -> (mt, nt): n-major round robin over all tiles, or (astat) every n-tile of an m-tile
     auto tile_at = [&](int i, int &mt, int &nt) -> bool {
         if (p.astat) {
@@ -538,7 +551,9 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_bhi, const __grid_const
             const uint32_t row = (uint32_t)mt * TC_BM + (uint32_t)r;
             const bool ok = (long)row < rows;
             uint32_t rr = ok ? row : 0u;                          // position of this row's neighbour in idx[]
-            if (p.units && ok) rr = unit_slot((uint32_t)__ldg(p.units + 1 + (row >> 3)), (uint32_t)p.g_ns, row & 7u);
+            if (p.units && ok)
+                rr = unit_slot((uint32_t)__ldg(p.units + 1 + (row >> p.unit_lg)), (uint32_t)p.g_ns, (uint32_t)p.unit_lg,
+                               row & ((1u << p.unit_lg) - 1u));
             const uint32_t scene = rr / rps, q = rr / (uint32_t)p.g_ns;
             const int a = __ldg(p.g_idx + rr);
             const float *src_f = p.g_points + ((size_t)scene * p.g_n + a) * src_pitch;
@@ -731,11 +746,11 @@ group_concat_split_kernel(long rows, int n, int c, int m, int ns, const float *_
 __global__ void __launch_bounds__(256, 6)
 hoist_expand_split_kernel(long rows, int n, int n1, int m, int ns, const float *__restrict__ xyz, const float *__restrict__ z,
                           int ldz, const float *__restrict__ wx, const float *__restrict__ new_xyz,
-                          const int *__restrict__ idx, const int *__restrict__ units, __nv_bfloat16 *__restrict__ hi,
-                          __nv_bfloat16 *__restrict__ lo, int kp)
+                          const int *__restrict__ idx, const int *__restrict__ units, int lgu,
+                          __nv_bfloat16 *__restrict__ hi, __nv_bfloat16 *__restrict__ lo, int kp)
 {
     extern __shared__ __align__(16) float hx_wx[];                      // [3][kp] zero padded
-    if (units) rows = (long)__ldg(units) * 8;                           // unit-list mode (TcParams::units): compact rows
+    if (units) rows = (long)__ldg(units) << lgu;                        // unit-list mode (TcParams::units): compact rows
     for (int i = threadIdx.x; i < 3 * kp; i += blockDim.x) {
         const int a = i / kp, k = i - a * kp;
         hx_wx[i] = k < n1 ? __ldg(wx + a * n1 + k) : 0.0f;
@@ -747,7 +762,7 @@ hoist_expand_split_kernel(long rows, int n, int n1, int m, int ns, const float *
     const int nchunk = kp >> 3;
     for (long row = warp0; row < rows; row += nwarps) {
         long src = row;                                                  // position of this row's neighbour in idx[]
-        if (units) src = unit_slot((uint32_t)__ldg(units + 1 + (row >> 3)), (uint32_t)ns, (uint32_t)row & 7u);
+        if (units) src = unit_slot((uint32_t)__ldg(units + 1 + (row >> lgu)), (uint32_t)ns, (uint32_t)lgu, (uint32_t)row & ((1u << lgu) - 1u));
         const long scene = src / rps, q = src / ns;
         const int a = __ldg(idx + src);
         const float *px = xyz + ((size_t)scene * n + a) * 3, *pc = new_xyz + (size_t)q * 3;
@@ -831,11 +846,12 @@ struct TcGather { int b, n, c, m, ns; const float *xyz, *points, *new_xyz; const
 static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const void *a_lo, const TcGather *g,
                             const void *b_hi, const void *b_lo, const float *scale, const float *shift, int relu, int pool,
                             const int *rowmask, float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split,
-                            cudaStream_t stream, const int *units = nullptr, int unit_pool = 0)
+                            cudaStream_t stream, const int *units = nullptr, int unit_pool = 0, int unit_rows = 8)
 {
     SSD3D_REQUIRE(rows >= 0 && kp > 0 && n > 0, "linear_tc: bad shape rows=%ld kp=%d n=%d", rows, kp, n);
     if (units) {
-        SSD3D_REQUIRE(rows % 8 == 0 && pool == 1 && rowmask == nullptr, "linear_tc (unit list): rows=%ld must be a multiple of 8, no pool / rowmask", rows);
+        SSD3D_REQUIRE(unit_rows == 8 || unit_rows == 4, "linear_tc (unit list): unit_rows=%d must be 8 or 4", unit_rows);
+        SSD3D_REQUIRE(rows % unit_rows == 0 && pool == 1 && rowmask == nullptr, "linear_tc (unit list): rows=%ld must be a multiple of %d, no pool / rowmask", rows, unit_rows);
         if (unit_pool) {
             SSD3D_REQUIRE(relu && out_f32 && !out_hi, "linear_tc (unit list): pooling combines post-ReLU values by atomicMax into out_f32 only");
             pool = 8;
@@ -922,7 +938,7 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
     SSD3D_REQUIRE(stages >= 2, "linear_tc: tile does not fit shared memory");
     p.stages = stages;
     p.scale = scale; p.shift = shift; p.relu = relu; p.pool = pool; p.rowmask = rowmask;
-    p.units = units; p.unit_pool = unit_pool;
+    p.units = units; p.unit_pool = unit_pool; p.unit_lg = unit_rows == 4 ? 2 : 3;
     p.out_f32 = out_f32; p.ld_f32 = ld_f32;
     p.out_hi = (__nv_bfloat16 *)out_hi; p.out_lo = (__nv_bfloat16 *)out_lo; p.ld_split = ld_split;
 
@@ -985,7 +1001,7 @@ static int linear_tc_launch(long rows, int kp, int n, const void *a_hi, const vo
 
 static int hoist_expand_split_launch(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z, int ldz,
                                      const float *wx, const float *new_xyz, const int *idx, const int *units, void *hi,
-                                     void *lo, int kp, ssd3d_stream_t stream)
+                                     void *lo, int kp, ssd3d_stream_t stream, int unit_rows = 8)
 {
     SSD3D_REQUIRE(b >= 0 && n > 0 && m >= 0 && n1 > 0 && nsample > 0 && ldz >= n1, "hoist_expand_split: bad shape");
     SSD3D_REQUIRE(kp % 16 == 0 && kp >= n1 && kp <= 4096, "hoist_expand_split: kp=%d must be a multiple of 16 in [n1, 4096]", kp);
@@ -997,7 +1013,8 @@ static int hoist_expand_split_launch(int b, int n, int n1, int m, int nsample, c
     const long blocks_want = (rows + 7) / 8;
     const int blocks = (int)(blocks_want < (long)kNumSMs * 32 ? blocks_want : (long)kNumSMs * 32);
     hoist_expand_split_kernel<<<blocks, 256, (size_t)3 * kp * sizeof(float), (cudaStream_t)stream>>>(
-        rows, n, n1, m, nsample, xyz, z, ldz, wx, new_xyz, idx, units, (__nv_bfloat16 *)hi, (__nv_bfloat16 *)lo, kp);
+        rows, n, n1, m, nsample, xyz, z, ldz, wx, new_xyz, idx, units, unit_rows == 4 ? 2 : 3, (__nv_bfloat16 *)hi,
+        (__nv_bfloat16 *)lo, kp);
     SSD3D_LAUNCH_CHECK("hoist_expand_split_kernel");
 }
 
@@ -1012,8 +1029,25 @@ extern "C" int ssd3d_hoist_expand_split_units(int b, int n, int n1, int m, int n
                                               int ldz, const float *wx, const float *new_xyz, const int *idx,
                                               const int *units, void *hi, void *lo, int kp, ssd3d_stream_t stream)
 {
-    SSD3D_REQUIRE(units && nsample % 8 == 0 && nsample <= 128, "hoist_expand_split_units: needs a unit list and nsample a multiple of 8, <= 128");
-    return hoist_expand_split_launch(b, n, n1, m, nsample, xyz, z, ldz, wx, new_xyz, idx, units, hi, lo, kp, stream);
+    return ssd3d_hoist_expand_split_units_ex(b, n, n1, m, nsample, xyz, z, ldz, wx, new_xyz, idx, units, hi, lo, kp, stream, 8);
+}
+
+// The unit lists of 8- and 4-row units (include/ssd3d.h): a list names at most 16 units per group, so 4-row units
+// cover nsample <= 64 and 8-row units nsample <= 128
+static bool unit_rows_ok(int unit_rows, int nsample)
+{
+    return (unit_rows == 8 || unit_rows == 4) && nsample % unit_rows == 0 && nsample <= 16 * unit_rows;
+}
+
+extern "C" int ssd3d_hoist_expand_split_units_ex(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z,
+                                                 int ldz, const float *wx, const float *new_xyz, const int *idx,
+                                                 const int *units, void *hi, void *lo, int kp, ssd3d_stream_t stream,
+                                                 int unit_rows)
+{
+    SSD3D_REQUIRE(units && unit_rows_ok(unit_rows, nsample),
+                  "hoist_expand_split_units: needs a unit list, unit_rows 8 or 4 and nsample a multiple of it, <= 16 * unit_rows (nsample=%d unit_rows=%d)",
+                  nsample, unit_rows);
+    return hoist_expand_split_launch(b, n, n1, m, nsample, xyz, z, ldz, wx, new_xyz, idx, units, hi, lo, kp, stream, unit_rows);
 }
 
 // Unit-list forms of ssd3d_linear_tc / ssd3d_linear_tc_hoisted (TcParams::units): the matrix has units[0] * 8 rows (`rows` /
@@ -1024,9 +1058,19 @@ extern "C" int ssd3d_linear_tc_units(long rows, int kp, int n, const void *a_hi,
                                      int unit_pool, float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split,
                                      ssd3d_stream_t stream)
 {
+    return ssd3d_linear_tc_units_ex(rows, kp, n, a_hi, a_lo, b_hi, b_lo, scale, shift, relu, units, unit_pool, out_f32, ld_f32,
+                                    out_hi, out_lo, ld_split, stream, 8);
+}
+
+// ... with units of unit_rows (8 or 4) rows: the matrix has units[0] * unit_rows rows
+extern "C" int ssd3d_linear_tc_units_ex(long rows, int kp, int n, const void *a_hi, const void *a_lo, const void *b_hi,
+                                        const void *b_lo, const float *scale, const float *shift, int relu, const int *units,
+                                        int unit_pool, float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split,
+                                        ssd3d_stream_t stream, int unit_rows)
+{
     SSD3D_REQUIRE(units, "linear_tc_units: null unit list");
     return linear_tc_launch(rows, kp, n, a_hi, a_lo, nullptr, b_hi, b_lo, scale, shift, relu, 1, nullptr, out_f32, ld_f32,
-                            out_hi, out_lo, ld_split, (cudaStream_t)stream, units, unit_pool);
+                            out_hi, out_lo, ld_split, (cudaStream_t)stream, units, unit_pool, unit_rows);
 }
 
 extern "C" int ssd3d_linear_tc_hoisted_units(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z,
@@ -1035,13 +1079,25 @@ extern "C" int ssd3d_linear_tc_hoisted_units(int b, int n, int n1, int m, int ns
                                              const float *scale, const float *shift, int relu, int unit_pool, float *out_f32,
                                              int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream)
 {
+    return ssd3d_linear_tc_hoisted_units_ex(b, n, n1, m, nsample, xyz, z, ldz, wx, new_xyz, idx, units, nout, b_hi, b_lo, scale,
+                                            shift, relu, unit_pool, out_f32, ld_f32, out_hi, out_lo, ld_split, stream, 8);
+}
+
+extern "C" int ssd3d_linear_tc_hoisted_units_ex(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z,
+                                                int ldz, const float *wx, const float *new_xyz, const int *idx,
+                                                const int *units, int nout, const void *b_hi, const void *b_lo,
+                                                const float *scale, const float *shift, int relu, int unit_pool, float *out_f32,
+                                                int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream,
+                                                int unit_rows)
+{
     SSD3D_REQUIRE(b >= 0 && n > 0 && m >= 0 && n1 > 0 && nsample > 0 && ldz >= n1, "linear_tc_hoisted_units: bad shape");
     SSD3D_REQUIRE(xyz && new_xyz && idx && z && wx && units, "linear_tc_hoisted_units: null pointer");
-    SSD3D_REQUIRE(nsample % 8 == 0 && nsample <= 128, "linear_tc_hoisted_units: nsample=%d must be a multiple of 8, <= 128", nsample);
+    SSD3D_REQUIRE(unit_rows_ok(unit_rows, nsample),
+                  "linear_tc_hoisted_units: nsample=%d must be a multiple of unit_rows=%d (8 or 4), <= 16 * unit_rows", nsample, unit_rows);
     TcGather g = {b, n, n1, m, nsample, xyz, z, new_xyz, idx, ldz, wx};
     const int kp = (n1 + 15) / 16 * 16;
     return linear_tc_launch((long)b * m * nsample, kp, nout, nullptr, nullptr, &g, b_hi, b_lo, scale, shift, relu, 1, nullptr,
-                            out_f32, ld_f32, out_hi, out_lo, ld_split, (cudaStream_t)stream, units, unit_pool);
+                            out_f32, ld_f32, out_hi, out_lo, ld_split, (cudaStream_t)stream, units, unit_pool, unit_rows);
 }
 
 extern "C" int ssd3d_linear_tc(long rows, int kp, int n, const void *a_hi, const void *a_lo, const void *b_hi,

@@ -49,10 +49,11 @@ __device__ __forceinline__ void split_store8(void *hi, void *lo, const float (&f
 // rows, the layout the wgmma descriptors (wg_desc(.., 128)) and the 128B-swizzled TMA boxes use
 __device__ __forceinline__ uint32_t sw128_chunk(uint32_t row, uint32_t c16) { return row * 128u + ((c16 ^ (row & 7u)) << 4); }
 
-// Unit lists (include/ssd3d.h, ssd3d_query_ball_point_multi_ws): desc = (group << 4) | j names rows 8j .. 8j+7 of
-// neighbour list `group`.  Row e (< 8) of the unit is entry unit_slot(desc, ns, e) of idx[] (grouped rows < 2^31).
+// Unit lists (include/ssd3d.h, ssd3d_query_ball_point_multi_ws_ex): desc = (group << 4) | j names rows U j .. U j + U-1
+// of neighbour list `group`, U = 1 << lgu rows per unit (8 or 4, fixed per list).  Row e (< U) of the unit is entry
+// unit_slot(desc, ns, lgu, e) of idx[] (grouped rows < 2^31).  Templated kernels pass lgu as a literal.
 __device__ __forceinline__ uint32_t unit_group(uint32_t desc) { return desc >> 4; }
-__device__ __forceinline__ uint32_t unit_slot(uint32_t desc, uint32_t ns, uint32_t e) { return (desc >> 4) * ns + ((desc & 15u) << 3) + e; }
+__device__ __forceinline__ uint32_t unit_slot(uint32_t desc, uint32_t ns, uint32_t lgu, uint32_t e) { return (desc >> 4) * ns + ((desc & 15u) << lgu) + e; }
 
 // Columns k0 .. k0+7 of a grouped operand row concat(src_f[0:c], src_x - ctr) cut at column kend (c + 3, or c when only
 // the features are wanted), zero beyond kend and for a row that does not exist (!ok).  vec: src_f is 16-byte aligned.

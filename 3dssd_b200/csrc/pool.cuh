@@ -30,4 +30,14 @@ __device__ __forceinline__ void quad_rowmax_transpose(float (&v)[N], int lane)
     colmax_step(v, lane, 4, N / 8);
 }
 
+// The same over the 4 lanes of a column quad that share lane bit 4 (rows 0-3 or 4-7 of a fragment half, the 4-row units of
+// a unit list): on return lane t owns, in v[i], i < N/4, the maximum of value slot i + (N/4)((t/4) % 4) over rows
+// 4(t/16) .. 4(t/16)+3.  N/2 + N/4 shuffles, one step fewer than the 8-row pool.
+template <int N>
+__device__ __forceinline__ void quad_rowmax4_transpose(float (&v)[N], int lane)
+{
+    colmax_step(v, lane, 8, N / 2);
+    colmax_step(v, lane, 4, N / 4);
+}
+
 }  // namespace ssd3d

@@ -26,7 +26,8 @@
 // (the ball query lists ceil(cnt / 8) units per non-empty group) instead of 128 consecutive rows; each unit is pooled by the
 // shuffle butterfly and the units of a group meet through atomicMax on the non-negative fp32 result, which the caller
 // zero-fills (= the cnt == 0 mask of layers_util.py:180).  Same bits as the dense schedule, 4-8x fewer rows on KITTI-like
-// clouds (DESIGN.md section 3.4).
+// clouds (DESIGN.md section 3.4).  Lists of 4-row units (SfParams::unit_lg == 2, nsample <= 64) put 32 units in a tile and
+// pool each with one butterfly step fewer; groups of 1-4 hits then convolve 4 rows instead of 8.
 //
 // Precision: same bf16 hi/lo split and 3-MMA scheme as mlp_tc.cu.
 #include <cuda_bf16.h>
@@ -56,6 +57,7 @@ struct SfParams {
     // names rows 8j..8j+7 of neighbour list `group` -- instead of 128 consecutive rows, units[0] is their number, and the
     // pooled result is combined across the units of a group with atomicMax on the (non-negative) fp32 output
     const int *units;
+    int unit_lg;                     // log2 of the rows per unit: 3 (8-row units) or 2 (4-row units)
     // hoisted first conv (see ssd3d_linear_tc_hoisted in include/ssd3d.h): `points` is the per-point table z (row pitch
     // ldz, c = its width n1), the operand row is relu(z[idx] + (xyz[idx] - new_xyz) . wx) with wx = [3][c], and the
     // stack starts at the scale's SECOND conv (K = c, no xyz columns appended)
@@ -140,6 +142,7 @@ struct SfDyn {
     __device__ __forceinline__ int ns() const { return p.ns; }
     __device__ __forceinline__ int c() const { return p.c; }
     __device__ __forceinline__ bool hoist() const { return p.hoist != 0; }
+    __device__ __forceinline__ int lgu() const { return p.unit_lg; }
     __device__ __forceinline__ int kp(int l) const { return p.kp[l]; }
     __device__ __forceinline__ int npad(int l) const { return p.npad[l]; }
     __device__ __forceinline__ int nout(int l) const { return p.nout[l]; }
@@ -155,8 +158,8 @@ struct SfDyn {
 };
 
 // Hoisted stacks of two convs (the shipped configuration): operand width K0 = n1 of the hoisted first conv, then
-// K0 -> N0 -> N1, NS neighbours per group.
-template <int K0, int N0, int N1, int NS>
+// K0 -> N0 -> N1, NS neighbours per group, unit lists (if any) of 1 << LGU rows per unit.
+template <int K0, int N0, int N1, int NS, int LGU = 3>
 struct SfStat {
     static constexpr bool kStatic = true;
     __device__ __forceinline__ explicit SfStat(const SfParams &) {}
@@ -165,6 +168,7 @@ struct SfStat {
     __device__ __forceinline__ constexpr int ns() const { return NS; }
     __device__ __forceinline__ constexpr int c() const { return K0; }
     __device__ __forceinline__ constexpr bool hoist() const { return true; }
+    __device__ __forceinline__ constexpr int lgu() const { return LGU; }
     __device__ __forceinline__ constexpr int kp(int l) const { return l == 0 ? KP0 : NP0; }
     __device__ __forceinline__ constexpr int npad(int l) const { return l == 0 ? NP0 : NP1; }
     __device__ __forceinline__ constexpr int nout(int l) const { return l == 0 ? N0 : N1; }
@@ -316,19 +320,21 @@ sa_fused_kernel(const SfParams p)
     const int tile0 = blockIdx.x * SLOTS + slot, tstep = gridDim.x * SLOTS;
     const int *units = p.units;
     __builtin_assume(units == nullptr || __isGlobal(units));
-    const bool compact = units != nullptr;
+    // (a compile-time twin of 4-row units is launched with a unit list only: its dense schedule is never compiled)
+    const bool compact = (C::kStatic && cfg.lgu() == 2) || units != nullptr;
     const int nunits = compact ? __ldg(units) : 0;
-    const int tiles = compact ? (nunits + 15) >> 4 : p.tiles;
+    const int lgu = cfg.lgu(), upt = 128 >> lgu;        // rows per unit (log2), units per tile
+    const int tiles = compact ? (nunits + upt - 1) / upt : p.tiles;
     // neighbour index (and, in unit-list mode, unit descriptor) of this thread's row, fetched one tile ahead
     // (rows < 2^31: checked by the launcher)
     auto fetch = [&](int tl, int &desc, int &a) {
         desc = -1; a = 0;
         if (tl >= tiles) return;
         if (compact) {
-            const int ui = tl * 16 + (r >> 3);
+            const int ui = tl * upt + (r >> lgu);
             if (ui < nunits) {
                 desc = __ldg(units + 1 + ui);
-                a = __ldg(p.idx + unit_slot((uint32_t)desc, (uint32_t)cfg.ns(), (uint32_t)r & 7u));
+                a = __ldg(p.idx + unit_slot((uint32_t)desc, (uint32_t)cfg.ns(), (uint32_t)lgu, (uint32_t)r & ((1u << lgu) - 1u)));
             }
         } else if ((long)tl * 128 + r < p.rows) {
             desc = 0;
@@ -451,6 +457,22 @@ sa_fused_kernel(const SfParams p)
                                     d[4 * j + 2] = fmaxf(fmaf(d[4 * j + 2], s2.x, h2.x), 0.0f);
                                     d[4 * j + 3] = fmaxf(fmaf(d[4 * j + 3], s2.y, h2.y), 0.0f);
                                 }
+                            }
+                            if (compact && lgu == 2) {
+                                // 4-row maxima: lane owns slots s = i + (W/8)((lane/4) % 4) of d, column 8(s/4) + cq + (s%2)
+                                // of rows 4(lane/16) .. +3 of the 8-row slab (s/2)%2 of its warp's 16 rows: one listed unit,
+                                // combined into its group by atomicMax
+                                quad_rowmax4_transpose<W / 2>(d, lane);
+#pragma unroll
+                                for (int i = 0; i < W / 8; i++) {
+                                    const int s = i + (W / 8) * ((lane >> 2) & 3);
+                                    const int ui = tile * 32 + 16 * hf + 4 * q + 2 * ((s >> 1) & 1) + (lane >> 4);
+                                    const int col = 64 * c + 8 * (s >> 2) + cq + (s & 1);
+                                    if (ui < nunits && col < nout)
+                                        atomic_max_nonneg(p.out_f32 + (size_t)unit_group((uint32_t)__ldg(units + 1 + ui)) * p.ld_f32 + col,
+                                                          finish(d[i], col));
+                                }
+                                continue;                              // (the row half's last step)
                             }
                             // 8-row maxima: lane owns slots s = i + (W/16)(lane/4) of d, column 8(s/4) + cq + (s%2) of the
                             // 8-row slab (s/2)%2 of its warp's 16 rows
@@ -575,20 +597,27 @@ static cudaError_t sf_launch(const SfParams &p, size_t smem, int per_sm, cudaStr
 
 // The hoisted two-conv stacks of the shipped 3DSSD configuration (configs/kitti/3dssd/3dssd.yaml:47-52) have compile-time
 // twins of the kernel: layer 1 [16 -> 16 -> 32] x32 and [32 -> 32 -> 64] x64 neighbours, layer 2 [64 -> 64 -> 128] x32 and
-// [64 -> 96 -> 128] x64.  Returns false when (shape, slots, warpgroups) has no twin: the caller takes the dynamic kernel.
+// [64 -> 96 -> 128] x64, each for 8-row units (and the dense schedule) and for lists of 4-row units.  Returns false when
+// (shape, slots, warpgroups) has no twin: the caller takes the dynamic kernel.
+template <int LGU>
+static bool sf_launch_static_lg(const SfParams &p, int slots, int wg, size_t smem, int per_sm, cudaStream_t st, cudaError_t *e)
+{
+    const int k0 = p.c, n0 = p.nout[0], n1 = p.nout[1], ns = p.ns;
+    if (slots == 1 && wg == 1) {
+        if (k0 == 16 && n0 == 16 && n1 == 32 && ns == 32) { *e = sf_launch<SfStat<16, 16, 32, 32, LGU>, 1, 1>(p, smem, per_sm, st); return true; }
+        if (k0 == 32 && n0 == 32 && n1 == 64 && ns == 64) { *e = sf_launch<SfStat<32, 32, 64, 64, LGU>, 1, 1>(p, smem, per_sm, st); return true; }
+    }
+    if (slots == 2 && wg == 2) {
+        if (k0 == 64 && n0 == 64 && n1 == 128 && ns == 32) { *e = sf_launch<SfStat<64, 64, 128, 32, LGU>, 2, 2>(p, smem, per_sm, st); return true; }
+        if (k0 == 64 && n0 == 96 && n1 == 128 && ns == 64) { *e = sf_launch<SfStat<64, 96, 128, 64, LGU>, 2, 2>(p, smem, per_sm, st); return true; }
+    }
+    return false;
+}
 static bool sf_launch_static(const SfParams &p, int slots, int wg, size_t smem, int per_sm, cudaStream_t st, cudaError_t *e)
 {
     if (!p.hoist || p.nl != 2) return false;
-    const int k0 = p.c, n0 = p.nout[0], n1 = p.nout[1], ns = p.ns;
-    if (slots == 1 && wg == 1) {
-        if (k0 == 16 && n0 == 16 && n1 == 32 && ns == 32) { *e = sf_launch<SfStat<16, 16, 32, 32>, 1, 1>(p, smem, per_sm, st); return true; }
-        if (k0 == 32 && n0 == 32 && n1 == 64 && ns == 64) { *e = sf_launch<SfStat<32, 32, 64, 64>, 1, 1>(p, smem, per_sm, st); return true; }
-    }
-    if (slots == 2 && wg == 2) {
-        if (k0 == 64 && n0 == 64 && n1 == 128 && ns == 32) { *e = sf_launch<SfStat<64, 64, 128, 32>, 2, 2>(p, smem, per_sm, st); return true; }
-        if (k0 == 64 && n0 == 96 && n1 == 128 && ns == 64) { *e = sf_launch<SfStat<64, 96, 128, 64>, 2, 2>(p, smem, per_sm, st); return true; }
-    }
-    return false;
+    return p.units && p.unit_lg == 2 ? sf_launch_static_lg<2>(p, slots, wg, smem, per_sm, st, e)
+                                     : sf_launch_static_lg<3>(p, slots, wg, smem, per_sm, st, e);
 }
 
 // w_blob: per layer { hi image | lo image }, each image = k-blocks of [npad x (64 | tail)] bf16 in the canonical
@@ -597,7 +626,8 @@ static bool sf_launch_static(const SfParams &p, int slots, int wg, size_t smem, 
 static int sa_mlp_fused_impl(int b, int n, int c, int m, int nsample, const float *xyz, const float *points, int ldz,
                              const float *wx, const float *new_xyz, const int *idx, const int *pts_cnt, const int *units, int nl,
                              const int *nout, const void *w_blob, const float *ss_blob, int last_scale_nonneg,
-                             float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream)
+                             float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream,
+                             int unit_rows)
 {
     const bool hoist = wx != nullptr;
     SSD3D_REQUIRE(b >= 0 && n > 0 && m >= 0 && c >= 0, "sa_mlp_fused: bad shape");
@@ -607,6 +637,8 @@ static int sa_mlp_fused_impl(int b, int n, int c, int m, int nsample, const floa
     SSD3D_REQUIRE(!hoist || (c > 0 && ldz >= c), "sa_mlp_fused_hoisted: bad table shape n1=%d ldz=%d", c, ldz);
     SSD3D_REQUIRE(out_f32 || (out_hi && out_lo), "sa_mlp_fused: no output requested");
     SSD3D_REQUIRE(!units || (out_f32 && !out_hi && !out_lo), "sa_mlp_fused: a unit list combines through atomicMax on the (zero-filled) fp32 output only");
+    SSD3D_REQUIRE(!units || unit_rows == 8 || (unit_rows == 4 && nsample <= 64),
+                  "sa_mlp_fused: unit_rows=%d must be 8, or 4 with nsample <= 64 (nsample=%d)", unit_rows, nsample);
     SSD3D_REQUIRE((reinterpret_cast<uintptr_t>(w_blob) & 15u) == 0, "sa_mlp_fused: weight blob must be 16-byte aligned");
     SSD3D_REQUIRE(!points || (c & 3) || (hoist && (ldz & 3)) || (reinterpret_cast<uintptr_t>(points) & 15u) == 0,
                   "sa_mlp_fused: points must be 16-byte aligned when c is a multiple of 4");
@@ -623,6 +655,7 @@ static int sa_mlp_fused_impl(int b, int n, int c, int m, int nsample, const floa
     SSD3D_REQUIRE(p.rows < (1L << 31) - 128, "sa_mlp_fused: too many grouped rows (%ld)", p.rows);
     p.tiles = (int)((p.rows + 127) / 128);
     p.xyz = xyz; p.points = points; p.new_xyz = new_xyz; p.idx = idx; p.cnt = pts_cnt; p.units = units;
+    p.unit_lg = units && unit_rows == 4 ? 2 : 3;
     p.hoist = hoist ? 1 : 0; p.ldz = ldz; p.wx = wx;
     p.pool_first = last_scale_nonneg ? 1 : 0;
     p.nl = nl;
@@ -685,7 +718,17 @@ extern "C" int ssd3d_sa_mlp_fused(int b, int n, int c, int m, int nsample, const
                                   float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream)
 {
     return sa_mlp_fused_impl(b, n, c, m, nsample, xyz, points, c, nullptr, new_xyz, idx, pts_cnt, units, nl, nout, w_blob, ss_blob,
-                             last_scale_nonneg, out_f32, ld_f32, out_hi, out_lo, ld_split, stream);
+                             last_scale_nonneg, out_f32, ld_f32, out_hi, out_lo, ld_split, stream, 8);
+}
+
+extern "C" int ssd3d_sa_mlp_fused_ex(int b, int n, int c, int m, int nsample, const float *xyz, const float *points,
+                                     const float *new_xyz, const int *idx, const int *pts_cnt, const int *units, int nl,
+                                     const int *nout, const void *w_blob, const float *ss_blob, int last_scale_nonneg,
+                                     float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream,
+                                     int unit_rows)
+{
+    return sa_mlp_fused_impl(b, n, c, m, nsample, xyz, points, c, nullptr, new_xyz, idx, pts_cnt, units, nl, nout, w_blob, ss_blob,
+                             last_scale_nonneg, out_f32, ld_f32, out_hi, out_lo, ld_split, stream, unit_rows);
 }
 
 // The fused SA scale with its first conv hoisted (see ssd3d_linear_tc_hoisted): z[b,n,ldz] per-point table (this scale's
@@ -696,7 +739,17 @@ extern "C" int ssd3d_sa_mlp_fused_hoisted(int b, int n, int n1, int m, int nsamp
                                           int last_scale_nonneg, float *out_f32, int ld_f32, void *out_hi, void *out_lo,
                                           int ld_split, ssd3d_stream_t stream)
 {
+    return ssd3d_sa_mlp_fused_hoisted_ex(b, n, n1, m, nsample, xyz, z, ldz, wx, new_xyz, idx, pts_cnt, units, nl, nout, w_blob,
+                                         ss_blob, last_scale_nonneg, out_f32, ld_f32, out_hi, out_lo, ld_split, stream, 8);
+}
+
+extern "C" int ssd3d_sa_mlp_fused_hoisted_ex(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z, int ldz,
+                                             const float *wx, const float *new_xyz, const int *idx, const int *pts_cnt,
+                                             const int *units, int nl, const int *nout, const void *w_blob, const float *ss_blob,
+                                             int last_scale_nonneg, float *out_f32, int ld_f32, void *out_hi, void *out_lo,
+                                             int ld_split, ssd3d_stream_t stream, int unit_rows)
+{
     SSD3D_REQUIRE(z && wx, "sa_mlp_fused_hoisted: null table pointer");
     return sa_mlp_fused_impl(b, n, n1, m, nsample, xyz, z, ldz, wx, new_xyz, idx, pts_cnt, units, nl, nout, w_blob, ss_blob,
-                             last_scale_nonneg, out_f32, ld_f32, out_hi, out_lo, ld_split, stream);
+                             last_scale_nonneg, out_f32, ld_f32, out_hi, out_lo, ld_split, stream, unit_rows);
 }

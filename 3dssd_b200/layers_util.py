@@ -42,13 +42,16 @@ def _conv_train(pp, scope, x, bn, bn_decay, relu=True, debug=None):
                                   decay=0.9 if bn_decay is None else float(bn_decay))[1][0]
 
 
-def _ball_query(xyz, new_xyz, radius_list, nsample_list, dilated_group, want_units=False):
+def _ball_query(xyz, new_xyz, radius_list, nsample_list, dilated_group, want_units=False, unit_rows=None):
     """The ball queries of all scales (:137-145) -> (idx_list, cnt_list, units_list); units_list holds the unit lists of
-    query_ball_point_multi(return_units=True) when want_units (up to 4 scales), else None per scale."""
+    query_ball_point_multi(return_units=True) when want_units (up to 4 scales), else None per scale; unit_rows: their
+    rows per unit, one per scale (None: 8)."""
     nscale = len(radius_list)
     min_r = [0.0 if (i == 0 or not dilated_group) else radius_list[i - 1] for i in range(nscale)]   # :137-141
     if nscale <= 4:   # one pass over the candidates for all shells
-        res = tf_ops.query_ball_point_multi(min_r, radius_list, nsample_list, xyz, new_xyz, dilated_group, return_units=want_units)
+        with tf_ops.unit_rows(unit_rows if want_units else None):
+            res = tf_ops.query_ball_point_multi(min_r, radius_list, nsample_list, xyz, new_xyz, dilated_group,
+                                                return_units=want_units)
         return res[0], res[1], res[2] if want_units else [None] * nscale
     idx_list, cnt_list = [], []
     for i in range(nscale):
@@ -132,6 +135,7 @@ def _part_bounds(npoint, fps_parts):
 
 
 COMPACT_GROUPS = True      # fused SA scales convolve only the 8-row units that hold distinct neighbours (tf_ops.sa_mlp_fused `units`)
+UNIT_ROWS = 4              # rows per unit of those lists where nsample <= 64 (DESIGN.md 3.4); 8 for wider groups
 HOIST_EXPAND_MIN_K = 256   # hoisted second convs at least this wide materialise their operand (tf_ops.hoist_expand_split)
 
 
@@ -145,8 +149,9 @@ def _route_plan(pp, scope, nsample_list, mlp_list, bn, c_feat, use_agg, mlp_mode
                  `stack`) run the whole scale in one kernel; layer by layer, the first operand is 'gather'ed in the
                  kernel (linear_tc_gather), materialised by group_concat_split ('split'), built from z by the producer
                  warps of linear_tc_hoisted ('hoisted') or materialised from z by hoist_expand_split ('expand', wide
-                 second convs).  zoff: its columns in z.  units: only the 8-row units of its unit list are convolved,
-                 and pooled into the zero-filled concat buffer;
+                 second convs).  zoff: its columns in z.  units: only the units of its unit list are convolved,
+                 and pooled into the zero-filled concat buffer; unit_rows: rows per unit of that list (UNIT_ROWS
+                 for nsample <= 64, else 8);
       compact    some scale uses its unit list;
       split_out  the aggregation conv's split operand is written by the scales' epilogues (else split once afterwards)."""
     tc = mlp_mode == "tc" and all(k in tf_ops.TC_POOL_WIDTHS for k in nsample_list) and all(m[-1] % 8 == 0 for m in mlp_list)
@@ -162,7 +167,8 @@ def _route_plan(pp, scope, nsample_list, mlp_list, bn, c_feat, use_agg, mlp_mode
     n1 = {i: pp.conv(scopes[i][0], bn).cout for i in plan.hoisted}
     ldz = sum(n1.values())
     for i, names in enumerate(scopes):
-        sc = SimpleNamespace(stack=stacks[i], zoff=None, units=COMPACT_GROUPS and len(mlp_list) <= 4)
+        sc = SimpleNamespace(stack=stacks[i], zoff=None, units=COMPACT_GROUPS and len(mlp_list) <= 4,
+                             unit_rows=UNIT_ROWS if nsample_list[i] <= 16 * UNIT_ROWS and nsample_list[i] % UNIT_ROWS == 0 else 8)
         if i in plan.hoisted:
             sc.zoff = sum(n1[h] for h in plan.hoisted[:plan.hoisted.index(i)])
         if sc.stack is not None:
@@ -222,7 +228,8 @@ def _group_and_mlp(pp, plan, table, xyz, points, new_xyz, radius_list, nsample_l
     """Everything of pointnet_sa_module_msg after the sampling, for one block of query points new_xyz (b, m_q, 3), on
     the routes of `plan`: ball queries (:137-145), grouping + MLP + max-pool + mask per scale (:157-180), concat +
     aggregation (:182-185).  table: _hoist_table's.  Returns (new_points, idx_list, cnt_list)."""
-    idx_list, cnt_list, units_list = _ball_query(xyz, new_xyz, radius_list, nsample_list, dilated_group, plan.compact)
+    idx_list, cnt_list, units_list = _ball_query(xyz, new_xyz, radius_list, nsample_list, dilated_group, plan.compact,
+                                                 [sc.unit_rows for sc in plan.scales] if plan.compact else None)
     if not plan.tc:
         outs = []
         for i, scopes in enumerate(plan.scopes):
@@ -239,7 +246,7 @@ def _group_and_mlp(pp, plan, table, xyz, points, new_xyz, radius_list, nsample_l
     bs, m_q = new_xyz.shape[:2]
     ctot = sum(m[-1] for m in mlp_list)
     concat = torch.empty((bs, m_q, ctot), dtype=torch.float32, device=xyz.device)
-    if plan.compact:                 # unit lists combine their 8-row units with atomicMax on the ZERO-FILLED buffer
+    if plan.compact:                 # unit lists combine their units with atomicMax on the ZERO-FILLED buffer
         tf_ops.fill_zero(concat)
     split = None
     if plan.split_out:
@@ -250,7 +257,7 @@ def _group_and_mlp(pp, plan, table, xyz, points, new_xyz, radius_list, nsample_l
     for i, sc in enumerate(plan.scales):
         idx, cnt = idx_list[i], cnt_list[i]
         units = units_list[i] if sc.units else None
-        if units is not None:        # the last conv pools every 8-row unit into its group's row
+        if units is not None:        # the last conv pools every unit into its group's row
             out = dict(out_f32=(concat, off), units=units, unit_pool=True)
         else:                        # :167-180 conv + BN + ReLU + max + mask
             out = dict(out_f32=(concat, off), out_split=None if split is None else split + (off,), pool=nsample_list[i], rowmask=cnt)

@@ -10,8 +10,10 @@ with the TF custom-op layer replaced by ctypes calls into libssd3d.so (include/s
 checks mirror the reference's OP_REQUIRES (InvalidArgument -> ValueError); outputs are allocated here, like
 TF's allocate_output, and the kernels run on torch's current stream (CUDA-graph capturable).
 """
+import contextlib
 import ctypes
 import math
+import threading
 
 import numpy as np
 import torch
@@ -286,18 +288,54 @@ def query_ball_point_dilated(min_radius, max_radius, nsample, xyz1, xyz2):
 
 BQ_GRID_MIN_N = 2048     # candidate sets at least this large take the spatially culled kernel (csrc/ball_query_grid.cu)
 
+# Rows per unit of the unit lists query_ball_point_multi(return_units=True) builds inside a unit_rows() block
+_UNIT_WIDTHS = threading.local()
 
-def query_ball_point_multi(min_radius_list, max_radius_list, nsample_list, xyz1, xyz2, dilated, grid=None, return_units=False):
+
+@contextlib.contextmanager
+def unit_rows(widths):
+    """Unit widths for the ball queries of this block: shell s of a query_ball_point_multi(return_units=True) call made
+    inside it lists units of widths[s] rows (8 or 4), unless the call passes unit_rows itself.  The lists carry their
+    width (`list.unit_rows`), which the unit-list kernels read, so only the query needs it."""
+    prev = getattr(_UNIT_WIDTHS, "w", None)
+    _UNIT_WIDTHS.w = None if widths is None else [int(w) for w in widths]
+    try:
+        yield
+    finally:
+        _UNIT_WIDTHS.w = prev
+
+
+def _unit_width(w, ns=None):
+    """A unit width: 8 or 4 rows, and 4 only for groups of at most 64 rows (a list names 16 units per group); ns: the
+    group size to check a 4-row width against."""
+    w = int(w)
+    if w not in (8, 4):
+        raise ValueError("unit_rows must be 8 or 4, got %d" % w)
+    if w == 4 and ns is not None and (ns > 16 * w or ns % w):
+        raise ValueError("%d-row units need nsample a multiple of %d and <= %d, got %d" % (w, w, 16 * w, ns))
+    return w
+
+
+def query_ball_point_multi(min_radius_list, max_radius_list, nsample_list, xyz1, xyz2, dilated, grid=None, return_units=False,
+                           unit_rows=None):
     """All radius shells of one SA layer in a single pass over the candidates (fast path; same results
     as calling query_ball_point[_dilated] once per shell).  Returns lists (idx_list, pts_cnt_list).
     grid: None = automatic (the culled kernel for ndataset >= BQ_GRID_MIN_N), True / False = force / forbid it;
     the outputs are identical either way.
     return_units: also return, per shell, the UNIT LIST of the grouped MLP (int32 tensor, include/ssd3d.h
-    ssd3d_query_ball_point_multi_ws), or None for nsample > 128: (idx_list, pts_cnt_list, units_list)."""
+    ssd3d_query_ball_point_multi_ws_ex), or None for nsample > 128: (idx_list, pts_cnt_list, units_list).
+    unit_rows: rows per unit of each shell's list, 8 or 4 (4 needs nsample <= 64); None = the enclosing unit_rows()
+    block's widths, else 8.  Each list records its width in its `unit_rows` attribute."""
     xyz1, xyz2 = _bq_shapes(xyz1, xyz2)
     nq = len(max_radius_list)
     if not (len(nsample_list) == nq and len(min_radius_list) == nq and 1 <= nq <= 4):
         raise ValueError("query_ball_point_multi takes 1..4 shells with matching list lengths")
+    if unit_rows is None:
+        unit_rows = getattr(_UNIT_WIDTHS, "w", None) or [8] * nq
+    if len(unit_rows) != nq:
+        raise ValueError("unit_rows needs one width per shell")
+    want_units = return_units and all(int(k) <= 128 for k in nsample_list)
+    widths = [_unit_width(w, int(k)) for w, k in zip(unit_rows, nsample_list)] if want_units else [8] * nq
     for r, k in zip(max_radius_list, nsample_list):
         if not r > 0:
             raise ValueError("QueryBallPoint expects positive radius")
@@ -319,15 +357,21 @@ def query_ball_point_multi(min_radius_list, max_radius_list, nsample_list, xyz1,
     ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=xyz1.device) if use_grid else None
     units = [None] * nq
     pu = ctypes.c_void_p(0)
-    if return_units and all(int(k) <= 128 for k in nsample_list):
-        units = [torch.empty((1 + b * m * ((int(k) + 7) // 8),), dtype=torch.int32, device=xyz1.device) for k in nsample_list]
+    if want_units:
+        units = [torch.empty((1 + b * m * ((int(k) + w - 1) // w),), dtype=torch.int32, device=xyz1.device)
+                 for k, w in zip(nsample_list, widths)]
+        for t, w in zip(units, widths):
+            t.unit_rows = w
         parr = (ctypes.c_void_p * nq)(*[t.data_ptr() for t in units])
         pu = ctypes.cast(parr, ctypes.c_void_p)
-    check(lib().ssd3d_query_ball_point_multi_ws(b, n, m, nq, 1 if dilated else 0, ctypes.cast(lo, ctypes.c_void_p),
-                                                ctypes.cast(hi, ctypes.c_void_p), ctypes.cast(ks, ctypes.c_void_p),
-                                                _p(xyz1), _p(xyz2), ctypes.cast(pi, ctypes.c_void_p),
-                                                ctypes.cast(pc, ctypes.c_void_p), pu, _p(ws), ws_bytes if use_grid else 0,
-                                                _stream()), "query_ball_point_multi")
+    args = [b, n, m, nq, 1 if dilated else 0, ctypes.cast(lo, ctypes.c_void_p), ctypes.cast(hi, ctypes.c_void_p),
+            ctypes.cast(ks, ctypes.c_void_p), _p(xyz1), _p(xyz2), ctypes.cast(pi, ctypes.c_void_p),
+            ctypes.cast(pc, ctypes.c_void_p), pu, _p(ws), ws_bytes if use_grid else 0, _stream()]
+    if all(w == 8 for w in widths):
+        check(lib().ssd3d_query_ball_point_multi_ws(*args), "query_ball_point_multi")
+    else:
+        wa = (ctypes.c_int * nq)(*widths)
+        check(lib().ssd3d_query_ball_point_multi_ws_ex(*args, ctypes.cast(wa, ctypes.c_void_p)), "query_ball_point_multi")
     if return_units:
         return idx, cnt, units
     return idx, cnt
@@ -545,18 +589,22 @@ def _outputs(lead, n, dev, want_f32, want_split, out_f32, out_split, pooled):
     return y, sp, [pf, ldf, ph, pl, lds]
 
 
-def _units_check(units, unit_pool, pool=1, rowmask=None, relu=True, out_f32=None, out_split=None, want_split=False):
-    """A unit list (query_ball_point_multi(return_units=True)) replaces pool / rowmask; with unit_pool the listed 8-row
-    units are max-pooled into the caller's zero-filled out_f32 by atomicMax, so there is no split output."""
+def _units_check(units, unit_pool, pool=1, rowmask=None, relu=True, out_f32=None, out_split=None, want_split=False,
+                 unit_rows=None, ns=None):
+    """A unit list (query_ball_point_multi(return_units=True)) replaces pool / rowmask; with unit_pool the listed units
+    are max-pooled into the caller's zero-filled out_f32 by atomicMax, so there is no split output.  Returns the rows
+    per unit: unit_rows, else the width the list records (8 for a list without one); ns: rows per group, when known."""
     if units is None:
         if unit_pool:
             raise ValueError("unit_pool needs a unit list")
-        return
+        return 8
+    w = _unit_width(getattr(units, "unit_rows", 8) if unit_rows is None else unit_rows, ns)
     _req(units, "units", torch.int32, copy=False)
     if int(pool) != 1 or rowmask is not None:
-        raise ValueError("a unit list replaces pool / rowmask (unit_pool=True pools the listed 8-row units)")
+        raise ValueError("a unit list replaces pool / rowmask (unit_pool=True pools the listed units)")
     if unit_pool and (not relu or out_f32 is None or out_split is not None or want_split):
         raise ValueError("a pooled unit list needs relu, out_f32=(zero-filled buffer, col_offset) and no split output")
+    return w
 
 
 def _pool(pool, group):
@@ -643,26 +691,28 @@ def group_concat_split(xyz, points, new_xyz, idx, kp=None):
     return hi, lo
 
 
-def _tc_epilogue(f, relu, pool, rowmask, lead, ns, dev, want_f32, want_split, out_f32, out_split, units, unit_pool):
+def _tc_epilogue(f, relu, pool, rowmask, lead, ns, dev, want_f32, want_split, out_f32, out_split, units, unit_pool,
+                 unit_rows=None):
     """Checks and output placement shared by the linear_tc* wrappers, for an operand of leading shape `lead` in groups
-    of ns rows -> (y, (hi, lo) or None, pool, rowmask, the layer's arguments, the output arguments)."""
-    _units_check(units, unit_pool, pool, rowmask, relu, out_f32, out_split, want_split)
+    of ns rows -> (y, (hi, lo) or None, pool, rowmask, the layer's arguments, the output arguments, rows per unit)."""
+    w = _units_check(units, unit_pool, pool, rowmask, relu, out_f32, out_split, want_split, unit_rows)
     pool = _pool(pool, ns)
     pooled = pool > 1 or unit_pool
     olead = lead[:-1] if pooled else lead
     rowmask = _rowmask(rowmask, math.prod(olead))
     y, sp, out = _outputs(olead, f.cout, dev, want_f32, want_split, out_f32, out_split, pooled)
-    return y, sp, pool, rowmask, [_p(f.b_hi), _p(f.b_lo), _p(f.scale), _p(f.shift), 1 if relu else 0], out
+    return y, sp, pool, rowmask, [_p(f.b_hi), _p(f.b_lo), _p(f.scale), _p(f.shift), 1 if relu else 0], out, w
 
 
 def linear_tc(a_hi, a_lo, f, relu=True, pool=1, rowmask=None, want_f32=True, want_split=False, out_f32=None,
-              out_split=None, units=None, unit_pool=False):
+              out_split=None, units=None, unit_pool=False, unit_rows=None):
     """One folded conv layer on the tensor cores.  a_hi/a_lo (..., kp) bf16; f: params.FoldedConv.
     Returns (y_f32 or None, (hi, lo) or None).  out_f32=(buffer, col_offset) / out_split=(hi_buf, lo_buf, col_offset)
     write into slices of preallocated (..., ld) buffers (the concat of the SA scales) instead of allocating.
     units: the operand holds COMPACT rows (8 per listed unit, include/ssd3d.h ssd3d_linear_tc_units) in its first
     units[0] * 8 rows; outputs are compact likewise, or -- unit_pool=True, the last conv of a scale -- every unit is
-    max-pooled and combined into out_f32[group] by atomicMax (buffer zero-filled by the caller)."""
+    max-pooled and combined into out_f32[group] by atomicMax (buffer zero-filled by the caller).  unit_rows: rows per
+    unit, 8 or 4 (ssd3d_linear_tc_units_ex); None = the width the list records."""
     a_hi, a_lo = _req(a_hi, "a_hi", torch.bfloat16), _req(a_lo, "a_lo", torch.bfloat16)
     if a_hi.shape != a_lo.shape:
         raise ValueError("a_hi / a_lo must be bfloat16 tensors of the same shape")
@@ -670,10 +720,12 @@ def linear_tc(a_hi, a_lo, f, relu=True, pool=1, rowmask=None, want_f32=True, wan
     if kp != f.kp:
         raise ValueError("operand K (%d) does not match the layer's padded K (%d)" % (kp, f.kp))
     lead = tuple(a_hi.shape[:-1])
-    y, sp, pool, rowmask, head, out = _tc_epilogue(f, relu, pool, rowmask, lead, lead[-1] if lead else 1, a_hi.device,
-                                                   want_f32, want_split, out_f32, out_split, units, unit_pool)
+    y, sp, pool, rowmask, head, out, w = _tc_epilogue(f, relu, pool, rowmask, lead, lead[-1] if lead else 1, a_hi.device,
+                                                      want_f32, want_split, out_f32, out_split, units, unit_pool, unit_rows)
     args = [a_hi.numel() // kp, kp, f.cout, _p(a_hi), _p(a_lo)] + head
-    if units is not None:
+    if units is not None and w != 8:
+        check(lib().ssd3d_linear_tc_units_ex(*args, _p(units), 1 if unit_pool else 0, *out, _stream(), w), "linear_tc_units")
+    elif units is not None:
         check(lib().ssd3d_linear_tc_units(*args, _p(units), 1 if unit_pool else 0, *out, _stream()), "linear_tc_units")
     else:
         check(lib().ssd3d_linear_tc(*args, pool, _p(rowmask), *out, _stream()), "linear_tc")
@@ -688,15 +740,15 @@ def linear_tc_gather(xyz, points, new_xyz, idx, f, relu=True, pool=1, rowmask=No
     xyz, points, new_xyz, idx, b, n, c, m, ns = _grouping(xyz, points, new_xyz, idx)
     if round16(c + 3) != f.kp or c + 3 != f.cin:
         raise ValueError("layer input width %d does not match c+3 = %d" % (f.cin, c + 3))
-    y, sp, pool, rowmask, head, out = _tc_epilogue(f, relu, pool, rowmask, (b, m, ns), ns, xyz.device, want_f32,
-                                                   want_split, out_f32, out_split, None, False)
+    y, sp, pool, rowmask, head, out, _ = _tc_epilogue(f, relu, pool, rowmask, (b, m, ns), ns, xyz.device, want_f32,
+                                                      want_split, out_f32, out_split, None, False)
     check(lib().ssd3d_linear_tc_gather(b, n, c, m, ns, _p(xyz), _p(points), _p(new_xyz), _p(idx), f.cout, *head, pool,
                                        _p(rowmask), *out, _stream()), "linear_tc_gather")
     return y, sp
 
 
 def linear_tc_hoisted(xyz, z, zoff, wx, new_xyz, idx, f, relu=True, pool=1, rowmask=None, want_f32=False, want_split=True,
-                      out_f32=None, out_split=None, units=None, unit_pool=False):
+                      out_f32=None, out_split=None, units=None, unit_pool=False, unit_rows=None):
     """Second conv of an SA scale fed by the hoisted first conv (include/ssd3d.h, ssd3d_linear_tc_hoisted).
     z: (b, n, ldz) fp32 per-point table = (features . Wf) * s1 + t1 for all scales of the layer, this scale's
     columns start at zoff; wx: (3, n1) fp32 = Wx * s1; f: params.FoldedConv of the second conv (cin == n1).
@@ -705,10 +757,14 @@ def linear_tc_hoisted(xyz, z, zoff, wx, new_xyz, idx, f, relu=True, pool=1, rowm
     zp, ldz, wx, n1 = _hoisted_table(z, zoff, wx, b, n)
     if f.cin != n1:
         raise ValueError("second conv expects %d inputs, the hoisted first conv has %d outputs" % (f.cin, n1))
-    y, sp, pool, rowmask, head, out = _tc_epilogue(f, relu, pool, rowmask, (b, m, ns), ns, xyz.device, want_f32,
-                                                   want_split, out_f32, out_split, units, unit_pool)
+    y, sp, pool, rowmask, head, out, w = _tc_epilogue(f, relu, pool, rowmask, (b, m, ns), ns, xyz.device, want_f32,
+                                                      want_split, out_f32, out_split, units, unit_pool, unit_rows)
     args = [b, n, n1, m, ns, _p(xyz), zp, ldz, _p(wx), _p(new_xyz), _p(idx)]
-    if units is not None:
+    if units is not None and w != 8:
+        _unit_width(w, ns)
+        check(lib().ssd3d_linear_tc_hoisted_units_ex(*args, _p(units), f.cout, *head, 1 if unit_pool else 0, *out, _stream(), w),
+              "linear_tc_hoisted_units")
+    elif units is not None:
         check(lib().ssd3d_linear_tc_hoisted_units(*args, _p(units), f.cout, *head, 1 if unit_pool else 0, *out, _stream()),
               "linear_tc_hoisted_units")
     else:
@@ -716,32 +772,35 @@ def linear_tc_hoisted(xyz, z, zoff, wx, new_xyz, idx, f, relu=True, pool=1, rowm
     return y, sp
 
 
-def hoist_expand_split(xyz, z, zoff, wx, new_xyz, idx, units=None):
+def hoist_expand_split(xyz, z, zoff, wx, new_xyz, idx, units=None, unit_rows=None):
     """The operand linear_tc_hoisted would build in its producer warps, materialised: (hi, lo) bf16 (b, m, nsample, kp) =
     split(relu(z[idx] + (xyz[idx] - new_xyz) . wx)).  Followed by the plain linear_tc this is the faster route for wide
     layers (K >= 256), where the resident operand of the in-kernel route leaves the weight ring two narrow stages.
-    units: only the listed 8-row units are built, as compact rows at the start of the buffers."""
+    units: only the listed units are built, as compact rows at the start of the buffers (unit_rows: as linear_tc)."""
     xyz, _, new_xyz, idx, b, n, _, m, ns = _grouping(xyz, None, new_xyz, idx)
     zp, ldz, wx, n1 = _hoisted_table(z, zoff, wx, b, n)
     if zoff % 4 or ldz % 4:                         # the kernel reads the table in 16-byte vectors
         raise ValueError("z must be (b, n, ldz) with ldz, zoff multiples of 4, zoff + n1 <= ldz, and wx (3, n1)")
-    _units_check(units, False)
+    w = _units_check(units, False, unit_rows=unit_rows, ns=ns)
     kp = round16(n1)
     hi = torch.empty((b, m, ns, kp), dtype=torch.bfloat16, device=xyz.device)
     lo = torch.empty_like(hi)
     args = [b, n, n1, m, ns, _p(xyz), zp, ldz, _p(wx), _p(new_xyz), _p(idx)]
-    if units is not None:
+    if units is not None and w != 8:
+        check(lib().ssd3d_hoist_expand_split_units_ex(*args, _p(units), _p(hi), _p(lo), kp, _stream(), w), "hoist_expand_split_units")
+    elif units is not None:
         check(lib().ssd3d_hoist_expand_split_units(*args, _p(units), _p(hi), _p(lo), kp, _stream()), "hoist_expand_split_units")
     else:
         check(lib().ssd3d_hoist_expand_split(*args, _p(hi), _p(lo), kp, _stream()), "hoist_expand_split")
     return hi, lo
 
 
-def _sa_fused(xyz, points, table, new_xyz, idx, cnt, stack, out_f32, out_split, units):
+def _sa_fused(xyz, points, table, new_xyz, idx, cnt, stack, out_f32, out_split, units, unit_rows):
     """The body of sa_mlp_fused (points, table None) and sa_mlp_fused_hoisted (table = (z, zoff, wx)) up to the entry
-    point -> (y, the entry point's arguments without the stream)."""
-    _units_check(units, units is not None, out_f32=out_f32, out_split=out_split)
+    point -> (y, the entry point's arguments without the stream, rows per unit)."""
+    w = _units_check(units, units is not None, out_f32=out_f32, out_split=out_split, unit_rows=unit_rows)
     xyz, points, new_xyz, idx, b, n, c, m, ns = _grouping(xyz, points, new_xyz, idx, cnt)
+    _unit_width(w, ns)
     if table is None:
         if c + 3 != stack.cin:
             raise ValueError("feature channels (%d) do not match the stack's input width (%d)" % (c, stack.cin - 3))
@@ -754,26 +813,32 @@ def _sa_fused(xyz, points, table, new_xyz, idx, cnt, stack, out_f32, out_split, 
     y, _, out = _outputs((b, m), stack.nout[-1], xyz.device, out_split is None, False, out_f32, out_split, True)
     nout = (ctypes.c_int * len(stack.nout))(*stack.nout)
     return y, [b, n] + src + [_p(new_xyz), _p(idx), _p(cnt), _p(units), len(stack.nout), ctypes.cast(nout, ctypes.c_void_p),
-                              _p(stack.w_blob), _p(stack.ss_blob), 1 if stack.last_scale_nonneg else 0] + out
+                              _p(stack.w_blob), _p(stack.ss_blob), 1 if stack.last_scale_nonneg else 0] + out, w
 
 
-def sa_mlp_fused(xyz, points, new_xyz, idx, cnt, stack, out_f32=None, out_split=None, units=None):
+def sa_mlp_fused(xyz, points, new_xyz, idx, cnt, stack, out_f32=None, out_split=None, units=None, unit_rows=None):
     """One SA scale in one kernel: gather + concat + conv stack + max-pool + mask (layers_util.py:157-180).
     stack: params.FusedStack.  out_f32=(buffer, col_offset) / out_split=(hi, lo, col_offset) as linear_tc;
     without them a fresh (b, m, C3) fp32 tensor is returned.
     units: the scale's unit list (query_ball_point_multi(return_units=True)): only the listed 8-row units are convolved
     -- the skipped rows repeat a group's first neighbour and cannot change the max-pool -- and results are combined with
-    atomicMax into out_f32, which must be zero-filled (fill_zero)."""
-    y, args = _sa_fused(xyz, points, None, new_xyz, idx, cnt, stack, out_f32, out_split, units)
-    check(lib().ssd3d_sa_mlp_fused(*args, _stream()), "sa_mlp_fused")
+    atomicMax into out_f32, which must be zero-filled (fill_zero).  unit_rows: as linear_tc."""
+    y, args, w = _sa_fused(xyz, points, None, new_xyz, idx, cnt, stack, out_f32, out_split, units, unit_rows)
+    if w != 8:
+        check(lib().ssd3d_sa_mlp_fused_ex(*args, _stream(), w), "sa_mlp_fused")
+    else:
+        check(lib().ssd3d_sa_mlp_fused(*args, _stream()), "sa_mlp_fused")
     return y
 
 
-def sa_mlp_fused_hoisted(xyz, z, zoff, wx, new_xyz, idx, cnt, stack, out_f32=None, out_split=None, units=None):
+def sa_mlp_fused_hoisted(xyz, z, zoff, wx, new_xyz, idx, cnt, stack, out_f32=None, out_split=None, units=None, unit_rows=None):
     """sa_mlp_fused with the scale's first conv hoisted into the per-point table z (see linear_tc_hoisted): `stack` is the
-    params.FusedStack of the REMAINING convs (its input width == wx.shape[1]).  units: as sa_mlp_fused."""
-    y, args = _sa_fused(xyz, None, (z, zoff, wx), new_xyz, idx, cnt, stack, out_f32, out_split, units)
-    check(lib().ssd3d_sa_mlp_fused_hoisted(*args, _stream()), "sa_mlp_fused_hoisted")
+    params.FusedStack of the REMAINING convs (its input width == wx.shape[1]).  units, unit_rows: as sa_mlp_fused."""
+    y, args, w = _sa_fused(xyz, None, (z, zoff, wx), new_xyz, idx, cnt, stack, out_f32, out_split, units, unit_rows)
+    if w != 8:
+        check(lib().ssd3d_sa_mlp_fused_hoisted_ex(*args, _stream(), w), "sa_mlp_fused_hoisted")
+    else:
+        check(lib().ssd3d_sa_mlp_fused_hoisted(*args, _stream()), "sa_mlp_fused_hoisted")
     return y
 
 

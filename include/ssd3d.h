@@ -148,6 +148,14 @@ int ssd3d_query_ball_point_multi_ws(int b, int n, int m, int nqueries, int dilat
                                     const float *max_radius, const int *nsample, const float *xyz1, const float *xyz2,
                                     int *const *idx, int *const *pts_cnt, int *const *units, void *workspace,
                                     size_t workspace_bytes, ssd3d_stream_t stream);
+/* The same with a unit width per shell: unit_rows (host array of nqueries ints, NULL = all 8) gives shell s units of
+ * W = unit_rows[s] rows, 8 or 4: [1 + u] = (group << 4) | j then names rows Wj..Wj+W-1, a group with cnt hits gets
+ * ceil(cnt/W) units and units[s] holds 1 + b*m*ceil(nsample[s]/W) ints.  j has 4 bits, so W = 4 needs nsample <= 64
+ * (W = 8: nsample <= 128).  The consumers of a list take the same width (the *_ex / *_units_ex calls below). */
+int ssd3d_query_ball_point_multi_ws_ex(int b, int n, int m, int nqueries, int dilated, const float *min_radius,
+                                       const float *max_radius, const int *nsample, const float *xyz1, const float *xyz2,
+                                       int *const *idx, int *const *pts_cnt, int *const *units, void *workspace,
+                                       size_t workspace_bytes, ssd3d_stream_t stream, const int *unit_rows);
 
 /* replaces groupPointLauncher(b,n,c,m,nsample,points,idx,out)
  *   grouping/tf_grouping.cpp:446, grouping/tf_grouping_g.cu:476-479, kernel :362-379.
@@ -251,12 +259,33 @@ int ssd3d_linear_tc_hoisted_units(int b, int n, int n1, int m, int nsample, cons
                                   const void *b_hi, const void *b_lo, const float *scale, const float *shift, int relu,
                                   int unit_pool, float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split,
                                   ssd3d_stream_t stream);
+/* The three unit-list calls for lists of unit_rows-row units (8 or 4, as the list was built with
+ * ssd3d_query_ball_point_multi_ws_ex; nsample a multiple of it and <= 16 * unit_rows): the matrix has units[0] * unit_rows
+ * rows, compact row Wu + e is neighbour slot Wj + e, and unit_pool pools every W-row unit.  Otherwise as above. */
+int ssd3d_hoist_expand_split_units_ex(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z, int ldz,
+                                      const float *wx, const float *new_xyz, const int *idx, const int *units, void *hi,
+                                      void *lo, int kp, ssd3d_stream_t stream, int unit_rows);
+int ssd3d_linear_tc_units_ex(long rows, int kp, int n, const void *a_hi, const void *a_lo, const void *b_hi,
+                             const void *b_lo, const float *scale, const float *shift, int relu, const int *units,
+                             int unit_pool, float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split,
+                             ssd3d_stream_t stream, int unit_rows);
+int ssd3d_linear_tc_hoisted_units_ex(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z, int ldz,
+                                     const float *wx, const float *new_xyz, const int *idx, const int *units, int nout,
+                                     const void *b_hi, const void *b_lo, const float *scale, const float *shift, int relu,
+                                     int unit_pool, float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split,
+                                     ssd3d_stream_t stream, int unit_rows);
 /* Same idea for a scale that fits the fused kernel (ssd3d_sa_mlp_fused): the stack passed here starts at the scale's
  * SECOND conv, the first operand row is relu(z[idx] + (xyz[idx] - new_xyz) . wx), built during the gather. */
 int ssd3d_sa_mlp_fused_hoisted(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z, int ldz,
                                const float *wx, const float *new_xyz, const int *idx, const int *pts_cnt, const int *units,
                                int nl, const int *nout, const void *w_blob, const float *ss_blob, int last_scale_nonneg,
                                float *out_f32, int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream);
+/* ... for a list of unit_rows-row units (8, or 4 with nsample <= 64; ignored without a list) */
+int ssd3d_sa_mlp_fused_hoisted_ex(int b, int n, int n1, int m, int nsample, const float *xyz, const float *z, int ldz,
+                                  const float *wx, const float *new_xyz, const int *idx, const int *pts_cnt,
+                                  const int *units, int nl, const int *nout, const void *w_blob, const float *ss_blob,
+                                  int last_scale_nonneg, float *out_f32, int ld_f32, void *out_hi, void *out_lo,
+                                  int ld_split, ssd3d_stream_t stream, int unit_rows);
 /* hi/lo[row, 0:kp] = split(x[row, 0:c]), zero padded (kp % 8 == 0). */
 int ssd3d_split_rows(long rows, int c, const float *x, int ldx, void *hi, void *lo, int kp, ssd3d_stream_t stream);
 /* ssd3d_group_concat fused with the split: hi/lo [b*m*nsample, kp] bf16. */
@@ -275,12 +304,17 @@ int ssd3d_group_concat_split(int b, int n, int c, int m, int nsample, const floa
  * listed 8-row units instead of all nsample rows of every group -- the rows it skips repeat a group's first neighbour and
  * cannot change the max-pool -- and combines the units of a group with atomicMax on out_f32, which the caller must have
  * ZERO-FILLED (zero is also the masked result of a group without neighbours); out_hi / out_lo must be NULL.  Identical
- * results; the work shrinks from b*m*nsample rows to 8 * sum(ceil(cnt / 8)). */
+ * results; the work shrinks from b*m*nsample rows to 8 * sum(ceil(cnt / 8)), or with a list of 4-row units
+ * (ssd3d_sa_mlp_fused_ex, unit_rows = 4, nsample <= 64) to 4 * sum(ceil(cnt / 4)). */
 size_t ssd3d_sa_fused_smem(int c, int nl, const int *nout);
 int ssd3d_sa_mlp_fused(int b, int n, int c, int m, int nsample, const float *xyz, const float *points,
                        const float *new_xyz, const int *idx, const int *pts_cnt, const int *units, int nl,
                        const int *nout, const void *w_blob, const float *ss_blob, int last_scale_nonneg, float *out_f32,
                        int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream);
+int ssd3d_sa_mlp_fused_ex(int b, int n, int c, int m, int nsample, const float *xyz, const float *points,
+                          const float *new_xyz, const int *idx, const int *pts_cnt, const int *units, int nl,
+                          const int *nout, const void *w_blob, const float *ss_blob, int last_scale_nonneg, float *out_f32,
+                          int ld_f32, void *out_hi, void *out_lo, int ld_split, ssd3d_stream_t stream, int unit_rows);
 
 /* ---- backward operators (training graphs) ---------------------------------------------------
  * Each zero-fills its output first, as the reference's TF ops do with cudaMemset before the launcher. */
