@@ -381,6 +381,25 @@ def test_new_entry_points_check_shapes_before_any_launch(fake_cuda):
     assert not failures, "\n".join(failures)
 
 
+POOL_SMEM_MAX = 227 * 1024           # the opt-in shared memory of one H100 CTA
+POOL_MAX_N = 17706                   # the largest scene the pool takes at nsample 512 and c_info 128
+
+
+def test_region_pool_shared_memory_limit():
+    """The pool stages the scene's xyz in shared memory: at nsample 512 and c_info 128 it takes scenes of up to
+    POOL_MAX_N points (tests/test_pointrcnn_rcnn_gpu.py runs that one), and one point more is rejected by the C ABI
+    before any CUDA call, so also on a machine without a GPU."""
+    pkg = importlib.import_module("3dssd_b200")
+    L = pkg.lib()
+    assert L.ssd3d_region_pool_smem(POOL_MAX_N, 512, 128) <= POOL_SMEM_MAX < L.ssd3d_region_pool_smem(POOL_MAX_N + 1, 512, 128)
+    assert L.ssd3d_region_pool_smem(POOL_MAX_N, 512, 128) == (POOL_MAX_N * 3 + 7 * 128 + 8 * 512) * 4
+    null = ctypes.c_void_p(None)
+    pool = lambda n, p: L.ssd3d_region_pool(1, n, p, 512, 128, 128, *[null] * 4, 9, null, 1.0, 0.5, *[null] * 8)
+    assert pool(POOL_MAX_N, 0) == 0                                         # accepted: no proposal, nothing to launch
+    assert pool(POOL_MAX_N + 1, 0) == -1 and "shared memory" in L.ssd3d_last_error().decode()
+    assert pool(POOL_MAX_N + 1, 100) == -1 and "shared memory" in L.ssd3d_last_error().decode()
+
+
 def test_stage2_sa_route_plan():
     """rcnn_layer1 / rcnn_layer2 at inference, from parameter shapes alone: the tensor-core route (K = 64 is a pooling
     width of its epilogue) with the first conv hoisted (c = 256 + 3 at layer 1, 128 + 3 at layer 2) and unit lists; the

@@ -104,23 +104,109 @@ def scenes():
     return {"synthetic": np.ascontiguousarray(syn, np.float32), "realscan": np.ascontiguousarray(real, np.float32)}
 
 
-@pytest.mark.parametrize("name", ["synthetic", "realscan"])
-def test_query_boxes_vs_reference_kernel(pkg, cuda, ref_query, name):
+CLUSTER_BOX = np.array([0, 0, 0, 2.0, 1.5, 2.0, 0.3], np.float32)   # placed on a cluster: its points >= 0.55 m off a face
+
+
+def edge_scene(n, rng, clusters):
+    """A scene of n points spread over x in [-30, 30], z in [0, 60], with point clusters far outside that region:
+    clusters is a list of index arrays, cluster j's points lie within 0.3 m of (50 + 10 j, -0.6, 80) horizontally and
+    0.4 m vertically.  Returns the xyz [n, 3] and one bottom-centred box per cluster (CLUSTER_BOX at the cluster's
+    foot) that holds exactly that cluster's points, also after the pool's expansion by 1 m."""
+    xyz = np.stack([rng.uniform(-30, 30, n), rng.uniform(-2.5, 1.0, n), rng.uniform(0, 60, n)], -1).astype(np.float32)
+    boxes = []
+    for j, members in enumerate(clusters):
+        c = np.array([50 + 10 * j, -0.6, 80], np.float32)
+        k = len(members)
+        xyz[members] = c + np.stack([rng.uniform(-0.3, 0.3, k), rng.uniform(-0.4, 0.4, k), rng.uniform(-0.3, 0.3, k)], -1)
+        boxes.append(CLUSTER_BOX + np.array([c[0], 0, c[2], 0, 0, 0, 0], np.float32))
+    return xyz, boxes
+
+
+def random_boxes(xyz, m, rng):
+    """m boxes on random scene points (with replacement), one holding every point, one far from all of them."""
+    pick = xyz[rng.integers(0, len(xyz), m)]
+    bx = np.zeros((m, 7), np.float32)
+    bx[:, 0], bx[:, 2] = pick[:, 0], pick[:, 2]
+    bx[:, 1] = pick[:, 1] + rng.uniform(0.2, 1.5, m)
+    bx[:, 3:6] = rng.uniform(1.0, 6.0, (m, 3))
+    bx[:, 6] = rng.uniform(-np.pi, np.pi, m)
+    bx[0] = [10, 2, 40, 200, 10, 200, 0.1]
+    bx[1] = [500, 0, 500, 2, 2, 2, 0]
+    return bx
+
+
+# kernel edges: name -> (n, nsample).  "n*": scenes whose last warp is partial (n = 1 and 33 are nearly nothing else),
+# with a cluster in that warp; "ns*": nsample around a warp and at its limit, with clusters of nsample - 1, nsample and
+# nsample + 1 points scattered through the scene's index order.
+EDGES = {"n1": (1, 512), "n33": (33, 512), "n1000": (1000, 512), "n16383": (16383, 512), "ns1": (8192, 1),
+         "ns31": (8192, 31), "ns32": (8192, 32), "ns33": (8192, 33), "ns1024": (8192, 1024)}
+
+
+def edge_case(name, m=24):
+    """(xyz [2, n, 3], boxes [2, m, 7], nsample, designed) for an EDGES shape: two scenes (another batch offset each),
+    the cluster boxes first, then random_boxes.  designed: (scene, row, the cluster's indices) of every cluster box."""
+    n, ns = EDGES[name]
+    rng = np.random.default_rng(sum(map(ord, name)))
+    xyz, boxes, designed = [], [], []
+    for s in range(2):
+        if name.startswith("n") and not name.startswith("ns"):
+            tail = np.arange(32 * ((n - 1) // 32), n)                 # the last warp, partial for every n here
+            clusters = [tail]
+        else:
+            perm = rng.permutation(n)
+            sizes = [max(ns - 1, 0), ns, ns + 1]
+            cuts = np.cumsum([0] + sizes)
+            clusters = [np.sort(perm[cuts[j]:cuts[j + 1]]) for j in range(3)]
+        x, cb = edge_scene(n, rng, clusters)
+        xyz.append(x)
+        boxes.append(np.concatenate([np.stack(cb), random_boxes(x, m - len(cb), rng)]))
+        designed += [(s, r, c) for r, c in enumerate(clusters)]
+    return np.stack(xyz), np.stack(boxes), ns, designed
+
+
+def query_case(name):
+    """(xyz, boxes, nsample, designed) of test_query_boxes_vs_reference_kernel's case"""
+    if name in EDGES:
+        return edge_case(name)
     xyz = scenes()[name]
     rng = np.random.default_rng(7)
-    boxes = np.stack([proposals_around(x, 100, rng, big=3) for x in xyz])
-    idx, cnt = pkg.tf_ops.query_boxes_3d_points(512, torch.from_numpy(xyz).to(cuda), torch.from_numpy(boxes).to(cuda))
-    ridx, rcnt = ref_query(512, xyz, boxes)
-    assert np.array_equal(cnt.cpu().numpy(), rcnt)
-    assert np.array_equal(idx.cpu().numpy(), ridx)
+    return xyz, np.stack([proposals_around(x, 100, rng, big=3) for x in xyz]), 512, []
+
+
+def assert_designed_hits(idx, cnt, ns, designed, what):
+    """Each cluster box lists its cluster's first ns points in index order, padded with the first one."""
+    for s, r, members in designed:
+        k = min(len(members), ns)
+        assert cnt[s, r] == k, "%s: cluster box %d of scene %d holds %d points, expected %d" % (what, r, s, cnt[s, r], k)
+        exp = np.full(ns, members[0] if k else 0, np.int32)
+        exp[:k] = members[:k]
+        np.testing.assert_array_equal(idx[s, r], exp, err_msg="%s: cluster box %d of scene %d" % (what, r, s))
+
+
+@pytest.mark.parametrize("name", ["synthetic", "realscan"] + list(EDGES))
+def test_query_boxes_vs_reference_kernel(pkg, cuda, ref_query, name):
+    xyz, boxes, ns, designed = query_case(name)
+    idx, cnt = pkg.tf_ops.query_boxes_3d_points(ns, torch.from_numpy(xyz).to(cuda), torch.from_numpy(boxes).to(cuda))
+    idx, cnt = idx.cpu().numpy(), cnt.cpu().numpy()
+    ridx, rcnt = ref_query(ns, xyz, boxes)
+    assert np.array_equal(cnt, rcnt)
+    assert np.array_equal(idx, ridx)
     c = rcnt.ravel()
-    assert (c == 512).sum() >= 3 and (c == 0).sum() >= 2 and ((c > 0) & (c < 512)).sum() > 50
+    if name in EDGES:
+        assert_designed_hits(idx, cnt, ns, designed, name)
+        assert (cnt[:, len(designed) // 2] == min(xyz.shape[1], ns)).all() and not cnt[:, len(designed) // 2 + 1].any()
+    else:
+        assert (c == 512).sum() >= 3 and (c == 0).sum() >= 2 and ((c > 0) & (c < 512)).sum() > 50
     # the numpy restatement agrees wherever no point lies within a few ulp of a face
+    rows = range(0, boxes.shape[1], 1 if name in EDGES else 7)
+    compared = 0
     for s in range(len(xyz)):
-        for r in range(0, 100, 7):
-            i, n, amb = scan_np(xyz[s], boxes[s, r], 512)
+        for r in rows:
+            i, n, amb = scan_np(xyz[s], boxes[s, r], ns)
             if amb == 0:
-                assert n == rcnt[s, r] and np.array_equal(i, ridx[s, r])
+                compared += 1
+                assert n == rcnt[s, r] and np.array_equal(i, ridx[s, r]), "scene %d box %d" % (s, r)
+    assert compared >= len(xyz) * len(rows) // 2
 
 
 def pool_inputs(pkg, cuda, xyz, rng, count):
@@ -164,6 +250,90 @@ def test_region_pool(pkg, cuda, ref_query, name):
             assert_close(torch.from_numpy(ofeat[s, r, :, :128]), torch.from_numpy(info_conv64(info, params)), "info conv")
             assert np.array_equal(ofeat[s, r, :, 128:], feat[s, k])
     assert np.array_equal(cnt > 0, (rcnt > 0) & (np.arange(100)[None] < count[:, None]))
+
+
+def info_params(co, rng):
+    """A random roi_pool/conv0 (5 -> co, with BN) under its variable names."""
+    sc = "roi_pool/conv0/"
+    return {sc + "weights": rng.standard_normal((5, co)).astype(np.float32), sc + "biases": rng.standard_normal(co).astype(np.float32) * 0.1,
+            sc + "bn/gamma": rng.uniform(0.5, 1.5, co).astype(np.float32), sc + "bn/beta": rng.standard_normal(co).astype(np.float32) * 0.1,
+            sc + "bn/moving_mean": rng.standard_normal(co).astype(np.float32) * 0.1,
+            sc + "bn/moving_variance": rng.uniform(0.5, 2.0, co).astype(np.float32)}
+
+
+# pool edges: name -> (query shape of EDGES, c_info, c_feat, width of a block row, count given).  c_feat = 0 passes null
+# features; "nmax" is the largest scene the pool takes at nsample 512 and c_info 128 (tests/test_pointrcnn_rcnn_cpu.py
+# checks that one point more is rejected).
+POOL_EDGES = {"n1": ("n1", 128, 128, 9, True), "n33": ("n33", 4, 4, 7, False), "n1000": ("n1000", 256, 0, 12, True),
+              "n16383": ("n16383", 128, 4, 9, True), "ns1": ("ns1", 4, 0, 9, True), "ns31": ("ns31", 128, 4, 7, True),
+              "ns32": ("ns32", 256, 4, 12, False), "ns33": ("ns33", 128, 128, 9, True),
+              "ns1024": ("ns1024", 256, 128, 9, True), "nmax": (None, 128, 128, 9, True)}
+POOL_MAX_N = 17706
+
+
+@pytest.mark.parametrize("name", list(POOL_EDGES))
+def test_region_pool_kernel_edges(pkg, cuda, ref_query, name):
+    """The fused pool at the kernel's edges, every row: the indices and counts against the reference kernel on the
+    expanded boxes (and the designed cluster hits), padding rows empty, the canonical xyz in float32, the info conv in
+    float64 with the mask of score >= 0.5 (exact 0.5 scores on cluster points), and the copied features bit for bit."""
+    from test_bench_step_gpu import conv64
+    shape, co, cf, ld, with_count = POOL_EDGES[name]
+    if shape is None:
+        rng = np.random.default_rng(5)
+        xyz, cb = edge_scene(POOL_MAX_N, rng, [np.arange(POOL_MAX_N - 40, POOL_MAX_N, 3)])
+        xyz = np.stack([xyz, xyz[::-1]])
+        boxes = np.stack([np.concatenate([cb, random_boxes(xyz[s], 23, rng)]) for s in range(2)])
+        ns, designed = 512, []
+    else:
+        xyz, boxes, ns, designed = edge_case(shape)
+        rng = np.random.default_rng(len(name))
+    b, n, _ = xyz.shape
+    m = boxes.shape[1]
+    count = np.array([m, m - 5], np.int32)
+    valid = np.arange(m)[None] < count[:, None] if with_count else np.ones((b, m), bool)
+    block = np.zeros((b, m, ld), np.float32)
+    block[..., :7] = boxes
+    block[..., 7:] = rng.standard_normal((b, m, ld - 7))                   # the NMS block's extra columns are not read
+    block[~valid, :7] = rng.uniform(-5, 5, (int((~valid).sum()), 7))       # padding rows are not scanned either
+    feat = rng.standard_normal((b, n, cf)).astype(np.float32)
+    score = rng.uniform(0, 1, (b, n)).astype(np.float32)
+    score[:, ::3] = 0.5                                                     # the threshold itself: mask 1
+    score[:, 1::3] = np.nextafter(np.float32(0.5), np.float32(0))          # one ulp below: mask 0
+    params = info_params(co, rng)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
+    f = t(feat) if cf else torch.empty((b, n, 0), device=cuda)
+    assert cf or f.data_ptr() == 0                                          # null features
+    oxyz, ofeat, idx, cnt = pkg.tf_ops.region_pool(t(xyz), f, t(score), t(block), t(count) if with_count else None,
+                                                   pkg.params.prepare(params, cuda).conv("roi_pool/conv0", True), nsample=ns)
+    torch.cuda.synchronize()
+    assert tuple(oxyz.shape) == (b * m, ns, 3) and tuple(ofeat.shape) == (b * m, ns, co + cf)
+    idx_np, cnt_np = idx.cpu().numpy(), cnt.cpu().numpy()
+    exp_boxes = np.stack([np.stack([expand(block[s, r]) for r in range(m)]) for s in range(b)])
+    ridx, rcnt = ref_query(ns, xyz, exp_boxes)
+    assert np.array_equal(cnt_np[valid], rcnt[valid]) and np.array_equal(idx_np[valid], ridx[valid])
+    assert not cnt_np[~valid].any() and not idx_np[~valid].any()           # padding pools nothing
+    assert_designed_hits(idx_np, cnt_np, ns, designed, name)
+    if name == "nmax":
+        assert (cnt_np[:, 0] == 14).all() and (cnt_np[:, 1] == 512).all()
+    for s in range(b):
+        for r in np.flatnonzero(valid[s]):
+            i, c, amb = scan_np(xyz[s], exp_boxes[s, r], ns)
+            if amb == 0:
+                assert c == cnt_np[s, r] and np.array_equal(i, idx_np[s, r]), "scene %d box %d" % (s, r)
+    # every row: canonical xyz, [info conv | features]
+    oxyz_np = oxyz.cpu().numpy().reshape(b, m, ns, 3)
+    for s in range(b):
+        for r in range(m):
+            can = canonical_np(xyz[s, idx_np[s, r]], block[s, r])
+            np.testing.assert_allclose(oxyz_np[s, r], can, rtol=0, atol=4 * np.spacing(np.float32(np.abs(can).max() + 1)))
+    k = idx.view(b, m * ns).long()
+    gx = torch.gather(t(xyz).double(), 1, k[..., None].expand(-1, -1, 3))
+    gs = torch.gather(t(score), 1, k)
+    info = torch.cat([oxyz.view(b, m * ns, 3).double(), (gs >= 0.5).double()[..., None], gx.norm(dim=-1, keepdim=True)], -1)
+    assert (gs == 0.5).any() and ((gs < 0.5).any() or n < 2)
+    assert_close(ofeat.view(b, m * ns, -1)[..., :co], conv64(params, "roi_pool/conv0", info, True, True), "%s: info conv" % name)
+    if cf:
+        assert torch.equal(ofeat.view(b, m * ns, -1)[..., co:], torch.gather(f, 1, k[..., None].expand(-1, -1, cf)))
 
 
 def test_decode_rows_and_counted_nms(pkg, cuda):
