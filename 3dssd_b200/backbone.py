@@ -53,7 +53,6 @@ class SABackbone:
         self.latency_mode = latency_mode
         self.fps_parts = fps_parts if isinstance(fps_parts, int) else list(fps_parts)
         self.head = head                      # optional head.DetectionHead: real detections instead of the stand-in block
-        self._graph = None
         self._split = {}                      # layer index -> (features, split features) of the FP layer the head reads
 
     def forward(self, points, return_debug=False):
@@ -65,50 +64,7 @@ class SABackbone:
     def forward_lists(self, xyz_list, feat_list, return_debug=False):
         """The layer loop on the given starting lists (forward starts from [xyz], [features] of the points; PointRCNN's
         stage 2 from [proposal centres, pooled xyz], [None, pooled features], double_stage_detector.py:210)."""
-        xyz_list, feat_list = list(xyz_list), list(feat_list)
-        fps_list = [None] * len(xyz_list)
-        dbg = []
-        for spec in self.arch:
-            (xyz_i, feat_i, radius, nsample, mlps, bn, rng, method, npoint, former, attn, ltype, scope, dilated,
-             vote_idx, agg) = spec
-            former_idx = fps_list[former] if former != -1 else None
-            vote_ctr = xyz_list[vote_idx] if vote_idx != -1 else None
-            if ltype == "SA_Layer":
-                parts = None
-                if self.latency_mode and len(radius) and vote_ctr is None:
-                    parts = self.fps_parts if (len(npoint) == 1 and method[0] == "D-FPS") else True
-                r = L.pointnet_sa_module_msg(xyz_list[xyz_i[0]], feat_list[feat_i[0]], radius, nsample, mlps, False,
-                                             None, bn, rng, method, npoint, former_idx, attn, scope, dilated, vote_ctr,
-                                             agg, params=self.params, ffps_mode=self.ffps_mode, aggregation=self.aggregation,
-                                             return_debug=True,
-                                             mlp_mode=self.mlp_mode, fuse_scale=self.fuse_scale,
-                                             gather_in_kernel=self.gather_in_kernel, hoist_first=self.hoist_first,
-                                             fps_cluster=self.fps_cluster, fps_parts=parts, fps_packet=self.fps_packet,
-                                             fps_bucket=self.fps_bucket)
-                xyz_list.append(r[0]); feat_list.append(r[1]); fps_list.append(r[2]); dbg.append(r[3])
-            elif ltype == "Vote_Layer":
-                nx, nf, off = L.vote_layer(xyz_list[xyz_i[0]], feat_list[feat_i[0]], mlps, False, None, bn, scope,
-                                           params=self.params, mlp_mode=self.mlp_mode)
-                xyz_list.append(nx); feat_list.append(nf); fps_list.append(None); dbg.append({"offsets": off})
-            elif ltype == "SA_Layer_SSG_Last":
-                xyz_list.append(None)
-                feat_list.append(L.pointnet_sa_module(xyz_list[xyz_i[0]], feat_list[feat_i[0]], mlps, False, None, bn,
-                                                      scope, params=self.params))
-                fps_list.append(None); dbg.append({})
-            elif ltype == "FP_Layer":
-                xyz_list.append(xyz_list[xyz_i[0]])
-                # the layer the head reads alone hands it its split features (the operand of the head's first convs)
-                li = len(feat_list)
-                split = self.head is not None and list(self.head.feature_index) == [li] and len(mlps) > 0
-                r = L.pointnet_fp_module(xyz_list[xyz_i[0]], xyz_list[xyz_i[1]], feat_list[feat_i[0]], feat_list[feat_i[1]],
-                                         mlps, False, None, scope, bn, params=self.params, want_split=split)
-                if split:
-                    r, sp = r
-                    self._split[li] = (r, sp)
-                feat_list.append(r)
-                fps_list.append(None); dbg.append({})
-            else:
-                raise ValueError("unknown layer type %r" % (ltype,))
+        xyz_list, feat_list, fps_list, dbg = run_layers(self.arch, xyz_list, feat_list, self.params, net=self)
         if return_debug:
             return xyz_list, feat_list, fps_list, dbg
         return xyz_list, feat_list, fps_list
@@ -156,35 +112,89 @@ class SABackbone:
         NMS writes into its send buffer and ncclAllGather is captured with the kernels) into one CUDA graph.  Returns
         replay(points=None) -> (forward outputs, (block, count)); with `gather` the pair holds this rank's views of the
         send buffer and gather.result() / gather.raw hold all ranks' detections after the replay."""
-        static_in = example_points.clone()
         out_buf = gather.out() if gather is not None else None
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(warmup):
-                out = self.forward(static_in)
-                blk = self.detections(out[0], out[1], out=out_buf)
-                if gather is not None:
-                    gather.gather()
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        # thread_local: NCCL's watchdog thread polls its events while this thread captures
-        kw = {"capture_error_mode": "thread_local"} if (gather is not None and gather.world > 1) else {}
-        with torch.cuda.graph(g, **kw):
-            out = self.forward(static_in)
+
+        def step(points):
+            out = self.forward(points)
             blk = self.detections(out[0], out[1], out=out_buf)
             if gather is not None:
                 gather.gather()
-        self._graph = (g, static_in, out, blk)
-
-        def replay(points=None):
-            if points is not None:
-                static_in.copy_(points, non_blocking=True)
-            g.replay()
             return out, blk
+        # thread_local: NCCL's watchdog thread polls its events while this thread captures
+        kw = {"capture_error_mode": "thread_local"} if (gather is not None and gather.world > 1) else {}
+        return capture_graph(step, example_points, warmup, **kw)
 
-        return replay
+
+def capture_graph(step, example_points, warmup=2, **graph_kw):
+    """Record step(points) into one CUDA graph (no allocation or host sync happens inside the kernels, include/ssd3d.h)
+    after `warmup` calls on a side stream.  Returns replay(points=None) -> what the recorded call returned, after copying
+    new points into the static input buffer.  graph_kw go to torch.cuda.graph."""
+    static_in = example_points.clone()
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for _ in range(warmup):
+            step(static_in)
+    torch.cuda.current_stream().wait_stream(s)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g, **graph_kw):
+        out = step(static_in)
+
+    def replay(points=None):
+        if points is not None:
+            static_in.copy_(points, non_blocking=True)
+        g.replay()
+        return out
+
+    return replay
+
+
+def run_layers(arch, xyz_list, feat_list, params, is_training=False, bn_decay=None, net=None):
+    """The layer loop (single_stage_detector.py:115-125, layer_builder.py:45-101): every layer of `arch` appends one
+    entry to the xyz / feature / fps-index / debug lists and addresses its inputs by index.  Returns the four lists.
+    Inference takes its FPS, route and latency options and the head's split operand from `net` (an SABackbone);
+    is_training=True runs the SA and vote layers with params.TrainableParams, batch-statistics BatchNorm and bn_decay."""
+    xyz_list, feat_list = list(xyz_list), list(feat_list)
+    fps_list, dbg = [None] * len(xyz_list), []
+    for spec in arch:
+        (xyz_i, feat_i, radius, nsample, mlps, bn, rng, method, npoint, former, attn, ltype, scope, dilated,
+         vote_idx, agg) = spec
+        xyz, feat, fps, d = xyz_list[xyz_i[0]], feat_list[feat_i[0]], None, {}
+        vote_ctr = xyz_list[vote_idx] if vote_idx != -1 else None
+        if ltype == "SA_Layer":
+            kw = {}
+            if not is_training:
+                parts = None
+                if net.latency_mode and len(radius) and vote_ctr is None:
+                    parts = net.fps_parts if (len(npoint) == 1 and method[0] == "D-FPS") else True
+                kw = dict(ffps_mode=net.ffps_mode, aggregation=net.aggregation, mlp_mode=net.mlp_mode, fuse_scale=net.fuse_scale,
+                          gather_in_kernel=net.gather_in_kernel, hoist_first=net.hoist_first, fps_cluster=net.fps_cluster,
+                          fps_parts=parts, fps_packet=net.fps_packet, fps_bucket=net.fps_bucket)
+            xyz, feat, fps, d = L.pointnet_sa_module_msg(xyz, feat, radius, nsample, mlps, is_training, bn_decay, bn, rng, method,
+                                                         npoint, fps_list[former] if former != -1 else None, attn, scope,
+                                                         dilated, vote_ctr, agg, params=params, return_debug=True, **kw)
+        elif ltype == "Vote_Layer":
+            kw = {} if is_training else {"mlp_mode": net.mlp_mode}
+            xyz, feat, off = L.vote_layer(xyz, feat, mlps, is_training, bn_decay, bn, scope, params=params, **kw)
+            d = {"offsets": off}
+        elif is_training:
+            raise ValueError("layer type %r has no training driver here" % (ltype,))
+        elif ltype == "SA_Layer_SSG_Last":
+            xyz, feat = None, L.pointnet_sa_module(xyz, feat, mlps, False, None, bn, scope, params=params)
+        elif ltype == "FP_Layer":
+            # the layer the head reads alone hands it its split features (the operand of the head's first convs)
+            li = len(feat_list)
+            split = net.head is not None and list(net.head.feature_index) == [li] and len(mlps) > 0
+            feat = L.pointnet_fp_module(xyz, xyz_list[xyz_i[1]], feat, feat_list[feat_i[1]], mlps, False, None, scope, bn,
+                                        params=params, want_split=split)
+            if split:
+                net._split[li] = feat
+                feat = feat[0]
+        else:
+            raise ValueError("unknown layer type %r" % (ltype,))
+        xyz_list.append(xyz); feat_list.append(feat); fps_list.append(fps); dbg.append(d)
+    return xyz_list, feat_list, fps_list, dbg
 
 
 class TrainOutputs(NamedTuple):
@@ -204,19 +214,8 @@ def train_forward(arch, tp, xyz, feat, *, bn_decay=None):
     bn_decay: the decay of every BatchNorm's moving statistics in this forward (model_forward(bn_decay),
     trainer.py:130; solver.Solver.bn_decay gives the scheduled value); None keeps the layers' default of 0.9."""
     from . import head as _head
-    xyz_l, feat_l, fps_l, offs, vote_base = [xyz], [feat], [None], [], None
-    for spec in arch:
-        (xyz_i, feat_i, radius, nsample, mlps, bn, rng, method, npoint, former, attn, ltype, scope, dilated, vote_idx, agg) = spec
-        if ltype == "SA_Layer":
-            r = L.pointnet_sa_module_msg(xyz_l[xyz_i[0]], feat_l[feat_i[0]], radius, nsample, mlps, True, bn_decay, bn, rng, method,
-                                         npoint, fps_l[former] if former != -1 else None, attn, scope, dilated,
-                                         xyz_l[vote_idx] if vote_idx != -1 else None, agg, params=tp)
-            xyz_l.append(r[0]); feat_l.append(r[1]); fps_l.append(r[2])
-        elif ltype == "Vote_Layer":
-            vote_base = xyz_l[xyz_i[0]]                                 # PRED_VOTE_BASE (layer_builder.py:96)
-            nx, nf, off = L.vote_layer(vote_base, feat_l[feat_i[0]], mlps, True, bn_decay, bn, scope, params=tp)
-            xyz_l.append(nx); feat_l.append(nf); fps_l.append(None); offs.append(off)
-        else:
-            raise ValueError("layer type %r has no training driver here" % (ltype,))
+    xyz_l, feat_l, _, dbg = run_layers(arch, [xyz], [feat], tp, True, bn_decay)
+    votes = [(spec[0][0], d["offsets"]) for spec, d in zip(arch, dbg) if spec[11] == "Vote_Layer"]
     f = tp.conv_train("conv1d_0", feat_l[-1], True, bn_decay)
-    return TrainOutputs(_head.box_regression_head(f, 1, 1, 6, True, True, params=tp, bn_decay=bn_decay), offs, xyz_l[-1], vote_base)
+    return TrainOutputs(_head.box_regression_head(f, 1, 1, 6, True, True, params=tp, bn_decay=bn_decay), [o for _, o in votes],
+                        xyz_l[-1], xyz_l[votes[-1][0]] if votes else None)   # vote_base: PRED_VOTE_BASE (layer_builder.py:96)

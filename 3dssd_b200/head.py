@@ -39,14 +39,18 @@ def _scope(scope, name):
     return name if scope == '' else scope + "/" + name
 
 
-def _conv_chain(pp, hi, lo, scopes_bn_relu):
+def head_convs(pp, scope, bn, mlp, hi, lo, want_f32=False):
+    """head_builder.py:93-113 at inference on the split features (hi, lo), on the tensor cores: one conv1d_i per width of
+    `mlp`, then the pred_cls_base -> pred_cls and pred_reg_base -> pred_reg chains.  Returns (features, (cls, reg)):
+    the last conv1d_i output in fp32 when want_f32 (None otherwise, or without conv1d_i), cls and reg in fp32."""
     y = None
-    for i, (sc, bn, relu) in enumerate(scopes_bn_relu):
-        last = i == len(scopes_bn_relu) - 1
-        y, sp = tf_ops.linear_tc(hi, lo, pp.conv(sc, bn), relu=relu, want_f32=last, want_split=not last)
-        if not last:
-            hi, lo = sp
-    return y
+    for i in range(len(mlp)):
+        y, (hi, lo) = tf_ops.linear_tc(hi, lo, pp.conv(_scope(scope, "conv1d_%d" % i), bn), want_f32=want_f32, want_split=True)
+    preds = []
+    for name in ("pred_cls", "pred_reg"):
+        _, (b_hi, b_lo) = tf_ops.linear_tc(hi, lo, pp.conv(_scope(scope, name + "_base"), bn), want_f32=False, want_split=True)
+        preds.append(tf_ops.linear_tc(b_hi, b_lo, pp.conv(_scope(scope, name), False), relu=False)[0])
+    return y, tuple(preds)
 
 
 def box_regression_head(feature_input, pred_cls_channel, pred_reg_base_num, pred_reg_channel_num, bn, is_training, *,
@@ -63,10 +67,8 @@ def box_regression_head(feature_input, pred_cls_channel, pred_reg_base_num, pred
                                                      False, bn_decay, relu=False)
         pred_cls, pred_reg = chain("pred_cls_base", "pred_cls"), chain("pred_reg_base", "pred_reg")
     else:
-        pp = prepare(params, feature_input.device)
-        hi, lo = tf_ops.split_rows(feature_input)
-        pred_cls = _conv_chain(pp, hi, lo, [(_scope(scope, "pred_cls_base"), bn, True), (_scope(scope, "pred_cls"), False, False)])
-        pred_reg = _conv_chain(pp, hi, lo, [(_scope(scope, "pred_reg_base"), bn, True), (_scope(scope, "pred_reg"), False, False)])
+        _, (pred_cls, pred_reg) = head_convs(prepare(params, feature_input.device), scope, bn, (),
+                                             *tf_ops.split_rows(feature_input))
     pred_reg = pred_reg.view(bs, n, pred_reg_base_num, pred_reg_channel_num + ANGLE_CLS_NUM * 2)
     return (pred_cls, pred_reg[..., :pred_reg_channel_num],
             pred_reg[..., pred_reg_channel_num:pred_reg_channel_num + ANGLE_CLS_NUM],
@@ -122,14 +124,10 @@ class DetectionHead:
         fs = [feature_list[i] for i in self.feature_index]
         xyz = xs[0] if len(xs) == 1 else torch.cat(xs, dim=1)
         feat = (fs[0] if len(fs) == 1 else torch.cat(fs, dim=1)).contiguous()
-        hi, lo = tf_ops.split_rows(feat) if split is None else split
-        y = feat
-        for i, ch in enumerate(self.mlp_list):                                    # :93-95
-            y, (hi, lo) = tf_ops.linear_tc(hi, lo, self.params.conv(_scope(self.scope, "conv1d_%d" % i), self.bn),
-                                           want_f32=True, want_split=True)
-        pp, sc, st = self.params, self.scope, self.stage
-        cls = _conv_chain(pp, hi, lo, [(_scope(sc, "pred_cls_base"), self.bn, True), (_scope(sc, "pred_cls"), False, False)])
-        reg = _conv_chain(pp, hi, lo, [(_scope(sc, "pred_reg_base"), self.bn, True), (_scope(sc, "pred_reg"), False, False)])
+        y, (cls, reg) = head_convs(self.params, self.scope, self.bn, self.mlp_list,
+                                   *(tf_ops.split_rows(feat) if split is None else split), want_f32=True)
+        y = feat if y is None else y
+        st = self.stage
         # decode + sigmoid (anchor_decoder.py:86-164, single_stage_detector.py:210-211): one kernel
         if st["REGRESSION"] == "Bin-Anchor":
             boxes, score = tf_ops.decode_bin_anchor(xyz, reg, cls, st["ANCHOR_SIZE"], st["HALF_BIN_SEARCH_RANGE"],

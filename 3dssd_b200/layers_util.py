@@ -412,42 +412,46 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
             parts.append((col, col + npoint, ev_main() if in_parts else None))
         col += width
 
+    # ---- the consumers (:113-187).  Latency mode: one per part of the sampling, each on its own stream as soon as its
+    # samples are final, joined at the end; otherwise one over every sample on the main stream once the sampling is done
     src_xyz = vote_ctr if vote_ctr is not None else xyz
-    debug = {"idx": [], "cnt": []}
-
-    if not in_parts:
+    if in_parts:
+        chunks = [(fps_idx[:, c0:c1], ev, _side_stream(dev, 8 + pi)) for pi, (c0, c1, ev) in enumerate(parts)]
+    else:
         for _, _, ev in parts:
             if ev is not None:
                 main.wait_event(ev)
         if former_fps_idx is not None:
             fps_idx = torch.cat([fps_idx, former_fps_idx], dim=-1).contiguous()    # :113-114
-        new_xyz = tf_ops.gather_point(src_xyz, fps_idx)                            # :116-119
-        if nscale and is_training:
-            new_points, idx, cnt, convs = _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_list,
-                                                               mlp_list, bn, bn_decay, dilated_group, use_agg)
-            debug = {"idx": idx, "cnt": cnt} if convs is None else {"idx": idx, "cnt": cnt, "convs": convs}
-        elif nscale:
-            table = _hoist_table(pp, plan, points)
-            new_points, idx, cnt = _group_and_mlp(pp, plan, table, xyz, points, new_xyz, radius_list, nsample_list,
-                                                  mlp_list, dilated_group)
-            debug = {"idx": idx, "cnt": cnt}
-        else:
-            new_points = tf_ops.gather_point(points.contiguous(), fps_idx)         # :186-187
-    else:
-        # ---- one consumer chain per part, each on its own stream, joined at the end
-        xyz_parts, pts_parts, found, done = [], [], [], []
-        for pi, (c0, c1, ev) in enumerate(parts):
-            st = _side_stream(dev, 8 + pi)
+        chunks = [(fps_idx, None, main)]
+    xyz_parts, pts_parts, found, done = [], [], [], []
+    for sel, ev, st in chunks:
+        if in_parts:
             st.wait_event(ev)
             if plan.hoisted:
                 st.wait_event(z_ready)
-            with torch.cuda.stream(st):
-                nx = tf_ops.gather_point(src_xyz, fps_idx[:, c0:c1])
+        with torch.cuda.stream(st):
+            nx = tf_ops.gather_point(src_xyz, sel)                                 # :116-119
+            dbg = {"idx": [], "cnt": []}
+            if not nscale:
+                npnts = tf_ops.gather_point(points.contiguous(), sel)              # :186-187
+            elif is_training:
+                npnts, idx, cnt, convs = _group_and_mlp_train(pp, scope, xyz, points, nx, radius_list, nsample_list, mlp_list,
+                                                              bn, bn_decay, dilated_group, use_agg)
+                dbg = {"idx": idx, "cnt": cnt} if convs is None else {"idx": idx, "cnt": cnt, "convs": convs}
+            else:
+                if not in_parts:
+                    table = _hoist_table(pp, plan, points)
                 npnts, idx, cnt = _group_and_mlp(pp, plan, table, xyz, points, nx, radius_list, nsample_list, mlp_list,
                                                  dilated_group)
-                e2 = torch.cuda.Event()
-                e2.record(st)
-            xyz_parts.append(nx); pts_parts.append(npnts); found.append((idx, cnt)); done.append(e2)
+                dbg = {"idx": idx, "cnt": cnt}
+            if in_parts:
+                done.append(torch.cuda.Event())
+                done[-1].record(st)
+        xyz_parts.append(nx); pts_parts.append(npnts); found.append(dbg)
+    if not in_parts:
+        new_xyz, new_points, debug = xyz_parts[0], pts_parts[0], found[0]
+    else:
         for e2 in done:
             main.wait_event(e2)
         for i in range(nside):
@@ -456,8 +460,7 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
         new_points = tf_ops.concat_rows(pts_parts)
         keep.extend(xyz_parts + pts_parts)
         if return_debug:
-            debug = {"idx": [torch.cat([f[0][i] for f in found], dim=1) for i in range(nscale)],
-                     "cnt": [torch.cat([f[1][i] for f in found], dim=1) for i in range(nscale)]}
+            debug = {k: [torch.cat([f[k][i] for f in found], dim=1) for i in range(nscale)] for k in ("idx", "cnt")}
         _KEEPALIVE.append((keep, found if not return_debug else None, table))
         del _KEEPALIVE[:-8]
     if return_debug:

@@ -17,8 +17,8 @@ import torch
 
 from . import config as _cfg
 from . import tf_ops
-from .backbone import SABackbone
-from .head import ANGLE_CLS_NUM, DetectionHead, _conv_chain, reg_channels
+from .backbone import SABackbone, capture_graph
+from .head import ANGLE_CLS_NUM, DetectionHead, head_convs, reg_channels
 from .params import init_head_params, init_params, init_rcnn_params, prepare
 
 
@@ -58,19 +58,6 @@ class PointRCNN:
         self.rcnn = SABackbone(_cfg.ARCH_POINTRCNN_RCNN, self.params, device=self.device, aggregation=False)
         (self.head_xyz, self.head_feat, _, self.head_mlp, self.head_bn, _, self.head_scope) = _cfg.HEAD_POINTRCNN_RCNN
         self.reg_channels = reg_channels(self.stage) + 2 * ANGLE_CLS_NUM
-        self._graph = None
-
-    def _head(self, ctr, feat):
-        """head_builder.py:81-113 on [B, P, 512]: conv1d_0 (BN), then pred_cls (2) / pred_reg (52) chains."""
-        b, p = ctr.shape[:2]
-        hi, lo = tf_ops.split_rows(feat.reshape(b, p, -1).contiguous())
-        sc = self.head_scope
-        for i in range(len(self.head_mlp)):
-            _, (hi, lo) = tf_ops.linear_tc(hi, lo, self.params.conv("%s/conv1d_%d" % (sc, i), self.head_bn),
-                                           want_f32=False, want_split=True)
-        cls = _conv_chain(self.params, hi, lo, [(sc + "/pred_cls_base", self.head_bn, True), (sc + "/pred_cls", False, False)])
-        reg = _conv_chain(self.params, hi, lo, [(sc + "/pred_reg_base", self.head_bn, True), (sc + "/pred_reg", False, False)])
-        return cls, reg
 
     def forward(self, points, return_debug=False):
         rxyz, rfeat, rfps, rdbg = self.rpn.forward(points, return_debug=True)
@@ -83,7 +70,9 @@ class PointRCNN:
                                                      context=pool[4], mask_thresh=self.mask_thresh)
         ctr = cast_bottom_to_center(props)[..., :3].contiguous()
         xyz_l, feat_l, fps_l, sdbg = self.rcnn.forward_lists([ctr, pxyz], [None, pfeat], return_debug=True)
-        cls, reg = self._head(xyz_l[self.head_xyz[0]], feat_l[self.head_feat[0]])
+        # head_builder.py:81-113 on the [B * P, 512] features as [B, P, 512]: conv1d_0, then the pred_cls / pred_reg chains
+        feat = feat_l[self.head_feat[0]].reshape(*xyz_l[self.head_xyz[0]].shape[:2], -1).contiguous()
+        _, (cls, reg) = head_convs(self.params, self.head_scope, self.head_bn, self.head_mlp, *tf_ops.split_rows(feat))
         st = self.stage
         boxes, scores = tf_ops.decode_bin_anchor_rows(props, reg, cls, pcnt, st["HALF_BIN_SEARCH_RANGE"], st["BIN_CLASS_NUM"],
                                                       ANGLE_CLS_NUM)
@@ -100,23 +89,4 @@ class PointRCNN:
 
     def capture(self, example_points, warmup=2):
         """Record forward into one CUDA graph; returns replay(points=None) -> (block, count) on the static buffers."""
-        static_in = example_points.clone()
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(warmup):
-                self.forward(static_in)
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            out = self.forward(static_in)
-        self._graph = (g, static_in, out)
-
-        def replay(points=None):
-            if points is not None:
-                static_in.copy_(points, non_blocking=True)
-            g.replay()
-            return out
-
-        return replay
+        return capture_graph(self.forward, example_points, warmup)

@@ -244,6 +244,66 @@ def dry(monkeypatch, oracle_ops):
         out = y.max(dim=-2).values
         return out * (rowmask > 0).unsqueeze(-1).to(out.dtype) if rowmask is not None else out
 
+    # ---- FP layers, decoders, NMS and PointRCNN's region pool
+    def fp_interp_split(xyz1, xyz2, points2, points1=None, kp=None):
+        d = ((xyz1.double()[:, :, None] - xyz2.double()[:, None]) ** 2).sum(-1)
+        dist, idx = d.topk(min(3, xyz2.shape[1]), dim=-1, largest=False)
+        inv = 1.0 / dist.clamp_min(1e-10)
+        w = inv / inv.sum(-1, keepdim=True)
+        x = (points2.double()[torch.arange(points2.shape[0])[:, None, None], idx] * w[..., None]).sum(2)
+        if points1 is not None:
+            x = torch.cat([x, points1.double()], -1)
+        return split_rows(x.float(), kp)
+
+    def decode_dist_anchor_free(center_xyz, pred_reg, pred_cls, angle_bins=12):
+        reg, cls = pred_reg.numpy(), pred_cls.numpy()
+        off, acls, ares = reg[..., :6], reg[..., 6:6 + angle_bins], reg[..., 6 + angle_bins:]
+        bins = np.argmax(acls, -1)
+        res = np.take_along_axis(ares, bins[..., None], -1)[..., 0]
+        ang = ((bins.astype(np.float32) + res) * np.float32(2 * np.pi / angle_bins)).astype(np.float32)
+        ctr = center_xyz.numpy() + off[..., :3]
+        ctr[..., 1] += off[..., 4]
+        boxes = np.concatenate([ctr, np.maximum(off[..., 3:6] * np.float32(2), np.float32(0.1)), ang[..., None]], -1).astype(np.float32)
+        return torch.from_numpy(boxes), torch.from_numpy((1 / (1 + np.exp(-cls[..., 0].astype(np.float64)))).astype(np.float32))
+
+    def decode_bin_anchor(center_xyz, pred_reg, pred_cls, anchor_lhw, half_bin_search_range=3.0, bin_num=12, angle_bins=12):
+        b, n, _ = center_xyz.shape
+        boxes = torch.cat([center_xyz, torch.tensor(anchor_lhw, dtype=torch.float32).expand(b, n, 3),
+                           pred_reg[..., :1]], -1)
+        return boxes.contiguous(), torch.sigmoid(pred_cls[..., 0]).contiguous()
+
+    def decode_bin_anchor_rows(anchors, pred_reg, pred_cls, pool_cnt=None, half_bin_search_range=1.5, bin_num=6, angle_bins=12):
+        score = torch.softmax(pred_cls[..., :2].double(), -1)[..., 1].float()
+        if pool_cnt is not None:
+            score = score * (pool_cnt > 0).float()
+        return anchors[..., :7].contiguous(), score
+
+    def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
+        blk, cnt = oracle_ops.bev_nms(n(boxes), n(scores), iou_threshold, max_output, cls_id)
+        if out is None:
+            return t(blk), t(cnt)
+        out[0].copy_(t(blk)); out[1].copy_(t(cnt))
+        return out
+
+    def bev_nms_counted(boxes, scores, n_valid, iou_threshold, max_output, cls_id=0, out=None):
+        m = (torch.arange(scores.shape[1])[None] < n_valid[:, None].long()).float()
+        return bev_nms(boxes, scores * m - (1 - m), iou_threshold, max_output, cls_id, out)
+
+    def region_pool(xyz, features, point_score, proposals, count, info_conv, nsample=512, context=1.0, mask_thresh=0.5):
+        """Each proposal pools the scene's first nsample points (cyclically), canonical = relative to its centre."""
+        b, nn = xyz.shape[:2]
+        p = proposals.shape[1]
+        idx = (torch.arange(nsample) % nn).to(torch.int32).expand(b, p, nsample).contiguous()
+        rows = torch.arange(nsample) % nn
+        cxyz = xyz[:, None, rows] - proposals[:, :, None, :3]
+        mask = (point_score[:, None, rows] >= mask_thresh).float().expand(b, p, nsample)
+        info = torch.cat([cxyz, mask[..., None], cxyz.norm(dim=-1, keepdim=True)], -1)
+        feat = torch.cat([conv(info, info_conv), features[:, None, rows].expand(b, p, nsample, -1)], -1)
+        cnt = torch.full((b, p), nsample, dtype=torch.int32)
+        if count is not None:
+            cnt = cnt * (torch.arange(p)[None] < count[:, None].long()).to(torch.int32)
+        return (cxyz.reshape(b * p, nsample, 3).contiguous(), feat.reshape(b * p, nsample, -1).contiguous(), idx, cnt)
+
     fakes = dict(
         fill_zero=lambda x: x.zero_(),
         split_rows=split_rows, linear_tc=linear_tc, linear_tc_gather=linear_tc_gather, linear_tc_hoisted=linear_tc_hoisted,
@@ -261,6 +321,8 @@ def dry(monkeypatch, oracle_ops):
         fps_temp_elems=lambda nn, c=3, npoint=0, **kw: 2 * nn,
         vote_translate=lambda xyz, off, rng: xyz + torch.minimum(torch.maximum(off[..., :3], torch.tensor(rng)), -torch.tensor(rng)),
         bn_train=bn_train, rowgroup_max=rowgroup_max,
+        fp_interp_split=fp_interp_split, decode_dist_anchor_free=decode_dist_anchor_free, decode_bin_anchor=decode_bin_anchor,
+        decode_bin_anchor_rows=decode_bin_anchor_rows, bev_nms=bev_nms, bev_nms_counted=bev_nms_counted, region_pool=region_pool,
     )
     for k, v in fakes.items():
         monkeypatch.setattr(T, k, v)
@@ -311,33 +373,11 @@ def test_backbone_orchestration_dry_run_matches_oracle_layers(dry, oracle_ops, l
         assert np.abs(got[1][li].numpy() - exp[1][li]).max() <= 1e-4 * max(1.0, np.abs(exp[1][li]).max()), "features of layer %d" % li
 
 
-def test_head_orchestration_dry_run_writes_into_gather_buffers(dry, oracle_ops, monkeypatch):
+def test_head_orchestration_dry_run_writes_into_gather_buffers(dry, oracle_ops):
     """DetectionHead + DetectionGather plumbing on the CPU: conv chain -> one-kernel decode -> NMS writing straight into
     the send buffer of the (single-rank) gather, against the oracle's head."""
     pkg = dry
     from oracle import head as ohead
-    T = pkg.tf_ops
-
-    def decode(center_xyz, pred_reg, pred_cls, angle_bins=12):
-        reg, cls = pred_reg.numpy(), pred_cls.numpy()
-        off, acls, ares = reg[..., :6], reg[..., 6:6 + angle_bins], reg[..., 6 + angle_bins:]
-        bins = np.argmax(acls, -1)
-        res = np.take_along_axis(ares, bins[..., None], -1)[..., 0]
-        ang = ((bins.astype(np.float32) + res) * np.float32(2 * np.pi / angle_bins)).astype(np.float32)
-        ctr = center_xyz.numpy() + off[..., :3]
-        ctr[..., 1] += off[..., 4]
-        boxes = np.concatenate([ctr, np.maximum(off[..., 3:6] * np.float32(2), np.float32(0.1)), ang[..., None]], -1).astype(np.float32)
-        return torch.from_numpy(boxes), torch.from_numpy((1 / (1 + np.exp(-cls[..., 0].astype(np.float64)))).astype(np.float32))
-
-    def nms(boxes, scores, thr, max_output, cls_id=0, out=None):
-        blk, cnt = oracle_ops.bev_nms(boxes.numpy(), scores.numpy(), thr, max_output, cls_id)
-        if out is None:
-            return torch.from_numpy(blk), torch.from_numpy(cnt)
-        out[0].copy_(torch.from_numpy(blk)); out[1].copy_(torch.from_numpy(cnt))
-        return out
-
-    monkeypatch.setattr(T, "decode_dist_anchor_free", decode)
-    monkeypatch.setattr(T, "bev_nms", nms)
     rng = np.random.default_rng(3)
     xyz = rng.uniform(-10, 10, (3, 64, 3)).astype(np.float32)
     feat = np.maximum(rng.standard_normal((3, 64, 512)), 0).astype(np.float32)
@@ -397,6 +437,55 @@ def test_training_mode_orchestration_dry_run_matches_oracle(dry, oracle_ops, dec
     assert np.abs(got_i[1].numpy() - exp_i[1]).max() <= 1e-4 * np.abs(exp_i[1]).max()
 
 
+def _scaled_pointrcnn(pkg, mp):
+    """PointRCNN's tables with smaller sample counts and 64 points per proposal, so its dry run is small; mp: a
+    monkeypatch context that restores them."""
+    cfg = pkg.config
+    for name, div in (("ARCH_POINTRCNN_RPN", 16), ("ARCH_POINTRCNN_RCNN", 8)):
+        arch = copy.deepcopy(getattr(cfg, name))
+        for spec in arch:
+            spec[8] = [p if p in (-1, 0) else max(1, p // div) for p in spec[8]]
+        mp.setattr(cfg, name, arch)
+    pool = list(cfg.POINTS_POOLER_POINTRCNN)
+    pool[3] = 64
+    mp.setattr(cfg, "POINTS_POOLER_POINTRCNN", pool)
+
+
+def _rpn_dry_run(pkg, mp, latency):
+    """PointRCNN's first stage: the SA and FP layers of its table and its Bin-Anchor DetectionHead."""
+    _scaled_pointrcnn(pkg, mp)
+    cfg = pkg.config
+    synth = importlib.import_module("3dssd_b200.synth")
+    params = pkg.rcnn.init_pointrcnn_params(seed=3)
+    head = pkg.DetectionHead(cfg.HEAD_POINTRCNN_RPN, params, device="cpu", stage=cfg.STAGE_POINTRCNN_RPN_TEST)
+    net = pkg.SABackbone(cfg.ARCH_POINTRCNN_RPN, params, in_channels=1, device="cpu", head=head, aggregation=False,
+                         latency_mode=latency)
+    xyz_l, feat_l, _ = net.forward(torch.from_numpy(synth.kitti_like(2, 1024, seed=42)))
+    blk, cnt = net.detections(xyz_l, feat_l)
+    assert blk.shape == (2, 100, 9) and feat_l[-1].shape == (2, 1024, 128)
+
+
+def _pointrcnn_dry_run(pkg, mp):
+    """PointRCNN.forward: RPN, region pool, stage-2 layers, RCNN head, row decode and the counted NMS."""
+    _scaled_pointrcnn(pkg, mp)
+    synth = importlib.import_module("3dssd_b200.synth")
+    net = pkg.PointRCNN(device="cpu", seed=3)
+    block, count = net.forward(torch.from_numpy(synth.kitti_like(2, 1024, seed=43)))
+    assert block.shape == (2, 100, 9) and count.shape == (2,)
+
+
+def _train_forward_dry_run(pkg):
+    """backbone.train_forward over the (scaled) 3DSSD table with TrainableParams."""
+    synth = importlib.import_module("3dssd_b200.synth")
+    arch = _scaled(pkg, 16)
+    d = dict(pkg.params.init_params(arch, 1, seed=4, random_bias=True))
+    d.update(pkg.params.init_head_params(pkg.config.layer_channels(arch, 1)[-1], seed=5))
+    pts = torch.from_numpy(synth.kitti_like(2, 1024, seed=44))
+    o = pkg.train_forward(arch, pkg.params.TrainableParams(d, "cpu"), pts[..., :3].contiguous(), pts[..., 3:].contiguous(),
+                          bn_decay=0.5)
+    assert o.head[0].shape == o.base_xyz.shape[:2] + (1,) and len(o.vote_offsets) == 1
+
+
 TRACE_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "launch_trace.json")
 
 
@@ -432,7 +521,8 @@ def test_launch_trace_matches_recording(dry, oracle_ops, monkeypatch):
     falls back (a FusedStack that no longer fits, a scale that loses its unit list) gives the same numbers but a
     different trace.  Every tf_ops stand-in of the dry fixture logs its name, stream, tensor shapes and scalar and
     keyword arguments; the streams and events log their waits and records.  The dry runs are the 18 route / latency
-    combinations of the backbone test and the training-mode layer.  SSD3D_RECORD_TRACE=<file> writes the traces to
+    combinations of the backbone test, the training-mode layer, the 3DSSD head, PointRCNN's RPN in both modes, the whole
+    PointRCNN forward and backbone.train_forward.  SSD3D_RECORD_TRACE=<file> writes the traces to
     <file> instead of comparing them with tests/golden/launch_trace.json."""
     T = dry.tf_ops
     for k, v in list(vars(T).items()):
@@ -445,6 +535,15 @@ def test_launch_trace_matches_recording(dry, oracle_ops, monkeypatch):
                 lambda r=route, lt=latency, p=parts: test_backbone_orchestration_dry_run_matches_oracle_layers(dry, oracle_ops, lt, p, *r)
     for decay in (None, 0.5):
         runs["training-decay%s" % decay] = lambda d=decay: test_training_mode_orchestration_dry_run_matches_oracle(dry, oracle_ops, d)
+    runs["head-3dssd"] = lambda: test_head_orchestration_dry_run_writes_into_gather_buffers(dry, oracle_ops)
+
+    def scaled(run, *a):
+        with monkeypatch.context() as mp:
+            run(dry, mp, *a)
+    for latency in (False, True):
+        runs["rpn-latency%d" % latency] = lambda lt=latency: scaled(_rpn_dry_run, lt)
+    runs["pointrcnn-forward"] = lambda: scaled(_pointrcnn_dry_run)
+    runs["train-forward"] = lambda: _train_forward_dry_run(dry)
     got = {}
     for key, run in runs.items():
         monkeypatch.setattr(dry.layers_util, "_SIDE_STREAMS", {})

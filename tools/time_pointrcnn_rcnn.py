@@ -79,7 +79,8 @@ def main():
     st = net.stage
 
     def head_decode_nms():
-        cls, reg = net._head(d["ctr"], d["rcnn_feat"][4])
+        feat = d["rcnn_feat"][4].reshape(*d["ctr"].shape[:2], -1).contiguous()
+        _, (cls, reg) = pkg.head.head_convs(net.params, net.head_scope, net.head_bn, net.head_mlp, *T.split_rows(feat))
         boxes, scores = T.decode_bin_anchor_rows(props, reg, cls, d["pool_cnt"], st["HALF_BIN_SEARCH_RANGE"], st["BIN_CLASS_NUM"])
         return T.bev_nms_counted(boxes, scores, pcount, st["NMS_THRESH"], st["MAX_OUTPUT_NUM"])
     res["head_decode_nms_ms"] = timed(head_decode_nms, a.reps, a.warmup)
