@@ -86,11 +86,19 @@ def _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_l
 _SIDE_STREAMS = {}
 
 
-def _side_stream(device, i=0):
-    key = (str(device), i)
+def _side_stream(device, role):
+    """The side stream of `role` on `device` ('hoist', ('fork', i) or ('part', i)), created on first use."""
+    key = (str(device), role)
     if key not in _SIDE_STREAMS:
         _SIDE_STREAMS[key] = torch.cuda.Stream(device=device)
     return _SIDE_STREAMS[key]
+
+
+def _ffps_direct(n, c):
+    """Whether F-FPS over n points of c concatenated channels takes the matrix-free kernel.  The 132-channel variant
+    walks a 131-long dependent fma chain per round: at layer-3 sizes (512 points) the small matrix is faster, so the
+    kernel serves where the matrix is the expensive part (c <= 68, layer 2)."""
+    return c <= 68 and tf_ops.ffps_supported(n, c)
 
 
 def ffps_indices(npoint, xyz, points, mode, out=None, idx_offset=0, cluster=None):
@@ -103,10 +111,7 @@ def ffps_indices(npoint, xyz, points, mode, out=None, idx_offset=0, cluster=None
     xyz / points may be [:, a:b] slices of dense tensors (read in place); out=(buffer, col) / idx_offset as in
     tf_ops.farthest_point_sample; cluster: the 'direct' kernel's CTA cap (tf_ops.farthest_point_sample_features)."""
     if mode == "direct":
-        c = xyz.shape[2] + points.shape[2]
-        # the 132-channel variant walks a 131-long dependent fma chain per round: at layer-3 sizes (512 points) the
-        # small matrix is faster, so 'direct' is used where the matrix is the expensive part (c <= 68, layer 2)
-        if c <= 68 and tf_ops.ffps_supported(xyz.shape[1], c):
+        if _ffps_direct(xyz.shape[1], xyz.shape[2] + points.shape[2]):
             kw = {} if cluster is None else {"cluster": cluster}
             return tf_ops.farthest_point_sample_features(npoint, xyz, points, out=out, idx_offset=idx_offset, **kw)
         mode = "matrix"
@@ -273,6 +278,29 @@ def _group_and_mlp(pp, plan, table, xyz, points, new_xyz, radius_list, nsample_l
     return tf_ops.linear_tc(cat_hi, cat_lo, pp.conv(plan.agg, plan.bn))[0], idx_list, cnt_list
 
 
+def _sampling_segments(n, fps_sample_range_list, fps_method_list, npoint_list, vote_ctr):
+    """The sampling table (:84-111) as segments in launch order, each (kind, lo, hi, npoint, col): kind 'iota', 'F'
+    (F-FPS) or 'D' (D-FPS) picks npoint indices among the rows [lo, hi) into the columns [col, col + npoint) of fps_idx.
+    A fusion-sampling entry is two segments over the same rows: its D-FPS half in the upper columns, listed first so that
+    it is forked before the F-FPS half in the lower columns starts."""
+    segs, last = [], 0
+    for rng, method, npoint in zip(fps_sample_range_list, fps_method_list, npoint_list):
+        lo, hi = last, n if rng == -1 else last + rng             # tf.slice size -1 (:86-87)
+        col = sum(sg[3] for sg in segs)
+        last += rng
+        if npoint == 0:                                           # :88-90
+            continue
+        if vote_ctr is not None:                                  # :91-93
+            segs.append(("iota", lo, hi, vote_ctr.shape[1], col))
+        elif method == "FS":                                      # :94-99 fusion sampling
+            segs += [("D", lo, hi, npoint, col + npoint), ("F", lo, hi, npoint, col)]
+        elif npoint == hi - lo:                                   # :100-101
+            segs.append(("iota", lo, hi, npoint, col))
+        else:                                                     # F-FPS :102-105, D-FPS :106-107
+            segs.append(("F" if method == "F-FPS" else "D", lo, hi, npoint, col))
+    return segs
+
+
 def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_training, bn_decay, bn,
                            fps_sample_range_list, fps_method_list, npoint_list, former_fps_idx, use_attention, scope,
                            dilated_group, vote_ctr=None, aggregation_channel=None, debugging=False, epsilon=1e-5, *,
@@ -286,16 +314,15 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
       fps_bucket   lone D-FPS kernel choice (tf_ops.farthest_point_sample `bucket_kernel`: None automatic, False = cluster kernel);
       fps_packet   D-FPS with the coordinates-in-packet kernel (64 KiB of shared memory per CTA instead of the whole
                    scene: other kernels can share its SMs);
-      fps_parts    latency mode.  FPS emits its samples in order, and a sample is final once its round is done, so the
-                   layer consumes the sampling IN PARTS: a lone D-FPS runs as resumable launches of rounds (an int =
-                   that many equal parts, or a list of fractions), a fusion-sampling layer hands over its F-FPS and
-                   D-FPS halves separately; ball query + grouped MLP + aggregation of a part run on a side stream
-                   while the sampling of the next part continues, and the per-part results are joined at the end.
+      fps_parts    latency mode (inference only).  FPS emits its samples in order, and a sample is final once its round
+                   is done, so the layer consumes the sampling IN PARTS: a lone D-FPS runs as resumable launches of
+                   rounds (an int = that many equal parts, or a list of fractions), an F-FPS of at least 256 samples on
+                   the matrix-free kernel as two, and every other segment is a part of its own; ball query + grouped
+                   MLP + aggregation of a part run on a side stream while the sampling of the next part continues, and
+                   the per-part results are joined at the end.
                    Captured in a CUDA graph this is a plain dependency graph -- nothing polls."""
     if use_attention:
         raise NotImplementedError("query_ball_point_withidx (use_attention) is unused by the shipped 3DSSD configs")
-    if is_training:
-        fps_parts = None                      # training takes the literal layer-by-layer schedule
     if mlp_mode not in ("tc", "fp32"):
         raise ValueError("mlp_mode must be 'tc' or 'fp32'")
     trainable = _trainable(params, is_training)
@@ -305,7 +332,7 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
     dev = xyz.device
     nscale = len(radius_list)
     main = torch.cuda.current_stream()
-    in_parts = bool(fps_parts) and nscale > 0 and former_fps_idx is None
+    in_parts = bool(fps_parts) and nscale > 0 and former_fps_idx is None and not is_training
     keep = []                                  # temporaries shared between streams stay alive until the final join
     use_agg = bool(aggregation and aggregation_channel is not None and aggregation_channel != -1)
 
@@ -316,153 +343,117 @@ def pointnet_sa_module_msg(xyz, points, radius_list, nsample_list, mlp_list, is_
         plan = _route_plan(pp, scope, nsample_list, mlp_list, bn, points.shape[-1], use_agg, mlp_mode, fuse_scale,
                            gather_in_kernel, hoist_first)
         if in_parts and plan.hoisted:          # overlaps the first rounds of the sampling
-            zs = _side_stream(dev, 7)
+            zs = _side_stream(dev, "hoist")
             zs.wait_stream(main)
             with torch.cuda.stream(zs):
                 table = _hoist_table(pp, plan, points)
             z_ready = torch.cuda.Event()
             z_ready.record(zs)
 
-    # ---- sampling (:84-111): every segment writes its indices, segment offset included, straight into fps_idx
-    segs, last = [], 0
-    for rng, method, npoint in zip(fps_sample_range_list, fps_method_list, npoint_list):
-        end = n if rng == -1 else last + rng                      # tf.slice size -1 (:86-87)
-        if npoint == 0:                                           # :88-90
-            last += rng
-            continue
-        if vote_ctr is not None:                                  # :91-93
-            kind, width = "iota", vote_ctr.shape[1]
-        elif method == "FS":                                      # :94-99 fusion sampling
-            kind, width = "FS", 2 * npoint
-        elif npoint == end - last:                                # :100-101
-            kind, width = "iota", npoint
-        elif method == "F-FPS":                                   # :102-105
-            kind, width = "F", npoint
-        else:                                                     # D-FPS :106-107
-            kind, width = "D", npoint
-        segs.append((kind, last, end, npoint, width))
-        last += rng
-    mtot = sum(sg[4] for sg in segs)
-    fps_idx = torch.empty((bs, mtot), dtype=torch.int32, device=dev)
-    parts = []                                 # (col0, col1, event): fps_idx[:, col0:col1] is complete at `event`
-    col, nside = 0, 0
-
-    def on_side(fn):
-        nonlocal nside
-        side = _side_stream(dev, nside)
-        nside += 1
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
-            fn()
-            ev = torch.cuda.Event()
-            ev.record(side)
-        return ev
-
-    def ev_main():
-        ev = torch.cuda.Event()
-        ev.record(main)
-        return ev
-
-    def ffps_segment(npoint, tmp_xyz, tmp_points, lo, col):
-        """F-FPS of one segment; in latency mode the matrix-free kernel runs as two resumable launches, so the first
-        half of its samples is handed to the consumers while the second half is still being picked."""
-        c = tmp_xyz.shape[2] + tmp_points.shape[2]
-        if in_parts and ffps_mode == "direct" and c <= 68 and npoint >= 256 and tf_ops.ffps_supported(tmp_xyz.shape[1], c):
-            temp = torch.empty((bs, tmp_xyz.shape[1]), dtype=torch.float32, device=dev)
+    # ---- sampling (:84-111): every segment writes its indices, segment offset included, straight into its columns of
+    # fps_idx, in one launch or in resumable launches of rounds, on the main stream or forked onto a side stream
+    segs = _sampling_segments(n, fps_sample_range_list, fps_method_list, npoint_list, vote_ctr)
+    fps_idx = torch.empty((bs, sum(sg[3] for sg in segs)), dtype=torch.int32, device=dev)
+    parts, forks = [], []                      # (col0, col1, event): fps_idx[:, col0:col1] is complete at `event`
+    for kind, lo, hi, npoint, col in segs:
+        seg_xyz, seg_points = xyz[:, lo:hi], points[:, lo:hi]      # read in place (scene-strided)
+        st, temp, rounds = main, None, [(0, npoint)]
+        if kind == "D" and len(segs) > 1:
+            # D-FPS next to other segments: independent latency-bound chains on a handful of SMs each, run concurrently
+            st = _side_stream(dev, ("fork", len(forks)))
+            forks.append(st)
+            st.wait_stream(main)
+        # latency mode: the lone D-FPS, and an F-FPS of at least 256 samples on the matrix-free kernel, run as resumable
+        # launches of rounds that carry their state in `temp`, so that earlier samples are consumed while later ones are
+        # still being picked
+        elif kind == "F" and in_parts and ffps_mode == "direct" and npoint >= 256 and \
+                _ffps_direct(seg_xyz.shape[1], seg_xyz.shape[2] + seg_points.shape[2]):
+            temp = torch.empty(seg_xyz.shape[:2], dtype=torch.float32, device=dev)
+            rounds = _part_bounds(npoint, 2)
+        elif kind == "D" and in_parts and not isinstance(fps_parts, bool) and tf_ops.fps_supports_rounds(hi - lo, 3):
+            temp = torch.empty((bs, tf_ops.fps_temp_elems(hi - lo, 3, npoint, bucket_kernel=fps_bucket)),
+                               dtype=torch.float32, device=dev)
+            rounds = _part_bounds(npoint, fps_parts)
+        if temp is not None:
             keep.append(temp)
-            for j0, j1 in _part_bounds(npoint, 2):
-                tf_ops.farthest_point_sample_features(npoint, tmp_xyz, tmp_points, out=(fps_idx, col), idx_offset=lo,
-                                                      rounds=(j0, j1), temp=temp)
-                parts.append((col + j0, col + j1, ev_main()))
-            return
-        ffps_indices(npoint, tmp_xyz, tmp_points, ffps_mode, out=(fps_idx, col), idx_offset=lo,
-                     cluster=fps_cluster if fps_cluster < 0 else None)
-        parts.append((col, col + npoint, ev_main() if in_parts else None))
-
-    lone = len(segs) == 1
-    for kind, lo, hi, npoint, width in segs:
-        tmp_xyz, tmp_points = xyz[:, lo:hi], points[:, lo:hi]     # read in place (scene-strided)
-        if kind == "iota":
-            tf_ops.iota_idx(bs, width, dev, out=(fps_idx, col), start=lo)
-            parts.append((col, col + width, ev_main() if in_parts else None))
-        elif kind == "FS":
-            # F-FPS and D-FPS are independent latency-bound chains on a handful of SMs each: run them concurrently
-            c0 = col
-            ev_d = on_side(lambda: tf_ops.farthest_point_sample(npoint, tmp_xyz, out=(fps_idx, c0 + npoint), idx_offset=lo,
-                                                                cluster=fps_cluster))
-            ffps_segment(npoint, tmp_xyz, tmp_points, lo, col)
-            parts.append((col + npoint, col + 2 * npoint, ev_d))
-        elif kind == "F":
-            ffps_segment(npoint, tmp_xyz, tmp_points, lo, col)
-        elif not lone:                                            # D-FPS segment next to other segments: side stream
-            c0 = col
-            ev_d = on_side(lambda: tf_ops.farthest_point_sample(npoint, tmp_xyz, out=(fps_idx, c0), idx_offset=lo,
-                                                                cluster=fps_cluster))
-            parts.append((col, col + npoint, ev_d))
-        elif in_parts and not isinstance(fps_parts, bool) and tf_ops.fps_supports_rounds(hi - lo, 3):
-            temp = torch.empty((bs, tf_ops.fps_temp_elems(hi - lo, 3, npoint, bucket_kernel=fps_bucket)), dtype=torch.float32, device=dev)
-            keep.append(temp)
-            for j0, j1 in _part_bounds(npoint, fps_parts):
-                tf_ops.farthest_point_sample(npoint, tmp_xyz, out=(fps_idx, col), idx_offset=lo, rounds=(j0, j1), temp=temp,
-                                             cluster=fps_cluster, bucket_kernel=fps_bucket)
-                parts.append((col + j0, col + j1, ev_main()))
-        else:
-            tf_ops.farthest_point_sample(npoint, tmp_xyz, out=(fps_idx, col), idx_offset=lo, cluster=fps_cluster,
-                                         packet_kernel=fps_packet, bucket_kernel=fps_bucket)
-            parts.append((col, col + npoint, ev_main() if in_parts else None))
-        col += width
+        out = (fps_idx, col)
+        with torch.cuda.stream(st):
+            for j0, j1 in rounds:
+                if kind == "iota":
+                    tf_ops.iota_idx(bs, npoint, dev, out=out, start=lo)
+                elif kind == "F" and temp is not None:
+                    tf_ops.farthest_point_sample_features(npoint, seg_xyz, seg_points, out=out, idx_offset=lo,
+                                                          rounds=(j0, j1), temp=temp)
+                elif kind == "F":
+                    ffps_indices(npoint, seg_xyz, seg_points, ffps_mode, out=out, idx_offset=lo,
+                                 cluster=fps_cluster if fps_cluster < 0 else None)
+                elif st is not main:
+                    tf_ops.farthest_point_sample(npoint, seg_xyz, out=out, idx_offset=lo, cluster=fps_cluster)
+                elif temp is not None:
+                    tf_ops.farthest_point_sample(npoint, seg_xyz, out=out, idx_offset=lo, rounds=(j0, j1), temp=temp,
+                                                 cluster=fps_cluster, bucket_kernel=fps_bucket)
+                else:
+                    tf_ops.farthest_point_sample(npoint, seg_xyz, out=out, idx_offset=lo, cluster=fps_cluster,
+                                                 packet_kernel=fps_packet, bucket_kernel=fps_bucket)
+                # final at an event recorded after the launch, or at once in main-stream order
+                ev = None
+                if in_parts or st is not main:
+                    ev = torch.cuda.Event()
+                    ev.record(st)
+                parts.append((col + j0, col + j1, ev))
+    parts.sort(key=lambda p: p[0])             # column order, in which the consumers' results are joined
 
     # ---- the consumers (:113-187).  Latency mode: one per part of the sampling, each on its own stream as soon as its
     # samples are final, joined at the end; otherwise one over every sample on the main stream once the sampling is done
     src_xyz = vote_ctr if vote_ctr is not None else xyz
-    if in_parts:
-        chunks = [(fps_idx[:, c0:c1], ev, _side_stream(dev, 8 + pi)) for pi, (c0, c1, ev) in enumerate(parts)]
-    else:
+    if not in_parts:
         for _, _, ev in parts:
             if ev is not None:
                 main.wait_event(ev)
         if former_fps_idx is not None:
             fps_idx = torch.cat([fps_idx, former_fps_idx], dim=-1).contiguous()    # :113-114
-        chunks = [(fps_idx, None, main)]
-    xyz_parts, pts_parts, found, done = [], [], [], []
-    for sel, ev, st in chunks:
-        if in_parts:
-            st.wait_event(ev)
-            if plan.hoisted:
-                st.wait_event(z_ready)
-        with torch.cuda.stream(st):
-            nx = tf_ops.gather_point(src_xyz, sel)                                 # :116-119
-            dbg = {"idx": [], "cnt": []}
-            if not nscale:
-                npnts = tf_ops.gather_point(points.contiguous(), sel)              # :186-187
-            elif is_training:
-                npnts, idx, cnt, convs = _group_and_mlp_train(pp, scope, xyz, points, nx, radius_list, nsample_list, mlp_list,
-                                                              bn, bn_decay, dilated_group, use_agg)
-                dbg = {"idx": idx, "cnt": cnt} if convs is None else {"idx": idx, "cnt": cnt, "convs": convs}
-            else:
+        parts = [(0, fps_idx.shape[1], None)]
+    if not nscale:
+        new_xyz = tf_ops.gather_point(src_xyz, fps_idx)                            # :116-119
+        new_points, debug = tf_ops.gather_point(points.contiguous(), fps_idx), {"idx": [], "cnt": []}   # :186-187
+    elif is_training:
+        new_xyz = tf_ops.gather_point(src_xyz, fps_idx)
+        new_points, idx, cnt, convs = _group_and_mlp_train(pp, scope, xyz, points, new_xyz, radius_list, nsample_list,
+                                                           mlp_list, bn, bn_decay, dilated_group, use_agg)
+        debug = {"idx": idx, "cnt": cnt} if convs is None else {"idx": idx, "cnt": cnt, "convs": convs}
+    else:
+        xyz_parts, pts_parts, found, done = [], [], [], []
+        for pi, (c0, c1, ev) in enumerate(parts):
+            st = main
+            if in_parts:
+                st = _side_stream(dev, ("part", pi))
+                st.wait_event(ev)
+                if plan.hoisted:
+                    st.wait_event(z_ready)
+            with torch.cuda.stream(st):
+                nx = tf_ops.gather_point(src_xyz, fps_idx[:, c0:c1])
                 if not in_parts:
                     table = _hoist_table(pp, plan, points)
                 npnts, idx, cnt = _group_and_mlp(pp, plan, table, xyz, points, nx, radius_list, nsample_list, mlp_list,
                                                  dilated_group)
-                dbg = {"idx": idx, "cnt": cnt}
-            if in_parts:
-                done.append(torch.cuda.Event())
-                done[-1].record(st)
-        xyz_parts.append(nx); pts_parts.append(npnts); found.append(dbg)
-    if not in_parts:
-        new_xyz, new_points, debug = xyz_parts[0], pts_parts[0], found[0]
-    else:
-        for e2 in done:
-            main.wait_event(e2)
-        for i in range(nside):
-            main.wait_stream(_side_stream(dev, i))
-        new_xyz = tf_ops.concat_rows(xyz_parts)
-        new_points = tf_ops.concat_rows(pts_parts)
-        keep.extend(xyz_parts + pts_parts)
-        if return_debug:
-            debug = {k: [torch.cat([f[k][i] for f in found], dim=1) for i in range(nscale)] for k in ("idx", "cnt")}
-        _KEEPALIVE.append((keep, found if not return_debug else None, table))
-        del _KEEPALIVE[:-8]
+                if in_parts:
+                    done.append(torch.cuda.Event())
+                    done[-1].record(st)
+            xyz_parts.append(nx); pts_parts.append(npnts); found.append({"idx": idx, "cnt": cnt})
+        if not in_parts:
+            new_xyz, new_points, debug = xyz_parts[0], pts_parts[0], found[0]
+        else:
+            for e in done:
+                main.wait_event(e)
+            for s in forks:
+                main.wait_stream(s)
+            new_xyz = tf_ops.concat_rows(xyz_parts)
+            new_points = tf_ops.concat_rows(pts_parts)
+            keep.extend(xyz_parts + pts_parts)
+            if return_debug:
+                debug = {k: [torch.cat([f[k][i] for f in found], dim=1) for i in range(nscale)] for k in ("idx", "cnt")}
+            _KEEPALIVE.append((keep, found if not return_debug else None, table))
+            del _KEEPALIVE[:-8]
     if return_debug:
         return new_xyz, new_points, fps_idx, debug
     return new_xyz, new_points, fps_idx

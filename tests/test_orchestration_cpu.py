@@ -77,7 +77,10 @@ def dry(monkeypatch, oracle_ops):
             assert temp is not None and temp.shape == (inp.shape[0], 2 * inp.shape[1])      # fps_temp_elems of the fake
         return place(o.farthest_point_sample(npoint, n(inp)), out, idx_offset, inp.shape[0], npoint, rounds)
 
-    def ffps(npoint, xyz, points=None, *, out=None, idx_offset=0, rounds=None, temp=None):
+    def ffps(npoint, xyz, points=None, *, out=None, idx_offset=0, rounds=None, temp=None, **kw):
+        assert set(kw) <= {"cluster"}                                # the real wrapper's CTA cap changes no index
+        if rounds is not None and tuple(rounds) != (0, npoint):
+            assert temp is not None and temp.shape == xyz.shape[:2]
         f = n(xyz) if points is None else np.concatenate([n(xyz), n(points)], -1)
         return place(o.farthest_point_sample_with_distance(npoint, o.calc_square_dist(f)), out, idx_offset, xyz.shape[0], npoint, rounds)
 
@@ -351,16 +354,28 @@ _LATENCY = [(False, None), (True, 2), (True, [0.5, 0.25, 0.25])]
 @pytest.mark.parametrize("mlp_mode,gather,hoist,fuse", _ROUTES)
 @pytest.mark.parametrize("latency,parts", _LATENCY)
 def test_backbone_orchestration_dry_run_matches_oracle_layers(dry, oracle_ops, latency, parts, mlp_mode, gather, hoist, fuse):
-    pkg = dry
+    kw = dict(fps_parts=parts) if parts is not None else {}
+    _backbone_dry_run(dry, _scaled(dry, 16), mlp_mode=mlp_mode, latency_mode=latency, gather_in_kernel=gather,
+                      hoist_first=hoist, fuse_scale=fuse, **kw)     # 1024 -> 256 -> 64+.. centres
+
+
+# two SA layers on the 1024 input points whose F-FPS samples 256 points on 4 channels: in latency mode the matrix-free
+# kernel hands over its two halves separately, next to a D-FPS half (fusion sampling) or a D-FPS segment on a side stream
+_HALVES = [[[0], [0], [0.4, 0.8], [16, 32], [[16, 16, 32], [16, 32, 48]], True, [-1], ['FS'], [256],
+            -1, False, 'SA_Layer', 'fs', True, -1, 64],
+           [[0], [0], [0.4, 0.8], [16, 32], [[16, 16, 32], [16, 32, 48]], True, [512, -1], ['F-FPS', 'D-FPS'], [256, 256],
+            -1, False, 'SA_Layer', 'fd', True, -1, 64]]
+
+
+def _backbone_dry_run(pkg, arch, **net_kw):
+    """SABackbone(arch, **net_kw).forward on two 1024-point scenes against the oracle's layers: every layer's fps_idx,
+    ball-query indices, xyz and features."""
     from oracle import layers as olayers
     synth = importlib.import_module("3dssd_b200.synth")
-    arch = _scaled(pkg, 16)                                       # 1024 -> 256 -> 64+.. centres
     params = pkg.params.init_params(arch, 1, seed=4, random_bias=True)
     pts = synth.kitti_like(2, 1024, seed=40)
     pts[..., 0] *= 0.2; pts[..., 2] *= 0.2
-    kw = dict(fps_parts=parts) if parts is not None else {}
-    net = pkg.SABackbone(arch, params, in_channels=1, device="cpu", mlp_mode=mlp_mode, latency_mode=latency,
-                         gather_in_kernel=gather, hoist_first=hoist, fuse_scale=fuse, **kw)
+    net = pkg.SABackbone(arch, params, in_channels=1, device="cpu", **net_kw)
     got = net.forward(torch.from_numpy(pts), return_debug=True)
     exp = olayers.backbone_forward(arch, pts, params, ffps_mode="matrix", return_debug=True)
     for li in range(1, len(arch) + 1):
@@ -511,7 +526,9 @@ def _traced(name, fn):
     def call(*a, **k):
         b = sig.bind(*a, **k)
         b.apply_defaults()
-        _log("%s@%s %s" % (name, _SYNC["stack"][-1].name, " ".join("%s=%s" % (p, _describe(v)) for p, v in b.arguments.items())))
+        # a **kwargs parameter shows only the keywords actually passed
+        args = [(p, v) for p, v in b.arguments.items() if sig.parameters[p].kind != inspect.Parameter.VAR_KEYWORD or v]
+        _log("%s@%s %s" % (name, _SYNC["stack"][-1].name, " ".join("%s=%s" % (p, _describe(v)) for p, v in args)))
         return fn(*a, **k)
     return call
 
@@ -522,7 +539,8 @@ def test_launch_trace_matches_recording(dry, oracle_ops, monkeypatch):
     different trace.  Every tf_ops stand-in of the dry fixture logs its name, stream, tensor shapes and scalar and
     keyword arguments; the streams and events log their waits and records.  The dry runs are the 18 route / latency
     combinations of the backbone test, the training-mode layer, the 3DSSD head, PointRCNN's RPN in both modes, the whole
-    PointRCNN forward and backbone.train_forward.  SSD3D_RECORD_TRACE=<file> writes the traces to
+    PointRCNN forward, backbone.train_forward, the throughput backbone with fps_cluster=-4, with the packet and with the
+    bucket D-FPS kernel, and latency mode on F-FPS segments of 256 samples.  SSD3D_RECORD_TRACE=<file> writes the traces to
     <file> instead of comparing them with tests/golden/launch_trace.json."""
     T = dry.tf_ops
     for k, v in list(vars(T).items()):
@@ -544,6 +562,12 @@ def test_launch_trace_matches_recording(dry, oracle_ops, monkeypatch):
         runs["rpn-latency%d" % latency] = lambda lt=latency: scaled(_rpn_dry_run, lt)
     runs["pointrcnn-forward"] = lambda: scaled(_pointrcnn_dry_run)
     runs["train-forward"] = lambda: _train_forward_dry_run(dry)
+    # the FPS options of bench.py's throughput step (fps_cluster=-4, automatic layer-1 kernel), the two other lone D-FPS
+    # kernels, and the F-FPS halves of latency mode
+    runs["backbone-throughput-cluster-4"] = lambda: _backbone_dry_run(dry, _scaled(dry, 16), fps_cluster=-4)
+    runs["backbone-fps-packet"] = lambda: _backbone_dry_run(dry, _scaled(dry, 16), fps_packet=True)
+    runs["backbone-fps-bucket"] = lambda: _backbone_dry_run(dry, _scaled(dry, 16), fps_bucket=True)
+    runs["backbone-ffps-halves-latency1"] = lambda: _backbone_dry_run(dry, _HALVES, latency_mode=True)
     got = {}
     for key, run in runs.items():
         monkeypatch.setattr(dry.layers_util, "_SIDE_STREAMS", {})
