@@ -66,6 +66,7 @@ _SIGNATURES = {
     "ssd3d_three_interpolate_grad": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_bev_nms": [c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "ssd3d_bev_nms_counted": [c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "ssd3d_bev_nms_classes": [c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p, c_void_p, c_void_p],
     "ssd3d_query_boxes_3d_points": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_region_pool_smem": [c_int, c_int, c_int],
     "ssd3d_region_pool": [c_int] * 6 + [c_void_p] * 4 + [c_int, c_void_p, c_float, c_float] + [c_void_p] * 8,
@@ -96,6 +97,8 @@ _SIGNATURES = {
     "ssd3d_vote_translate": [c_long, c_void_p, c_void_p, c_int, c_float, c_float, c_float, c_void_p, c_void_p],
     "ssd3d_decode_dist_anchor_free": [c_long, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                       c_void_p],
+    "ssd3d_decode_dist_anchor_free_classes": [c_long, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                              c_void_p, c_void_p],
     "ssd3d_decode_bin_anchor": [c_long, c_int, c_float, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                 c_void_p, c_void_p],
     "ssd3d_linear_wgrad_workspace": [c_long, c_int, c_int],
@@ -109,12 +112,19 @@ _SIGNATURES = {
                                 c_void_p],
     "ssd3d_vote_translate_grad": [c_long, c_void_p, c_int, c_void_p, c_float, c_float, c_float, c_void_p, c_void_p],
     "ssd3d_det_assign": [c_int, c_int, c_int, c_int, c_int] + [c_void_p] * 15,
+    "ssd3d_det_assign_classes": [c_int, c_int, c_int, c_int, c_int, c_int] + [c_void_p] * 15,
     "ssd3d_det_loss_workspace": [c_int],
     "ssd3d_det_loss": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
                        c_void_p, c_int] + [c_void_p] * 12,
     "ssd3d_det_loss_grad": [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
                             c_int, c_void_p, c_int] + [c_void_p] * 11 + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
                                                                          c_void_p, c_int, c_void_p, c_void_p],
+    "ssd3d_det_loss_classes": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
+                               c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 12,
+    "ssd3d_det_loss_grad_classes": [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
+                                    c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 11 + [c_void_p, c_int, c_void_p, c_int,
+                                                                                          c_void_p, c_int, c_void_p, c_int,
+                                                                                          c_void_p, c_void_p],
     "ssd3d_grad_clip_scale_workspace": [c_long],
     "ssd3d_grad_clip_scale": [c_void_p, c_long, c_float, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_peer_allreduce_resident_ctas": [],

@@ -112,6 +112,9 @@ class SABackbone:
         NMS writes into its send buffer and ncclAllGather is captured with the kernels) into one CUDA graph.  Returns
         replay(points=None) -> (forward outputs, (block, count)); with `gather` the pair holds this rank's views of the
         send buffer and gather.result() / gather.raw hold all ranks' detections after the replay."""
+        if gather is not None and self.head is not None and gather.max_output != self.head.max_output:
+            raise ValueError("capture: the gather carries %d rows per scene, the head writes %d (max_output = classes x %d)"
+                             % (gather.max_output, self.head.max_output, self.head.stage["MAX_OUTPUT_NUM"]))
         out_buf = gather.out() if gather is not None else None
 
         def step(points):
@@ -211,11 +214,13 @@ def train_forward(arch, tp, xyz, feat, *, bn_decay=None):
     """The backbone loop of SABackbone.forward in training mode (SA and vote layers, batch-statistics BatchNorm) with
     params.TrainableParams, then conv1d_0 and the box-regression head of the 3DSSD head on the last layer's features
     (single_stage_detector.py:115-125, head_builder.py:81-114).  Everything is differentiable w.r.t. tp's parameters.
+    The head has as many class channels as tp's pred_cls/weights has columns.
     bn_decay: the decay of every BatchNorm's moving statistics in this forward (model_forward(bn_decay),
     trainer.py:130; solver.Solver.bn_decay gives the scheduled value); None keeps the layers' default of 0.9."""
     from . import head as _head
     xyz_l, feat_l, _, dbg = run_layers(arch, [xyz], [feat], tp, True, bn_decay)
     votes = [(spec[0][0], d["offsets"]) for spec, d in zip(arch, dbg) if spec[11] == "Vote_Layer"]
     f = tp.conv_train("conv1d_0", feat_l[-1], True, bn_decay)
-    return TrainOutputs(_head.box_regression_head(f, 1, 1, 6, True, True, params=tp, bn_decay=bn_decay), [o for _, o in votes],
+    cls = tp.tensors["pred_cls/weights"].shape[1]
+    return TrainOutputs(_head.box_regression_head(f, cls, 1, 6, True, True, params=tp, bn_decay=bn_decay), [o for _, o in votes],
                         xyz_l[-1], xyz_l[votes[-1][0]] if votes else None)   # vote_base: PRED_VOTE_BASE (layer_builder.py:96)

@@ -67,6 +67,30 @@ ARCH_POINTRCNN_RPN = [
 ]
 AGGREGATION_POINTRCNN = False      # MODEL.NETWORK.AGGREGATION_SA_FEATURE (tiny_pointrcnn_stage1.yaml:45)
 
+# The class list of the single-stage model (DATASET.KITTI.CLS_LIST): label k is the 1-based place of the class in the
+# list, 0 is padding.  The valid names are the eight KITTI keys of g_type_mean_size (lib/utils/model_util.py:19-26),
+# with their mean (l, h, w) in metres.
+CLS_LIST = ('Car',)
+CLASS_MEAN_SIZE = {
+    'Car': (3.88311640418, 1.62856739989, 1.52563191462), 'Van': (5.06763659, 1.9007158, 2.20532825),
+    'Truck': (10.13586957, 2.58549199, 3.2520595), 'Pedestrian': (0.84422524, 1.76255119, 0.66068622),
+    'Person_sitting': (0.80057803, 1.27450867, 0.5983815), 'Cyclist': (1.76282397, 1.73698127, 0.59706367),
+    'Tram': (16.17150617, 2.53246914, 3.53079012), 'Misc': (3.64300781, 1.54298177, 1.92320313),
+}
+
+
+def check_cls_list(cls_list):
+    """A class list as a tuple of names: a comma-separated string or a sequence of 1..8 distinct names of
+    CLASS_MEAN_SIZE.  Anything else raises ValueError."""
+    names = tuple(c.strip() for c in cls_list.split(",")) if isinstance(cls_list, str) else tuple(cls_list)
+    bad = [c for c in names if c not in CLASS_MEAN_SIZE]
+    if bad:
+        raise ValueError("unknown class name(s) %s; the valid names are %s" % (bad, ", ".join(CLASS_MEAN_SIZE)))
+    if not 1 <= len(names) <= len(CLASS_MEAN_SIZE) or len(set(names)) != len(names):
+        raise ValueError("a class list holds 1..%d distinct names, got %r" % (len(CLASS_MEAN_SIZE), names))
+    return names
+
+
 # Detection heads: (xyz_index, feature_index, op_type, mlp_list, bn, layer_type, scope), with the MODEL.FIRST_STAGE
 # constants that select and parametrise their regression and post-processing.
 HEAD_3DSSD = [[6], [6], 'conv1d', [128], True, 'Det', '']                     # 3dssd.yaml:68

@@ -7,7 +7,9 @@
 //                    'Dist-Anchor-free' regression, the corner loss and the vote loss: per-scene partial sums in double,
 //                    then one fixed-order sum over the scenes
 //   det_loss_grad    their gradients w.r.t. the head outputs, the candidate points and the raw vote offsets
-// No float atomics anywhere: every run gives the same bits.
+// Each takes a class count C (the *_classes entry points, DESIGN.md section 3.17; the single-class ones are C = 1): the
+// targets stay class-agnostic but the centre-ness label, which goes to column label - 1 of [rows, C]; the classification
+// loss is the class mean of the sigmoid cross-entropy.  No float atomics anywhere: every run gives the same bits.
 #include <math.h>
 
 #include "box_geom.cuh"
@@ -58,7 +60,7 @@ __device__ __forceinline__ bool box_valid(const float *b)
 }
 
 __global__ void __launch_bounds__(kDetThreads) det_assign_kernel(
-    int n, int nv, int g, int nbins, const float *__restrict__ base, const float *__restrict__ vbase,
+    int n, int nv, int g, int nbins, int ncls, const float *__restrict__ base, const float *__restrict__ vbase,
     const float *__restrict__ boxes, const int *__restrict__ labels, int *__restrict__ a_idx, float *__restrict__ a_box,
     float *__restrict__ pmask, float *__restrict__ nmask, float *__restrict__ cls_label, int *__restrict__ a_bin,
     float *__restrict__ a_res, float *__restrict__ off_t, float *__restrict__ vmask, float *__restrict__ vtarget)
@@ -107,7 +109,8 @@ __global__ void __launch_bounds__(kDetThreads) det_assign_kernel(
             const float dist = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
             const bool pos = hit >= 0 && dist <= kSampleRange;
             float label = 0.f;
-            if (pos && labels[(size_t)s * g + a] == 1) {                       // one_hot(label - 1) of the one class
+            const int lab = pos ? labels[(size_t)s * g + a] : 0;
+            if (lab >= 1 && lab <= ncls) {                                      // one_hot(label - 1, ncls): column lab - 1
                 // centre-ness (loss_builder.py:99-137) in double, rounded once
                 const double ry = bx[6], c = cos(ry), sn = sin(ry);
                 const double ex = (double)t[0] - bx[0], ey = (double)t[1] - bx[1], ez = (double)t[2] - bx[2];
@@ -124,7 +127,7 @@ __global__ void __launch_bounds__(kDetThreads) det_assign_kernel(
             for (int k = 0; k < 7; k++) a_box[r * 7 + k] = bx[k];
             pmask[r] = pos ? 1.f : 0.f;
             nmask[r] = hit < 0 ? 1.f : 0.f;
-            cls_label[r] = label;
+            for (int c = 0; c < ncls; c++) cls_label[r * ncls + c] = c == lab - 1 ? label : 0.f;
             a_bin[r] = bin;
             a_res[r] = res;
             float *o = off_t + r * 6;
@@ -154,6 +157,7 @@ __global__ void __launch_bounds__(kDetThreads) det_assign_kernel(
 struct LossIn {
     const float *base, *cls, *off, *acls, *ares, *vote;
     int ld_cls, ld_off, ld_acls, ld_ares, ld_vote;
+    int ncls;                     // classification columns: pred_cls columns 0:ncls, label [rows, ncls]
     const float *box, *pmask, *nmask, *label, *res, *vmask, *vtarget;
     const int *bin;
 };
@@ -216,8 +220,12 @@ __global__ void __launch_bounds__(kDetThreads) det_loss_partial_kernel(int n, in
     for (int p = threadIdx.x; p < n; p += blockDim.x) {
         const size_t r = (size_t)s * n + p;
         const double pm = in.pmask[r], cm = pm + in.nmask[r];
-        const double x = in.cls[r * in.ld_cls], z = in.label[r];
-        acc[0] += (fmax(x, 0.0) - x * z + log1p(exp(-fabs(x)))) * cm;            // sigmoid_cross_entropy_with_logits
+        double ce = 0.0;                                                          // sigmoid_cross_entropy_with_logits
+        for (int c = 0; c < in.ncls; c++) {
+            const double x = in.cls[r * in.ld_cls + c], z = in.label[r * in.ncls + c];
+            ce += fmax(x, 0.0) - x * z + log1p(exp(-fabs(x)));
+        }
+        acc[0] += ce / in.ncls * cm;                                              // the mean over the classes
         const float *o = in.off + r * in.ld_off;
         float t[6];
         target_of(in, r, t);
@@ -294,8 +302,10 @@ __global__ void __launch_bounds__(kDetThreads) det_loss_grad_kernel(int b, int n
         const double pm = in.pmask[r], cm = pm + in.nmask[r];
         const double s_cls = (double)gl[0] / norm[0], s_off = (double)gl[1] / norm[1], s_bin = (double)gl[2] / norm[1],
                      s_res = (double)gl[3] / norm[1], s_cor = (double)gl[4] / norm[1];
-        const double x = in.cls[r * in.ld_cls];
-        gcls[r * ldgc] = cm != 0.0 ? (float)((1.0 / (1.0 + exp(-x)) - in.label[r]) * cm * s_cls) : 0.f;
+        for (int c = 0; c < in.ncls; c++) {
+            const double x = in.cls[r * in.ld_cls + c];
+            gcls[r * ldgc + c] = cm != 0.0 ? (float)((1.0 / (1.0 + exp(-x)) - in.label[r * in.ncls + c]) * cm * s_cls / in.ncls) : 0.f;
+        }
         const float *o = in.off + r * in.ld_off;
         float t[6];
         target_of(in, r, t);
@@ -360,54 +370,77 @@ static double bin_interval(int nbins) { return (double)(float)(2.0 * M_PI / nbin
 
 using namespace ssd3d;
 
+static int det_assign(const char *op, int b, int n, int nv, int g, int angle_bins, int cls_num, const float *base_xyz,
+                      const float *vote_base, const float *gt_boxes, const int *gt_labels, int *assigned_idx, float *assigned_box,
+                      float *pmask, float *nmask, float *cls_label, int *angle_bin, float *angle_res, float *offset_target,
+                      float *vote_mask, float *vote_target, ssd3d_stream_t stream)
+{
+    SSD3D_REQUIRE(b >= 0 && n >= 0 && nv >= 0 && g >= 0 && angle_bins >= 1 && angle_bins <= kMaxBins && cls_num >= 1 &&
+                  cls_num <= SSD3D_MAX_CLASSES, "%s: bad shape b=%d n=%d nv=%d g=%d bins=%d classes=%d", op, b, n, nv, g,
+                  angle_bins, cls_num);
+    if (b == 0 || (n == 0 && nv == 0)) return 0;
+    SSD3D_REQUIRE((n == 0 || (base_xyz && assigned_idx && assigned_box && pmask && nmask && cls_label && angle_bin && angle_res &&
+                              offset_target)) && (nv == 0 || (vote_base && vote_mask && vote_target)) &&
+                  (g == 0 || (gt_boxes && gt_labels)), "%s: null pointer", op);
+    det_assign_kernel<<<b, kDetThreads, 0, (cudaStream_t)stream>>>(n, nv, g, angle_bins, cls_num, base_xyz, vote_base, gt_boxes,
+                                                                   gt_labels, assigned_idx, assigned_box, pmask, nmask, cls_label,
+                                                                   angle_bin, angle_res, offset_target, vote_mask, vote_target);
+    SSD3D_LAUNCH_CHECK("det_assign_kernel");
+}
+
 extern "C" int ssd3d_det_assign(int b, int n, int nv, int g, int angle_bins, const float *base_xyz, const float *vote_base,
                                 const float *gt_boxes, const int *gt_labels, int *assigned_idx, float *assigned_box,
                                 float *pmask, float *nmask, float *cls_label, int *angle_bin, float *angle_res,
                                 float *offset_target, float *vote_mask, float *vote_target, ssd3d_stream_t stream)
 {
-    SSD3D_REQUIRE(b >= 0 && n >= 0 && nv >= 0 && g >= 0 && angle_bins >= 1 && angle_bins <= kMaxBins,
-                  "det_assign: bad shape b=%d n=%d nv=%d g=%d bins=%d", b, n, nv, g, angle_bins);
-    if (b == 0 || (n == 0 && nv == 0)) return 0;
-    SSD3D_REQUIRE((n == 0 || (base_xyz && assigned_idx && assigned_box && pmask && nmask && cls_label && angle_bin && angle_res &&
-                              offset_target)) && (nv == 0 || (vote_base && vote_mask && vote_target)) &&
-                  (g == 0 || (gt_boxes && gt_labels)), "det_assign: null pointer");
-    det_assign_kernel<<<b, kDetThreads, 0, (cudaStream_t)stream>>>(n, nv, g, angle_bins, base_xyz, vote_base, gt_boxes, gt_labels,
-                                                                   assigned_idx, assigned_box, pmask, nmask, cls_label, angle_bin,
-                                                                   angle_res, offset_target, vote_mask, vote_target);
-    SSD3D_LAUNCH_CHECK("det_assign_kernel");
+    return det_assign("det_assign", b, n, nv, g, angle_bins, 1, base_xyz, vote_base, gt_boxes, gt_labels, assigned_idx,
+                      assigned_box, pmask, nmask, cls_label, angle_bin, angle_res, offset_target, vote_mask, vote_target, stream);
+}
+
+extern "C" int ssd3d_det_assign_classes(int b, int n, int nv, int g, int angle_bins, int cls_num, const float *base_xyz,
+                                        const float *vote_base, const float *gt_boxes, const int *gt_labels, int *assigned_idx,
+                                        float *assigned_box, float *pmask, float *nmask, float *cls_label, int *angle_bin,
+                                        float *angle_res, float *offset_target, float *vote_mask, float *vote_target,
+                                        ssd3d_stream_t stream)
+{
+    return det_assign("det_assign_classes", b, n, nv, g, angle_bins, cls_num, base_xyz, vote_base, gt_boxes, gt_labels,
+                      assigned_idx, assigned_box, pmask, nmask, cls_label, angle_bin, angle_res, offset_target, vote_mask,
+                      vote_target, stream);
 }
 
 extern "C" size_t ssd3d_det_loss_workspace(int b) { return (size_t)(b > 0 ? b : 0) * 9 * sizeof(double); }
 
-static int det_loss_in(int n, int nv, int angle_bins, const float *base_xyz, const float *pred_cls, int ld_cls,
+static int det_loss_in(int n, int nv, int angle_bins, int cls_num, const float *base_xyz, const float *pred_cls, int ld_cls,
                        const float *pred_offset, int ld_offset, const float *pred_angle_cls, int ld_angle_cls,
                        const float *pred_angle_res, int ld_angle_res, const float *vote_offset, int ld_vote,
                        const float *assigned_box, const float *pmask, const float *nmask, const float *cls_label,
                        const int *angle_bin, const float *angle_res, const float *vote_mask,
                        const float *vote_target, LossIn &in)
 {
-    SSD3D_REQUIRE(angle_bins >= 1 && angle_bins <= kMaxBins && ld_cls >= 1 && ld_offset >= 6 && ld_angle_cls >= angle_bins &&
+    SSD3D_REQUIRE(cls_num >= 1 && cls_num <= SSD3D_MAX_CLASSES, "det_loss: bad class count %d", cls_num);
+    SSD3D_REQUIRE(angle_bins >= 1 && angle_bins <= kMaxBins && ld_cls >= cls_num && ld_offset >= 6 && ld_angle_cls >= angle_bins &&
                   ld_angle_res >= angle_bins && ld_vote >= 3, "det_loss: bad row strides or bins=%d", angle_bins);
     SSD3D_REQUIRE(n == 0 || (base_xyz && pred_cls && pred_offset && pred_angle_cls && pred_angle_res && assigned_box && pmask &&
                              nmask && cls_label && angle_bin && angle_res), "det_loss: null pointer");
     SSD3D_REQUIRE(nv == 0 || (vote_offset && vote_mask && vote_target), "det_loss: null pointer");
     in = LossIn{base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, ld_cls, ld_offset, ld_angle_cls,
-                ld_angle_res, ld_vote, assigned_box, pmask, nmask, cls_label, angle_res, vote_mask, vote_target,
+                ld_angle_res, ld_vote, cls_num, assigned_box, pmask, nmask, cls_label, angle_res, vote_mask, vote_target,
                 angle_bin};
     return 0;
 }
 
-extern "C" int ssd3d_det_loss(int b, int n, int nv, int angle_bins, const float *base_xyz, const float *pred_cls, int ld_cls,
-                              const float *pred_offset, int ld_offset, const float *pred_angle_cls, int ld_angle_cls,
-                              const float *pred_angle_res, int ld_angle_res, const float *vote_offset, int ld_vote,
-                              const float *assigned_box, const float *pmask, const float *nmask, const float *cls_label,
-                              const int *angle_bin, const float *angle_res, const float *vote_mask,
-                              const float *vote_target, void *workspace, float *loss, float *norm, ssd3d_stream_t stream)
+extern "C" int ssd3d_det_loss_classes(int b, int n, int nv, int angle_bins, int cls_num, const float *base_xyz,
+                                      const float *pred_cls, int ld_cls, const float *pred_offset, int ld_offset,
+                                      const float *pred_angle_cls, int ld_angle_cls, const float *pred_angle_res, int ld_angle_res,
+                                      const float *vote_offset, int ld_vote, const float *assigned_box, const float *pmask,
+                                      const float *nmask, const float *cls_label, const int *angle_bin, const float *angle_res,
+                                      const float *vote_mask, const float *vote_target, void *workspace, float *loss, float *norm,
+                                      ssd3d_stream_t stream)
 {
     SSD3D_REQUIRE(b >= 1 && n >= 0 && nv >= 0, "det_loss: bad shape b=%d n=%d nv=%d", b, n, nv);
     SSD3D_REQUIRE(workspace && loss && norm, "det_loss: null pointer");
     LossIn in;
-    const int st = det_loss_in(n, nv, angle_bins, base_xyz, pred_cls, ld_cls, pred_offset, ld_offset, pred_angle_cls, ld_angle_cls,
+    const int st = det_loss_in(n, nv, angle_bins, cls_num, base_xyz, pred_cls, ld_cls, pred_offset, ld_offset, pred_angle_cls, ld_angle_cls,
                                pred_angle_res, ld_angle_res, vote_offset, ld_vote, assigned_box, pmask, nmask, cls_label, angle_bin,
                                angle_res, vote_mask, vote_target, in);
     if (st) return st;
@@ -417,6 +450,47 @@ extern "C" int ssd3d_det_loss(int b, int n, int nv, int angle_bins, const float 
     if (e) return e;
     det_loss_final_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(b, (const double *)workspace, loss, norm);
     SSD3D_LAUNCH_CHECK("det_loss_final_kernel");
+}
+
+extern "C" int ssd3d_det_loss_grad_classes(int b, int n, int nv, int angle_bins, int cls_num, const float *base_xyz,
+                                           const float *pred_cls, int ld_cls, const float *pred_offset, int ld_offset,
+                                           const float *pred_angle_cls, int ld_angle_cls, const float *pred_angle_res,
+                                           int ld_angle_res, const float *vote_offset, int ld_vote, const float *assigned_box,
+                                           const float *pmask, const float *nmask, const float *cls_label, const int *angle_bin,
+                                           const float *angle_res, const float *vote_mask, const float *vote_target,
+                                           const float *grad_loss, const float *norm, float *grad_base_xyz, float *grad_cls,
+                                           int ldg_cls, float *grad_offset, int ldg_offset, float *grad_angle_cls,
+                                           int ldg_angle_cls, float *grad_angle_res, int ldg_angle_res, float *grad_vote_offset,
+                                           ssd3d_stream_t stream)
+{
+    SSD3D_REQUIRE(b >= 0 && n >= 0 && nv >= 0, "det_loss_grad: bad shape b=%d n=%d nv=%d", b, n, nv);
+    SSD3D_REQUIRE(ldg_cls >= cls_num && ldg_offset >= 6 && ldg_angle_cls >= angle_bins && ldg_angle_res >= angle_bins,
+                  "det_loss_grad: bad gradient row strides");
+    const long rows = (long)b * (n > nv ? n : nv);
+    if (rows == 0) return 0;
+    SSD3D_REQUIRE(grad_loss && norm && (n == 0 || (grad_base_xyz && grad_cls && grad_offset && grad_angle_cls && grad_angle_res)) &&
+                  (nv == 0 || grad_vote_offset), "det_loss_grad: null pointer");
+    LossIn in;
+    const int st = det_loss_in(n, nv, angle_bins, cls_num, base_xyz, pred_cls, ld_cls, pred_offset, ld_offset, pred_angle_cls, ld_angle_cls,
+                               pred_angle_res, ld_angle_res, vote_offset, ld_vote, assigned_box, pmask, nmask, cls_label, angle_bin,
+                               angle_res, vote_mask, vote_target, in);
+    if (st) return st;
+    det_loss_grad_kernel<<<ceil_div(rows, kDetThreads), kDetThreads, 0, (cudaStream_t)stream>>>(
+        b, n, nv, angle_bins, bin_interval(angle_bins), in, grad_loss, norm, grad_base_xyz, grad_cls, ldg_cls, grad_offset, ldg_offset,
+        grad_angle_cls, ldg_angle_cls, grad_angle_res, ldg_angle_res, grad_vote_offset);
+    SSD3D_LAUNCH_CHECK("det_loss_grad_kernel");
+}
+
+extern "C" int ssd3d_det_loss(int b, int n, int nv, int angle_bins, const float *base_xyz, const float *pred_cls, int ld_cls,
+                              const float *pred_offset, int ld_offset, const float *pred_angle_cls, int ld_angle_cls,
+                              const float *pred_angle_res, int ld_angle_res, const float *vote_offset, int ld_vote,
+                              const float *assigned_box, const float *pmask, const float *nmask, const float *cls_label,
+                              const int *angle_bin, const float *angle_res, const float *vote_mask,
+                              const float *vote_target, void *workspace, float *loss, float *norm, ssd3d_stream_t stream)
+{
+    return ssd3d_det_loss_classes(b, n, nv, angle_bins, 1, base_xyz, pred_cls, ld_cls, pred_offset, ld_offset, pred_angle_cls,
+                                  ld_angle_cls, pred_angle_res, ld_angle_res, vote_offset, ld_vote, assigned_box, pmask, nmask,
+                                  cls_label, angle_bin, angle_res, vote_mask, vote_target, workspace, loss, norm, stream);
 }
 
 extern "C" int ssd3d_det_loss_grad(int b, int n, int nv, int angle_bins, const float *base_xyz, const float *pred_cls, int ld_cls,
@@ -429,20 +503,9 @@ extern "C" int ssd3d_det_loss_grad(int b, int n, int nv, int angle_bins, const f
                                    float *grad_angle_cls, int ldg_angle_cls, float *grad_angle_res, int ldg_angle_res,
                                    float *grad_vote_offset, ssd3d_stream_t stream)
 {
-    SSD3D_REQUIRE(b >= 0 && n >= 0 && nv >= 0, "det_loss_grad: bad shape b=%d n=%d nv=%d", b, n, nv);
-    SSD3D_REQUIRE(ldg_cls >= 1 && ldg_offset >= 6 && ldg_angle_cls >= angle_bins && ldg_angle_res >= angle_bins,
-                  "det_loss_grad: bad gradient row strides");
-    const long rows = (long)b * (n > nv ? n : nv);
-    if (rows == 0) return 0;
-    SSD3D_REQUIRE(grad_loss && norm && (n == 0 || (grad_base_xyz && grad_cls && grad_offset && grad_angle_cls && grad_angle_res)) &&
-                  (nv == 0 || grad_vote_offset), "det_loss_grad: null pointer");
-    LossIn in;
-    const int st = det_loss_in(n, nv, angle_bins, base_xyz, pred_cls, ld_cls, pred_offset, ld_offset, pred_angle_cls, ld_angle_cls,
-                               pred_angle_res, ld_angle_res, vote_offset, ld_vote, assigned_box, pmask, nmask, cls_label, angle_bin,
-                               angle_res, vote_mask, vote_target, in);
-    if (st) return st;
-    det_loss_grad_kernel<<<ceil_div(rows, kDetThreads), kDetThreads, 0, (cudaStream_t)stream>>>(
-        b, n, nv, angle_bins, bin_interval(angle_bins), in, grad_loss, norm, grad_base_xyz, grad_cls, ldg_cls, grad_offset, ldg_offset,
-        grad_angle_cls, ldg_angle_cls, grad_angle_res, ldg_angle_res, grad_vote_offset);
-    SSD3D_LAUNCH_CHECK("det_loss_grad_kernel");
+    return ssd3d_det_loss_grad_classes(b, n, nv, angle_bins, 1, base_xyz, pred_cls, ld_cls, pred_offset, ld_offset, pred_angle_cls,
+                                       ld_angle_cls, pred_angle_res, ld_angle_res, vote_offset, ld_vote, assigned_box, pmask, nmask,
+                                       cls_label, angle_bin, angle_res, vote_mask, vote_target, grad_loss, norm, grad_base_xyz,
+                                       grad_cls, ldg_cls, grad_offset, ldg_offset, grad_angle_cls, ldg_angle_cls, grad_angle_res,
+                                       ldg_angle_res, grad_vote_offset, stream);
 }

@@ -73,8 +73,8 @@ __global__ void vote_translate_kernel(long rows, const float *__restrict__ xyz, 
 }
 
 // one thread per candidate point
-__global__ void decode_kernel(long rows, int nbins, const float *__restrict__ ctr, const float *__restrict__ reg, int ldreg,
-                              const float *__restrict__ cls, int ldcls, float bin_interval, float *__restrict__ boxes,
+__global__ void decode_kernel(long rows, int nbins, int ncls, const float *__restrict__ ctr, const float *__restrict__ reg,
+                              int ldreg, const float *__restrict__ cls, int ldcls, float bin_interval, float *__restrict__ boxes,
                               float *__restrict__ scores)
 {
     const long r = blockIdx.x * (long)blockDim.x + threadIdx.x;
@@ -99,7 +99,7 @@ __global__ void decode_kernel(long rows, int nbins, const float *__restrict__ ct
     o[6] = angle;
     // the sigmoid in double, rounded once: in float, expf's own 2-ulp error plus the rounding of the add and the divide
     // put some scores more than 2 ulp away from the exact sigmoid
-    scores[r] = (float)(1.0 / (1.0 + exp(-(double)cls[r * ldcls])));
+    for (int c = 0; c < ncls; c++) scores[r * ncls + c] = (float)(1.0 / (1.0 + exp(-(double)cls[r * ldcls + c])));
 }
 
 // argmax over nb logits, ties to the first index (tf.argmax)
@@ -244,18 +244,35 @@ extern "C" int ssd3d_vote_translate(long rows, const float *xyz, const float *of
     SSD3D_LAUNCH_CHECK("vote_translate_kernel");
 }
 
+static int decode_dist_anchor_free(const char *op, long rows, int angle_bins, int cls_num, const float *center_xyz,
+                                   const float *pred_reg, int ld_reg, const float *pred_cls, int ld_cls, float *boxes, float *scores,
+                                   ssd3d_stream_t stream)
+{
+    SSD3D_REQUIRE(rows >= 0 && angle_bins >= 1 && ld_reg >= 6 + 2 * angle_bins && cls_num >= 1 && cls_num <= SSD3D_MAX_CLASSES &&
+                  ld_cls >= cls_num, "%s: bad shape rows=%ld bins=%d ld_reg=%d ld_cls=%d cls_num=%d", op, rows, angle_bins, ld_reg,
+                  ld_cls, cls_num);
+    if (rows == 0) return 0;
+    SSD3D_REQUIRE(center_xyz && pred_reg && pred_cls && boxes && scores, "%s: null pointer", op);
+    const float interval = (float)(2.0 * 3.14159265358979323846 / angle_bins);
+    decode_kernel<<<(int)((rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>(rows, angle_bins, cls_num, center_xyz, pred_reg,
+                                                                              ld_reg, pred_cls, ld_cls, interval, boxes, scores);
+    SSD3D_LAUNCH_CHECK("decode_kernel");
+}
+
 extern "C" int ssd3d_decode_dist_anchor_free(long rows, int angle_bins, const float *center_xyz, const float *pred_reg,
                                              int ld_reg, const float *pred_cls, int ld_cls, float *boxes, float *scores,
                                              ssd3d_stream_t stream)
 {
-    SSD3D_REQUIRE(rows >= 0 && angle_bins >= 1 && ld_reg >= 6 + 2 * angle_bins && ld_cls >= 1,
-                  "decode_dist_anchor_free: bad shape rows=%ld bins=%d ld_reg=%d ld_cls=%d", rows, angle_bins, ld_reg, ld_cls);
-    if (rows == 0) return 0;
-    SSD3D_REQUIRE(center_xyz && pred_reg && pred_cls && boxes && scores, "decode_dist_anchor_free: null pointer");
-    const float interval = (float)(2.0 * 3.14159265358979323846 / angle_bins);
-    decode_kernel<<<(int)((rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>(rows, angle_bins, center_xyz, pred_reg, ld_reg,
-                                                                              pred_cls, ld_cls, interval, boxes, scores);
-    SSD3D_LAUNCH_CHECK("decode_kernel");
+    return decode_dist_anchor_free("decode_dist_anchor_free", rows, angle_bins, 1, center_xyz, pred_reg, ld_reg, pred_cls, ld_cls,
+                                   boxes, scores, stream);
+}
+
+extern "C" int ssd3d_decode_dist_anchor_free_classes(long rows, int angle_bins, int cls_num, const float *center_xyz,
+                                                     const float *pred_reg, int ld_reg, const float *pred_cls, int ld_cls,
+                                                     float *boxes, float *scores, ssd3d_stream_t stream)
+{
+    return decode_dist_anchor_free("decode_dist_anchor_free_classes", rows, angle_bins, cls_num, center_xyz, pred_reg, ld_reg,
+                                   pred_cls, ld_cls, boxes, scores, stream);
 }
 
 extern "C" int ssd3d_decode_bin_anchor(long rows, int bin_num, float half_bin_search_range, int angle_bins,

@@ -36,9 +36,9 @@ __device__ __forceinline__ uint32_t nms_f2ord(float x)
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
-__device__ __forceinline__ unsigned long long nms_key(const float *sc, int i)
+__device__ __forceinline__ unsigned long long nms_key(const float *sc, int lds, int i)
 {
-    return ((unsigned long long)nms_f2ord(sc[i]) << 32) | (unsigned long long)(0xffffffffu - (uint32_t)i);
+    return ((unsigned long long)nms_f2ord(sc[(size_t)i * lds]) << 32) | (unsigned long long)(0xffffffffu - (uint32_t)i);
 }
 __device__ __forceinline__ int nms_key_index(unsigned long long key) { return (int)(0xffffffffu - (uint32_t)(key & 0xffffffffull)); }
 
@@ -83,7 +83,7 @@ __device__ __forceinline__ void nms_sort_desc(unsigned long long *keys, int npow
 }
 
 // The fixed-size output block of one scene from the kept sorted positions (or, kept_src, the kept box indices)
-__device__ __forceinline__ void nms_write_block(int cnt, const int *kept_src, const float *bx, const float *sc, int max_out,
+__device__ __forceinline__ void nms_write_block(int cnt, const int *kept_src, const float *bx, const float *sc, int lds, int max_out,
                                                 int cls_id, float *ob)
 {
     for (int e = threadIdx.x; e < max_out * 9; e += blockDim.x) {
@@ -91,15 +91,84 @@ __device__ __forceinline__ void nms_write_block(int cnt, const int *kept_src, co
         float v = 0.0f;
         if (k < cnt) {
             const int src = kept_src[k];
-            v = f < 7 ? bx[(size_t)src * 7 + f] : (f == 7 ? sc[src] : (float)cls_id);
+            v = f < 7 ? bx[(size_t)src * 7 + f] : (f == 7 ? sc[(size_t)src * lds] : (float)cls_id);
         }
         ob[e] = v;
     }
 }
 
-// Shared memory of the kernel: keys[npow2] | kept rect[kcap] | kept area[kcap] | kept src[kcap] (kcap = min(n, max_out))
+// Shared memory of the kernels: keys[npow2] | kept rect[kcap] | kept area[kcap] | kept src[kcap] (kcap = min(n, max_out))
 __host__ __device__ static size_t nms_keys_bytes(int npow2) { return ((size_t)npow2 * 8 + 15) & ~(size_t)15; }
 static size_t nms_smem_bytes(int npow2, int kcap) { return nms_keys_bytes(npow2) + (size_t)kcap * (16 + 4 + 4); }
+
+// The static shared state of one chunked walk
+struct NmsChunk {
+    float4 crect[NMS_CHUNK];
+    float carea[NMS_CHUNK];
+    uint32_t cself[NMS_CHUNK];     // cself[t] bit j: chunk candidate j (< t) suppresses candidate t
+    uint32_t cbykept;              // bit t: candidate t is suppressed by an already kept box
+    int nkept;
+};
+
+// The greedy NMS of one scene by the whole CTA: candidates 0 .. nv-1 with scores sc[i * lds] sorted by key, then walked
+// in chunks of 32.  On return (after a barrier) ch.nkept boxes are kept, their box indices in ksrc[0 .. nkept).
+__device__ __forceinline__ void nms_walk(int npow2, int kcap, int nv, const float *bx, const float *sc, int lds, float iou_thr,
+                                         int max_out, unsigned char *smem, NmsChunk &ch, int *&ksrc_out)
+{
+    unsigned long long *keys = reinterpret_cast<unsigned long long *>(smem);
+    float4 *krect = reinterpret_cast<float4 *>(smem + nms_keys_bytes(npow2));
+    float *karea = reinterpret_cast<float *>(krect + kcap);
+    int *ksrc = reinterpret_cast<int *>(karea + kcap);
+    ksrc_out = ksrc;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+    for (int i = tid; i < npow2; i += NMS_THREADS) keys[i] = i < nv ? nms_key(sc, lds, i) : 0ull;
+    if (tid == 0) ch.nkept = 0;
+    __syncthreads();
+    nms_sort_desc(keys, npow2);
+
+    for (int base = 0; base < nv; base += NMS_CHUNK) {
+        const int nk = ch.nkept;              // read by all threads after the barrier that ended the last step
+        if (nk >= max_out) break;
+        const int cn = min(NMS_CHUNK, nv - base);
+        if (tid < cn) {
+            const float4 r = nms_rect(bx + (size_t)nms_key_index(keys[base + tid]) * 7);
+            ch.crect[tid] = r;
+            ch.carea[tid] = nms_area(r);
+        }
+        if (tid == 0) ch.cbykept = 0u;
+        __syncthreads();
+        // candidate `lane` against kept boxes warp, warp + 32, ...; warp t also builds row t of the chunk's own matrix
+        if (lane < cn) {
+            const float4 a = ch.crect[lane];
+            const float aa = ch.carea[lane];
+            bool hit = false;
+            for (int u = warp; u < nk && !hit; u += NMS_THREADS / 32) hit = nms_over(krect[u], karea[u], a, aa, iou_thr);
+            if (hit) atomicOr(&ch.cbykept, 1u << lane);
+        }
+        if (warp < cn) {
+            const bool sup = lane < warp && nms_over(ch.crect[lane], ch.carea[lane], ch.crect[warp], ch.carea[warp], iou_thr);
+            const uint32_t row = __ballot_sync(0xffffffffu, sup);
+            if (lane == 0) ch.cself[warp] = row;
+        }
+        __syncthreads();
+        if (tid == 0) {                       // greedy, in sorted order, within the chunk
+            const uint32_t alive = ~ch.cbykept;
+            uint32_t taken = 0u;
+            int k = nk;
+            for (int t = 0; t < cn && k < max_out; t++) {
+                if (!((alive >> t) & 1u) || (ch.cself[t] & taken)) continue;
+                taken |= 1u << t;
+                krect[k] = ch.crect[t];
+                karea[k] = ch.carea[t];
+                ksrc[k] = nms_key_index(keys[base + t]);
+                k++;
+            }
+            ch.nkept = k;
+        }
+        __syncthreads();
+    }
+}
 
 __global__ void __launch_bounds__(NMS_THREADS)
 bev_nms_kernel(int n, int npow2, int kcap, const float *__restrict__ boxes, const float *__restrict__ scores,
@@ -107,76 +176,71 @@ bev_nms_kernel(int n, int npow2, int kcap, const float *__restrict__ boxes, cons
                      int *__restrict__ out_cnt)
 {
     extern __shared__ __align__(16) unsigned char nms_smem[];
-    unsigned long long *keys = reinterpret_cast<unsigned long long *>(nms_smem);
-    float4 *krect = reinterpret_cast<float4 *>(nms_smem + nms_keys_bytes(npow2));
-    float *karea = reinterpret_cast<float *>(krect + kcap);
-    int *ksrc = reinterpret_cast<int *>(karea + kcap);
-    __shared__ float4 crect[NMS_CHUNK];
-    __shared__ float carea[NMS_CHUNK];
-    __shared__ uint32_t cself[NMS_CHUNK];     // cself[t] bit j: chunk candidate j (< t) suppresses candidate t
-    __shared__ uint32_t cbykept;              // bit t: candidate t is suppressed by an already kept box
-    __shared__ int nkept;
-
-    const int scene = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    __shared__ NmsChunk ch;
+    const int scene = blockIdx.x;
     const float *bx = boxes + (size_t)scene * n * 7;
     const float *sc = scores + (size_t)scene * n;
-    // candidates n_valid[scene] .. n-1 are padding: key 0 sorts them last and the walk below stops before them
+    // candidates n_valid[scene] .. n-1 are padding: key 0 sorts them last and the walk stops before them
     const int nv = n_valid == nullptr ? n : max(0, min(n, n_valid[scene]));
+    int *ksrc;
+    nms_walk(npow2, kcap, nv, bx, sc, 1, iou_thr, max_out, nms_smem, ch, ksrc);
+    const int cnt = ch.nkept;
+    nms_write_block(cnt, ksrc, bx, sc, 1, max_out, cls_id, out_block + (size_t)scene * max_out * 9);
+    if (threadIdx.x == 0) out_cnt[scene] = cnt;
+}
 
-    for (int i = tid; i < npow2; i += NMS_THREADS) keys[i] = i < nv ? nms_key(sc, i) : 0ull;
-    if (tid == 0) nkept = 0;
-    __syncthreads();
-    nms_sort_desc(keys, npow2);
-
-    for (int base = 0; base < nv; base += NMS_CHUNK) {
-        const int nk = nkept;                 // read by all threads after the barrier that ended the last step
-        if (nk >= max_out) break;
-        const int cn = min(NMS_CHUNK, nv - base);
-        if (tid < cn) {
-            const float4 r = nms_rect(bx + (size_t)nms_key_index(keys[base + tid]) * 7);
-            crect[tid] = r;
-            carea[tid] = nms_area(r);
+// Per-class NMS of one scene by a cluster of ncls CTAs (DESIGN.md section 3.17): CTA rank c walks class c's scores
+// (scores[scene, i, c]); the kept counts are exchanged over distributed shared memory, so that each CTA writes its rows
+// at the sum of the lower ranks' counts, class-major and compacted, in the same launch.
+__global__ void __launch_bounds__(NMS_THREADS)
+bev_nms_classes_kernel(int n, int npow2, int kcap, int ncls, const float *__restrict__ boxes, const float *__restrict__ scores,
+                       float iou_thr, int max_out, float *__restrict__ out_block, int *__restrict__ out_cnt)
+{
+    extern __shared__ __align__(16) unsigned char nms_smem[];
+    __shared__ NmsChunk ch;
+    __shared__ int row0, total;
+    const int c = (int)cluster_ctarank(), scene = (int)cluster_id_x();
+    const float *bx = boxes + (size_t)scene * n * 7;
+    const float *sc = scores + (size_t)scene * n * ncls + c;
+    int *ksrc;
+    nms_walk(npow2, kcap, n, bx, sc, ncls, iou_thr, max_out, nms_smem, ch, ksrc);
+    cluster_sync_all();                                    // every rank's ch.nkept is final
+    if (threadIdx.x == 0) {
+        int below = 0, all = 0;
+        const uint32_t at = smem_u32(&ch.nkept);
+        for (int r = 0; r < ncls; r++) {
+            int v;
+            asm volatile("ld.shared::cluster.s32 %0, [%1];" : "=r"(v) : "r"(mapa(at, (uint32_t)r)) : "memory");
+            if (r < c) below += v;
+            all += v;
         }
-        if (tid == 0) cbykept = 0u;
-        __syncthreads();
-        // candidate `lane` against kept boxes warp, warp + 32, ...; warp t also builds row t of the chunk's own matrix
-        if (lane < cn) {
-            const float4 a = crect[lane];
-            const float aa = carea[lane];
-            bool hit = false;
-            for (int u = warp; u < nk && !hit; u += NMS_THREADS / 32) hit = nms_over(krect[u], karea[u], a, aa, iou_thr);
-            if (hit) atomicOr(&cbykept, 1u << lane);
-        }
-        if (warp < cn) {
-            const bool sup = lane < warp && nms_over(crect[lane], carea[lane], crect[warp], carea[warp], iou_thr);
-            const uint32_t row = __ballot_sync(0xffffffffu, sup);
-            if (lane == 0) cself[warp] = row;
-        }
-        __syncthreads();
-        if (tid == 0) {                       // greedy, in sorted order, within the chunk
-            const uint32_t alive = ~cbykept;
-            uint32_t taken = 0u;
-            int k = nk;
-            for (int t = 0; t < cn && k < max_out; t++) {
-                if (!((alive >> t) & 1u) || (cself[t] & taken)) continue;
-                taken |= 1u << t;
-                krect[k] = crect[t];
-                karea[k] = carea[t];
-                ksrc[k] = nms_key_index(keys[base + t]);
-                k++;
-            }
-            nkept = k;
-        }
-        __syncthreads();
+        row0 = below;
+        total = all;
     }
-    const int cnt = nkept;
-    nms_write_block(cnt, ksrc, bx, sc, max_out, cls_id, out_block + (size_t)scene * max_out * 9);
-    if (tid == 0) out_cnt[scene] = cnt;
+    cluster_sync_all();                                    // no CTA leaves while a peer may still read its count
+    const int cnt = ch.nkept, rows = ncls * max_out;
+    float *ob = out_block + (size_t)scene * rows * 9;
+    for (int e = threadIdx.x; e < cnt * 9; e += blockDim.x) {
+        const int k = e / 9, f = e - k * 9, src = ksrc[k];
+        ob[(size_t)row0 * 9 + e] = f < 7 ? bx[(size_t)src * 7 + f] : (f == 7 ? sc[(size_t)src * ncls] : (float)c);
+    }
+    if (c == ncls - 1)
+        for (int e = total * 9 + threadIdx.x; e < rows * 9; e += blockDim.x) ob[e] = 0.0f;
+    if (c == 0 && threadIdx.x == 0) out_cnt[scene] = total;
 }
 
 }  // namespace ssd3d
 
 using namespace ssd3d;
+
+// The shared memory of one scene's walk: sort keys of npow2 >= n candidates and kcap = min(n, max_output) kept boxes
+static size_t nms_plan(int n, int max_output, int &npow2, int &kcap)
+{
+    npow2 = 1;
+    while (npow2 < n) npow2 <<= 1;
+    kcap = max_output < n ? max_output : n;
+    return nms_smem_bytes(npow2, kcap);
+}
 
 static int bev_nms_launch(const char *op, int b, int n, const float *boxes, const float *scores, const int *n_valid,
                           float iou_threshold, int max_output, int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream)
@@ -185,10 +249,8 @@ static int bev_nms_launch(const char *op, int b, int n, const float *boxes, cons
     SSD3D_REQUIRE(n <= NMS_MAX_N, "%s: at most %d candidates per scene (got %d)", op, NMS_MAX_N, n);
     if (b == 0) return 0;                    // nothing read or written: an empty tensor may have a null data pointer
     SSD3D_REQUIRE(boxes && scores && out_block && out_cnt, "%s: null pointer", op);
-    int npow2 = 1;
-    while (npow2 < n) npow2 <<= 1;
-    const int kcap = max_output < n ? max_output : n;
-    const size_t smem = nms_smem_bytes(npow2, kcap);
+    int npow2, kcap;
+    const size_t smem = nms_plan(n, max_output, npow2, kcap);
     SSD3D_REQUIRE(smem <= NMS_SMEM_MAX, "%s: max_output=%d at n=%d needs %zu bytes of shared memory (at most %zu)",
                   op, max_output, n, smem, NMS_SMEM_MAX);
     const int e = cuda_status(cudaFuncSetAttribute(bev_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
@@ -213,4 +275,43 @@ extern "C" int ssd3d_bev_nms_counted(int b, int n, const float *boxes, const flo
     if (b > 0) SSD3D_REQUIRE(n_valid != nullptr, "bev_nms_counted: null n_valid");
     return bev_nms_launch("bev_nms_counted", b, n, boxes, scores, n_valid, iou_threshold, max_output, cls_id, out_block,
                           out_cnt, stream);
+}
+
+extern "C" int ssd3d_bev_nms_classes(int b, int n, int cls_num, const float *boxes, const float *scores, float iou_threshold,
+                                     int max_output, float *out_block, int *out_cnt, ssd3d_stream_t stream)
+{
+    SSD3D_REQUIRE(b >= 0 && n > 0 && max_output > 0 && cls_num >= 1 && cls_num <= SSD3D_MAX_CLASSES,
+                  "bev_nms_classes: bad shape b=%d n=%d max_output=%d cls_num=%d (1..%d)", b, n, max_output, cls_num,
+                  SSD3D_MAX_CLASSES);
+    SSD3D_REQUIRE(n <= NMS_MAX_N, "bev_nms_classes: at most %d candidates per scene (got %d)", NMS_MAX_N, n);
+    if (b == 0) return 0;
+    SSD3D_REQUIRE(boxes && scores && out_block && out_cnt, "bev_nms_classes: null pointer");
+    int npow2, kcap;
+    const size_t smem = nms_plan(n, max_output, npow2, kcap);
+    SSD3D_REQUIRE(smem <= NMS_SMEM_MAX, "bev_nms_classes: max_output=%d at n=%d needs %zu bytes of shared memory (at most %zu)",
+                  max_output, n, smem, NMS_SMEM_MAX);
+    int e = cuda_status(cudaFuncSetAttribute(bev_nms_classes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                        "bev_nms_classes_kernel shared memory");
+    if (e) return e;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(b * cls_num));
+    cfg.blockDim = dim3(NMS_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = (cudaStream_t)stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cls_num;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    e = cuda_status(cudaOccupancyMaxActiveClusters(&clusters, bev_nms_classes_kernel, &cfg), "bev_nms_classes occupancy");
+    if (e) return e;
+    SSD3D_REQUIRE(clusters >= 1, "bev_nms_classes: a cluster of %d CTAs with %zu bytes of shared memory each cannot be placed",
+                  cls_num, smem);
+    e = cuda_status(cudaLaunchKernelEx(&cfg, bev_nms_classes_kernel, n, npow2, kcap, cls_num, boxes, scores, iou_threshold,
+                                       max_output, out_block, out_cnt), "bev_nms_classes_kernel");
+    if (e) return e;
+    SSD3D_LAUNCH_CHECK("bev_nms_classes_kernel");
 }

@@ -1,7 +1,7 @@
 """Detection head, box decoding and post-processing of the single-stage 3DSSD detector (SURVEY.md section 8f, rows f1/f2).
 
 Mirrors, for inference with the shipped 3DSSD configuration (anchor-free 'Dist-Anchor-free' regression, sigmoid
-classification, one class, `HEAD: [[[6], [6], 'conv1d', [128,], True, 'Det', '']]`, configs/kitti/3dssd/3dssd.yaml:68):
+classification over the classes of CLS_LIST (one by default), `HEAD: [[[6], [6], 'conv1d', [128,], True, 'Det', '']]`, configs/kitti/3dssd/3dssd.yaml:68):
   HeadBuilder.build_layer            /root/reference/lib/modeling/head_builder.py:81-114
   box_regression_head                /root/reference/lib/utils/head_util.py:26-59
   decode_dist_anchor_free            /root/reference/lib/utils/anchor_decoder.py:86-112
@@ -95,27 +95,45 @@ def decode_dist_anchor_free(center_xyz, det_forced_6_distance, det_angle_cls, de
 
 
 def postprocess(pred_anchors_3d, pred_score, max_output=MAX_OUTPUT_NUM, nms_threshold=NMS_THRESH):
-    """PostProcessor.forward for one class: pred_anchors_3d (bs, n, 1, 7), pred_score (bs, n, 1) ->
-    fixed-size block (bs, max_output, 9) + count (bs,)."""
+    """PostProcessor.forward: pred_anchors_3d (bs, n, 1, 7), pred_score (bs, n, C) -> fixed-size block
+    (bs, C * max_output, 9) + count (bs,).  One class: tf_ops.bev_nms; C > 1: the per-class NMS over the shared boxes
+    (postprocessor.py:49-120), class-major rows tagged with the 0-based class in column 8."""
     boxes = pred_anchors_3d[:, :, 0, :].contiguous()
-    return tf_ops.bev_nms(boxes, pred_score[:, :, 0].contiguous(), nms_threshold, max_output, cls_id=0)
+    c = pred_score.shape[-1]
+    if c == 1:
+        return tf_ops.bev_nms(boxes, pred_score[:, :, 0].contiguous(), nms_threshold, max_output, cls_id=0)
+    return tf_ops.bev_nms(boxes, pred_score.contiguous(), nms_threshold, max_output, cls_num=c)
 
 
 class DetectionHead:
     """HeadBuilder (head_builder.py) + test_forward + PostProcessor for a 'conv1d' / 'Det' head spec.  stage: the
     MODEL.FIRST_STAGE constants (config.STAGE_3DSSD, the default, or config.STAGE_POINTRCNN_RPN): REGRESSION selects the
     decode ('Dist-Anchor-free': tf_ops.decode_dist_anchor_free, 'Bin-Anchor': tf_ops.decode_bin_anchor on one anchor of
-    ANCHOR_SIZE per point), MAX_OUTPUT_NUM and NMS_THRESH the post-processing."""
+    ANCHOR_SIZE per point), MAX_OUTPUT_NUM and NMS_THRESH the post-processing.
+    A 'Dist-Anchor-free' head has as many sigmoid classes C as its pred_cls/weights has columns (1..8); cls_num, when
+    given, must agree.  C > 1 decodes C scores per point and runs the per-class NMS: the block is
+    [bs, C * MAX_OUTPUT_NUM, 9] (max_output), class-major, column 8 the 0-based class."""
 
-    def __init__(self, head_cfg=None, params=None, device="cuda", cls_num=1, stage=None):
+    def __init__(self, head_cfg=None, params=None, device="cuda", cls_num=None, stage=None):
         self.cfg = HEAD_3DSSD if head_cfg is None else head_cfg
         self.xyz_index, self.feature_index, self.op_type, self.mlp_list, self.bn, self.layer_type, self.scope = self.cfg
         if self.op_type != 'conv1d' or self.layer_type != 'Det':
             raise NotImplementedError("only 'conv1d' / 'Det' heads are built")
         self.stage = _cfg.STAGE_3DSSD if stage is None else stage
         self.reg_channels = reg_channels(self.stage)
-        self.cls_num = cls_num
         self.params = prepare(params, device)
+        raw = self.params.raw
+        key = _scope(self.scope, "pred_cls") + "/weights"
+        width = None if raw is None or key not in raw else int(raw[key].shape[-1])
+        if self.stage["REGRESSION"] == "Dist-Anchor-free" and width is not None:
+            if cls_num is not None and int(cls_num) != width:
+                raise ValueError("DetectionHead: cls_num=%d but %s has %d columns" % (cls_num, key, width))
+            if not 1 <= width <= tf_ops.MAX_CLASSES:
+                raise ValueError("DetectionHead: %s has %d columns; 1..%d classes are built" % (key, width, tf_ops.MAX_CLASSES))
+            cls_num = width
+        self.cls_num = 1 if cls_num is None else int(cls_num)
+        self.multi = self.stage["REGRESSION"] == "Dist-Anchor-free" and self.cls_num > 1
+        self.max_output = self.stage["MAX_OUTPUT_NUM"] * (self.cls_num if self.multi else 1)   # rows of the block
 
     def forward(self, xyz_list, feature_list, return_raw=False, out=None, split=None):
         """out=(block, count): preallocated outputs of the NMS (the send buffer of the multi-GPU gather).  split: the
@@ -132,14 +150,19 @@ class DetectionHead:
         if st["REGRESSION"] == "Bin-Anchor":
             boxes, score = tf_ops.decode_bin_anchor(xyz, reg, cls, st["ANCHOR_SIZE"], st["HALF_BIN_SEARCH_RANGE"],
                                                     st["BIN_CLASS_NUM"], ANGLE_CLS_NUM)
+        elif self.multi:
+            boxes, score = tf_ops.decode_dist_anchor_free(xyz, reg, cls, ANGLE_CLS_NUM, cls_num=self.cls_num)
         else:
             boxes, score = tf_ops.decode_dist_anchor_free(xyz, reg, cls, ANGLE_CLS_NUM)
-        block, cnt = tf_ops.bev_nms(boxes, score, st["NMS_THRESH"], st["MAX_OUTPUT_NUM"], cls_id=0, out=out)   # postprocessor.py:52-120
+        if self.multi:                                                             # postprocessor.py:49-120, every class
+            block, cnt = tf_ops.bev_nms(boxes, score, st["NMS_THRESH"], st["MAX_OUTPUT_NUM"], out=out, cls_num=self.cls_num)
+        else:
+            block, cnt = tf_ops.bev_nms(boxes, score, st["NMS_THRESH"], st["MAX_OUTPUT_NUM"], cls_id=0, out=out)   # postprocessor.py:52-120
         if return_raw:
             bs, n, _ = reg.shape
             r4 = reg.view(bs, n, 1, self.reg_channels + 2 * ANGLE_CLS_NUM)
             k = self.reg_channels
-            return block, cnt, {"boxes": boxes.unsqueeze(2), "score": score.unsqueeze(-1), "cls": cls, "reg": reg,
+            return block, cnt, {"boxes": boxes.unsqueeze(2), "score": score if self.multi else score.unsqueeze(-1), "cls": cls, "reg": reg,
                                 "offset": r4[..., :k], "angle_cls": r4[..., k:k + ANGLE_CLS_NUM],
                                 "angle_res": r4[..., k + ANGLE_CLS_NUM:], "feat": y}
         return block, cnt

@@ -9,8 +9,12 @@ The two seams of the reference's training step, on the GPU:
 Both take the tensors head.box_regression_head and vote_layer return; the work is csrc/det_loss.cu.
 
     outs = backbone.train_forward(arch, tp, xyz, feat)
-    tg = assign_targets(outs.base_xyz, outs.vote_base, gt_boxes, gt_labels)
-    losses = detection_loss(outs.base_xyz, *outs.head, outs.vote_offset, tg)
+    tg = assign_targets(outs.base_xyz, outs.vote_base, gt_boxes, gt_labels, cls_num)
+    losses = detection_loss(outs.base_xyz, *outs.head, outs.vote_offset, tg, cls_num)
+
+cls_num (the head's pred_cls width C, labels 1..C): C > 1 takes the class forms of the kernels, whose classification
+target is one_hot(label - 1, C) * centre-ness and whose classification loss is the mean over the classes
+(loss_builder.py:58-96); C = 1 (or None) is the single-class path.
     losses["total"].backward()
 """
 from typing import NamedTuple
@@ -31,7 +35,7 @@ LOSS_NAMES = ("cls_loss", "offset_loss", "bin_angle_loss", "res_angle_loss", "co
 
 class Targets(NamedTuple):
     """Per candidate point [b, n]: assigned_idx (int32), assigned_box [.., 7], pmask, nmask, cls_label (the centre-ness
-    classification target), angle_bin (int32), angle_res, offset_target [.., 6]; per vote base point [b, nv]: vote_mask,
+    classification target; [b, n, C] for C > 1 classes), angle_bin (int32), angle_res, offset_target [.., 6]; per vote base point [b, nv]: vote_mask,
     vote_target [.., 3].  No gradient flows into any of them."""
     assigned_idx: torch.Tensor
     assigned_box: torch.Tensor
@@ -45,22 +49,27 @@ class Targets(NamedTuple):
     vote_target: torch.Tensor
 
 
-def assign_targets(base_xyz, vote_base, gt_boxes, gt_labels):
+def _classes(cls_num):
+    """The cls_num of the tf_ops calls: None (the single-class entry points) for one class."""
+    return None if cls_num is None or int(cls_num) == 1 else int(cls_num)
+
+
+def assign_targets(base_xyz, vote_base, gt_boxes, gt_labels, cls_num=None):
     """base_xyz (b, n, 3) candidate points (the CG layer's centres), vote_base (b, nv, 3) the vote layer's input points,
     gt_boxes (b, g, 7) camera-frame (x, y, z, l, h, w, ry) padded with rows of zeros, gt_labels (b, g) -> Targets.
     A scene without a valid box gives all negatives and zero targets (include/ssd3d.h, ssd3d_det_assign)."""
     labels = gt_labels if isinstance(gt_labels, torch.Tensor) and gt_labels.dtype == torch.int32 else torch.as_tensor(
         gt_labels, device=base_xyz.device).to(torch.int32)
     with torch.no_grad():
-        t = tf_ops.det_assign(base_xyz.detach(), vote_base.detach(), gt_boxes, labels, ANGLE_CLS_NUM)
+        t = tf_ops.det_assign(base_xyz.detach(), vote_base.detach(), gt_boxes, labels, ANGLE_CLS_NUM, cls_num=_classes(cls_num))
     return Targets(**t)
 
 
-def detection_loss(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, targets):
+def detection_loss(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, targets, cls_num=None):
     """The six losses of the 3DSSD head on `targets` -> dict of 0-d device tensors named LOSS_NAMES plus "total", their
     sum.  Differentiable w.r.t. base_xyz, the four head outputs (read in place) and the raw vote offsets."""
     loss = tf_ops.det_loss_train(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset,
-                                 targets._asdict(), ANGLE_CLS_NUM)
+                                 targets._asdict(), ANGLE_CLS_NUM, cls_num=_classes(cls_num))
     out = {name: loss[i] for i, name in enumerate(LOSS_NAMES)}
     out["total"] = loss.sum()
     return out

@@ -56,9 +56,10 @@ def _pinned(a, dev):
     return t.pin_memory() if dev.type == "cuda" else t
 
 
-def run_batch(frames, device="cuda", with_db=False):
+def run_batch(frames, device="cuda", with_db=False, db_classes=_mixup.CLASS_INDEX):
     """Preprocess a batch of read frames -> (list of (position, sample dict) to write, skipped {position: reason},
-    ObjectDatabase of the written frames (frames = their positions) or None)."""
+    ObjectDatabase of the written frames (frames = their positions) or None).  db_classes: the labels whose rows become
+    database objects (label k = the k-th class of the frames' class list)."""
     dev = torch.device(device)
     gt = frames[0].boxes is not None
     sizes = [len(f.points) for f in frames]
@@ -106,7 +107,7 @@ def run_batch(frames, device="cuda", with_db=False):
             dpts = torch.cat([kept[k_off[s]:k_off[s + 1]] for s in rows]).float()
             doff = np.concatenate([[0], np.cumsum(n_kept[rows])])
             sel = rows
-        db = _mixup.ObjectDatabase.build(dpts, doff, boxes[sel], labels[sel], device=dev)
+        db = _mixup.ObjectDatabase.build(dpts, doff, boxes[sel], labels[sel], classes=db_classes, device=dev)
         pos = torch.as_tensor(np.asarray([frames[s].position for s in rows], np.int32), device=db.frames.device)
         db.frames = pos[db.frames.long()] if len(db) else db.frames
     return [(frames[s].position, d) for s, d in out], skipped, db

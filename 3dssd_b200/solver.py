@@ -160,6 +160,7 @@ class Trainer:
         elif dp.tp is not tp:
             raise ValueError("Trainer: dp must be the DataParallel of the same TrainableParams")
         self.dp = dp
+        self.cls_num = int(tp.tensors["pred_cls/weights"].shape[1])   # the head's classes (labels 1..cls_num)
         tp.refresh_operands()                # a DataParallel's constructor may have broadcast rank 0's weights
         self.global_step = 0                 # host mirror of the device's global_step: schedules need no device read
 
@@ -170,8 +171,8 @@ class Trainer:
         self.dp.zero_grad()
         with self.dp.recording():
             o = backbone.train_forward(self.arch, self.tp, xyz, feat, bn_decay=decay)
-        tg = loss.assign_targets(o.base_xyz, o.vote_base, gt_boxes, gt_labels)
-        losses = loss.detection_loss(o.base_xyz, *o.head, o.vote_offsets[-1], tg)
+        tg = loss.assign_targets(o.base_xyz, o.vote_base, gt_boxes, gt_labels, self.cls_num)
+        losses = loss.detection_loss(o.base_xyz, *o.head, o.vote_offsets[-1], tg, self.cls_num)
         losses["total"].backward()
         mean = self.dp.exchange(losses)
         self.adam.step()

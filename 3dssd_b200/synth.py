@@ -86,3 +86,42 @@ def kitti_like_with_boxes(batch, npoints, max_boxes, seed=0, surface_frac=0.3):
         pts[s, at, 1] = cy + b[:, 1]
         pts[s, at, 2] = -sn * cx + c * cz + b[:, 2]
     return pts, boxes, labels
+
+
+def kitti_like_multiclass(batch, npoints, max_boxes, classes=("Car", "Pedestrian", "Cyclist"), seed=0, surface_frac=0.3):
+    """kitti_like_with_boxes for several classes: each box draws a class of `classes` (names of config.CLASS_MEAN_SIZE)
+    uniformly, its label is the class's 1-based place in `classes`, and its (l, h, w) lies within +-15 % of the class's
+    mean size (g_type_mean_size, lib/utils/model_util.py:19-26).  Same points-on-the-boxes recipe; a random stream of its
+    own (kitti_like_with_boxes is left as it is)."""
+    from .config import CLASS_MEAN_SIZE, check_cls_list
+    classes = check_cls_list(classes)
+    pts = kitti_like(batch, npoints, seed=seed)
+    boxes = np.zeros((batch, max_boxes, 7), np.float32)
+    labels = np.zeros((batch, max_boxes), np.int32)
+    for s in range(batch):
+        rng = np.random.default_rng(seed + 104729 * (s + 1))
+        g = int(rng.integers(max(1, max_boxes // 2), max_boxes + 1)) if max_boxes else 0
+        for j in range(g):
+            k = int(rng.integers(len(classes)))
+            l, h, w = (m * rng.uniform(0.85, 1.15) for m in CLASS_MEAN_SIZE[classes[k]])
+            boxes[s, j] = (rng.uniform(-30, 30), 1.65 + 0.05 * rng.standard_normal(), rng.uniform(4, 60), l, h, w,
+                           rng.uniform(-np.pi, np.pi))
+            labels[s, j] = k + 1
+        if g == 0:
+            continue
+        kpts = int(round(surface_frac * npoints))
+        owner = rng.integers(0, g, kpts)
+        b = boxes[s, owner].astype(np.float64)
+        u = rng.uniform(-0.5, 0.5, (kpts, 3))
+        face = rng.integers(0, 6, kpts)                       # 0..3: a side, 4: the top, 5: inside
+        u[face == 0, 0], u[face == 1, 0] = 0.5, -0.5
+        u[face == 2, 2], u[face == 3, 2] = 0.5, -0.5
+        u[face == 4, 1] = -0.5
+        u[face == 5] *= 0.9
+        cx, cy, cz = u[:, 0] * b[:, 3], (u[:, 1] - 0.5) * b[:, 4], u[:, 2] * b[:, 5]
+        c, sn = np.cos(b[:, 6]), np.sin(b[:, 6])
+        at = rng.choice(npoints, kpts, replace=False)
+        pts[s, at, 0] = c * cx + sn * cz + b[:, 0]
+        pts[s, at, 1] = cy + b[:, 1]
+        pts[s, at, 2] = -sn * cx + c * cz + b[:, 2]
+    return pts, boxes, labels

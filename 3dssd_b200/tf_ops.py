@@ -13,6 +13,7 @@ TF's allocate_output, and the kernels run on torch's current stream (CUDA-graph 
 import contextlib
 import ctypes
 import math
+import operator
 import threading
 
 import numpy as np
@@ -842,28 +843,60 @@ def sa_mlp_fused_hoisted(xyz, z, zoff, wx, new_xyz, idx, cnt, stack, out_f32=Non
     return y
 
 
-def _nms_io(boxes, scores, max_output, out):
+MAX_CLASSES = 8               # SSD3D_MAX_CLASSES: the eight KITTI class names, the portable cluster size
+
+
+def _classes(cls_num):
+    """A class count of the multi-class entry points, 1 <= cls_num <= MAX_CLASSES."""
+    try:
+        c = None if isinstance(cls_num, bool) else operator.index(cls_num)
+    except TypeError:
+        c = None
+    if c is None or not 1 <= c <= MAX_CLASSES:
+        raise ValueError("cls_num must be an integer in 1..%d, got %r" % (MAX_CLASSES, cls_num))
+    return c
+
+
+def _nms_io(boxes, scores, max_output, out, cls_num=None):
     boxes = _req(boxes, "boxes", torch.float32, 3, 7)
-    scores = _req(scores, "scores", torch.float32, 2)
     b, n, _ = boxes.shape
-    if scores.shape != (b, n):
-        raise ValueError("scores must be (b, n)")
+    if cls_num is None:
+        scores = _req(scores, "scores", torch.float32, 2)
+        if scores.shape != (b, n):
+            raise ValueError("scores must be (b, n)")
+        rows = int(max_output)
+    else:
+        scores = _req(scores, "scores", torch.float32, 3)
+        if tuple(scores.shape) != (b, n, cls_num):
+            raise ValueError("scores must be (b, n, cls_num) = (%d, %d, %d), got %s" % (b, n, cls_num, tuple(scores.shape)))
+        rows = cls_num * int(max_output)
     if out is None:
-        block = torch.empty((b, int(max_output), 9), dtype=torch.float32, device=boxes.device)
+        block = torch.empty((b, rows, 9), dtype=torch.float32, device=boxes.device)
         cnt = torch.empty((b,), dtype=torch.int32, device=boxes.device)
     else:
         block, cnt = _req(out[0], "out block", torch.float32, 3, 9, copy=False), _req(out[1], "out count", torch.int32, 1, copy=False)
-        if tuple(block.shape) != (b, int(max_output), 9) or tuple(cnt.shape) != (b,):
-            raise ValueError("out must be (float32 (b, max_output, 9), int32 (b,)) contiguous tensors")
+        if tuple(block.shape) != (b, rows, 9) or tuple(cnt.shape) != (b,):
+            raise ValueError("out must be (float32 (b, %s, 9), int32 (b,)) contiguous tensors"
+                             % ("max_output" if cls_num is None else "cls_num * max_output"))
     return boxes, scores, block, cnt
 
 
-def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None):
+def bev_nms(boxes, scores, iou_threshold, max_output, cls_id=0, out=None, cls_num=None):
     """Greedy BEV NMS per scene (postprocessor.py:76-88): boxes (b,n,7) = (x,y,z,l,h,w,ry), scores (b,n) ->
     block (b,max_output,9) = (box7, score, class) zero padded, count (b,) int32.  out=(block, count) writes into
     preallocated contiguous tensors (the send buffer of the multi-GPU gather).  Descending score, ties (-0 and +0
     included) to the lower index; rectangles and IoU by the float32 recipe of DESIGN.md §3.5, which the CPU
-    restatements of the test suite share decision for decision.  NaN scores are outside the contract."""
+    restatements of the test suite share decision for decision.  NaN scores are outside the contract.
+    cls_num=C (1..MAX_CLASSES): the per-class NMS of postprocessor.py:49-120 in one launch (ssd3d_bev_nms_classes):
+    scores (b,n,C) -> block (b, C*max_output, 9), class 0's kept rows first, then class 1's, ..., column 8 = the class
+    (cls_id is not used), count (b,) = rows kept over all classes."""
+    if cls_num is not None:
+        cls_num = _classes(cls_num)
+        boxes, scores, block, cnt = _nms_io(boxes, scores, max_output, out, cls_num)
+        b, n, _ = boxes.shape
+        check(lib().ssd3d_bev_nms_classes(b, n, cls_num, _p(boxes), _p(scores), float(iou_threshold), int(max_output), _p(block),
+                                          _p(cnt), _stream()), "bev_nms_classes")
+        return block, cnt
     boxes, scores, block, cnt = _nms_io(boxes, scores, max_output, out)
     b, n, _ = boxes.shape
     check(lib().ssd3d_bev_nms(b, n, _p(boxes), _p(scores), float(iou_threshold), int(max_output), int(cls_id),
@@ -1237,15 +1270,26 @@ def vote_translate(xyz, offsets, min_range):
     return out
 
 
-def decode_dist_anchor_free(center_xyz, pred_reg, pred_cls, angle_bins=12):
+def decode_dist_anchor_free(center_xyz, pred_reg, pred_cls, angle_bins=12, cls_num=None):
     """anchor_decoder.decode_dist_anchor_free + decode_class2angle + sigmoid in one kernel: center_xyz (b, n, 3),
-    pred_reg (b, n, 6 + 2*angle_bins), pred_cls (b, n, >= 1) -> boxes (b, n, 7), scores (b, n)."""
+    pred_reg (b, n, 6 + 2*angle_bins), pred_cls (b, n, >= 1) -> boxes (b, n, 7), scores (b, n).
+    cls_num=C: pred_cls (b, n, C) -> the same boxes and scores (b, n, C), one sigmoid per class."""
     center_xyz = _req(center_xyz, "center_xyz", torch.float32, 3, 3)
     pred_reg = _req(pred_reg, "pred_reg", torch.float32, 3)
     pred_cls = _req(pred_cls, "pred_cls", torch.float32, 3)
     b, n, _ = center_xyz.shape
     if pred_reg.shape[:2] != (b, n) or pred_cls.shape[:2] != (b, n) or pred_reg.shape[2] < 6 + 2 * angle_bins:
         raise ValueError("pred_reg must be (b, n, >= 6 + 2*angle_bins) and pred_cls (b, n, >= 1)")
+    if cls_num is not None:
+        cls_num = _classes(cls_num)
+        if pred_cls.shape[2] != cls_num:
+            raise ValueError("pred_cls must be (b, n, cls_num = %d), got %s" % (cls_num, tuple(pred_cls.shape)))
+        boxes = torch.empty((b, n, 7), dtype=torch.float32, device=center_xyz.device)
+        scores = torch.empty((b, n, cls_num), dtype=torch.float32, device=center_xyz.device)
+        check(lib().ssd3d_decode_dist_anchor_free_classes(b * n, int(angle_bins), cls_num, _p(center_xyz), _p(pred_reg),
+                                                          pred_reg.shape[2], _p(pred_cls), cls_num, _p(boxes), _p(scores),
+                                                          _stream()), "decode_dist_anchor_free_classes")
+        return boxes, scores
     boxes = torch.empty((b, n, 7), dtype=torch.float32, device=center_xyz.device)
     scores = torch.empty((b, n), dtype=torch.float32, device=center_xyz.device)
     check(lib().ssd3d_decode_dist_anchor_free(b * n, int(angle_bins), _p(center_xyz), _p(pred_reg), pred_reg.shape[2],
@@ -1592,9 +1636,12 @@ DET_TARGETS = ("assigned_idx", "assigned_box", "pmask", "nmask", "cls_label", "a
 _LOSS_TARGETS = ("assigned_box", "pmask", "nmask", "cls_label", "angle_bin", "angle_res", "vote_mask", "vote_target")
 
 
-def det_assign(base_xyz, vote_base, gt_boxes, gt_labels, angle_bins=12):
+def det_assign(base_xyz, vote_base, gt_boxes, gt_labels, angle_bins=12, cls_num=None):
     """'Mask' assignment + vote targets (ssd3d_det_assign): base_xyz (b, n, 3), vote_base (b, nv, 3), gt_boxes (b, g, 7)
-    zero-padded, gt_labels (b, g) int32 -> dict of the DET_TARGETS tensors."""
+    zero-padded, gt_labels (b, g) int32 -> dict of the DET_TARGETS tensors.  cls_num=C (ssd3d_det_assign_classes): labels
+    1..C, cls_label (b, n, C) = one_hot(label - 1, C) * centre-ness; the other targets are the same."""
+    if cls_num is not None:
+        cls_num = _classes(cls_num)
     base_xyz = _req(base_xyz, "base_xyz", torch.float32, 3, 3)
     vote_base = _req(vote_base, "vote_base", torch.float32, 3, 3)
     gt_boxes = _req(gt_boxes, "gt_boxes", torch.float32, 3, 7)
@@ -1607,10 +1654,15 @@ def det_assign(base_xyz, vote_base, gt_boxes, gt_labels, angle_bins=12):
     dev = base_xyz.device
     f = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
     i = lambda *s: torch.empty(s, dtype=torch.int32, device=dev)
-    t = dict(assigned_idx=i(b, n), assigned_box=f(b, n, 7), pmask=f(b, n), nmask=f(b, n), cls_label=f(b, n),
-             angle_bin=i(b, n), angle_res=f(b, n), offset_target=f(b, n, 6), vote_mask=f(b, nv), vote_target=f(b, nv, 3))
-    check(lib().ssd3d_det_assign(b, n, nv, g, int(angle_bins), _p(base_xyz), _p(vote_base), _p(gt_boxes), _p(gt_labels),
-                                 *[_p(t[k]) for k in DET_TARGETS], _stream()), "det_assign")
+    t = dict(assigned_idx=i(b, n), assigned_box=f(b, n, 7), pmask=f(b, n), nmask=f(b, n),
+             cls_label=f(b, n) if cls_num is None else f(b, n, cls_num), angle_bin=i(b, n), angle_res=f(b, n),
+             offset_target=f(b, n, 6), vote_mask=f(b, nv), vote_target=f(b, nv, 3))
+    if cls_num is None:
+        check(lib().ssd3d_det_assign(b, n, nv, g, int(angle_bins), _p(base_xyz), _p(vote_base), _p(gt_boxes), _p(gt_labels),
+                                     *[_p(t[k]) for k in DET_TARGETS], _stream()), "det_assign")
+    else:
+        check(lib().ssd3d_det_assign_classes(b, n, nv, g, int(angle_bins), cls_num, _p(base_xyz), _p(vote_base), _p(gt_boxes),
+                                             _p(gt_labels), *[_p(t[k]) for k in DET_TARGETS], _stream()), "det_assign_classes")
     return t
 
 
@@ -1626,12 +1678,17 @@ def _rows(t, name, b, n, width):
     return t, ld
 
 
-def _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins):
+def _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins, cls_num=None):
     base_xyz = _req(base_xyz, "base_xyz", torch.float32, 3, 3)
     b, n, _ = base_xyz.shape
     nv = tg["vote_mask"].shape[1]
+    if cls_num is not None:
+        cls_num = _classes(cls_num)
+        lab = tg["cls_label"]
+        if not isinstance(lab, torch.Tensor) or lab.dtype != torch.float32 or tuple(lab.shape) != (b, n, cls_num):
+            raise ValueError("target cls_label must be float32 (%d, %d, %d), got %s" % (b, n, cls_num, tuple(getattr(lab, "shape", ()))))
     ins = [(base_xyz,)]
-    for t, name, w in ((pred_cls, "pred_cls", 1), (pred_offset, "pred_offset", 6), (pred_angle_cls, "pred_angle_cls", angle_bins),
+    for t, name, w in ((pred_cls, "pred_cls", 1 if cls_num is None else cls_num), (pred_offset, "pred_offset", 6), (pred_angle_cls, "pred_angle_cls", angle_bins),
                        (pred_angle_res, "pred_angle_res", angle_bins)):
         ins.append(_rows(t, name, b, n, w))
     ins.append(_rows(vote_offset, "vote_offset", b, nv, 3))
@@ -1648,33 +1705,46 @@ def _det_args(ins, tg):
     return args + [_p(tg[k]) for k in _LOSS_TARGETS]
 
 
-def det_loss(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins=12):
+def det_loss(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins=12, cls_num=None):
     """The six detection losses (ssd3d_det_loss) -> (loss (6,) = cls, offset, angle bin, angle residual, corner, vote;
-    norm (3,) = the classification, positive and vote normalisers).  The head outputs are read in place."""
-    b, n, nv, ins = _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins)
+    norm (3,) = the classification, positive and vote normalisers).  The head outputs are read in place.
+    cls_num=C (ssd3d_det_loss_classes): pred_cls (b, n, [1,] C), tg of det_assign(cls_num=C); the classification loss
+    is the mean over the classes of the sigmoid cross-entropy."""
+    b, n, nv, ins = _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins,
+                                cls_num)
     dev = ins[0][0].device
     ws = torch.empty((int(lib().ssd3d_det_loss_workspace(b)),), dtype=torch.uint8, device=dev)
     loss = torch.empty((6,), dtype=torch.float32, device=dev)
     norm = torch.empty((3,), dtype=torch.float32, device=dev)
-    check(lib().ssd3d_det_loss(b, n, nv, int(angle_bins), *_det_args(ins, tg), _p(ws), _p(loss), _p(norm), _stream()), "det_loss")
+    if cls_num is None:
+        check(lib().ssd3d_det_loss(b, n, nv, int(angle_bins), *_det_args(ins, tg), _p(ws), _p(loss), _p(norm), _stream()), "det_loss")
+    else:
+        check(lib().ssd3d_det_loss_classes(b, n, nv, int(angle_bins), int(cls_num), *_det_args(ins, tg), _p(ws), _p(loss), _p(norm),
+                                           _stream()), "det_loss_classes")
     return loss, norm
 
 
-def det_loss_grad(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, grad_loss, norm, angle_bins=12):
+def det_loss_grad(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, grad_loss, norm, angle_bins=12,
+                  cls_num=None):
     """Backward of det_loss from grad_loss (6,) -> (grad_base_xyz (b, n, 3), grad_cls (b, n, 1), grad_reg (b, n, 6 + 2 *
-    angle_bins) laid out as the head's [offset | angle logits | angle residuals], grad_vote_offset (b, nv, 3))."""
-    b, n, nv, ins = _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins)
+    angle_bins) laid out as the head's [offset | angle logits | angle residuals], grad_vote_offset (b, nv, 3)).
+    cls_num=C (ssd3d_det_loss_grad_classes): grad_cls is (b, n, C)."""
+    b, n, nv, ins = _det_inputs(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins,
+                                cls_num)
     grad_loss, norm = _req(grad_loss, "grad_loss", torch.float32, 1, 6), _req(norm, "norm", torch.float32, 1, 3)
     dev = ins[0][0].device
     ldr = 6 + 2 * angle_bins
+    c = 1 if cls_num is None else int(cls_num)
     gbase = torch.empty((b, n, 3), dtype=torch.float32, device=dev)
-    gcls = torch.empty((b, n, 1), dtype=torch.float32, device=dev)
+    gcls = torch.empty((b, n, c), dtype=torch.float32, device=dev)
     greg = torch.empty((b, n, ldr), dtype=torch.float32, device=dev)
     gvote = torch.empty((b, nv, 3), dtype=torch.float32, device=dev)
-    check(lib().ssd3d_det_loss_grad(b, n, nv, int(angle_bins), *_det_args(ins, tg), _p(grad_loss), _p(norm), _p(gbase), _p(gcls), 1,
-                                    _p(greg), ldr, ctypes.c_void_p(greg.data_ptr() + 4 * 6), ldr,
-                                    ctypes.c_void_p(greg.data_ptr() + 4 * (6 + angle_bins)), ldr, _p(gvote), _stream()),
-          "det_loss_grad")
+    rest = (_p(grad_loss), _p(norm), _p(gbase), _p(gcls), c, _p(greg), ldr, ctypes.c_void_p(greg.data_ptr() + 4 * 6), ldr,
+            ctypes.c_void_p(greg.data_ptr() + 4 * (6 + angle_bins)), ldr, _p(gvote), _stream())
+    if cls_num is None:
+        check(lib().ssd3d_det_loss_grad(b, n, nv, int(angle_bins), *_det_args(ins, tg), *rest), "det_loss_grad")
+    else:
+        check(lib().ssd3d_det_loss_grad_classes(b, n, nv, int(angle_bins), c, *_det_args(ins, tg), *rest), "det_loss_grad_classes")
     return gbase, gcls, greg, gvote
 
 
@@ -1682,10 +1752,10 @@ class _DetLoss(torch.autograd.Function):
     """det_loss forward; det_loss_grad backward (one kernel for every input's gradient)."""
 
     @staticmethod
-    def forward(ctx, base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins):
-        loss, norm = det_loss(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins)
+    def forward(ctx, base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins, cls_num):
+        loss, norm = det_loss(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins, cls_num)
         ctx.save_for_backward(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, norm)
-        ctx.tg, ctx.angle_bins = tg, angle_bins
+        ctx.tg, ctx.angle_bins, ctx.cls_num = tg, angle_bins, cls_num
         return loss
 
     @staticmethod
@@ -1693,14 +1763,17 @@ class _DetLoss(torch.autograd.Function):
         base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, norm = ctx.saved_tensors
         nb = ctx.angle_bins
         gbase, gcls, greg, gvote = det_loss_grad(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset,
-                                                 ctx.tg, g.contiguous(), norm, nb)
+                                                 ctx.tg, g.contiguous(), norm, nb, ctx.cls_num)
         return (gbase, gcls.reshape(pred_cls.shape), greg[..., :6].reshape(pred_offset.shape),
-                greg[..., 6:6 + nb].reshape(pred_angle_cls.shape), greg[..., 6 + nb:].reshape(pred_angle_res.shape), gvote, None, None)
+                greg[..., 6:6 + nb].reshape(pred_angle_cls.shape), greg[..., 6 + nb:].reshape(pred_angle_res.shape), gvote, None, None,
+                None)
 
 
-def det_loss_train(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins=12):
-    """Differentiable det_loss -> loss (6,); gradients reach base_xyz, the four head outputs and vote_offset."""
-    return _DetLoss.apply(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, int(angle_bins))
+def det_loss_train(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, angle_bins=12, cls_num=None):
+    """Differentiable det_loss -> loss (6,); gradients reach base_xyz, the four head outputs and vote_offset.
+    cls_num=C: the class form of det_loss / det_loss_grad."""
+    return _DetLoss.apply(base_xyz, pred_cls, pred_offset, pred_angle_cls, pred_angle_res, vote_offset, tg, int(angle_bins),
+                          None if cls_num is None else _classes(cls_num))
 
 
 # ---- training-scene augmentation (csrc/augment.cu, DESIGN.md section 3.12) -------------------------------------------

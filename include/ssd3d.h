@@ -350,6 +350,19 @@ int ssd3d_bev_nms(int b, int n, const float *boxes, const float *scores, float i
 int ssd3d_bev_nms_counted(int b, int n, const float *boxes, const float *scores, const int *n_valid, float iou_threshold,
                           int max_output, int cls_id, float *out_block, int *out_cnt, ssd3d_stream_t stream);
 
+/* The most classes of the multi-class entry points: the eight KITTI class names of the reference
+ * (g_type_mean_size, lib/utils/model_util.py:19-26), and the portable thread-block cluster size. */
+#define SSD3D_MAX_CLASSES 8
+/* Per-class BEV NMS of postprocessor.py:49-120 in one launch (DESIGN.md section 3.17): for every class c < cls_num
+ * (1..SSD3D_MAX_CLASSES) the NMS of ssd3d_bev_nms on scores[b, n, cls_num] column c over the shared boxes [b, n, 7],
+ * at most max_output boxes per class.  out_block [b, cls_num * max_output, 9] holds class 0's kept rows in kept order,
+ * then class 1's, and so on, column 8 = c; out_cnt [b] = rows kept over all classes; rows at or past it are zero.  Each
+ * class's rows are the bits ssd3d_bev_nms(..., cls_id = c) writes on that column, so at cls_num = 1 the block is
+ * ssd3d_bev_nms's.  One thread-block cluster of cls_num CTAs per scene; fails before launching when such a cluster
+ * (each CTA with the shared memory of ssd3d_bev_nms at n, max_output) cannot be placed on the device. */
+int ssd3d_bev_nms_classes(int b, int n, int cls_num, const float *boxes, const float *scores, float iou_threshold,
+                          int max_output, float *out_block, int *out_cnt, ssd3d_stream_t stream);
+
 /* ---- PointRCNN's region pool (DESIGN.md section 3.16) -------------------------------------------- */
 
 /* query_boxes_3d_points (lib/utils/tf_ops/grouping/tf_grouping_g.cu:27-94, queryBoxes3dPointsLauncher :447-449):
@@ -458,6 +471,11 @@ int ssd3d_vote_translate(long rows, const float *xyz, const float *offsets, int 
  * -> boxes[rows,7] = (x, y, z, l, h, w, ry), scores[rows]. */
 int ssd3d_decode_dist_anchor_free(long rows, int angle_bins, const float *center_xyz, const float *pred_reg, int ld_reg,
                                   const float *pred_cls, int ld_cls, float *boxes, float *scores, ssd3d_stream_t stream);
+/* ssd3d_decode_dist_anchor_free with cls_num (1..SSD3D_MAX_CLASSES, <= ld_cls) sigmoid scores per row:
+ * scores[rows, cls_num], column c from pred_cls column c as the single-class form computes column 0; the same boxes. */
+int ssd3d_decode_dist_anchor_free_classes(long rows, int angle_bins, int cls_num, const float *center_xyz, const float *pred_reg,
+                                          int ld_reg, const float *pred_cls, int ld_cls, float *boxes, float *scores,
+                                          ssd3d_stream_t stream);
 /* decode_bin_anchor on the anchors of generate_3d_anchors_by_point_tf + the score sigmoid (lib/utils/anchor_decoder.py:
  * 115-164, lib/utils/generate_anchors.py:33-65; PointRCNN's 'Bin-Anchor' regression, one anchor size per point).
  * pred_reg[rows, ld_reg] = [x_bin | x_res | z_bin | z_res (bin_num each) | y_res | 3 size residuals | angle_bins logits |
@@ -504,6 +522,14 @@ int ssd3d_det_assign(int b, int n, int nv, int g, int angle_bins, const float *b
                      const float *gt_boxes, const int *gt_labels, int *assigned_idx, float *assigned_box, float *pmask,
                      float *nmask, float *cls_label, int *angle_bin, float *angle_res, float *offset_target, float *vote_mask,
                      float *vote_target, ssd3d_stream_t stream);
+/* ssd3d_det_assign for cls_num classes (1..SSD3D_MAX_CLASSES; labels 1..cls_num): every target but cls_label is the
+ * class-agnostic one of ssd3d_det_assign, bit for bit.  cls_label [b, n, cls_num]: column c is the centre-ness label of
+ * a positive whose box has label c + 1, else 0 (one_hot(label - 1, cls_num) * centre-ness, loss_builder.py:58-96); a
+ * label outside 1..cls_num gives a zero row and stays a regression positive. */
+int ssd3d_det_assign_classes(int b, int n, int nv, int g, int angle_bins, int cls_num, const float *base_xyz,
+                             const float *vote_base, const float *gt_boxes, const int *gt_labels, int *assigned_idx,
+                             float *assigned_box, float *pmask, float *nmask, float *cls_label, int *angle_bin, float *angle_res,
+                             float *offset_target, float *vote_mask, float *vote_target, ssd3d_stream_t stream);
 /* The six losses of LossBuilder.forward (loss_builder.py) for 'Center-ness' sigmoid classification, 'Dist-Anchor-free'
  * regression, the corner loss and the vote loss, from the head outputs read in place through row strides
  * (pred_cls [b, n, ld_cls] column 0, pred_offset [.., ld_offset] columns 0:6, pred_angle_cls / pred_angle_res columns
@@ -522,6 +548,16 @@ int ssd3d_det_loss(int b, int n, int nv, int angle_bins, const float *base_xyz, 
                    const float *assigned_box, const float *pmask, const float *nmask, const float *cls_label,
                    const int *angle_bin, const float *angle_res, const float *vote_mask, const float *vote_target,
                    void *workspace, float *loss, float *norm, ssd3d_stream_t stream);
+/* ssd3d_det_loss for cls_num sigmoid classes (1..SSD3D_MAX_CLASSES): pred_cls columns 0:cls_num (ld_cls >= cls_num),
+ * cls_label [b, n, cls_num] of ssd3d_det_assign_classes.  The classification term of a row is the mean over the classes
+ * of the sigmoid cross-entropy, summed over the classes in order in double; the other five losses are ssd3d_det_loss's.
+ * At cls_num = 1 it is ssd3d_det_loss bit for bit. */
+int ssd3d_det_loss_classes(int b, int n, int nv, int angle_bins, int cls_num, const float *base_xyz, const float *pred_cls,
+                           int ld_cls, const float *pred_offset, int ld_offset, const float *pred_angle_cls, int ld_angle_cls,
+                           const float *pred_angle_res, int ld_angle_res, const float *vote_offset, int ld_vote,
+                           const float *assigned_box, const float *pmask, const float *nmask, const float *cls_label,
+                           const int *angle_bin, const float *angle_res, const float *vote_mask, const float *vote_target,
+                           void *workspace, float *loss, float *norm, ssd3d_stream_t stream);
 /* Backward of ssd3d_det_loss from grad_loss[6] (device) and the norm[3] it wrote: grad_base_xyz [b, n, 3] (through the
  * offset target and the corner loss's decoded box; none through the centre-ness label, which TF stops),
  * grad_cls / grad_offset / grad_angle_cls / grad_angle_res with row strides ldg_* (the residual gradient only at the
@@ -536,6 +572,18 @@ int ssd3d_det_loss_grad(int b, int n, int nv, int angle_bins, const float *base_
                         float *grad_cls, int ldg_cls, float *grad_offset, int ldg_offset, float *grad_angle_cls,
                         int ldg_angle_cls, float *grad_angle_res, int ldg_angle_res, float *grad_vote_offset,
                         ssd3d_stream_t stream);
+/* Backward of ssd3d_det_loss_classes: grad_cls columns 0:cls_num (ldg_cls >= cls_num) = (sigmoid(x_c) - label_c) *
+ * cls_mask * grad_loss[0] / norm[0] / cls_num; every other gradient is ssd3d_det_loss_grad's.  At cls_num = 1 it is
+ * ssd3d_det_loss_grad bit for bit. */
+int ssd3d_det_loss_grad_classes(int b, int n, int nv, int angle_bins, int cls_num, const float *base_xyz, const float *pred_cls,
+                                int ld_cls, const float *pred_offset, int ld_offset, const float *pred_angle_cls, int ld_angle_cls,
+                                const float *pred_angle_res, int ld_angle_res, const float *vote_offset, int ld_vote,
+                                const float *assigned_box, const float *pmask, const float *nmask, const float *cls_label,
+                                const int *angle_bin, const float *angle_res, const float *vote_mask, const float *vote_target,
+                                const float *grad_loss, const float *norm, float *grad_base_xyz,
+                                float *grad_cls, int ldg_cls, float *grad_offset, int ldg_offset, float *grad_angle_cls,
+                                int ldg_angle_cls, float *grad_angle_res, int ldg_angle_res, float *grad_vote_offset,
+                                ssd3d_stream_t stream);
 
 /* ---- sharded step: exchange over NVLink peer memory ---------------------------------------- */
 

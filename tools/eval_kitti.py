@@ -36,10 +36,14 @@ def main(argv=None):
     ap.add_argument("--classes", default="Car", help="comma-separated class list of the model")
     ap.add_argument("--model", default="3dssd", choices=("3dssd", "pointrcnn", "pointrcnn-rpn"))
     args = ap.parse_args(argv)
+    pkg = importlib.import_module("3dssd_b200")
+    try:
+        cls_list = pkg.config.check_cls_list(args.classes)
+    except ValueError as e:
+        raise SystemExit("eval_kitti.py: --classes: %s" % e)
 
     import numpy as np
     import torch
-    pkg = importlib.import_module("3dssd_b200")
     io, ev = pkg.kitti_io, pkg.evaluation
     if not torch.cuda.is_available():
         raise SystemExit("eval_kitti.py needs a CUDA device (there is no CPU path)")
@@ -48,16 +52,20 @@ def main(argv=None):
     if not paths:
         raise SystemExit("no *.npy sample dicts under %s" % args.samples)
     weights = io.params_from_tf_variables(dict(np.load(args.weights)))
+    if args.model == "3dssd":
+        width = np.asarray(weights["pred_cls/weights"]).shape[-1] if "pred_cls/weights" in weights else None
+        if width != len(cls_list):
+            raise SystemExit("eval_kitti.py: the weights' pred_cls has %s class column(s), --classes names %d (%s)"
+                             % (width, len(cls_list), ",".join(cls_list)))
     if args.model == "pointrcnn-rpn":
         return rpn_recall(pkg, args, paths, weights, dev)
     if args.model == "pointrcnn":
         rcnn = pkg.PointRCNN(params=weights, device=dev)
         detect = lambda pts: rcnn.forward(pts)
     else:
-        head = pkg.DetectionHead(params=weights, device=dev)
+        head = pkg.DetectionHead(params=weights, device=dev, cls_num=len(cls_list))
         net = pkg.SABackbone(params=weights, in_channels=1, device=dev, head=head)
         detect = lambda pts: net.detections(*net.forward(pts)[:2])
-    cls_list = tuple(c.strip() for c in args.classes.split(","))
     acc = ev.EvalAccumulator(cls_list=cls_list, cls_thresh=args.cls_thresh)
     for i in range(0, len(paths), args.batch):
         samples = [io.read_sample(p) for p in paths[i:i + args.batch]]

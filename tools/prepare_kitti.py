@@ -47,7 +47,8 @@ def run(root, split, list_path, out, classes=("Car",), gt=True, mixup_db=None, b
             t1 = time.perf_counter()
             st["t_read"] += t1 - t0
             nxt = pool.submit(read, first + batch) if first + batch < len(ids) else None
-            written, skipped, db = PR.run_batch(frames, device, with_db=bool(mixup_db))
+            written, skipped, db = PR.run_batch(frames, device, with_db=bool(mixup_db),
+                                                db_classes=tuple(range(1, len(classes) + 1)))
             t2 = time.perf_counter()
             st["t_gpu"] += t2 - t1
             for pos, d in written:
@@ -86,11 +87,15 @@ def main(argv=None):
     ap.add_argument("--mixup-db", default=None, help="also write the mixup object database of the written frames (.npz)")
     ap.add_argument("--batch", type=int, default=PR.BATCH, help="frames per GPU batch")
     a = ap.parse_args(argv)
+    try:
+        classes = pkg.config.check_cls_list(a.classes)
+    except ValueError as e:
+        raise SystemExit("prepare_kitti.py: --classes: %s" % e)
     if not torch.cuda.is_available():
         raise SystemExit("prepare_kitti.py runs the filters on a CUDA device; none is available (there is no CPU path)")
     if a.batch < 1:
         raise SystemExit("--batch must be at least 1")
-    run(a.root, a.split, a.list, a.out, tuple(c.strip() for c in a.classes.split(",")), not a.no_gt, a.mixup_db, a.batch,
+    run(a.root, a.split, a.list, a.out, classes, not a.no_gt, a.mixup_db, a.batch,
         torch.device("cuda", 0))
     return 0
 

@@ -4,7 +4,9 @@ loss, per-rank clip, rank-ordered gradient mean, TF-style Adam under the step-dr
     python tools/train.py --steps N [--batch 4] [--gpus G] [--ckpt DIR] [--resume FILE] [--data DIR] [--augment]
     torchrun --nproc_per_node G tools/train.py --gpus G ...
 
-Scenes are synth.kitti_like_with_boxes draws (a fresh seed every step) or, with --data, the reference's per-frame sample
+--classes Car,Pedestrian,Cyclist (default Car) sets the head's class channels (labels 1..C in that order, as
+tools/prepare_kitti.py --classes writes them).  Scenes are synth.kitti_like_with_boxes draws for the one class Car,
+synth.kitti_like_multiclass draws over --classes otherwise (a fresh seed every step) or, with --data, the reference's per-frame sample
 dicts (*.npy, kitti_io.read_sample) taken in order, --batch per rank.  The losses are logged every --log-interval steps
 (reading them synchronises; the steps in between do not), a checkpoint named model-<global_step>.npz is written to --ckpt
 every Solver.checkpoint_interval steps and after the last one (rank 0), and --resume continues from such a file at its
@@ -13,8 +15,8 @@ step, learning rate and BatchNorm decay.
 With --augment the scenes go through the reference's training augmentation on the GPU (augment.Augmentor: flip,
 per-object noise, global rotation and scale, the context filter, then the choice of --points points), with draws seeded
 from (--seed, step, rank); without it the points are chosen on the host and nothing is augmented.  --mixup DB.npz (an
-object database of tools/build_mixup_db.py) adds the mixup paste before those stages: each scene draws 15 Car objects at
-each step (mixup.Sampler, seeded from --seed, rank and the scene's place in the batch) and keeps those that collide with
+object database of tools/build_mixup_db.py) adds the mixup paste before those stages: each scene draws --mixup-numbers
+objects of each of --mixup-classes (default 15 Car) at each step (mixup.Sampler, seeded from --seed, rank and the scene's place in the batch) and keeps those that collide with
 nothing, standing on the frame's ground plane -- read from --planes DIR (<DIR>/%06d.txt per sample name) with --data,
 the flat y = 1.65 plane of the synthetic scenes without it."""
 import argparse
@@ -34,8 +36,11 @@ S = importlib.import_module("3dssd_b200.solver")
 synth = importlib.import_module("3dssd_b200.synth")
 
 
-def synthetic_batch(step, rank, world, batch, points, max_boxes):
-    p, b, l = synth.kitti_like_with_boxes(world * batch, points, max_boxes, seed=1000 + step)
+def synthetic_batch(step, rank, world, batch, points, max_boxes, classes=("Car",)):
+    if tuple(classes) == ("Car",):
+        p, b, l = synth.kitti_like_with_boxes(world * batch, points, max_boxes, seed=1000 + step)
+    else:
+        p, b, l = synth.kitti_like_multiclass(world * batch, points, max_boxes, classes, seed=1000 + step)
     return tuple(pkg.dist.shard_batch(torch.from_numpy(x), rank, world) for x in (p, b, l))
 
 
@@ -48,8 +53,8 @@ def file_batch(files, step, rank, world, batch, points):
     return block, torch.from_numpy(boxes), torch.from_numpy(labels)
 
 
-def synthetic_ragged(step, rank, world, batch, points, max_boxes):
-    p, b, l = synthetic_batch(step, rank, world, batch, points, max_boxes)
+def synthetic_ragged(step, rank, world, batch, points, max_boxes, classes=("Car",)):
+    p, b, l = synthetic_batch(step, rank, world, batch, points, max_boxes, classes)
     n = p.shape[0]
     offsets = torch.arange(0, (n + 1) * points, points, dtype=torch.int32)
     return p.reshape(-1, 4), offsets, None, b, l
@@ -62,7 +67,7 @@ def file_ragged(files, step, rank, world, batch):
                                                      for i, s in enumerate(samples)]
 
 
-def main():
+def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, required=True, help="training steps to run in this invocation")
     ap.add_argument("--batch", type=int, default=4, help="scenes per rank (BATCH_SIZE of 3dssd.yaml)")
@@ -78,7 +83,18 @@ def main():
     ap.add_argument("--seed", type=int, default=0, help="seed of the augmentation draws")
     ap.add_argument("--mixup", default=None, help="object database (.npz of tools/build_mixup_db.py): paste objects first")
     ap.add_argument("--planes", default=None, help="directory of the KITTI ground planes of --data (with --mixup)")
-    a = ap.parse_args()
+    ap.add_argument("--classes", default="Car", help="comma-separated class list of the head (DATASET.KITTI.CLS_LIST)")
+    ap.add_argument("--mixup-classes", default="Car", help="comma-separated classes the mixup paste draws (names of --classes)")
+    ap.add_argument("--mixup-numbers", default="15", help="comma-separated objects per scene of each --mixup-classes entry")
+    a = ap.parse_args(argv)
+    try:
+        classes = pkg.config.check_cls_list(a.classes)
+        mix_names = pkg.config.check_cls_list(a.mixup_classes)
+        mix_numbers = tuple(int(v) for v in a.mixup_numbers.split(","))
+    except ValueError as e:
+        raise SystemExit("train.py: %s" % e)
+    if a.mixup and (any(c not in classes for c in mix_names) or len(mix_numbers) != len(mix_names) or min(mix_numbers) < 0):
+        raise SystemExit("train.py: --mixup-classes must name classes of --classes, with one --mixup-numbers entry (>= 0) each")
     if a.mixup and not a.augment:
         raise SystemExit("--mixup works with --augment")
     if a.mixup and a.data and not a.planes:
@@ -93,7 +109,7 @@ def main():
     torch.cuda.set_device(dev)
     arch, solver = pkg.config.ARCH_3DSSD, S.Solver()
     d = pkg.params.init_params(arch, 1, seed=0)
-    d.update(pkg.params.init_head_params(pkg.config.layer_channels(arch, 1)[-1], seed=1))
+    d.update(pkg.params.init_head_params(pkg.config.layer_channels(arch, 1)[-1], cls_channels=len(classes), seed=1))
     tp = pkg.params.TrainableParams(d, dev)
     dp = None
     if world > 1:
@@ -112,7 +128,8 @@ def main():
     aug = pkg.augment.Augmentor(a.points, dev) if a.augment else None
     MX = pkg.mixup
     db = MX.ObjectDatabase.load(a.mixup, dev) if a.mixup else None
-    sampler = MX.Sampler(db, seed=a.seed) if db is not None else None
+    sampler = (MX.Sampler(db, seed=a.seed, classes=tuple(classes.index(c) + 1 for c in mix_names), numbers=mix_numbers)
+               if db is not None else None)
     log("start at global_step %d: learning rate %.6g, bn decay %.6g, %d rank(s) x %d scenes"
         % (tr.global_step, solver.learning_rate(tr.global_step), solver.bn_decay(tr.global_step), world, a.batch))
 
@@ -133,7 +150,7 @@ def main():
             save()
         if aug is not None:
             if files is None:
-                cloud, offsets, sem, boxes, labels = synthetic_ragged(step, rank, world, a.batch, a.points, a.max_boxes)
+                cloud, offsets, sem, boxes, labels = synthetic_ragged(step, rank, world, a.batch, a.points, a.max_boxes, classes)
                 names = None
             else:
                 (cloud, offsets, sem, boxes, labels), names = file_ragged(files, step, rank, world, a.batch)
@@ -149,7 +166,7 @@ def main():
             draws = pkg.augment.draw(boxes.shape[0], rows, total, a.points, gen, dev)
             pts, boxes, labels = aug(cloud, offsets, sem, boxes, labels, draws, mixup=mix)
         elif files is None:
-            pts, boxes, labels = synthetic_batch(step, rank, world, a.batch, a.points, a.max_boxes)
+            pts, boxes, labels = synthetic_batch(step, rank, world, a.batch, a.points, a.max_boxes, classes)
         else:
             pts, boxes, labels = file_batch(files, step, rank, world, a.batch, a.points)
         xyz, feat = pkg.tf_ops.split_points(pts.to(dev, non_blocking=True))
