@@ -131,6 +131,14 @@ _SIGNATURES = {
     "ssd3d_peer_allreduce_mean": [c_void_p, ctypes.c_size_t, c_void_p, c_void_p, c_int, c_int, c_int] + [ctypes.c_size_t] * 10 +
                                  [c_void_p, c_void_p],
     "ssd3d_bn_moving_update_ranks": [c_void_p, c_long, c_void_p, c_long, c_int, c_float, c_void_p],
+    "ssd3d_bn_sync_area_bytes": [c_int, c_int],
+    "ssd3d_bn_sync_resident_ctas": [],
+    "ssd3d_bn_train_sync": [c_long, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_void_p,
+                            c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int,
+                            ctypes.c_size_t, c_void_p, c_void_p],
+    "ssd3d_bn_train_grad_sync": [c_long, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int,
+                                 ctypes.c_size_t, c_void_p, c_void_p],
     "ssd3d_adam_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_long, c_void_p, c_float, c_float, c_float, c_int, c_void_p,
                         c_void_p, c_void_p],
     "ssd3d_weight_operands": [c_void_p, c_void_p, c_int, c_long, c_void_p, c_void_p],
@@ -176,7 +184,7 @@ def lib():
                                                    "ssd3d_linear_wgrad_workspace", "ssd3d_bn_train_grad_workspace",
                                                    "ssd3d_det_loss_workspace", "ssd3d_grad_clip_scale_workspace",
                                                    "ssd3d_eval_workspace", "ssd3d_augment_workspace", "ssd3d_region_pool_smem",
-                                                   "ssd3d_prepare_workspace") else c_int
+                                                   "ssd3d_prepare_workspace", "ssd3d_bn_sync_area_bytes") else c_int
             if name == "ssd3d_fps_temp_elems":
                 fn.restype = c_long
         l.ssd3d_last_error.restype = ctypes.c_char_p

@@ -70,6 +70,7 @@ AGGREGATION_POINTRCNN = False      # MODEL.NETWORK.AGGREGATION_SA_FEATURE (tiny_
 # The class list of the single-stage model (DATASET.KITTI.CLS_LIST): label k is the 1-based place of the class in the
 # list, 0 is padding.  The valid names are the eight KITTI keys of g_type_mean_size (lib/utils/model_util.py:19-26),
 # with their mean (l, h, w) in metres.
+SYNC_BN = False                # MODEL.NETWORK.SYNC_BN: BatchNorm statistics over every GPU's scenes (dist.DataParallel)
 CLS_LIST = ('Car',)
 CLASS_MEAN_SIZE = {
     'Car': (3.88311640418, 1.62856739989, 1.52563191462), 'Van': (5.06763659, 1.9007158, 2.20532825),

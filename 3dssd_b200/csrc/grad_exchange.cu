@@ -35,24 +35,13 @@
 // CTAs of a launch must be co-resident on their device (ssd3d_peer_allreduce_resident_ctas); a wait of ~4 s gives up,
 // counts itself in state[2] instead of hanging the GPU, and that CTA writes NaN into its part of the gradient.
 #include "common.cuh"
+#include "peer_sync.cuh"
 
 namespace ssd3d {
 
 constexpr int CLIP_BLOCKS = 256, CLIP_THREADS = 256;   // the fixed reduction tree of the norm (ssd3d.h)
 constexpr int AR_THREADS = 256;
 static_assert(CLIP_BLOCKS == CLIP_THREADS, "the finalize reads one partial per thread");
-constexpr long long kSpinLimit = 1LL << 33;            // ~4 s of clock64 at H100 clocks
-
-__device__ __forceinline__ int ar_ld_acquire_sys(const int *p)
-{
-    int v;
-    asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void ar_st_release_sys(int *p, int v)
-{
-    asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
 
 // s[0..CLIP_THREADS) -> s[0], halving strides: the same tree in every block and in the finalize
 __device__ __forceinline__ double tree_sum(double *s, int tid)
@@ -113,8 +102,8 @@ struct AllreduceParams {
 __device__ __forceinline__ int ar_wait(const int *flag, int seq, int *state)
 {
     const long long t0 = clock64();
-    while (ar_ld_acquire_sys(flag) < seq) {
-        if (clock64() - t0 > kSpinLimit) { atomicAdd(state + 2, 1); return 0; }   // a peer never came: counted, not hung
+    while (ld_acquire_sys(flag) < seq) {
+        if (clock64() - t0 > kPeerSpinLimit) { atomicAdd(state + 2, 1); return 0; }   // a peer never came: counted, not hung
     }
     return 1;
 }
@@ -159,7 +148,7 @@ peer_allreduce_mean_kernel(const AllreduceParams p)
     __threadfence_system();
     __syncthreads();
     if (tid == 0) {
-        for (int q = 0; q < G; q++) ar_st_release_sys(reinterpret_cast<int *>(p.peer_base[q] + f1o) + (size_t)me * gridDim.x + j, seq);
+        for (int q = 0; q < G; q++) st_release_sys(reinterpret_cast<int *>(p.peer_base[q] + f1o) + (size_t)me * gridDim.x + j, seq);
         for (int q = 0; q < G; q++) s_ok &= ar_wait(reinterpret_cast<const int *>(mine + f1o) + (size_t)q * gridDim.x + j, seq, p.state);
     }
     __syncthreads();
@@ -186,7 +175,7 @@ peer_allreduce_mean_kernel(const AllreduceParams p)
     __threadfence_system();
     __syncthreads();
     if (tid == 0) {
-        for (int q = 0; q < G; q++) ar_st_release_sys(reinterpret_cast<int *>(p.peer_base[q] + f2o) + (size_t)me * gridDim.x + j, seq);
+        for (int q = 0; q < G; q++) st_release_sys(reinterpret_cast<int *>(p.peer_base[q] + f2o) + (size_t)me * gridDim.x + j, seq);
         for (int q = 0; q < G; q++) s_ok &= ar_wait(reinterpret_cast<const int *>(mine + f2o) + (size_t)q * gridDim.x + j, seq, p.state);
     }
     __syncthreads();

@@ -18,19 +18,9 @@
 // copy-out included -- has finished (same stream).  Every rank must call the exchange the same number of times.  A wait
 // that lasts ~4 s gives up and counts itself in state[2] (a rank that died must not hang the others' GPUs).
 #include "common.cuh"
+#include "peer_sync.cuh"
 
 namespace ssd3d {
-
-__device__ __forceinline__ int ld_acquire_sys(const int *p)
-{
-    int v;
-    asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release_sys(int *p, int v)
-{
-    asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
 
 struct PeerGatherParams {
     const uint4 *src;          // my slice (slice_bytes, 16-byte multiple)
@@ -60,7 +50,7 @@ peer_allgather_kernel(const PeerGatherParams p)
         const int *flag = reinterpret_cast<const int *>(mine + p.flag_off[par]) + peer;
         const long long t0 = clock64();
         while (ld_acquire_sys(flag) < seq) {
-            if (clock64() - t0 > (1LL << 33)) { atomicAdd(p.state + 2, 1); break; }   // ~4 s: a peer never came (counted, not hung)
+            if (clock64() - t0 > kPeerSpinLimit) { atomicAdd(p.state + 2, 1); break; }   // ~4 s: a peer never came (counted, not hung)
         }
     }
     __syncthreads();

@@ -12,6 +12,7 @@ gathered result is read through views of the receive buffer -- no pack / unpack 
 beyond graph.replay().
 """
 import contextlib
+import functools
 import os
 from typing import NamedTuple
 
@@ -190,6 +191,92 @@ def gather_detections(block, count, total_scenes, group=None):
     return g.result()
 
 
+# ---- SyncBN (DESIGN.md section 3.18) --------------------------------------------------------------------------------
+
+BN_SYNC_THREADS = 128         # channels per exchange CTA of csrc/bn.cu's SyncBN finalize
+
+
+def bn_sync_area_bytes(world, c):
+    """Bytes of one (BN scope, direction) area of csrc/bn.cu's SyncBN (ssd3d_bn_sync_area_bytes): per parity a data block
+    [world][3][c] of doubles and a flag block [world][ceil(c / 128)] of int32, each rounded up to 16 bytes."""
+    world, c = int(world), int(c)
+    if world < 1 or c < 1:
+        raise ValueError("bn_sync_area_bytes: world=%d c=%d" % (world, c))
+    data = _round(world * 3 * c * 8, 16)
+    flags = _round(world * (-(-c // BN_SYNC_THREADS)) * 4, 16)
+    return 2 * data + 2 * flags
+
+
+class BnSyncLayout(NamedTuple):
+    """areas[scope] = (forward area offset, backward area offset) in bytes inside every rank's symmetric buffer;
+    nbytes: the share's size."""
+    areas: dict
+    nbytes: int
+
+
+def bn_sync_layout(channels, world, base=0):
+    """BnSyncLayout of the BN scopes `channels` = [(scope, c), ...] over `world` ranks from byte offset `base` (a 16-byte
+    multiple): every scope gets its own forward area, then its own backward area, in the order given."""
+    base = int(base)
+    if base % 16:
+        raise ValueError("bn_sync_layout: base=%d must be a 16-byte multiple" % base)
+    areas, off = {}, base
+    for scope, c in channels:
+        if scope in areas:
+            raise ValueError("bn_sync_layout: scope %s listed twice" % scope)
+        n = bn_sync_area_bytes(world, c)
+        areas[scope] = (off, off + n)
+        off += 2 * n
+    return BnSyncLayout(areas, off - base)
+
+
+def _bn_channels(tp):
+    return [(s, tp.tensors[s + "/bn/moving_mean"].numel()) for s in tp.bn_scopes()]
+
+
+class BnSync:
+    """The SyncBN handle of one rank (TrainableParams.start_bn_sync): which ranks (peers, world, rank), where each BN
+    scope's forward and backward exchange live in the symmetric buffers (bn_sync_layout from byte `base`), and their
+    replay counters and time-out counts (state [scopes, 2, 4] int32 on the device).  Every scope has its own areas,
+    flags and counters, so the order in which scopes exchange does not matter; each must exchange once per step in each
+    direction on every rank.  before_exchange(scope, direction): optional host callable run just before each launch
+    (direction 0 forward, 1 backward): tests that simulate ranks on one device bring the ranks together with it."""
+
+    def __init__(self, tp, peers, world, rank, base=0, before_exchange=None):
+        from .tf_ops import BnSyncSlot
+        self.world, self.rank = int(world), int(rank)
+        if not 0 <= self.rank < self.world:
+            raise ValueError("BnSync: rank=%d outside world=%d" % (rank, world))
+        if not isinstance(peers, torch.Tensor) or peers.dtype != torch.int64 or peers.numel() != self.world:
+            raise ValueError("BnSync: peers must be an int64 tensor of world=%d bases" % self.world)
+        self.layout = bn_sync_layout(_bn_channels(tp), self.world, base)
+        self.state = torch.zeros((len(self.layout.areas), 2, 4), dtype=torch.int32, device=tp.device)
+        self._slots = {}
+        for i, (scope, offs) in enumerate(self.layout.areas.items()):
+            self._slots[scope] = tuple(
+                BnSyncSlot(peers, self.world, self.rank, off, self.state[i, d],
+                           None if before_exchange is None else functools.partial(before_exchange, scope, d))
+                for d, off in enumerate(offs))
+
+    @staticmethod
+    def symmetric_bytes(tp, world):
+        return bn_sync_layout(_bn_channels(tp), world).nbytes
+
+    def slots(self, scope):
+        """(forward, backward) tf_ops.BnSyncSlot of `scope`."""
+        if scope not in self._slots:
+            raise ValueError("BnSync: %s has no BatchNorm" % scope)
+        return self._slots[scope]
+
+    def replays(self):
+        """[scopes, 2] exchanges completed per scope and direction (a view of the device state)."""
+        return self.state[:, :, 0]
+
+    def timeouts(self):
+        """Waits that gave up (a peer that never arrived): 0 in a healthy run.  Synchronises."""
+        return int(self.state[:, :, 2].sum().item())
+
+
 # ---- data-parallel training (DESIGN.md section 3.9) -----------------------------------------------------------------
 
 ALLREDUCE_CTAS = 64           # CTAs per rank of one allreduce launch; all must be co-resident on the device
@@ -246,6 +333,9 @@ class DataParallel:
     tf_util.py:438-443): each rank clips its own gradient to global norm 5, the clipped gradients are averaged in rank
     order, and every rank's batch statistics update the moving averages, in rank order.  Every rank ends a step with the
     same gradient bits and the same statistics; with the same elementwise optimizer the replicas stay identical.
+    sync_bn=True (the reference's MODEL.NETWORK.SYNC_BN) normalises every BatchNorm with the statistics of all ranks'
+    rows instead (BnSync, DESIGN.md section 3.18); the moving statistics are then updated once per step, in the forward,
+    with those statistics, and exchange() leaves them alone.
 
         dp = DataParallel(tp, arena)                # arena: PeerArena of >= DataParallel.symmetric_bytes(tp, world)
         for step ...:
@@ -261,7 +351,8 @@ class DataParallel:
     rank=r) runs ranks simulated on one device (tests); nothing is broadcast.  Every rank must call exchange() the same
     number of times; nothing in a step synchronises the host."""
 
-    def __init__(self, tp, arena=None, *, peers=None, world=None, rank=None, ctas=ALLREDUCE_CTAS, clip_norm=CLIP_NORM):
+    def __init__(self, tp, arena=None, *, peers=None, world=None, rank=None, ctas=ALLREDUCE_CTAS, clip_norm=CLIP_NORM,
+                 sync_bn=False, before_exchange=None):
         from . import tf_ops
         self._tf_ops = tf_ops
         self.tp, self.clip_norm = tp, float(clip_norm)
@@ -286,10 +377,13 @@ class DataParallel:
         self.slice_floats = _round(_HEAD_FLOATS + self.nstats, 4)
         self.slice_bytes = 4 * self.slice_floats
         ar_bytes, ga_bytes = self._share_bytes(self.grad.numel(), self.slice_bytes, self.world, ctas)
+        sb_bytes = BnSync.symmetric_bytes(tp, self.world) if sync_bn else 0
         if arena is not None:
             ar_base, ga_base = arena.take(ar_bytes), arena.take(ga_bytes)
+            sb_base = arena.take(sb_bytes) if sync_bn else 0
         else:
             ar_base, ga_base = 0, _round(ar_bytes, 256)
+            sb_base = ga_base + _round(ga_bytes, 256)
         self.layout = allreduce_layout(self.grad.numel(), self.world, ctas, base=ar_base)
         recv, flag, _ = peer_layout(self.world, self.slice_bytes)
         self.recv_off = (ga_base + recv[0], ga_base + recv[1])
@@ -303,6 +397,7 @@ class DataParallel:
                                      device=dev)
         self.state_allreduce = torch.zeros((4,), dtype=torch.int32, device=dev)
         self.state_gather = torch.zeros((4,), dtype=torch.int32, device=dev)
+        self.bn_sync = BnSync(tp, self.peers, self.world, self.rank, sb_base, before_exchange) if sync_bn else None
         self.decay = None
 
     @staticmethod
@@ -310,12 +405,13 @@ class DataParallel:
         return allreduce_layout(n, world, ctas).nbytes, peer_layout(world, slice_bytes)[2]
 
     @staticmethod
-    def symmetric_bytes(tp, world, ctas=ALLREDUCE_CTAS):
+    def symmetric_bytes(tp, world, ctas=ALLREDUCE_CTAS, sync_bn=False):
         """Bytes of symmetric memory one DataParallel over `world` ranks takes (size a PeerArena with at least this)."""
         n = sum(t.numel() for t in tp.parameters())
         nstats = sum(tp.tensors[s + suffix].numel() for s in tp.bn_scopes() for suffix in tp._STATS)
         ar, ga = DataParallel._share_bytes(n, 4 * _round(_HEAD_FLOATS + nstats, 4), world, ctas)
-        return _round(ar, 256) + _round(ga, 256)
+        sb = BnSync.symmetric_bytes(tp, world) if sync_bn else 0
+        return _round(ar, 256) + _round(ga, 256) + _round(sb, 256)
 
     def _broadcast(self, group):
         src = dist.get_global_rank(group, 0)
@@ -330,20 +426,26 @@ class DataParallel:
     @contextlib.contextmanager
     def recording(self):
         """The forward of a step: every training BatchNorm records its batch statistics (exactly once per scope, one decay)
-        into this rank's slice of the per-step gather instead of updating the moving statistics in place."""
-        self.tp.start_bn_record(self.record)
+        into this rank's slice of the per-step gather instead of updating the moving statistics in place.  With sync_bn
+        every training BatchNorm is synchronised over the ranks instead (exactly once per scope, one decay)."""
+        sync = self.bn_sync is not None
+        if sync:
+            self.tp.start_bn_sync(self.bn_sync)
+        else:
+            self.tp.start_bn_record(self.record)
         ok = False
         try:
             yield self
             ok = True
         finally:
-            decay = self.tp.finish_bn_record(check=ok)
+            decay = self.tp.finish_bn_sync(check=ok) if sync else self.tp.finish_bn_record(check=ok)
         self.decay = decay
 
     def exchange(self, losses):
         """After backward(): clip scale -> allreduce mean of the clipped gradients (in place in every .grad) -> gather of
         losses, norms and batch statistics -> BN moving-statistics update of every rank.  losses: dict with
-        loss.LOSS_NAMES and "total" (0-d tensors).  Returns the rank-averaged losses (summed in double in rank order)."""
+        loss.LOSS_NAMES and "total" (0-d tensors).  Returns the rank-averaged losses (summed in double in rank order).
+        With sync_bn the forward has already updated the moving statistics, so the BN update is skipped."""
         from .loss import LOSS_NAMES
         keys = LOSS_NAMES + ("total",)
         if self.decay is None:
@@ -355,7 +457,8 @@ class DataParallel:
         T.peer_allreduce_mean(self.grad, self.scale, self.peers, W, self.rank, self.layout, self.state_allreduce)
         T.peer_allgather(self.send.view(torch.uint8), self.peers, W, self.rank, self.slice_bytes, self.recv_off, self.flag_off,
                          self.state_gather, self.gathered.view(-1).view(torch.uint8))
-        T.bn_moving_update_ranks(self.tp.stats_flat, self.gathered[:, _HEAD_FLOATS:_HEAD_FLOATS + self.nstats], W, self.decay)
+        if self.bn_sync is None:
+            T.bn_moving_update_ranks(self.tp.stats_flat, self.gathered[:, _HEAD_FLOATS:_HEAD_FLOATS + self.nstats], W, self.decay)
         self.decay = None
         g = self.gathered[:, :len(keys)].double()
         acc = g[0].clone()
@@ -370,4 +473,5 @@ class DataParallel:
 
     def timeouts(self):
         """Waits that gave up (a peer that never arrived): 0 in a healthy run.  Synchronises."""
-        return int(self.state_allreduce[2].item()) + int(self.state_gather[2].item())
+        n = int(self.state_allreduce[2].item()) + int(self.state_gather[2].item())
+        return n + (self.bn_sync.timeouts() if self.bn_sync is not None else 0)

@@ -352,6 +352,7 @@ class TrainableParams:
         self.grad_flat = self.grad_offsets = None          # flat_grads()
         self.stats_flat = self.bn_offsets = None           # flat_stats()
         self._bn_record = None                             # start_bn_record() .. finish_bn_record()
+        self._bn_sync = None                               # start_bn_sync() .. finish_bn_sync()
         self.param_flat = self.param_offsets = None        # flat_params()
         self.operand_cache = None                          # enable_operand_cache(): {scope: (forward fold, grad-x fold)}
 
@@ -370,7 +371,8 @@ class TrainableParams:
 
     def conv_train(self, scope, x, bn=True, bn_decay=None, relu=True, debug=None):
         """One conv (+ training BatchNorm when bn) (+ ReLU) of `scope`, differentiable (tf_ops.conv_train).  While a BN
-        record is open (start_bn_record) the batch statistics go to the record instead of the moving statistics."""
+        record is open (start_bn_record) the batch statistics go to the record instead of the moving statistics; while a
+        BN sync is open (start_bn_sync) the BatchNorm is synchronised over the ranks of its handle (SyncBN)."""
         from . import tf_ops
         t = self.tensors
         g = lambda k: t.get(scope + k)
@@ -382,6 +384,9 @@ class TrainableParams:
         if bn and self._bn_record is not None:
             stats_out, moving = self._record_slot(scope, decay), (None, None)
         extra = {} if self.operand_cache is None else {"operands": self.operand_cache[scope]}
+        if bn and self._bn_sync is not None:
+            self._claim(self._bn_sync, "BN sync", scope, decay)
+            extra["sync"] = self._bn_sync["handle"].slots(scope)
         return tf_ops.conv_train(x, t[scope + "/weights"], b, g("/bn/gamma"), g("/bn/beta"), moving[0], moving[1], bn=bn, relu=relu,
                                  decay=decay, debug=debug, stats_out=stats_out, **extra)
 
@@ -497,20 +502,24 @@ class TrainableParams:
                 record.numel() < self.stats_flat.numel() or record.device != self.stats_flat.device:
             raise ValueError("start_bn_record: record must be a float32 vector of >= %d elements on %s"
                              % (self.stats_flat.numel(), self.stats_flat.device))
-        if self._bn_record is not None:
-            raise ValueError("start_bn_record: a BN record is already open")
+        if self._bn_record is not None or self._bn_sync is not None:
+            raise ValueError("start_bn_record: a BN record or BN sync is already open")
         self._bn_record = {"buf": record, "seen": set(), "decay": None}
+
+    def _claim(self, rec, what, scope, decay):
+        """The once-per-scope, one-decay bookkeeping of an open BN record or BN sync."""
+        if scope not in self.bn_offsets:
+            raise ValueError("%s: %s has no moving statistics" % (what, scope))
+        if scope in rec["seen"]:
+            raise ValueError("%s: %s recorded twice in one step" % (what, scope))
+        if rec["decay"] is not None and decay != rec["decay"]:
+            raise ValueError("%s: %s uses decay %g, the step uses %g" % (what, scope, decay, rec["decay"]))
+        rec["seen"].add(scope)
+        rec["decay"] = decay
 
     def _record_slot(self, scope, decay):
         rec = self._bn_record
-        if scope not in self.bn_offsets:
-            raise ValueError("BN record: %s has no moving statistics" % scope)
-        if scope in rec["seen"]:
-            raise ValueError("BN record: %s recorded twice in one step" % scope)
-        if rec["decay"] is not None and decay != rec["decay"]:
-            raise ValueError("BN record: %s uses decay %g, the step uses %g" % (scope, decay, rec["decay"]))
-        rec["seen"].add(scope)
-        rec["decay"] = decay
+        self._claim(rec, "BN record", scope, decay)
         off, c = self.bn_offsets[scope]
         return rec["buf"][off:off + c], rec["buf"][off + c:off + 2 * c]
 
@@ -519,10 +528,31 @@ class TrainableParams:
         rec, self._bn_record = self._bn_record, None
         if rec is None:
             raise ValueError("finish_bn_record: no BN record is open")
+        return self._finish(rec, "BN record", check)
+
+    def _finish(self, rec, what, check):
         missing = [s for s in self.bn_offsets if s not in rec["seen"]]
         if check and missing:
-            raise ValueError("BN record: %d scope(s) did not record, e.g. %s" % (len(missing), missing[0]))
+            raise ValueError("%s: %d scope(s) did not record, e.g. %s" % (what, len(missing), missing[0]))
         return rec["decay"]
+
+    def start_bn_sync(self, handle):
+        """Open a BN sync: until finish_bn_sync(), every training BatchNorm runs SyncBN over the ranks of `handle`
+        (dist.BnSync: handle.slots(scope) -> the scope's (forward, backward) tf_ops.BnSyncSlot) and updates the moving
+        statistics in place with the statistics of every rank's rows.  Each scope exactly once, with one decay."""
+        self.flat_stats()
+        if not callable(getattr(handle, "slots", None)):
+            raise ValueError("start_bn_sync: handle must be a dist.BnSync")
+        if self._bn_sync is not None or self._bn_record is not None:
+            raise ValueError("start_bn_sync: a BN sync or BN record is already open")
+        self._bn_sync = {"handle": handle, "seen": set(), "decay": None}
+
+    def finish_bn_sync(self, check=True):
+        """Close the BN sync and return its decay.  check: every BN scope must have been synchronised exactly once."""
+        rec, self._bn_sync = self._bn_sync, None
+        if rec is None:
+            raise ValueError("finish_bn_sync: no BN sync is open")
+        return self._finish(rec, "BN sync", check)
 
 
 def prepare(params, device="cuda"):

@@ -148,17 +148,23 @@ class Trainer:
     """The loop body of the reference's trainer (trainer.py:177-207) for one rank: forward at the scheduled BatchNorm
     decay, targets, the six losses, backward, the clip / allreduce / BN update of dist.DataParallel, and the Adam step.
     dp: a dist.DataParallel over tp for several GPUs; None trains on one GPU through the same exchange at world size 1
-    (its clip is the pinned one and its BN update equals the in-place one bit for bit)."""
+    (its clip is the pinned one and its BN update equals the in-place one bit for bit).  sync_bn: SyncBN (the reference's
+    MODEL.NETWORK.SYNC_BN) for the DataParallel built here; None takes config.SYNC_BN.  A given dp brings its own."""
 
-    def __init__(self, arch, tp, solver, dp=None):
-        from . import dist
+    def __init__(self, arch, tp, solver, dp=None, sync_bn=None):
+        from . import config, dist
         self.arch, self.tp, self.solver = arch, tp, solver
         self.adam = Adam(tp, solver)
         if dp is None:
-            self._sym = torch.zeros((dist.DataParallel.symmetric_bytes(tp, 1),), dtype=torch.uint8, device=tp.device)
-            dp = dist.DataParallel(tp, peers=[self._sym.data_ptr()], world=1, rank=0, clip_norm=solver.clip_norm)
+            sync_bn = config.SYNC_BN if sync_bn is None else bool(sync_bn)
+            self._sym = torch.zeros((dist.DataParallel.symmetric_bytes(tp, 1, sync_bn=sync_bn),), dtype=torch.uint8,
+                                    device=tp.device)
+            dp = dist.DataParallel(tp, peers=[self._sym.data_ptr()], world=1, rank=0, clip_norm=solver.clip_norm,
+                                   sync_bn=sync_bn)
         elif dp.tp is not tp:
             raise ValueError("Trainer: dp must be the DataParallel of the same TrainableParams")
+        elif sync_bn is not None and bool(sync_bn) != (dp.bn_sync is not None):
+            raise ValueError("Trainer: sync_bn=%s but the given DataParallel has sync_bn=%s" % (sync_bn, dp.bn_sync is not None))
         self.dp = dp
         self.cls_num = int(tp.tensors["pred_cls/weights"].shape[1])   # the head's classes (labels 1..cls_num)
         tp.refresh_operands()                # a DataParallel's constructor may have broadcast rank 0's weights

@@ -15,6 +15,7 @@ import ctypes
 import math
 import operator
 import threading
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -1367,6 +1368,20 @@ def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=
     Returns (y, scale, shift, batch_mean, batch_var); (scale, shift) is the folded per-channel form.
     stats_out: optional (mean, var) float32 CUDA tensors [c] that receive the batch statistics and are returned as
     batch_mean / batch_var (the BN record of data-parallel training writes them straight into its exchange buffer)."""
+    return _bn_train(x, gamma, beta, moving_mean, moving_var, decay, relu, eps, stats_out, None)
+
+
+def bn_train_sync(x, gamma, beta, sync, moving_mean=None, moving_var=None, decay=0.9, relu=True, eps=BN_EPS, stats_out=None):
+    """bn_train of one rank's shard of a batch sharded over sync.world ranks (SyncBN, DESIGN.md section 3.18): the
+    statistics are those of every rank's rows, summed in rank order in double, so every rank gets the same scale, shift,
+    batch_mean and batch_var bits; the moving statistics are updated in place with them.  sync: the BnSyncSlot of this
+    BN scope's forward.  Every rank must make the same sequence of calls on a slot."""
+    if not isinstance(sync, BnSyncSlot):
+        raise ValueError("bn_train_sync: sync must be a BnSyncSlot, got %r" % (sync,))
+    return _bn_train(x, gamma, beta, moving_mean, moving_var, decay, relu, eps, stats_out, sync)
+
+
+def _bn_train(x, gamma, beta, moving_mean, moving_var, decay, relu, eps, stats_out, sync):
     x = _req(x, "x", torch.float32)
     c = x.shape[-1]
     rows = x.numel() // c
@@ -1375,6 +1390,7 @@ def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=
             _vec(t, name, c)
     if (moving_mean is None) != (moving_var is None):
         raise ValueError("moving_mean and moving_var go together")
+    sargs = None if sync is None else _sync_args(sync, "bn_train_sync")
     dev = x.device
     y = torch.empty_like(x)
     scale, shift = (torch.empty((c,), dtype=torch.float32, device=dev) for _ in range(2))
@@ -1383,10 +1399,50 @@ def bn_train(x, gamma, beta, moving_mean=None, moving_var=None, decay=0.9, relu=
     else:
         bmean, bvar = _vec(stats_out[0], "stats_out mean", c), _vec(stats_out[1], "stats_out var", c)
     ws = torch.empty((int(lib().ssd3d_bn_train_workspace(c)),), dtype=torch.uint8, device=dev)
-    check(lib().ssd3d_bn_train(rows, c, _p(x), c, _p(gamma), _p(beta), _p(moving_mean), _p(moving_var), float(decay), float(eps),
-                               _p(ws), _p(scale), _p(shift), _p(bmean), _p(bvar), 1 if relu else 0, _p(y), c, _stream()),
-          "bn_train")
+    args = (rows, c, _p(x), c, _p(gamma), _p(beta), _p(moving_mean), _p(moving_var), float(decay), float(eps), _p(ws), _p(scale),
+            _p(shift), _p(bmean), _p(bvar), 1 if relu else 0, _p(y), c)
+    if sync is None:
+        check(lib().ssd3d_bn_train(*args, _stream()), "bn_train")
+    else:
+        if sync.before is not None:
+            sync.before()
+        check(lib().ssd3d_bn_train_sync(*args, *sargs, _stream()), "bn_train_sync")
     return y, scale, shift, bmean, bvar
+
+
+class BnSyncSlot(NamedTuple):
+    """One (BN scope, direction) of SyncBN (ssd3d_bn_train_sync / ssd3d_bn_train_grad_sync): peers, an int64 CUDA tensor
+    [world] of every rank's symmetric-buffer base as mapped here; area, the byte offset (16-byte multiple) of this slot's
+    ssd3d_bn_sync_area_bytes(world, c) bytes in every rank's buffer; state, an int32 CUDA tensor [>= 3], zero-initialised,
+    owned by this slot.  before: optional callable run on the host just before the launch (tests that simulate ranks on
+    one device use it to bring the ranks to the exchange together).  dist.BnSync hands these out."""
+    peers: torch.Tensor
+    world: int
+    rank: int
+    area: int
+    state: torch.Tensor
+    before: object = None
+
+
+def _sync_args(sync, what):
+    world, rank, area = int(sync.world), int(sync.rank), int(sync.area)
+    if not 1 <= world <= 64 or not 0 <= rank < world:
+        raise ValueError("%s: bad world=%d rank=%d" % (what, world, rank))
+    if area < 0 or area % 16:
+        raise ValueError("%s: area offset %d must be a non-negative 16-byte multiple" % (what, area))
+    _req(sync.peers, "peers", torch.int64, 1, copy=False)
+    _req(sync.state, "state", torch.int32, 1, copy=False)
+    if sync.peers.numel() < world or sync.state.numel() < 3:
+        raise ValueError("%s: peers must hold >= world=%d bases and state >= 3 words" % (what, world))
+    return _p(sync.peers), world, rank, area, _p(sync.state)
+
+
+def bn_sync_resident_ctas():
+    """SyncBN exchange CTAs that fit co-resident on the current device (occupancy API)."""
+    n = int(lib().ssd3d_bn_sync_resident_ctas())
+    if n < 0:
+        check(n, "bn_sync_resident_ctas")
+    return n
 
 
 def rowgroup_max(y, pool, rowmask=None):
@@ -1423,6 +1479,19 @@ def linear_wgrad(x, dz, want_bias=True):
 def bn_train_grad(x, grad_out, scale, shift, batch_mean, batch_var, gamma, relu=True, eps=BN_EPS):
     """Backward of bn_train (+ ReLU) from its input x (the pre-BN conv output) and its outputs (scale, shift, batch_mean,
     batch_var) -> (grad_x, grad_gamma, grad_beta).  The moving statistics are not touched."""
+    return _bn_train_grad(x, grad_out, scale, shift, batch_mean, batch_var, gamma, relu, eps, None)
+
+
+def bn_train_grad_sync(x, grad_out, scale, shift, batch_mean, batch_var, gamma, sync, relu=True, eps=BN_EPS):
+    """Backward of bn_train_sync: sum g and sum g x^ are added over the ranks in rank order, so grad_x is the gradient of
+    the BatchNorm over every rank's rows; grad_gamma and grad_beta stay this rank's own sums (gamma and beta act per
+    rank; the data-parallel allreduce averages them).  sync: the BnSyncSlot of this BN scope's backward."""
+    if not isinstance(sync, BnSyncSlot):
+        raise ValueError("bn_train_grad_sync: sync must be a BnSyncSlot, got %r" % (sync,))
+    return _bn_train_grad(x, grad_out, scale, shift, batch_mean, batch_var, gamma, relu, eps, sync)
+
+
+def _bn_train_grad(x, grad_out, scale, shift, batch_mean, batch_var, gamma, relu, eps, sync):
     x, grad_out = _req(x, "x", torch.float32), _req(grad_out, "grad_out", torch.float32)
     if grad_out.shape != x.shape:
         raise ValueError("bn_train_grad: grad_out %s must have the shape of x %s" % (tuple(grad_out.shape), tuple(x.shape)))
@@ -1430,13 +1499,19 @@ def bn_train_grad(x, grad_out, scale, shift, batch_mean, batch_var, gamma, relu=
     rows = x.numel() // c
     for t, name in ((scale, "scale"), (shift, "shift"), (batch_mean, "batch_mean"), (batch_var, "batch_var"), (gamma, "gamma")):
         _vec(t, name, c)
+    sargs = None if sync is None else _sync_args(sync, "bn_train_grad_sync")
     dev = x.device
     gx = torch.empty_like(x)
     gg, gbeta = (torch.empty((c,), dtype=torch.float32, device=dev) for _ in range(2))
     ws = torch.empty((int(lib().ssd3d_bn_train_grad_workspace(c)),), dtype=torch.uint8, device=dev)
-    check(lib().ssd3d_bn_train_grad(rows, c, _p(x), c, _p(grad_out), c, _p(scale), _p(shift), _p(batch_mean), _p(batch_var),
-                                    _p(gamma), float(eps), 1 if relu else 0, _p(ws), _p(gg), _p(gbeta), _p(gx), c, _stream()),
-          "bn_train_grad")
+    args = (rows, c, _p(x), c, _p(grad_out), c, _p(scale), _p(shift), _p(batch_mean), _p(batch_var), _p(gamma), float(eps),
+            1 if relu else 0, _p(ws), _p(gg), _p(gbeta), _p(gx), c)
+    if sync is None:
+        check(lib().ssd3d_bn_train_grad(*args, _stream()), "bn_train_grad")
+    else:
+        if sync.before is not None:
+            sync.before()
+        check(lib().ssd3d_bn_train_grad_sync(*args, *sargs, _stream()), "bn_train_grad_sync")
     return gx, gg, gbeta
 
 
@@ -1486,16 +1561,18 @@ def vote_translate_grad(offsets, grad_out, min_range):
 
 
 def linear_bn_train(x, f, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9,
-                    stats_out=None):
+                    stats_out=None, sync=None):
     """Forward of one training-mode layer: split_rows -> linear_tc with the BN-less fold f (params.FoldedConv with
     scale = 1, shift = bias) -> bn_train (bn=True: batch statistics, moving statistics updated in place) -> ReLU.
     Returns (y, r): y the conv output before BatchNorm, r bn_train's (out, scale, shift, batch_mean, batch_var), or (y,)
-    when bn=False.  stats_out: see bn_train."""
+    when bn=False.  stats_out: see bn_train.  sync: a BnSyncSlot -> bn_train_sync instead of bn_train."""
     hi, lo = split_rows(x)
     y, _ = linear_tc(hi, lo, f, relu=bool(relu and not bn), want_f32=True, want_split=False)
     if not bn:
         return y, (y,)
     extra = {} if stats_out is None else {"stats_out": stats_out}
+    if sync is not None:
+        return y, bn_train_sync(y, gamma, beta, sync, moving_mean, moving_var, decay=decay, relu=relu, **extra)
     return y, bn_train(y, gamma, beta, moving_mean, moving_var, decay=decay, relu=relu, **extra)
 
 
@@ -1510,15 +1587,17 @@ class _ConvTrain(torch.autograd.Function):
     def forward(ctx, x, w, b, gamma, beta, opts):
         bn, relu, decay, moving, debug, stats_out = opts[:6]
         operands = opts[6] if len(opts) > 6 else None
+        sync = opts[7] if len(opts) > 7 else None
         x = x if x.is_contiguous() else x.contiguous()
         if operands is None:
             f = FoldedConv(w.detach(), torch.ones((w.shape[1],), dtype=torch.float32, device=x.device), b.detach())
         else:
             f = operands[0]
         y, r = linear_bn_train(x, f, gamma.detach(), beta.detach(), moving[0], moving[1],
-                               bn=bn, relu=relu, decay=decay, stats_out=stats_out)
+                               bn=bn, relu=relu, decay=decay, stats_out=stats_out, sync=None if sync is None else sync[0])
         out = r[0]
         ctx.bn, ctx.relu = bn, relu
+        ctx.sync = None if sync is None else sync[1]
         ctx.wt = None if operands is None else operands[1]
         if bn:
             ctx.save_for_backward(x, w, y, *r[1:], gamma)       # scale, shift, batch_mean, batch_var
@@ -1535,7 +1614,10 @@ class _ConvTrain(torch.autograd.Function):
         ggamma = gbeta = None
         if ctx.bn:
             scale, shift, bmean, bvar, gamma = ctx.saved_tensors[3:]
-            dz, ggamma, gbeta = bn_train_grad(y, g, scale, shift, bmean, bvar, gamma, relu=ctx.relu)
+            if ctx.sync is None:
+                dz, ggamma, gbeta = bn_train_grad(y, g, scale, shift, bmean, bvar, gamma, relu=ctx.relu)
+            else:
+                dz, ggamma, gbeta = bn_train_grad_sync(y, g, scale, shift, bmean, bvar, gamma, ctx.sync, relu=ctx.relu)
         elif ctx.relu:
             dz = torch.where(y > 0, g, torch.zeros((), dtype=g.dtype, device=g.device))   # ReluGrad: output > 0
         else:
@@ -1554,22 +1636,25 @@ class _ConvTrain(torch.autograd.Function):
 
 
 def conv_train(x, w, b, gamma=None, beta=None, moving_mean=None, moving_var=None, bn=True, relu=True, decay=0.9, debug=None,
-               stats_out=None, operands=None):
+               stats_out=None, operands=None, sync=None):
     """Differentiable conv (+bias) -> training BatchNorm (bn=True; updates moving_mean / moving_var in place) -> ReLU of
     one layer over the last axis of x, with the forward bits of the non-trainable training path.  x (..., cin),
     w (cin, cout), b / gamma / beta (cout,).  debug: a list that receives (pre-BN conv output, layer output).
     stats_out: optional (mean, var) [cout] that receive the batch statistics (bn=True; kept for the backward).
     operands: optional (forward fold of w with scale 1 and shift b, grad-x fold of w^T with scale 1 and shift 0), current
-    for w -- the caller's promise; both are otherwise built here on every call."""
+    for w -- the caller's promise; both are otherwise built here on every call.
+    sync: optional (forward BnSyncSlot, backward BnSyncSlot) of this scope: SyncBN (bn_train_sync / bn_train_grad_sync)."""
     if not isinstance(x, torch.Tensor) or x.dtype != torch.float32:     # the device is checked by the kernels' wrappers
         raise ValueError("x must be a float32 tensor")
     if w.dim() != 2 or x.shape[-1] != w.shape[0] or tuple(b.shape) != (w.shape[1],):
         raise ValueError("conv_train: x %s, w %s, b %s do not match" % (tuple(x.shape), tuple(w.shape), tuple(b.shape)))
     if bn and (gamma is None or beta is None):
         raise ValueError("conv_train: bn=True needs gamma and beta")
+    if sync is not None and (not bn or len(sync) != 2 or not all(isinstance(s, BnSyncSlot) for s in sync)):
+        raise ValueError("conv_train: sync must be (forward BnSyncSlot, backward BnSyncSlot) of a layer with bn=True")
     z = torch.zeros((0,), dtype=torch.float32, device=x.device)
-    return _ConvTrain.apply(x, w, b, gamma if bn else z, beta if bn else z,
-                            (bool(bn), bool(relu), float(decay), (moving_mean, moving_var), debug, stats_out, operands))
+    opts = (bool(bn), bool(relu), float(decay), (moving_mean, moving_var), debug, stats_out, operands)
+    return _ConvTrain.apply(x, w, b, gamma if bn else z, beta if bn else z, opts if sync is None else opts + (tuple(sync),))
 
 
 class _GroupMax(torch.autograd.Function):

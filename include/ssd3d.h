@@ -401,7 +401,7 @@ int ssd3d_rowgroup_max(long groups, int pool, int c, const float *y, int ldy, co
  * inv = gamma * rsqrt(var + eps), and -- when moving_mean / moving_var are given -- their in-place update
  * v -= (v - batch) * (1 - decay).  scale / shift [c] receive (inv, beta - mean*inv): the folded form the inference
  * kernels take.  batch_mean / batch_var [c] are optional outputs.  workspace: ssd3d_bn_train_workspace(c) bytes.
- * x and out may alias.  Statistics couple all rows: a batch sharded over GPUs needs its own reduction (not built). */
+ * x and out may alias.  Statistics couple all rows: a batch sharded over GPUs reduces them with ssd3d_bn_train_sync. */
 size_t ssd3d_bn_train_workspace(int c);
 int ssd3d_bn_train(long rows, int c, const float *x, int ldx, const float *gamma, const float *beta, float *moving_mean,
                    float *moving_var, float decay, float eps, void *workspace, float *scale, float *shift,
@@ -634,6 +634,29 @@ int ssd3d_peer_allreduce_mean(float *grad, size_t n, const float *scale, void *c
  * stats[n] and each rank's batch[.., n] hold means and variances at the same offsets. */
 int ssd3d_bn_moving_update_ranks(float *stats, long n, const float *batch, long ld_batch, int world, float decay,
                                  ssd3d_stream_t stream);
+
+/* SyncBN (csrc/bn.cu, DESIGN.md section 3.18): ssd3d_bn_train / ssd3d_bn_train_grad of a batch sharded over `world` ranks.
+ * Each is the same partial kernel, then ONE exchange-and-finalize launch of ceil(c / 128) CTAs, then the same apply
+ * kernel.  The exchange adds every rank's per-channel (rows, sum, sum of squares) -- backward: (rows, sum g, sum g x^) --
+ * in rank order in double, so the statistics (and the backward's coef) are those of all ranks' rows and every rank holds
+ * the same bits; with world = 1 the results equal the plain calls bit for bit.  The moving statistics are updated in
+ * place with the global statistics; grad_gamma / grad_beta stay this rank's own sums.
+ * peer_base: DEVICE array [world] of every rank's symmetric allocation as mapped here; area_off (16-byte multiple): the
+ * byte offset, in every rank's allocation, of this (scope, direction)'s area of ssd3d_bn_sync_area_bytes(world, c)
+ * bytes, zero-initialised; state: int32 [>= 3] zero-initialised, owned by this (scope, direction): [0] replays,
+ * [2] waits that gave up after ~4 s (that CTA's channels then come out NaN).  Every rank makes the same sequence of
+ * calls per area; the world's exchange CTAs of one call must be co-resident (ssd3d_bn_sync_resident_ctas per device).
+ * Capturable: no host sync, no allocation, no float atomics. */
+size_t ssd3d_bn_sync_area_bytes(int world, int c);
+int ssd3d_bn_sync_resident_ctas(void);
+int ssd3d_bn_train_sync(long rows, int c, const float *x, int ldx, const float *gamma, const float *beta, float *moving_mean,
+                        float *moving_var, float decay, float eps, void *workspace, float *scale, float *shift,
+                        float *batch_mean, float *batch_var, int relu, float *out, int ldo, void *const *peer_base, int world,
+                        int rank, size_t area_off, int *state, ssd3d_stream_t stream);
+int ssd3d_bn_train_grad_sync(long rows, int c, const float *x, int ldx, const float *grad_out, int ldg, const float *scale,
+                             const float *shift, const float *batch_mean, const float *batch_var, const float *gamma, float eps,
+                             int relu, void *workspace, float *grad_gamma, float *grad_beta, float *grad_x, int ldgx,
+                             void *const *peer_base, int world, int rank, size_t area_off, int *state, ssd3d_stream_t stream);
 
 /* ---- the solver: Adam and the weight operands (csrc/solver.cu, DESIGN.md section 3.11) ------------------------------
  * The update of tf.train.AdamOptimizer (lib/core/trainer.py:74-75) under the learning-rate schedule of

@@ -83,6 +83,8 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=0, help="seed of the augmentation draws")
     ap.add_argument("--mixup", default=None, help="object database (.npz of tools/build_mixup_db.py): paste objects first")
     ap.add_argument("--planes", default=None, help="directory of the KITTI ground planes of --data (with --mixup)")
+    ap.add_argument("--sync-bn", action="store_true",
+                    help="normalise BatchNorm with the statistics of every GPU's scenes (MODEL.NETWORK.SYNC_BN)")
     ap.add_argument("--classes", default="Car", help="comma-separated class list of the head (DATASET.KITTI.CLS_LIST)")
     ap.add_argument("--mixup-classes", default="Car", help="comma-separated classes the mixup paste draws (names of --classes)")
     ap.add_argument("--mixup-numbers", default="15", help="comma-separated objects per scene of each --mixup-classes entry")
@@ -113,8 +115,9 @@ def main(argv=None):
     tp = pkg.params.TrainableParams(d, dev)
     dp = None
     if world > 1:
-        dp = D.DataParallel(tp, D.PeerArena(D.DataParallel.symmetric_bytes(tp, world), dev), clip_norm=solver.clip_norm)
-    tr = S.Trainer(arch, tp, solver, dp)
+        dp = D.DataParallel(tp, D.PeerArena(D.DataParallel.symmetric_bytes(tp, world, sync_bn=a.sync_bn), dev),
+                            clip_norm=solver.clip_norm, sync_bn=a.sync_bn)
+    tr = S.Trainer(arch, tp, solver, dp, sync_bn=a.sync_bn)
     if a.resume:
         tr.load(a.resume)
     elif a.warm_start:

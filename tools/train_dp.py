@@ -29,6 +29,8 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--max-boxes", type=int, default=40)
+    ap.add_argument("--sync-bn", action="store_true",
+                    help="normalise BatchNorm with the statistics of every GPU's scenes (MODEL.NETWORK.SYNC_BN)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("train_dp.py measures on CUDA devices; none is available")
@@ -48,12 +50,12 @@ def main():
     d = pkg.params.init_params(arch, 1, seed=0, random_bias=True)
     d.update(pkg.params.init_head_params(pkg.config.layer_channels(arch, 1)[-1], seed=1))
     tp = pkg.params.TrainableParams(d, dev)
-    nbytes = D.DataParallel.symmetric_bytes(tp, world)
+    nbytes = D.DataParallel.symmetric_bytes(tp, world, sync_bn=a.sync_bn)
     if world > 1:
-        dp = D.DataParallel(tp, D.PeerArena(nbytes, dev))
+        dp = D.DataParallel(tp, D.PeerArena(nbytes, dev), sync_bn=a.sync_bn)
     else:
         sym = torch.zeros((nbytes,), dtype=torch.uint8, device=dev)
-        dp = D.DataParallel(tp, peers=[sym.data_ptr()], world=1, rank=0)
+        dp = D.DataParallel(tp, peers=[sym.data_ptr()], world=1, rank=0, sync_bn=a.sync_bn)
     assert D.ALLREDUCE_CTAS <= pkg.tf_ops.peer_allreduce_resident_ctas()
     opt = torch.optim.Adam(tp.parameters(), lr=1e-3)
     synth = importlib.import_module("3dssd_b200.synth")
@@ -94,7 +96,7 @@ def main():
     if rank == 0:
         print("card: %s, power limit / max SM clock: %s" % (card, power))
         print(json.dumps({"card": card, "power_limit_max_sm_clock": power, "world": world, "scenes_per_rank": a.batch,
-                          "points": a.points, "step_ms": round(step_ms, 3), "exchange_ms": round(ex_ms, 4),
+                          "points": a.points, "sync_bn": a.sync_bn, "step_ms": round(step_ms, 3), "exchange_ms": round(ex_ms, 4),
                           "scenes_per_s": round(world * a.batch / (step_ms * 1e-3), 2),
                           "grad_floats": dp.grad.numel(), "bn_stat_floats": dp.nstats, "timeouts": timeouts,
                           "total_loss": float(mean["total"])}))
