@@ -141,6 +141,7 @@ _SIGNATURES = {
                                  ctypes.c_size_t, c_void_p, c_void_p],
     "ssd3d_adam_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_long, c_void_p, c_float, c_float, c_float, c_int, c_void_p,
                         c_void_p, c_void_p],
+    "ssd3d_momentum_step": [c_void_p, c_void_p, c_void_p, c_long, c_void_p, c_float, c_int, c_void_p, c_void_p, c_void_p],
     "ssd3d_weight_operands": [c_void_p, c_void_p, c_int, c_long, c_void_p, c_void_p],
     "ssd3d_box_iou": [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "ssd3d_box_iou_matched": [c_long, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],

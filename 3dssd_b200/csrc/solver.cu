@@ -17,6 +17,15 @@
 //                     block that counts last is the only writer of the new state, so no block can see it half updated.
 //                     The library is built with -fmad=true: the arithmetic is spelled with __f*_rn so that contraction
 //                     cannot change a bit.  Non-finite gradients propagate into m, v and p.
+//   momentum_step     ONE launch of tf.train.MomentumOptimizer(lr, momentum) (use_nesterov=False, TF's ApplyMomentum) over
+//                     the same flat buffer, with the same schedule and the same state block and "last block publishes"
+//                     protocol; beta1_power and beta2_power are left as they are.  Per element, with the OLD state's lr:
+//                       accum' = rn(rn(accum * momentum) + g)
+//                       p'     = rn(p - rn(accum' * lr))
+//                     TF states this as an Eigen expression (accum * momentum + grad; var -= accum * lr) and it is not
+//                     known whether the reference's GPU build contracted either line into an fma.  The uncontracted form
+//                     is the one chosen here: every product and sum rounded once, spelled with __f*_rn.  Non-finite
+//                     gradients propagate into accum and p.
 //   weight_operands   ONE launch that rebuilds the split-bf16 tensor-core operands (operand.cuh) of every conv weight
 //                     from the flat parameter buffer: for W [cin, cout] the forward operand = split of W^T
 //                     [cout, round16(cin)] and the grad-x operand = split of W [cin, round16(cout)], zero padded.  A
@@ -49,6 +58,29 @@ struct AdamCoef {
     float alpha, omb1, omb2, eps;
 };
 
+// Thread 0 of every block: the old state and the learning rate it selects (piecewise_constant; boundaries increase, so the
+// last boundary below global_step wins).  Nothing is written: the state changes only after every block counted itself done.
+__device__ __forceinline__ float read_state(const AdamState *state, const AdamSchedule &sch, long long &step, float &b1p, float &b2p)
+{
+    const volatile AdamState *st = state;
+    step = st->global_step;
+    float lr = sch.values[0];
+#pragma unroll                                          // constant indices: the schedule stays in the parameter bank
+    for (int k = 0; k < ADAM_MAX_BOUNDARIES; k++)
+        if (k < sch.nb && step > sch.boundaries[k]) lr = sch.values[k + 1];
+    b1p = st->beta1_power; b2p = st->beta2_power;
+    return lr;
+}
+
+// Thread 0 of every block, after the block's last element: the block that counts last writes the new state.
+__device__ __forceinline__ bool last_block_done(AdamState *state)
+{
+    __threadfence();
+    if (atomicAdd(&state->done, 1u) != gridDim.x - 1) return false;
+    state->done = 0;
+    return true;
+}
+
 __device__ __forceinline__ void adam_one(float &p, float g, float &m, float &v, const AdamCoef c)
 {
     m = __fadd_rn(m, __fmul_rn(__fsub_rn(g, m), c.omb1));
@@ -63,15 +95,7 @@ adam_step_kernel(float *__restrict__ param, const float *__restrict__ grad, floa
     __shared__ long long s_step;
     __shared__ float s_b1p, s_b2p, s_lr;
     const int tid = threadIdx.x;
-    if (tid == 0) {                                     // the state changes only after every block has counted itself done
-        const volatile AdamState *st = state;
-        const long long step = st->global_step;
-        float lr = sch.values[0];
-#pragma unroll                                          // constant indices: the schedule stays in the parameter bank
-        for (int k = 0; k < ADAM_MAX_BOUNDARIES; k++)
-            if (k < sch.nb && step > sch.boundaries[k]) lr = sch.values[k + 1];   // boundaries increase: the last hit wins
-        s_step = step; s_b1p = st->beta1_power; s_b2p = st->beta2_power; s_lr = lr;
-    }
+    if (tid == 0) s_lr = read_state(state, sch, s_step, s_b1p, s_b2p);
     __syncthreads();
     const float lr = s_lr, b1p = s_b1p, b2p = s_b2p;
     AdamCoef c;
@@ -96,14 +120,52 @@ adam_step_kernel(float *__restrict__ param, const float *__restrict__ grad, floa
     }
     __syncthreads();
     if (tid == 0) {
-        __threadfence();
-        if (atomicAdd(&state->done, 1u) == gridDim.x - 1) {   // every block has read the old state: publish the new one
-            state->done = 0;
+        if (last_block_done(state)) {                   // every block has read the old state: publish the new one
             state->beta1_power = __fmul_rn(b1p, beta1);
             state->beta2_power = __fmul_rn(b2p, beta2);
             state->lr_used = lr;
             state->global_step = s_step + 1;
         }
+    }
+}
+
+__device__ __forceinline__ void momentum_one(float &p, float g, float &a, float mom, float lr)
+{
+    a = __fadd_rn(__fmul_rn(a, mom), g);
+    p = __fsub_rn(p, __fmul_rn(a, lr));
+}
+
+__global__ void __launch_bounds__(ADAM_THREADS)
+momentum_step_kernel(float *__restrict__ param, const float *__restrict__ grad, float *__restrict__ accum, long n, AdamState *state,
+                     float momentum, const AdamSchedule sch)
+{
+    __shared__ long long s_step;
+    __shared__ float s_b1p, s_b2p, s_lr;
+    const int tid = threadIdx.x;
+    if (tid == 0) s_lr = read_state(state, sch, s_step, s_b1p, s_b2p);
+    __syncthreads();
+    const float lr = s_lr;
+
+    const long n4 = n / 4, stride = (long)gridDim.x * ADAM_THREADS;
+    float4 *p4 = reinterpret_cast<float4 *>(param), *a4 = reinterpret_cast<float4 *>(accum);
+    const float4 *g4 = reinterpret_cast<const float4 *>(grad);
+    for (long i = (long)blockIdx.x * ADAM_THREADS + tid; i < n4; i += stride) {
+        float4 p = p4[i], a = a4[i];
+        const float4 g = __ldg(g4 + i);
+        momentum_one(p.x, g.x, a.x, momentum, lr); momentum_one(p.y, g.y, a.y, momentum, lr);
+        momentum_one(p.z, g.z, a.z, momentum, lr); momentum_one(p.w, g.w, a.w, momentum, lr);
+        p4[i] = p; a4[i] = a;
+    }
+    if (blockIdx.x == 0 && 4 * n4 + tid < n) {          // the tail of an n that is not a multiple of 4
+        const long i = 4 * n4 + tid;
+        float p = param[i], a = accum[i];
+        momentum_one(p, __ldg(grad + i), a, momentum, lr);
+        param[i] = p; accum[i] = a;
+    }
+    __syncthreads();
+    if (tid == 0 && last_block_done(state)) {           // the beta powers are Adam's: left as they are
+        state->lr_used = lr;
+        state->global_step = s_step + 1;
     }
 }
 
@@ -146,32 +208,61 @@ weight_operands_kernel(const float *__restrict__ param, const long long *__restr
 
 using namespace ssd3d;
 
+// The schedule of both solver entries, checked and packed into the launch's parameters; 0 or the error's return code.
+static int pack_schedule(const char *what, int nb, const long long *boundaries, const float *values, AdamSchedule &sch)
+{
+    SSD3D_REQUIRE(values && nb >= 0 && nb <= ADAM_MAX_BOUNDARIES && (nb == 0 || boundaries), "%s: nb=%d must be in [0, %d]",
+                  what, nb, ADAM_MAX_BOUNDARIES);
+    sch = AdamSchedule{};
+    sch.nb = nb;
+    for (int i = 0; i < nb; i++) {
+        SSD3D_REQUIRE(i == 0 || boundaries[i] > boundaries[i - 1], "%s: boundaries must increase", what);
+        sch.boundaries[i] = boundaries[i];
+    }
+    for (int i = 0; i <= nb; i++) sch.values[i] = values[i];
+    return 0;
+}
+
+static int solver_blocks(long n)
+{
+    const long want = (n / 4 + ADAM_THREADS - 1) / ADAM_THREADS;
+    return (int)(want < 1 ? 1 : (want < (long)kNumSMs * 8 ? want : (long)kNumSMs * 8));
+}
+
 extern "C" int ssd3d_adam_step(float *param, const float *grad, float *m, float *v, long n, void *state, float beta1,
                                float beta2, float epsilon, int nb, const long long *boundaries, const float *values,
                                ssd3d_stream_t stream)
 {
     SSD3D_REQUIRE(n > 0, "adam_step: n=%ld must be > 0", n);
     SSD3D_REQUIRE(param && grad && m && v && state && values, "adam_step: null pointer");
-    SSD3D_REQUIRE(nb >= 0 && nb <= ADAM_MAX_BOUNDARIES && (nb == 0 || boundaries), "adam_step: nb=%d must be in [0, %d]", nb,
-                  ADAM_MAX_BOUNDARIES);
     SSD3D_REQUIRE(((reinterpret_cast<uintptr_t>(param) | reinterpret_cast<uintptr_t>(grad) | reinterpret_cast<uintptr_t>(m) |
                     reinterpret_cast<uintptr_t>(v)) & 15u) == 0, "adam_step: param, grad, m and v must be 16-byte aligned");
     SSD3D_REQUIRE((reinterpret_cast<uintptr_t>(state) & 7u) == 0, "adam_step: state must be 8-byte aligned");
     SSD3D_REQUIRE(beta1 >= 0.0f && beta1 < 1.0f && beta2 >= 0.0f && beta2 < 1.0f && epsilon >= 0.0f,
                   "adam_step: beta1=%g, beta2=%g must be in [0, 1) and epsilon=%g >= 0", beta1, beta2, epsilon);
-    AdamSchedule sch = {};
-    sch.nb = nb;
-    for (int i = 0; i < nb; i++) {
-        SSD3D_REQUIRE(i == 0 || boundaries[i] > boundaries[i - 1], "adam_step: boundaries must increase");
-        sch.boundaries[i] = boundaries[i];
-    }
-    for (int i = 0; i <= nb; i++) sch.values[i] = values[i];
-    const long want = (n / 4 + ADAM_THREADS - 1) / ADAM_THREADS;
-    const int blocks = (int)(want < 1 ? 1 : (want < (long)kNumSMs * 8 ? want : (long)kNumSMs * 8));
+    AdamSchedule sch;
+    if (const int rc = pack_schedule("adam_step", nb, boundaries, values, sch)) return rc;
+    const int blocks = solver_blocks(n);
     const float omb1 = 1.0f - beta1, omb2 = 1.0f - beta2;    // float32 differences, rounded once
     adam_step_kernel<<<blocks, ADAM_THREADS, 0, (cudaStream_t)stream>>>(param, grad, m, v, n, (AdamState *)state, beta1, beta2,
                                                                         omb1, omb2, epsilon, sch);
     SSD3D_LAUNCH_CHECK("adam_step_kernel");
+}
+
+extern "C" int ssd3d_momentum_step(float *param, const float *grad, float *accum, long n, void *state, float momentum, int nb,
+                                   const long long *boundaries, const float *values, ssd3d_stream_t stream)
+{
+    SSD3D_REQUIRE(n > 0, "momentum_step: n=%ld must be > 0", n);
+    SSD3D_REQUIRE(param && grad && accum && state, "momentum_step: null pointer");
+    SSD3D_REQUIRE(((reinterpret_cast<uintptr_t>(param) | reinterpret_cast<uintptr_t>(grad) | reinterpret_cast<uintptr_t>(accum)) &
+                   15u) == 0, "momentum_step: param, grad and accum must be 16-byte aligned");
+    SSD3D_REQUIRE((reinterpret_cast<uintptr_t>(state) & 7u) == 0, "momentum_step: state must be 8-byte aligned");
+    SSD3D_REQUIRE(momentum >= 0.0f && momentum <= 1.0f, "momentum_step: momentum=%g must be in [0, 1]", momentum);
+    AdamSchedule sch;
+    if (const int rc = pack_schedule("momentum_step", nb, boundaries, values, sch)) return rc;
+    momentum_step_kernel<<<solver_blocks(n), ADAM_THREADS, 0, (cudaStream_t)stream>>>(param, grad, accum, n, (AdamState *)state,
+                                                                                      momentum, sch);
+    SSD3D_LAUNCH_CHECK("momentum_step_kernel");
 }
 
 extern "C" int ssd3d_weight_operands(const float *param, const long long *table, int nw, long tiles, void *arena,

@@ -238,8 +238,11 @@ class BnSync:
     """The SyncBN handle of one rank (TrainableParams.start_bn_sync): which ranks (peers, world, rank), where each BN
     scope's forward and backward exchange live in the symmetric buffers (bn_sync_layout from byte `base`), and their
     replay counters and time-out counts (state [scopes, 2, 4] int32 on the device).  Every scope has its own areas,
-    flags and counters, so the order in which scopes exchange does not matter; each must exchange once per step in each
-    direction on every rank.  before_exchange(scope, direction): optional host callable run just before each launch
+    flags and counters, so the order in which scopes exchange does not matter.  Each scope exchanges once per step in the
+    forward on every rank.  In the backward it exchanges once per step on every rank, or, when nothing below its
+    BatchNorm needs a gradient (a frozen layer below the lowest trained one, TrainableParams(trainable=...)), on no rank:
+    every rank freezes the same set, so the ranks skip the same scopes and each scope's counter stays in step across them.
+    before_exchange(scope, direction): optional host callable run just before each launch
     (direction 0 forward, 1 backward): tests that simulate ranks on one device bring the ranks together with it."""
 
     def __init__(self, tp, peers, world, rank, base=0, before_exchange=None):
@@ -416,8 +419,9 @@ class DataParallel:
     def _broadcast(self, group):
         src = dist.get_global_rank(group, 0)
         with torch.no_grad():
-            for _, t in self.tp.named_parameters():
-                dist.broadcast(t.data, src=src, group=group)
+            for k, t in self.tp.tensors.items():                # frozen tensors too: no step ever makes them agree
+                if not k.endswith(self.tp._STATS):
+                    dist.broadcast(t.data, src=src, group=group)
             dist.broadcast(self.tp.stats_flat, src=src, group=group)
 
     def zero_grad(self):

@@ -334,30 +334,60 @@ class PreparedParams:
         return self
 
 
+def trained_names(names, prefixes=None):
+    """The variables of `names` that training updates, as the reference's TRAIN.CONFIG.TRAIN_PARAM_PREFIX selects them
+    (lib/core/trainer.py:42, trainer_utils.get_trainable_parameter: the scope filter of tf.get_collection): name v is
+    trained iff re.match(prefix, v) for some prefix.  None or [] trains every name.  A prefix that matches no name is an
+    error (a misspelt scope would otherwise freeze everything it meant to train).  Returns the trained names in the
+    order of `names`."""
+    import re
+    names = list(names)
+    if not prefixes:
+        return names
+    prefixes = [str(p) for p in prefixes]
+    for p in prefixes:
+        if not any(re.match(p, v) for v in names):
+            raise ValueError("trainable prefix %r matches no variable (e.g. %s)" % (p, names[0] if names else "none"))
+    return [v for v in names if any(re.match(p, v) for p in prefixes)]
+
+
 class TrainableParams:
     """The parameters of a params dict as device tensors for training (layers with is_training=True run their
     differentiable path when given one of these): weights, biases, gamma and beta are leaf tensors with
     requires_grad=True, the moving statistics plain tensors that training forwards update in place.  Keys are the TF
     variable names.  Nothing folded is cached: every forward reads the live tensors, so an optimizer step is seen by the
-    next forward.  to_params() returns the numpy dict (moving statistics included) for prepare() / SABackbone."""
+    next forward.  to_params() returns the numpy dict (moving statistics included) for prepare() / SABackbone.
+
+    trainable: the reference's TRAIN_PARAM_PREFIX (trained_names; None or [] trains everything).  A tensor it does not
+    select is frozen: requires_grad=False, so autograd drops every layer below the lowest trained one and no gradient,
+    clip, allreduce or optimizer slot covers it.  Frozen layers still run in training mode (batch statistics, moving
+    statistics updated in place), as the reference's batch_norm_template does for every layer."""
 
     _STATS = ("/bn/moving_mean", "/bn/moving_variance")
 
-    def __init__(self, params, device="cuda"):
+    def __init__(self, params, device="cuda", trainable=None):
         self.device = torch.device(device)
         self.tensors = {}
+        self.trainable = tuple(trainable) if trainable else ()
+        trained = set(trained_names([k for k in params if not k.endswith(self._STATS)], self.trainable))
         for k, v in params.items():
             t = torch.from_numpy(np.array(v, dtype=np.float32, copy=True)).to(self.device)
-            self.tensors[k] = t if k.endswith(self._STATS) else t.requires_grad_(True)
+            self.tensors[k] = t if k.endswith(self._STATS) else t.requires_grad_(k in trained)
         self.grad_flat = self.grad_offsets = None          # flat_grads()
         self.stats_flat = self.bn_offsets = None           # flat_stats()
         self._bn_record = None                             # start_bn_record() .. finish_bn_record()
         self._bn_sync = None                               # start_bn_sync() .. finish_bn_sync()
         self.param_flat = self.param_offsets = None        # flat_params()
         self.operand_cache = None                          # enable_operand_cache(): {scope: (forward fold, grad-x fold)}
+        self.frozen_flat = None                            # enable_operand_cache(): the frozen weights, one buffer
 
     def named_parameters(self):
+        """(TF name, tensor) of every trained tensor."""
         return [(k, t) for k, t in self.tensors.items() if t.requires_grad]
+
+    def frozen_names(self):
+        """Weights, biases, gamma and beta that training leaves alone (TrainableParams(trainable=...))."""
+        return [k for k, t in self.tensors.items() if not (t.requires_grad or k.endswith(self._STATS))]
 
     def parameters(self):
         return [t for _, t in self.named_parameters()]
@@ -396,55 +426,76 @@ class TrainableParams:
         the offsets of flat_grads): the tensors stay autograd leaves and become views of it, so one kernel can update all
         of them.  Returns param_flat."""
         if self.param_flat is None:
-            named = self.named_parameters()
-            flat = torch.empty((sum(t.numel() for _, t in named),), dtype=torch.float32, device=self.device)
-            self.param_offsets, off = {}, 0
-            for k, t in named:
-                view = flat[off:off + t.numel()].view(t.shape)
-                view.copy_(t.detach())
-                t.data = view
-                self.param_offsets[k] = off
-                off += t.numel()
-            self.param_flat = flat
+            self.param_flat, self.param_offsets = self._flatten(self.named_parameters())
         return self.param_flat
 
+    def _flatten(self, named):
+        """Move the tensors of `named` into one new flat float32 buffer (they become views of it and stay autograd
+        leaves) -> (buffer, {name: its first element})."""
+        flat = torch.empty((sum(t.numel() for _, t in named),), dtype=torch.float32, device=self.device)
+        offsets, off = {}, 0
+        for k, t in named:
+            view = flat[off:off + t.numel()].view(t.shape)
+            view.copy_(t.detach())
+            t.data = view
+            offsets[k] = off
+            off += t.numel()
+        return flat, offsets
+
     def weight_scopes(self):
+        """Scopes of the trained conv weights."""
         return [k[: -len("/weights")] for k, _ in self.named_parameters() if k.endswith("/weights")]
 
+    def frozen_weight_scopes(self):
+        return [k[: -len("/weights")] for k in self.frozen_names() if k.endswith("/weights")]
+
     def enable_operand_cache(self):
-        """Keep the split tensor-core operands of every conv weight in one bf16 arena (operand_layout) and hand them to
+        """Keep the split tensor-core operands of every conv weight in a bf16 arena (operand_layout) and hand them to
         conv_train instead of rebuilding them in every forward and backward.  The cache holds what refresh_operands() last
         built: it is valid from then until the next write to a weight, so whatever writes weights calls refresh_operands()
-        (solver.Adam.step does).  The biases are read live (shift is a view of them)."""
+        (solver.Adam.step does).  The biases are read live (shift is a view of them).  Frozen weights move into a second
+        flat buffer (frozen_flat) with an arena of its own whose rows are built here once: refresh_operands() rebuilds
+        only the trained weights' rows unless told that the frozen weights were written too (a load or a broadcast)."""
         if self.operand_cache is not None:
             return
         self.flat_params()
-        scopes = self.weight_scopes()
+        frozen = self.frozen_weight_scopes()
+        self.frozen_flat, frozen_offsets = self._flatten([(s + "/weights", self.tensors[s + "/weights"]) for s in frozen])
+        self.operand_cache = {}
+        self._operands = [self._operand_rows(self.weight_scopes(), self.param_flat, self.param_offsets),
+                          self._operand_rows(frozen, self.frozen_flat, frozen_offsets)]
+        self.operand_arena = None if self._operands[0] is None else self._operands[0][3]
+        self.refresh_operands(frozen=True)
+
+    def _operand_rows(self, scopes, flat, offsets):
+        """Operand cache entries for the weights of `scopes`, which live in `flat` at `offsets` -> the arguments of
+        tf_ops.weight_operands that rebuild them (flat, table, tiles, arena), or None without a scope."""
+        if not scopes:
+            return None
         shapes = [tuple(self.tensors[s + "/weights"].shape) for s in scopes]
-        table, elems, self._operand_tiles = operand_layout([(self.param_offsets[s + "/weights"], ci, co)
-                                                            for s, (ci, co) in zip(scopes, shapes)])
-        self._operand_table = torch.from_numpy(table).to(self.device)
-        self.operand_arena = torch.zeros((elems,), dtype=torch.bfloat16, device=self.device)
+        table, elems, tiles = operand_layout([(offsets[s + "/weights"], ci, co) for s, (ci, co) in zip(scopes, shapes)])
+        arena = torch.zeros((elems,), dtype=torch.bfloat16, device=self.device)
         width = max(max(sh) for sh in shapes)
         ones = torch.ones((width,), dtype=torch.float32, device=self.device)
         zeros = torch.zeros((width,), dtype=torch.float32, device=self.device)
-        cache = {}
         for s, (ci, co), row in zip(scopes, shapes, table.tolist()):
             w = self.tensors[s + "/weights"].detach()
             b = self.tensors.get(s + "/biases")
-            blk = lambda o, r, c: self.operand_arena[o:o + r * c].view(r, c)
+            blk = lambda o, r, c: arena[o:o + r * c].view(r, c)
             fwd = FoldedConv.from_operands(w, ones[:co], zeros[:co] if b is None else b.detach(),
                                            blk(row[3], co, round16(ci)), blk(row[4], co, round16(ci)))
             bwd = FoldedConv.from_operands(w.t(), ones[:ci], zeros[:ci], blk(row[5], ci, round16(co)), blk(row[6], ci, round16(co)))
-            cache[s] = (fwd, bwd)
-        self.operand_cache = cache
-        self.refresh_operands()
+            self.operand_cache[s] = (fwd, bwd)
+        return flat, torch.from_numpy(table).to(self.device), tiles, arena
 
-    def refresh_operands(self):
-        """Rebuild the operand cache from the current weights (one launch); nothing to do when the cache is not enabled."""
+    def refresh_operands(self, frozen=False):
+        """Rebuild the operand cache of the trained weights from their current values (one launch), with frozen=True that
+        of the frozen weights too (one more); nothing to do when the cache is not enabled."""
         if self.operand_cache is not None:
             from . import tf_ops
-            tf_ops.weight_operands(self.param_flat, self._operand_table, self._operand_tiles, self.operand_arena)
+            for rows in self._operands[:2 if frozen else 1]:
+                if rows is not None:
+                    tf_ops.weight_operands(*rows)
 
     # ---- data-parallel training (dist.DataParallel): both capabilities are opt-in; unused, nothing above changes -----
     def flat_grads(self):

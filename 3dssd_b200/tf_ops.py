@@ -1187,7 +1187,7 @@ def bn_moving_update_ranks(stats, batch, world, decay):
     return stats
 
 
-# ---- the solver: Adam and the weight operands (csrc/solver.cu, DESIGN.md section 3.11) -------------------------------
+# ---- the solver: Adam, Momentum and the weight operands (csrc/solver.cu, DESIGN.md sections 3.11, 3.19) -------------------------------
 
 ADAM_STATE_INTS = 8           # the 32-byte state block as int32: [0:2] global_step, [2:5] float bits, [5] block counter
 
@@ -1204,13 +1204,39 @@ def adam_step(param, grad, m, v, state, boundaries, values, beta1=0.9, beta2=0.9
         raise ValueError("adam_step: param, grad, m, v must hold the same n > 0 floats and state %d int32" % ADAM_STATE_INTS)
     if any(t.data_ptr() % 16 for t in bufs) or state.data_ptr() % 8:
         raise ValueError("adam_step: param, grad, m, v must be 16-byte and state 8-byte aligned")
-    nb = len(boundaries)
-    if nb > 8 or len(values) != nb + 1:
-        raise ValueError("adam_step: %d boundaries (at most 8) need %d values, got %d" % (nb, nb + 1, len(values)))
-    bd = (ctypes.c_longlong * max(nb, 1))(*[int(b) for b in boundaries])
-    vals = (ctypes.c_float * (nb + 1))(*[float(x) for x in values])
+    nb, bd, vals = _schedule("adam_step", boundaries, values)
     check(lib().ssd3d_adam_step(*[_p(t) for t in bufs], n, _p(state), float(beta1), float(beta2), float(epsilon), nb,
                                 ctypes.cast(bd, ctypes.c_void_p), ctypes.cast(vals, ctypes.c_void_p), _stream()), "adam_step")
+    return param
+
+
+def _schedule(what, boundaries, values):
+    nb = len(boundaries)
+    if nb > 8 or len(values) != nb + 1:
+        raise ValueError("%s: %d boundaries (at most 8) need %d values, got %d" % (what, nb, nb + 1, len(values)))
+    if any(int(b) <= int(a) for a, b in zip(boundaries, boundaries[1:])):
+        raise ValueError("%s: boundaries %r must increase" % (what, tuple(boundaries)))
+    bd = (ctypes.c_longlong * max(nb, 1))(*[int(b) for b in boundaries])
+    vals = (ctypes.c_float * (nb + 1))(*[float(x) for x in values])
+    return nb, bd, vals
+
+
+def momentum_step(param, grad, accum, state, boundaries, values, momentum=0.9):
+    """One step of tf.train.MomentumOptimizer (use_nesterov=False) of the flat float32 buffers param / accum (in place)
+    from grad, in one launch (include/ssd3d.h, ssd3d_momentum_step).  state, boundaries and values as in adam_step; the
+    state's beta powers are left alone."""
+    bufs = [_req(t, name, torch.float32, 1, copy=False) for name, t in (("param", param), ("grad", grad), ("accum", accum))]
+    state = _req(state, "state", torch.int32, 1, copy=False)
+    n = bufs[0].numel()
+    if n == 0 or any(t.numel() != n for t in bufs) or state.numel() < ADAM_STATE_INTS:
+        raise ValueError("momentum_step: param, grad, accum must hold the same n > 0 floats and state %d int32" % ADAM_STATE_INTS)
+    if any(t.data_ptr() % 16 for t in bufs) or state.data_ptr() % 8:
+        raise ValueError("momentum_step: param, grad, accum must be 16-byte and state 8-byte aligned")
+    if not 0.0 <= float(momentum) <= 1.0:
+        raise ValueError("momentum_step: momentum=%g must be in [0, 1]" % momentum)
+    nb, bd, vals = _schedule("momentum_step", boundaries, values)
+    check(lib().ssd3d_momentum_step(*[_p(t) for t in bufs], n, _p(state), float(momentum), nb, ctypes.cast(bd, ctypes.c_void_p),
+                                    ctypes.cast(vals, ctypes.c_void_p), _stream()), "momentum_step")
     return param
 
 
@@ -1579,7 +1605,9 @@ def linear_bn_train(x, f, gamma=None, beta=None, moving_mean=None, moving_var=No
 class _ConvTrain(torch.autograd.Function):
     """conv (+bias) -> [training BatchNorm] -> [ReLU] of one layer (tf_util.conv2d / conv1d with is_training=True).
     Forward: linear_bn_train with a fold of the live weights, the sequence of the non-trainable training path.
-    Backward: bn_train_grad -> split -> linear_tc with W^T (grad_x) and linear_wgrad (grad_w, grad_b).
+    Backward: bn_train_grad -> split -> linear_tc with W^T (grad_x) and linear_wgrad (grad_w, grad_b).  Only what an input
+    that needs a gradient asks for runs: no linear_tc without x, no linear_wgrad without w or b, and no gamma / beta
+    gradient for a frozen BatchNorm (its dz is still formed when x or the weights need it).
     opts may end with operands = (forward fold, grad-x fold) prebuilt from the same weights (params.TrainableParams'
     operand cache): they are then used instead of building both folds here."""
 
@@ -1622,16 +1650,20 @@ class _ConvTrain(torch.autograd.Function):
             dz = torch.where(y > 0, g, torch.zeros((), dtype=g.dtype, device=g.device))   # ReluGrad: output > 0
         else:
             dz = g
+        need = ctx.needs_input_grad
+        ggamma, gbeta = (ggamma if need[3] else None), (gbeta if need[4] else None)
         cin, cout = w.shape
-        gx = None
-        if ctx.needs_input_grad[0]:
+        gx = gw = gb = None
+        if need[0]:
             d_hi, d_lo = split_rows(dz)
             wt = ctx.wt
             if wt is None:
                 wt = FoldedConv(w.detach().t().contiguous(), torch.ones((cin,), dtype=torch.float32, device=dz.device),
                                 torch.zeros((cin,), dtype=torch.float32, device=dz.device))
             gx, _ = linear_tc(d_hi, d_lo, wt, relu=False, want_f32=True, want_split=False)
-        gw, gb = linear_wgrad(x, dz, want_bias=True)
+        if need[1] or need[2]:
+            gw, gb = linear_wgrad(x, dz, want_bias=True)
+            gw, gb = (gw if need[1] else None), (gb if need[2] else None)
         return gx, gw, gb, ggamma, gbeta, None
 
 

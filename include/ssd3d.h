@@ -658,10 +658,10 @@ int ssd3d_bn_train_grad_sync(long rows, int c, const float *x, int ldx, const fl
                              int relu, void *workspace, float *grad_gamma, float *grad_beta, float *grad_x, int ldgx,
                              void *const *peer_base, int world, int rank, size_t area_off, int *state, ssd3d_stream_t stream);
 
-/* ---- the solver: Adam and the weight operands (csrc/solver.cu, DESIGN.md section 3.11) ------------------------------
- * The update of tf.train.AdamOptimizer (lib/core/trainer.py:74-75) under the learning-rate schedule of
- * tf.train.piecewise_constant (lib/core/trainer_utils.py:7-13), with every float32 operation rounded once.  Neither
- * entry allocates, uses float atomics or synchronises the host; both are CUDA-graph capturable. */
+/* ---- the solver: Adam, Momentum and the weight operands (csrc/solver.cu, DESIGN.md sections 3.11, 3.19) -------------
+ * The updates of tf.train.AdamOptimizer and tf.train.MomentumOptimizer (lib/core/trainer.py:72-75) under the
+ * learning-rate schedule of tf.train.piecewise_constant (lib/core/trainer_utils.py:7-13), with every float32 operation
+ * rounded once.  No entry allocates, uses float atomics or synchronises the host; all are CUDA-graph capturable. */
 
 /* One Adam step over flat buffers param, m, v (updated in place) and grad [n], all 16-byte aligned, in ONE launch.
  * state: the caller's 32-byte, 8-byte aligned device block { int64 global_step; float beta1_power; float beta2_power;
@@ -676,6 +676,15 @@ int ssd3d_bn_train_grad_sync(long rows, int c, const float *x, int ldx, const fl
  * lr_used = lr.  Non-finite gradients propagate. */
 int ssd3d_adam_step(float *param, const float *grad, float *m, float *v, long n, void *state, float beta1, float beta2,
                     float epsilon, int nb, const long long *boundaries, const float *values, ssd3d_stream_t stream);
+/* One step of tf.train.MomentumOptimizer(lr, momentum), use_nesterov=False (TF's ApplyMomentum), over flat buffers param
+ * and accum (updated in place) and grad [n], all 16-byte aligned, in ONE launch.  state, boundaries, values and the
+ * launch protocol are those of ssd3d_adam_step; momentum is in [0, 1] and accum starts at 0.  With lr read from the
+ * state as it was BEFORE the launch:
+ *   accum = rn(rn(accum * momentum) + g);  param = rn(param - rn(accum * lr))
+ * and, once every element is done: global_step += 1, lr_used = lr.  beta1_power and beta2_power are not touched.
+ * Non-finite gradients propagate. */
+int ssd3d_momentum_step(float *param, const float *grad, float *accum, long n, void *state, float momentum, int nb,
+                        const long long *boundaries, const float *values, ssd3d_stream_t stream);
 /* The split-bf16 tensor-core operands of nw conv weights, rebuilt from the flat parameter buffer in ONE launch.
  * table: DEVICE int64 [nw][8], row = { offset of W [cin, cout] in param (floats), cin, cout, then offsets in arena (bf16
  * elements, multiples of 8) of fwd_hi, fwd_lo [cout, round16(cin)] = split of W^T and of bwd_hi, bwd_lo

@@ -1,5 +1,6 @@
 """Train the 3DSSD backbone + head with the reference's solver (solver.Trainer: scheduled BatchNorm decay, detection
-loss, per-rank clip, rank-ordered gradient mean, TF-style Adam under the step-driven learning rate; DESIGN.md 3.11).
+loss, per-rank clip, rank-ordered gradient mean, TF-style Adam or Momentum under the step-driven learning rate;
+DESIGN.md 3.11, 3.19).
 
     python tools/train.py --steps N [--batch 4] [--gpus G] [--ckpt DIR] [--resume FILE] [--data DIR] [--augment]
     torchrun --nproc_per_node G tools/train.py --gpus G ...
@@ -11,6 +12,11 @@ dicts (*.npy, kitti_io.read_sample) taken in order, --batch per rank.  The losse
 (reading them synchronises; the steps in between do not), a checkpoint named model-<global_step>.npz is written to --ckpt
 every Solver.checkpoint_interval steps and after the last one (rank 0), and --resume continues from such a file at its
 step, learning rate and BatchNorm decay.
+
+Fine-tuning (DESIGN.md 3.19): --train-prefix layer4,conv1d_0,pred_ trains only the variables whose names start with one
+of the prefixes (TRAIN.CONFIG.TRAIN_PARAM_PREFIX; re.match, as the reference's scope filter) and freezes the rest, which
+still run in training mode and update their BatchNorm statistics; usually after --warm-start.  --solver momentum
+(SOLVER.TYPE 'SGD') replaces Adam with tf.train.MomentumOptimizer(lr, --momentum) under the same schedule.
 
 With --augment the scenes go through the reference's training augmentation on the GPU (augment.Augmentor: flip,
 per-object noise, global rotation and scale, the context filter, then the choice of --points points), with draws seeded
@@ -88,6 +94,10 @@ def main(argv=None):
     ap.add_argument("--classes", default="Car", help="comma-separated class list of the head (DATASET.KITTI.CLS_LIST)")
     ap.add_argument("--mixup-classes", default="Car", help="comma-separated classes the mixup paste draws (names of --classes)")
     ap.add_argument("--mixup-numbers", default="15", help="comma-separated objects per scene of each --mixup-classes entry")
+    ap.add_argument("--train-prefix", default="",
+                    help="comma-separated variable-name prefixes to train, the rest frozen (TRAIN_PARAM_PREFIX; default all)")
+    ap.add_argument("--solver", choices=("adam", "momentum"), default="adam", help="SOLVER.TYPE: Adam, or 'SGD' (Momentum)")
+    ap.add_argument("--momentum", type=float, default=0.9, help="SOLVER.MOMENTUM of --solver momentum")
     a = ap.parse_args(argv)
     try:
         classes = pkg.config.check_cls_list(a.classes)
@@ -109,10 +119,13 @@ def main(argv=None):
         raise SystemExit("--gpus %d but WORLD_SIZE is %d (launch G > 1 ranks with torchrun)" % (a.gpus, world))
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
-    arch, solver = pkg.config.ARCH_3DSSD, S.Solver()
+    arch, solver = pkg.config.ARCH_3DSSD, S.Solver(type=a.solver, momentum=a.momentum)
     d = pkg.params.init_params(arch, 1, seed=0)
     d.update(pkg.params.init_head_params(pkg.config.layer_channels(arch, 1)[-1], cls_channels=len(classes), seed=1))
-    tp = pkg.params.TrainableParams(d, dev)
+    try:
+        tp = pkg.params.TrainableParams(d, dev, trainable=[p for p in a.train_prefix.split(",") if p])
+    except ValueError as e:
+        raise SystemExit("train.py: --train-prefix: %s" % e)
     dp = None
     if world > 1:
         dp = D.DataParallel(tp, D.PeerArena(D.DataParallel.symmetric_bytes(tp, world, sync_bn=a.sync_bn), dev),
